@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Benchmark of the exact-inference hot path (see the contract in the task brief).
+"""Benchmark of the exact-inference hot path on the H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload grid10x10|asia_1m|dag50]
                     [--rows R] [--impl b200|reference] [--no-extras] [--no-cpu-baseline]
+                    [--dump-outputs DIR]
 
 A *step* is one pass of the hot path over one batch of synthetic evidence rows:
 `rows` independent exact-inference queries (same query variables, same evidence
@@ -24,8 +25,13 @@ Rank 0 prints ONE JSON line:
              iterations per GPU)
 
 `--impl reference` times the CPU arm instead: the reference's `pointwise_mul` / `sum_out`
-(oracle/_ref, copied from /root/reference by oracle/build_ref.py) driven in min-fill order, one
+(oracle/_ref, copied from the reference project by oracle/build_ref.py) driven in min-fill order, one
 process per host core, a bounded sample of the same workload per step.
+
+`--dump-outputs DIR` (GPU arm) writes what the timed path returned in its last timed step --
+the posteriors, float32 [Q, rows] -- to DIR/posterior.npy.  The evidence rows are seeded, so two
+builds run with the same arguments can be compared output for output.  Above DUMP_BYTES a fixed,
+seeded sample of the rows is written instead, with their indices in DIR/posterior_rows.npy.
 """
 from __future__ import annotations
 
@@ -60,7 +66,30 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the `extra` block (the other BASELINE configs)")
     ap.add_argument("--dump", default="", help="write per-launch timings (JSON) here")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the posteriors of the last timed step to DIR/*.npy")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
+
+
+DUMP_BYTES = 64 << 20  # --dump-outputs: at most this much in all
+
+
+def dump_outputs(directory, posterior):
+    """Write the posteriors [Q, rows] of the last timed step as float32; past DUMP_BYTES, a fixed
+    seeded sample of rows (columns) and their indices (float64)."""
+    os.makedirs(directory, exist_ok=True)
+    posterior = np.ascontiguousarray(posterior, dtype=np.float32)
+    q, n = posterior.shape
+    arrays = {"posterior": posterior}
+    if posterior.nbytes > DUMP_BYTES:
+        keep = DUMP_BYTES // (4 * q + 8)
+        cols = np.sort(np.random.default_rng(0).choice(n, size=keep, replace=False))
+        arrays = {"posterior": np.ascontiguousarray(posterior[:, cols]), "posterior_rows": cols.astype(np.float64)}
+    for name, arr in arrays.items():
+        np.save(os.path.join(directory, f"{name}.npy"), arr)
 
 
 # ------------------------------------------------------------------ clocks sampling
@@ -72,7 +101,7 @@ class ClockSampler:
     def __init__(self, index: int):
         self.index = index
         self.sm, self.reasons_seen = [], 0
-        self.max_sm = None
+        self.max_sm = self.power_limit_w = None
         self._stop = threading.Event()
         self._ready = threading.Event()
         self._active = False
@@ -88,6 +117,7 @@ class ClockSampler:
             pynvml.nvmlInit()
             h = pynvml.nvmlDeviceGetHandleByIndex(self.index)
             self.max_sm = float(pynvml.nvmlDeviceGetMaxClockInfo(h, pynvml.NVML_CLOCK_SM))
+            self.power_limit_w = pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
             self._ok = True
             self._ready.set()
             while not self._stop.is_set():
@@ -115,12 +145,13 @@ class ClockSampler:
 
     def summary(self):
         if not self._ok or not self.sm:
-            return {"sm_mhz": None, "sm_max_mhz": self.max_sm, "reasons": [], "samples": 0}
+            return {"sm_mhz": None, "sm_max_mhz": self.max_sm, "power_limit_w": self.power_limit_w, "reasons": [],
+                    "samples": 0}
         bits = {"hw_slowdown": 0x8, "sw_power_cap": 0x4, "hw_thermal_slowdown": 0x40, "sw_thermal_slowdown": 0x20,
                 "hw_power_brake_slowdown": 0x80}
         reasons = [n for n, b in bits.items() if self.reasons_seen & b]
-        return {"sm_mhz": float(np.median(self.sm)), "sm_max_mhz": self.max_sm, "reasons": reasons,
-                "samples": len(self.sm)}
+        return {"sm_mhz": float(np.median(self.sm)), "sm_max_mhz": self.max_sm, "power_limit_w": self.power_limit_w,
+                "reasons": reasons, "samples": len(self.sm)}
 
 
 # ------------------------------------------------------------------------ CPU legs
@@ -303,19 +334,7 @@ def measured_peak():
                 return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic(workload: str):
-    """Per-launch DRAM traffic of the dominant kernel from the committed ncu capture."""
-    path = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(path):
-        try:
-            with open(path) as f:
-                return json.load(f).get(workload)
-        except Exception:
-            return None
-    return None
+    return 3350.0, "data sheet (H100 SXM, HBM3 3.35 TB/s)"
 
 
 def workload_config(wl, rows, world):
@@ -347,7 +366,7 @@ def run_reference(args, rank, world):
         arm.close()
     value = float(np.mean(rates))
     what = ("oracle/_ref = the reference's own pandas pointwise_mul / sum_out (bayes_net.py:54-256, copied unmodified "
-            "from /root/reference by oracle/build_ref.py) driven in min-fill order; the reference's own set-order "
+            "from the reference project by oracle/build_ref.py) driven in min-fill order; the reference's own set-order "
             "elimination is OOM-killed on the grid" if kind == "reference" else
             "oracle/ve_oracle.py, numpy port of the reference's variable elimination (oracle/_ref did not travel)")
     cpu = {"value": value, "unit": UNIT, "cores": cores, "kind": kind,
@@ -381,7 +400,7 @@ def run_reference(args, rank, world):
     print(json.dumps(line), flush=True)
 
 
-# ---------------------------------------------------------------------- B200 arm
+# ----------------------------------------------------------------------- GPU arm
 class Timer:
     """Device timing of `steps` calls of fn(): CUDA events on the current stream, a barrier +
     synchronize on both sides, optional L2 flush (a 256 MB write) before every timed call."""
@@ -459,7 +478,7 @@ def exact_workload(ctx, wl, rows, steps, warmup, want_profile=False, counts=None
     out_host = engine.PinnedArray((Q, rows), np.float32)
     distributed = world > 1
     step_bytes = plan.bytes_per_row() * rows
-    flush = step_bytes < 512e6  # working set could sit in the 126 MB L2: flush between steps
+    flush = step_bytes < 512e6  # working set could partly sit in the 50 MB L2: flush between steps
 
     if distributed:
         sp = sharding.ShardedProgram(prog, Q, n_ev, rows, dst=0, device=dev)
@@ -483,6 +502,9 @@ def exact_workload(ctx, wl, rows, steps, warmup, want_profile=False, counts=None
     launches0 = prog.info()["launches"]
     dev_ms = tm.device_ms(device_step, steps, flush)
     launches = prog.info()["launches"] - launches0
+    last_output = None  # what the last timed step returned to its caller, on rank 0
+    if rank == 0:
+        last_output = (sp.gathered.permute(1, 0, 2).reshape(Q, -1) if distributed else d_out[:, :rows]).cpu().numpy()
     for _ in range(max(1, warmup // 2)):
         host_step()
     e2e_s = tm.wall_s(host_step, steps)
@@ -501,7 +523,7 @@ def exact_workload(ctx, wl, rows, steps, warmup, want_profile=False, counts=None
         "plan": plan, "prog": prog, "bn": bn, "codes_host": codes_host, "rows": rows, "flush": flush,
         "ms_per_step": ms_per_step, "value": total_rows / (ms_per_step * 1e-3),
         "e2e_ms_per_step": 1e3 * e2e_s / steps, "e2e_value": total_rows / (e2e_s / steps),
-        "h2d": int(n_ev * rows) * world, "d2h": int(Q * rows * 4) * world, "e2e_api": e2e_api,
+        "h2d": int(n_ev * rows) * world, "d2h": int(Q * rows * 4) * world, "e2e_api": e2e_api, "last_output": last_output,
         "launches": int(launches) * world, "ok": ok, "same": same, "total_rows": total_rows,
         # bytes the launches as issued move: paired steps keep their intermediate in registers
         "bytes_issued_per_row": plan.bytes_per_row() - prog.info()["pair_bytes_saved_per_row"],
@@ -528,7 +550,7 @@ def summarise_exact(res, wl):
         "algorithmic_bytes_per_row": plan.bytes_per_row(), "bytes_per_row_as_issued": res["bytes_issued_per_row"],
         "hbm_roofline_frac_whole_step": res["whole_step_frac"],
         "launches_per_step": res["launches"] // max(1, res.get("steps", 1)),
-        "l2": "flushed (256 MB write) between timed steps" if res["flush"] else "not flushed (step streams >> 126 MB)",
+        "l2": "flushed (256 MB write) between timed steps" if res["flush"] else "not flushed (step streams >> 50 MB L2)",
         "checks": {"posteriors_sum_to_one": res["ok"], "host_path_equals_device_path": res["same"]},
     }
 
@@ -632,6 +654,8 @@ def run_b200(args, rank, world, local_rank):
     clocks.end()
     clock_summary = clocks.summary()
     clocks.close()
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, res["last_output"])
 
     # ---- the other BASELINE configs, a few seconds each (every rank takes part in the collectives)
     extra = {}
@@ -677,7 +701,6 @@ def run_b200(args, rank, world, local_rank):
             info = prog.info()
             kernel_bytes = float(sum(sb) - info["pair_bytes_saved_per_row"]) * rows
             achieved = kernel_bytes / (kernel_ms * 1e-3) / 1e9
-            traffic = ncu_traffic(wl.name) if rows == wl.default_rows else None
             n_batched = int(sum(1 for st in plan.steps if st.kind == planner.KIND_BATCHED))
             # per kernel family: bytes its launches move / their share of the timed step (roles from the engine)
             roles = prog.step_roles()
@@ -706,25 +729,19 @@ def run_b200(args, rank, world, local_rank):
                 d["share_of_step"] = d["ms"] / ms_per_step
             # headline = the dominant kernel family, per launch; the aggregate over every step kernel beside it
             dom_name, dom = max(fams.items(), key=lambda kv: kv[1]["ms"])
-            dom_traffic = None
-            if traffic and traffic.get("by_kernel", {}).get(dom_name):
-                tk = traffic["by_kernel"][dom_name]
-                dom_traffic = tk["dram_bytes"] / max(1, tk["launches"])
             roofline.update({
                 "kernel": f"{dom_name} ({dom['launches']} launches per step, {dom['share_of_step']:.0%} of the step)",
                 "achieved": dom["achieved_gbs"], "frac": dom["frac"],
                 "algorithmic_bytes_per_launch": dom["bytes_per_row"] * rows / max(1, dom["launches"]),
                 "avg_launch_ms": dom["ms"] / max(1, dom["launches"]),
-                "traffic": dom_traffic,
                 "all_step_kernels": {
                     "achieved": achieved, "frac": achieved / peak, "algorithmic_bytes_per_step": kernel_bytes,
                     "kernel_ms_per_step": kernel_ms, "kernel_share_of_step": share,
                     "launches_per_step": n_batched - info["pairs"], "fused_launches": info["pairs"],
                     "bytes_per_row_one_launch_per_step": int(sum(sb)),
                     "bytes_per_row_as_issued": int(sum(sb) - info["pair_bytes_saved_per_row"]),
-                    "traffic": (traffic or {}).get("dram_bytes_per_step"),
                 },
-                "by_kernel": fams, "traffic_detail": traffic,
+                "by_kernel": fams,
             })
             if args.dump:
                 with open(args.dump, "w") as f:
@@ -737,7 +754,7 @@ def run_b200(args, rank, world, local_rank):
         else:
             achieved = res["bytes_issued_per_row"] * rows / (ms_per_step * 1e-3) / 1e9
             roofline.update({"kernel": "whole step (per-launch profile only at N = 1)", "achieved": achieved,
-                             "frac": achieved / peak, "traffic": None})
+                             "frac": achieved / peak})
 
         cpu = None
         if not args.no_cpu_baseline and not distributed:
@@ -751,7 +768,8 @@ def run_b200(args, rank, world, local_rank):
 
         cfg = workload_config(wl, rows, world)
         line = {
-            "metric": METRIC, "value": res["value"], "unit": UNIT, "n_gpus": world, "steps": args.steps,
+            "metric": METRIC, "value": res["value"], "unit": UNIT, "n_gpus": world, "gpu": torch.cuda.get_device_name(dev),
+            "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": cfg,
@@ -760,7 +778,7 @@ def run_b200(args, rank, world, local_rank):
                 "elimination_steps": len(plan.steps), "max_factor_entries_per_row": plan.max_factor_per_row(),
                 "algorithmic_bytes_per_row": plan.bytes_per_row(), "bytes_per_row_as_issued": res["bytes_issued_per_row"],
                 "l2": ("flushed (256 MB write) between timed steps" if res["flush"] else
-                       f"not flushed: each step streams {plan.bytes_per_row() * rows / 1e9:.2f} GB of factors >> 126 MB L2"),
+                       f"not flushed: each step streams {plan.bytes_per_row() * rows / 1e9:.2f} GB of factors >> 50 MB L2"),
             },
             "e2e": {"value": res["e2e_value"], "unit": UNIT, "h2d_bytes_per_step": res["h2d"],
                     "d2h_bytes_per_step": res["d2h"], "ms_per_step": res["e2e_ms_per_step"], "api": res["e2e_api"]},

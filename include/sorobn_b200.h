@@ -1,5 +1,5 @@
 /*
- * sorobn_b200 -- C ABI of the B200 exact-inference engine.
+ * sorobn_b200 -- C ABI of the H100 (sm_90a) exact-inference engine.
  *
  * This is the drop-in boundary for the exact-inference path of MaxHalford/sorobn.
  * The reference has no native layer: the whole path is Python over pandas
@@ -48,7 +48,7 @@ extern "C" {
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
 #define SBN_E_CUDA (-2)      /* CUDA runtime error (see sbn_last_error)     */
 #define SBN_E_NOMEM (-3)     /* scratch does not fit the device             */
-#define SBN_E_NODEVICE (-4)  /* no usable sm_100 GPU                        */
+#define SBN_E_NODEVICE (-4)  /* no usable sm_90 GPU                         */
 
 typedef struct sbn_program sbn_program;
 

@@ -158,6 +158,34 @@ def synthetic_cases(ref, synthetic, spec, n_cases, n_ev_range, seed, n_query=(1,
     return cases
 
 
+def ordered_golden(ref):
+    """tests/golden/ordered_grid4x4s3.json: the reference's operators driven in the device program's
+    min-fill order (oracle/ref_driver.py, what the CPU legs of bench.py time) on a small grid, so that
+    the test pinning that driver to the oracle runs where the reference itself is absent."""
+    from sorobn_b200 import BayesNet, planner, synthetic
+
+    kwargs = dict(rows=4, cols=4, n_states=3, seed=11)
+    spec = synthetic.grid(**kwargs)
+    net = synthetic.load(spec, BayesNet)._compiled
+    bn = synthetic.load(spec, ref.BayesNet)
+    query, evs = ("g0303",), ("g0001", "g0102", "g0203", "g0300")
+    plan = planner.build_plan(net, [net.index[q] for q in query], [net.index[e] for e in evs])
+    order = [net.names[v] for v in plan.order]
+    events = synthetic.random_events(spec, evs, 3, seed=5)
+    cases = []
+    import warnings
+
+    for b in range(len(events)):
+        event = {v: int(events[v].iloc[b]) for v in evs}
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            cases.append(run_case_ordered(ref, bn, query, event, order))
+    with open(os.path.join(OUT, "ordered_grid4x4s3.json"), "w") as f:
+        json.dump({"network": "grid4x4s3", "kind": "ordered", "generator": "grid", "kwargs": kwargs,
+                   "digest": spec_digest(spec), "order": order, "cases": cases}, f)
+    print(f"ordered grid4x4s3: {len(cases)} cases")
+
+
 def main():
     ref = import_reference()
     sys.path.insert(0, ROOT)
@@ -233,6 +261,8 @@ def main():
             json.dump({"network": name, "kind": "synthetic", "generator": kind, "kwargs": kwargs,
                        "digest": spec_digest(spec), "cases": cases}, f)
         print(f"{name}: {len(cases)} cases in {time.time() - t:.1f}s")
+    if not only_workload:
+        ordered_golden(ref)
 
     # ---- the benchmark grid (BASELINE.json configs[2]): a few rows of the real workload
     from sorobn_b200 import workloads

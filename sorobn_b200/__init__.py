@@ -1,8 +1,8 @@
-"""sorobn_b200: B200-native exact inference for Bayesian networks.
+"""sorobn_b200: GPU-native exact inference for Bayesian networks on the NVIDIA H100.
 
 A drop-in for the exact-inference path of MaxHalford/sorobn
 (`BayesNet.query(..., algorithm="exact")`, `BayesNet.impute`), with the
-factor-product / sum-out loop running as hand-written sm_100a CUDA kernels.
+factor-product / sum-out loop running as hand-written sm_90a CUDA kernels.
 """
 from . import examples, planner, sharding, structure, synthetic, workloads
 from .bayes_net import BayesNet

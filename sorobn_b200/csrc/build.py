@@ -1,4 +1,4 @@
-"""Build libsorobn_b200.so (hand-written sm_100a kernels + C ABI) in-tree with nvcc.
+"""Build libsorobn_b200.so (hand-written sm_90a kernels + C ABI) in-tree with nvcc.
 
 No torch, no pybind: the library's only dependency is the CUDA runtime (linked
 statically), so it loads with ctypes from any process.
@@ -18,6 +18,7 @@ HEADERS = [os.path.join(HERE, h) for h in ("sbn_kernels.cuh", "sbn_gibbs.cuh", "
                                             "sbn_launch_impl.cuh")] + [
     os.path.join(os.path.dirname(PKG), "include", "sorobn_b200.h")]
 OBJ_DIR = os.path.join(HERE, "build")
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 
 
 def nvcc_path() -> str:
@@ -42,14 +43,14 @@ def _stale(target: str, deps) -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile every translation unit for sm_100a (in parallel, each only when it is stale) and link
+    """Compile every translation unit for sm_90a (in parallel, each only when it is stale) and link
     libsorobn_b200.so in-tree."""
     if not force and up_to_date():
         return LIB
     from concurrent.futures import ThreadPoolExecutor
 
     os.makedirs(OBJ_DIR, exist_ok=True)
-    flags = ["-Xcompiler", "-fPIC", "-O3", "-std=c++17", "-lineinfo", "-gencode", "arch=compute_100a,code=sm_100a",
+    flags = ["-Xcompiler", "-fPIC", "-O3", "-std=c++17", "-lineinfo", *GENCODE,
              "-Xptxas", "-v" if verbose else "-O3"]
 
     def compile_one(src):
@@ -71,7 +72,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if errors:
         sys.stderr.write("\n".join(errors))
         raise RuntimeError("nvcc failed building libsorobn_b200.so")
-    res = subprocess.run([nvcc_path(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB,
+    res = subprocess.run([nvcc_path(), "-shared", *GENCODE, "-o", LIB,
                           *[obj for obj, _ in results]], capture_output=True, text=True)
     if res.returncode != 0:
         sys.stderr.write(res.stdout + res.stderr)

@@ -200,9 +200,8 @@ constexpr int64_t kTileTableMax = 1 << 23;  // int32 words per step
 
 // Tables staged per CTA: SBN_SMEM_BUDGET keeps several CTAs per SM.  Opt-in experiment
 // (SOROBN_B200_SMEM_BIG=<KB>, up to 200): a launch around a larger CPT (8^5 entries = 128 KB) stages
-// it with ONE CTA per SM walking every tile of its rows.  Measured on dag50: no gain (4 warps per
-// SM are latency-bound on the shared-memory gathers: 2.65 vs 2.13 ms and 2.03 vs 2.21 ms on the two
-// launches it applies to), so the default leaves such tables to the L1/L2 gathers of the plain kernel.
+// it with ONE CTA per SM walking every tile of its rows.  4 warps per SM are latency-bound on the
+// shared-memory gathers, so the default leaves such tables to the L1/L2 gathers of the plain kernel.
 int64_t smem_big() {
     static const int64_t v = [] {
         const char *e = getenv("SOROBN_B200_SMEM_BIG");
@@ -225,8 +224,8 @@ int64_t smem_big() {
 int64_t slice_budget() {
     static const int64_t v = [] {
         const char *e = getenv("SOROBN_B200_SLICE_KB");
-        // swept on B200 (dag50, 1M rows): 64 KB -> 8.46 ms, 32 KB -> 8.14 ms (more CTAs per SM),
-        // 16 KB -> 10.8 ms (the launch with two 128 KB CPTs no longer fits and leaves the tiled kernel)
+        // 32 KB: more CTAs per SM than 64 KB, while a launch with two 128 KB CPTs still fits
+        // (at 16 KB it would leave the tiled kernel)
         const int64_t kb = e ? atoll(e) : 32;
         return std::max<int64_t>(1024, std::min<int64_t>(kb * 1024, SBN_SMEM_BUDGET));
     }();
@@ -587,23 +586,23 @@ void build_params(const sbn_program *P, const StepDesc &st, const uint8_t *ev, i
     if (tiled) {
         const int64_t rows_per_cta = static_cast<int64_t>(tiled_threads()) * kRowsPerThread;
         const int64_t n_rblocks = (n_rows + rows_per_cta - 1) / rows_per_cta;
-        // enough CTAs for ~8 waves (148 SMs x ~6 resident CTAs), otherwise as many
+        // enough CTAs for ~8 waves (SMs x ~6 resident CTAs), otherwise as many
         // consecutive tiles per CTA as possible (neighbouring tiles share operands in L1)
         static const int64_t target_env = [] {
             const char *e = getenv("SOROBN_B200_TARGET_CTAS");
             return e ? atoll(e) : 0LL;
         }();
-        // swept on B200 (grid workload): 3552 -> 4.20 ms, 7104 -> 4.10 ms, 14208 -> 4.23 ms
+        const int64_t sms = P->n_sms;
         // big tables: one CTA per SM, so few CTAs that each amortise their 100+ KB of staging
-        int64_t target = st.big_tables ? 4 * 148 : (target_env > 0 ? target_env : 8 * 148 * 6);
+        int64_t target = st.big_tables ? 4 * sms : (target_env > 0 ? target_env : 8 * sms * 6);
         static const int64_t small_env = [] {
             const char *e = getenv("SOROBN_B200_SMALL_WAVE");
             return e ? atoll(e) : 2000LL;
         }();
         // A launch with few tiles in total (at one tile per CTA: under ~4.5 waves) runs as ONE wave
         // of CTAs that each walk all their tiles: staging and the first loads are paid once per CTA,
-        // not once per tile (grid: 3.305 -> 3.264 ms; the 125-entry table-only launches 22 -> 17 us).
-        if (small_env > 0 && !st.big_tables && st.n_tiles * n_rblocks <= small_env) target = 3 * 148;
+        // not once per tile.
+        if (small_env > 0 && !st.big_tables && st.n_tiles * n_rblocks <= small_env) target = 3 * sms;
         int64_t chunks = std::max<int64_t>(1, std::min<int64_t>(st.n_tiles, target / std::max<int64_t>(1, n_rblocks)));
         int64_t tpc = (st.n_tiles + chunks - 1) / chunks;
         if (st.slice_pos >= 0) tpc = st.slice_tpc;  // the slices were cut for this chunk size
@@ -636,10 +635,10 @@ void build_params(const sbn_program *P, const StepDesc &st, const uint8_t *ev, i
         const int64_t n_bblocks = (n_rows + rows_per_cta - 1) / rows_per_cta;
         const int64_t rest = st.n_out / (static_cast<int64_t>(c0) * c1);
         // Tile = axis 0 x tile1 digits of axis 1.  Start from ~32 outputs per thread and
-        // shrink while the grid is below two full waves (148 SMs x 16 CTAs).
+        // shrink while the grid is below two full waves (SMs x 16 CTAs).
         int tile1 = std::max(1, std::min(c1, 32 / std::max(1, c0)));
         auto ctas = [&](int t1) { return n_bblocks * ((c1 + t1 - 1) / t1) * rest; };
-        while (tile1 > 1 && ctas(tile1) < 2 * 148 * 16) tile1 = (tile1 + 1) / 2;
+        while (tile1 > 1 && ctas(tile1) < 2 * static_cast<int64_t>(P->n_sms) * 16) tile1 = (tile1 + 1) / 2;
         q->tile1 = tile1;
         q->n_tile1 = (c1 + tile1 - 1) / tile1;
         q->n_bblocks = static_cast<int32_t>(n_bblocks);
@@ -756,9 +755,8 @@ int run_table_steps(sbn_program *P) {
 // slab / TMA / plain variants) and its whole output is ONE tile (Q <= T x T joint query states).
 inline bool fold_normalise(const sbn_program *P, const StepDesc &st, const SbnStep &q) {
 #if !SBN_FOLD_NORMALISE
-    // Compiled out by default (sbn_kernels.cuh): measured on B200, the extra epilogue in every instantiation of
-    // the tiled kernel costs ~10 % on ALL launches (grid 3.14 -> 3.46 ms, dag50 7.26 -> 7.64 ms) to save one
-    // 6 us launch (Asia 30 -> 24 us).
+    // Compiled out by default (sbn_kernels.cuh): the extra epilogue lands in every instantiation of the
+    // tiled kernel, so every launch pays for it to save one small normalisation launch.
     (void)P;
     (void)st;
     (void)q;
@@ -966,8 +964,10 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
     SBN_CUDA_P(cudaSetDevice(device));
     cudaDeviceProp prop;
     SBN_CUDA_P(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return bail(fail(SBN_E_NODEVICE, "device %d is sm_%d%d; this library is built for sm_100a only",
-                                           device, prop.major, prop.minor));
+    if (prop.major != 9 || prop.minor != 0)
+        return bail(fail(SBN_E_NODEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major,
+                         prop.minor));
+    P->n_sms = prop.multiProcessorCount;
     SBN_CUDA_P(cudaStreamCreateWithFlags(&P->stream, cudaStreamNonBlocking));
     for (int k = 0; k < sbn_program::kBranches; ++k)
         SBN_CUDA_P(cudaStreamCreateWithFlags(&P->branch[k], cudaStreamNonBlocking));
@@ -1182,7 +1182,7 @@ static int run_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int
     // cut into column ranges of the same staging buffers, H2D / kernels / D2H run on three streams
     // chained by events, so a range's posteriors drain while the next range computes and the one
     // after uploads -- PCIe is full duplex.  Launch-heavy programs (the grid: 48 launches per run,
-    // 5 MB of copies against 3 ms of kernels) keep the single CUDA-graph replay.
+    // 5 MB of copies against milliseconds of kernels) keep the single CUDA-graph replay.
     int64_t launches_per_run = 1;
     for (size_t k = 0; k < P->steps.size(); ++k)
         if (!hoisted(P, P->steps[k])) ++launches_per_run;
@@ -1195,8 +1195,7 @@ static int run_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int
         constexpr int kMaxRanges = 8;
         static const int kRanges = [] {
             const char *e = getenv("SOROBN_B200_PIPE_RANGES");
-            // swept on B200 (Asia, 1M rows, 4 MB in + 8 MB out): 2 / 3 / 4 / 6 / 8 ranges -> 0.240 / 0.235 / 0.245 /
-            // 0.251 / 0.253 ms, unpipelined 0.268 ms: the copies (51 GB/s for both directions together) are the bound
+            // few ranges: each range adds copies and launches, and the copies are the bound
             const int v = e ? atoi(e) : 3;
             return v >= 2 && v <= kMaxRanges ? v : 3;
         }();
@@ -1207,8 +1206,8 @@ static int run_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int
         cudaStream_t s_in = P->branch[0], s_run = P->stream, s_out = P->branch[1];
         const int64_t range = round_up((n_rows + kRanges - 1) / kRanges, 32);
         // the whole fan-out is issued into a stream capture and replayed as ONE graph launch when the
-        // host buffers are pinned (a dozen copies, launches and event edges cost more CPU time than
-        // the 0.2 ms they overlap); the graph is kept for the (buffers, rows) it was built for
+        // host buffers are pinned (a dozen copies, launches and event edges cost CPU time of the order
+        // of what they overlap); the graph is kept for the (buffers, rows) it was built for
         auto pinned = [](const void *ptr) {
             cudaPointerAttributes a;
             if (cudaPointerGetAttributes(&a, ptr) != cudaSuccess) {

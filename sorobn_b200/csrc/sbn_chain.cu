@@ -581,8 +581,7 @@ bool chainable(const sbn_program *P, const StepDesc &st, int64_t tab_max) {
 int input_class(const StepDesc &st, int i) { return i < st.nu ? 0 : i < st.nu + st.na ? 1 : i < st.nu + st.na + st.nb ? 2 : 3; }
 
 int chain_grid(const sbn_program *P, const SbnSegment &seg) {
-    int sms = 148;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, P->device);
+    const int sms = P->n_sms;
     int per_sm = 1;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sbn_chain_kernel, seg.threads, seg.smem_bytes) != cudaSuccess || per_sm < 1) {
         cudaGetLastError();
@@ -599,9 +598,8 @@ void sbn_chain_plan(sbn_program *P) {
     P->seg_first.assign(P->steps.size(), -1);
     if (P->mode != 1 || P->f64) return;
     // Segments are planned for every batched program (cheap) but only USED when the program's
-    // use_chain switch is on: SOROBN_B200_CHAIN=1 or sbn_program_set_tiled(prog, 7).  Measured on
-    // B200 (DESIGN.md "On-chip segments"): the benchmark grid runs 4.85 ms through one 47-step
-    // segment against 3.16 ms through the per-step launches, so the default stays the latter.
+    // use_chain switch is on: SOROBN_B200_CHAIN=1 or sbn_program_set_tiled(prog, 7).  The default stays
+    // the per-step launches (DESIGN.md "On-chip segments").
     static const int min_steps = env_int("SOROBN_B200_CHAIN_MIN", 4);
     static const int tab_kb = env_int("SOROBN_B200_CHAIN_TAB_KB", 32);  // tables of one step
     const int64_t tab_max = static_cast<int64_t>(tab_kb) * 1024 / 4;

@@ -22,9 +22,7 @@
 //   * every CPT is staged in shared memory when the network's tables fit (42 KB for the 100-node
 //     benchmark grid), the chain states live there as [variable][chain] bytes (conflict-free);
 //   * the weights of the <= 8 states stay in registers (SBN_GIBBS_MAX_CARD falls back to local memory).
-// 64 chains per CTA: 10k chains make 157 CTAs, one or two per SM on all 148 of them.
-// (round 1: CSR arrays and CPTs in global memory, w[64] in local memory: 2.9 us per update;
-//  now ~0.15 us, the device time of 10k chains x 10k iterations went from 28.8 ms to ~2 ms.)
+// 64 chains per CTA: 10k chains make 157 CTAs, one or two per SM on all 132 SMs of an H100.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -245,7 +243,7 @@ __global__ void __launch_bounds__(SBN_GIBBS_CHAINS) sbn_gibbs_kernel(const __gri
 // padded with a dummy state slot that is always 0 and a dummy 1.0 table entry (stride 0).  Every
 // word of the record, every state byte and every table entry of an update is then an independent
 // load: the update's latency is three dependent shared-memory reads deep instead of one per loop
-// iteration of the generic kernel (measured: 1.26 us -> ~0.2 us per update).  Arithmetic and random
+// iteration of the generic kernel.  Arithmetic and random
 // stream are the generic kernel's, bit for bit (padding multiplies by 1.0f).
 #define SBN_GF_GROUPS 5
 #define SBN_GF_TERMS 4

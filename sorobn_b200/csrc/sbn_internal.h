@@ -65,6 +65,7 @@ struct SbnPair;     // sbn_pair.h
 
 struct sbn_program {
     int device = 0;
+    int n_sms = 1;     // multiprocessors of `device`: the grid-size heuristics count waves in them
     bool f64 = false;  // single-event programs computed and returned in double
     int mode = 0, n_ev = 0, Q = 0, post_slot = 0, post_batched = 0;
     std::vector<std::pair<int64_t, int64_t>> tables;  // (offset, size) in floats

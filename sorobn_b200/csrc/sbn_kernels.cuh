@@ -1,4 +1,4 @@
-// sorobn_b200 -- sm_100a kernels for the factor-product / sum-out step.
+// sorobn_b200 -- sm_90a kernels for the factor-product / sum-out step.
 //
 // One launch computes, for every output entry o and evidence row b,
 //
@@ -134,23 +134,11 @@ __device__ __forceinline__ void sbn_pdl_entry() {
     asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 
-// Packed fp32 FMA (fma.rn.f32x2 -> SASS FFMA2): two evidence rows per issue slot.  Same FP32 rate as two FFMA
-// (tools/micro/ffma2_bench.cu: 71 vs 73 TFLOP/s), half the instructions.
-#ifndef SBN_FFMA2
-#define SBN_FFMA2 1
-#endif
+// FMA of two evidence rows held in a register pair.  sm_90 has no packed fp32 FMA, so this is two scalar
+// FFMA with the same rounding (one fused multiply-add per row).
 __device__ __forceinline__ void sbn_fma2(float (&acc)[2], const float (&a)[2], const float (&b)[2]) {
-#if SBN_FFMA2
-    unsigned long long ra, rb, rc;
-    memcpy(&ra, a, 8);
-    memcpy(&rb, b, 8);
-    memcpy(&rc, acc, 8);
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(rc) : "l"(ra), "l"(rb));
-    memcpy(acc, &rc, 8);
-#else
     acc[0] = fmaf(a[0], b[0], acc[0]);
     acc[1] = fmaf(a[1], b[1], acc[1]);
-#endif
 }
 
 __device__ __forceinline__ float4 sbn_mul4(float4 a, float4 b) {

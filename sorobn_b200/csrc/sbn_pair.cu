@@ -46,8 +46,8 @@ __device__ __forceinline__ void pair_step(const float (&in)[SBN_PAIR_T][SBN_PAIR
                                           const float *k, const int (&e)[V], const PairG &G) {
     constexpr int T = SBN_PAIR_T, PW = SBN_PAIR_PW;
     // per-row coefficients that arrive one value (CE) or one row pair (GB / GC) at a time are kept as (row 0, row 1)
-    // register pairs and go through the packed FFMA2; float4 loads (B, CU) fill four registers of ONE row, pairing
-    // them up would cost more moves than the packed FMA saves
+    // register pairs and go through sbn_fma2; float4 loads (B, CU) fill four registers of ONE row and are
+    // accumulated one register at a time
     constexpr bool PACKED = V == 2 && (MODE == SBN_PAIR_CE || MODE == SBN_PAIR_GB || MODE == SBN_PAIR_GC);
 #pragma unroll
     for (int d0 = 0; d0 < T; ++d0)
@@ -98,8 +98,7 @@ __device__ __forceinline__ void pair_step(const float (&in)[SBN_PAIR_T][SBN_PAIR
 //   step 2: out[w][z] = sum_y c2[y][w][z] * pre2[y][w] * mid[y][w]
 // Coefficients past a real cardinality are zero, F indices past one are clamped: the loop nest is
 // always T x T x T and only the stores are predicated.
-// Five CTAs per SM (96 registers, a handful of spilled bytes): measured on B200, grid 100k rows, 2 / 3 / 4 / 5 / 6 / 8
-// resident CTAs -> 2.65 / 2.65 / 2.57 / 2.52 / 2.60 / 2.92 ms per step.  (Four with a batched coefficient operand: its
+// Five CTAs per SM (96 registers, a handful of spilled bytes).  (Four with a batched coefficient operand: its
 // fifteen pre-scaled offsets would spill at 96 registers.)
 template <int M1, int M2>
 __global__ void __launch_bounds__(SBN_PAIR_ROWS / kV, (M1 >= SBN_PAIR_GB ? 4 : 5)) sbn_pair_kernel(const __grid_constant__ SbnPairParams p) {
@@ -800,7 +799,7 @@ static cudaError_t triple_launch(sbn_program *P, const SbnPair &pr, int64_t n_ro
         const char *e = getenv("SOROBN_B200_TRIPLE_TPC");
         return e ? atoll(e) : 1LL;
     }();
-    // measured on B200 (grid, 100k rows): 3 CTAs / SM (128 registers) 440-453 us, 2 CTAs (152 registers) 464-515 us
+    // resident CTAs per SM the triple kernel is compiled for: 3 (128 registers) by default, 1 or 2 on request
     static const int minb = [] {
         const char *e = getenv("SOROBN_B200_TRIPLE_MINB");
         return e ? atoi(e) : 3;
@@ -846,10 +845,11 @@ cudaError_t sbn_pair_launch(sbn_program *P, const SbnPair &pr, const uint8_t *d_
     q.canon = P->d_pair_canon + pr.canon_pos;
     q.tile_off = P->d_pair_tiles + pr.tile_off_pos;
     const int64_t n_rblocks = (n_rows + SBN_PAIR_ROWS - 1) / SBN_PAIR_ROWS;
-    static const int64_t target = [] {
+    static const int64_t target_env = [] {
         const char *e = getenv("SOROBN_B200_PAIR_CTAS");
-        return e ? atoll(e) : 8LL * 148 * 6;
+        return e ? atoll(e) : 0LL;
     }();
+    const int64_t target = target_env > 0 ? target_env : 8LL * P->n_sms * 6;  // ~8 waves of 6 CTAs per SM
     const int64_t chunks = std::max<int64_t>(1, std::min<int64_t>(q.n_tiles, target / std::max<int64_t>(1, n_rblocks)));
     const int64_t tpc = (q.n_tiles + chunks - 1) / chunks;
     q.tiles_per_cta = static_cast<int32_t>(tpc);

@@ -396,8 +396,7 @@ cudaError_t sbn_tma_launch(sbn_program *P, const StepDesc &st, const uint8_t *d_
     }
     // Tensor maps.  Preferred: a 4-D view (rows, tile digit, eliminated state, entry) of the factor whose
     // box (256, tn, CX, 1) is the whole operand block of a tile -- ONE TMA instruction per operand
-    // and stage (25 one-entry boxes per stage saturate the TMA unit's issue rate before HBM:
-    // measured 98 us against 92 us for the register-preload kernel on `625 <- sum_5 t x B625`).
+    // and stage (25 one-entry boxes per stage saturate the TMA unit's issue rate before HBM).
     // The view needs non-zero strides for both axes; otherwise fall back to (rows, entries) with
     // one-entry boxes.
     static const int big_env = env_int("SOROBN_B200_TMA_BIGBOX", 1);
@@ -445,8 +444,7 @@ cudaError_t sbn_tma_launch(sbn_program *P, const StepDesc &st, const uint8_t *d_
     while (S > 2 && smem_of(S) > 110 * 1024) --S;
     if (smem_of(S) > 200 * 1024) return cudaErrorInvalidConfiguration;
     q.n_stages = S;
-    int sms = 148;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, P->device);
+    const int sms = P->n_sms;
     const int per_sm = smem_of(S) + 2048 <= 113 * 1024 ? 2 : 1;
     const int grid = static_cast<int>(std::min<int64_t>(q.n_items, static_cast<int64_t>(sms) * per_sm));
     const size_t smem = smem_of(S);

@@ -3,7 +3,7 @@
 This is the "thin C-ABI/ctypes shim" between the Python host (`BayesNet.query`) and
 the CUDA kernels.  There is deliberately no fallback: if the library has not been
 built (`python -m sorobn_b200.csrc.build` / `__graft_entry__.build()`), cannot be
-loaded, or no sm_100 GPU is visible, construction raises.
+loaded, or no sm_90 GPU is visible, construction raises.
 """
 from __future__ import annotations
 

@@ -60,9 +60,8 @@ MAX_EV = 8  # evidence axes per input (SBN_MAX_EV)
 TILE_EDGE = 5  # largest register-tile edge of sbn_step_tiled
 MAX_ELIM = 3  # variables summed out by one launch (SBN_MAX_ELIM)
 MAX_Z = 256  # joint states of the variables summed out by one launch
-# Largest table (entries) that may keep evidence axes.  Swept on B200: 4096 is best on all three
-# benchmark networks (grid 4.21 ms against 4.34 ms without and 4.38 ms at 16384, where a consumer
-# ends up gathering from a 62 KB table for every output).
+# Largest table (entries) that may keep evidence axes.  Much larger tables make a consumer gather
+# from a big table (62 KB at 16384 entries on the grid) for every output.
 LIFT_MAX = int(os.environ.get("SOROBN_B200_LIFT_MAX", "4096"))
 TILED_MAX_IN = 4  # inputs of one launch of the tiled kernel (csrc: kTiledMaxIn)
 SLICE_MIN_BYTES = 64 * 1024  # tables of one launch beyond this are laid out for sliced staging (csrc: SBN_SMEM_BUDGET)

@@ -2,7 +2,7 @@
 
 The golden vectors were produced by the real reference (oracle/gen_golden.py); the
 hand-written values below are the reference's own doctest outputs
-(/root/reference/sorobn/bayes_net.py and examples.py)."""
+(sorobn/bayes_net.py and examples.py of MaxHalford/sorobn)."""
 import numpy as np
 import pytest
 
@@ -162,35 +162,41 @@ def test_oracle_gibbs_conditionals_match_reference(name):
 
 
 def test_reference_copy_driven_in_min_fill_order_matches_the_oracle():
-    """`oracle/_ref` (the reference itself, copied by oracle/build_ref.py) driven through
-    oracle/ref_driver.ordered_query -- what bench.py's CPU legs time -- gives the oracle's
-    posterior.  Skipped where the copy was not built."""
+    """The reference's operators driven through oracle/ref_driver.ordered_query in the device
+    program's min-fill order -- what bench.py's CPU legs time -- give the oracle's posterior.
+    The reference's answers are stored in tests/golden/ordered_grid4x4s3.json (oracle/gen_golden.py);
+    where `oracle/_ref` was built, the live copy must reproduce them too."""
+    from conftest import spec_digest
     from oracle import build_ref, ref_driver
-    from sorobn_b200 import planner, synthetic
+    from sorobn_b200 import BayesNet, planner, synthetic
 
-    if not build_ref.available():
-        pytest.skip("oracle/_ref not built (python oracle/build_ref.py needs /root/reference)")
     import warnings
 
-    ref = build_ref.import_reference()
-    from sorobn_b200 import BayesNet
-
-    spec = synthetic.grid(4, 4, 3, seed=11)
+    golden = load_golden("ordered_grid4x4s3")
+    spec = synthetic.grid(**golden["kwargs"])
+    assert spec_digest(spec) == golden["digest"], "synthetic generator drifted: regenerate tests/golden"
     ours = synthetic.load(spec, BayesNet)
-    theirs = synthetic.load(spec, ref.BayesNet)
     net = ours._compiled
     query, evs = ("g0303",), ("g0001", "g0102", "g0203", "g0300")
     plan = planner.build_plan(net, [net.index[q] for q in query], [net.index[e] for e in evs])
     order = [net.names[v] for v in plan.order]
+    assert order == golden["order"]
     dn = oracle_net(ours)
     events = synthetic.random_events(spec, evs, 3, seed=5)
-    for b in range(len(events)):
+    ref = build_ref.import_reference() if build_ref.available() else None
+    theirs = synthetic.load(spec, ref.BayesNet) if ref is not None else None
+    assert len(golden["cases"]) == len(events)
+    for b, case in enumerate(golden["cases"]):
         event = {v: int(events[v].iloc[b]) for v in evs}
-        with warnings.catch_warnings():
-            warnings.simplefilter("ignore")
-            got = ref_driver.ordered_query(ref, theirs, query, event, order)
+        assert case_event(case) == event and case["names"] == list(query)
         want = ve_oracle.query(dn, *query, event=event)[1].reshape(-1)
-        dense = np.zeros_like(want)
-        for k, v in got.items():
-            dense[dn.domains[query[0]].index(k)] = v
-        assert np.allclose(dense, want, rtol=1e-12, atol=0)
+        stored = dense_answer(case, dn.domains)
+        assert np.allclose(stored, want, rtol=1e-12, atol=0)
+        if ref is not None:
+            with warnings.catch_warnings():
+                warnings.simplefilter("ignore")
+                got = ref_driver.ordered_query(ref, theirs, query, event, order)
+            dense = np.zeros_like(want)
+            for k, v in got.items():
+                dense[dn.domains[query[0]].index(k)] = v
+            assert np.allclose(dense, stored, rtol=1e-12, atol=0)
