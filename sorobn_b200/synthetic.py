@@ -47,10 +47,12 @@ def _random_cpt(rng, parent_cards, card, alpha=1.0):
     return arr
 
 
-def grid(rows: int, cols: int, n_states: int, seed: int = 0, alpha: float = 1.0) -> NetSpec:
+def grid(rows: int, cols: int, n_states, seed: int = 0, alpha: float = 1.0) -> NetSpec:
     """rows x cols lattice; node (i, j) has parents (i-1, j) and (i, j-1).
 
     Node names are strings "gRRCC" so that lexicographic order == row-major order.
+    `n_states` is one cardinality for every node or a sequence cycled over the nodes in
+    row-major order.
     """
     rng = np.random.default_rng(seed)
     name = lambda i, j: f"g{i:02d}{j:02d}"
@@ -58,7 +60,6 @@ def grid(rows: int, cols: int, n_states: int, seed: int = 0, alpha: float = 1.0)
     for i in range(rows):
         for j in range(cols):
             n = name(i, j)
-            nodes.append(n)
             ps = []
             if i > 0:
                 ps.append(name(i - 1, j))
@@ -67,10 +68,13 @@ def grid(rows: int, cols: int, n_states: int, seed: int = 0, alpha: float = 1.0)
             ps.sort()
             if ps:
                 parents[n] = ps
-            cards[n] = n_states
+            k = len(nodes)
+            cards[n] = int(n_states) if np.isscalar(n_states) else int(n_states[k % len(n_states)])
+            nodes.append(n)
     for n in nodes:
         cpt[n] = _random_cpt(rng, [cards[p] for p in parents.get(n, [])], cards[n], alpha)
-    return NetSpec(f"grid{rows}x{cols}s{n_states}", nodes, parents, cards, cpt)
+    tag = n_states if np.isscalar(n_states) else "x".join(map(str, n_states))
+    return NetSpec(f"grid{rows}x{cols}s{tag}", nodes, parents, cards, cpt)
 
 
 def random_dag(n_nodes: int, max_parents: int, n_states, seed: int = 0, alpha: float = 1.0,

@@ -209,7 +209,9 @@ def test_tiled_and_plain_kernels_agree_with_oracle(cards):
     from oracle import ve_oracle
     from sorobn_b200 import BayesNet, engine, planner, synthetic
 
-    rng = np.random.default_rng(hash(str(cards)) % 2**32)
+    import zlib
+
+    rng = np.random.default_rng(zlib.crc32(str(cards).encode()))  # stable across processes, unlike hash()
     worst = 0.0
     for trial in range(3):
         spec = synthetic.random_dag(14, 3, cards, seed=40 + trial, window=5)
@@ -262,10 +264,11 @@ def test_full_size_grid_properties():
     perm = np.random.default_rng(0).permutation(B)
     shuffled = prog.run(np.ascontiguousarray(codes[:, perm]), B)
     assert np.array_equal(shuffled, out[:, perm])
-    # chunking invariance: a second program restricted to 4096-row chunks agrees bitwise
+    # chunking invariance: the batch run as 4096-row pieces (the last one partial) agrees bitwise.  (A
+    # reservation alone does not chunk: a run grows it to the batch when device memory allows.)
     small = engine.Program(plan)
-    small.reserve(4096)
-    assert np.array_equal(small.run(codes, B), out)
+    pieces = [small.run(np.ascontiguousarray(codes[:, lo:lo + 4096]), min(4096, B - lo)) for lo in range(0, B, 4096)]
+    assert np.array_equal(np.concatenate(pieces, axis=1), out)
     # oracle on a sample of rows
     dn = ve_oracle.dense_from_pandas(bn.P, bn.parents, bn.nodes)
     order = [net.names[v] for v in plan.order]
