@@ -18,6 +18,7 @@
 #include "sbn_chain.h"
 #include "sbn_gibbs.cuh"
 #include "sbn_internal.h"
+#include "sbn_join.h"
 #include "sbn_kernels.cuh"
 #include "sbn_launch.h"
 #include "sbn_pair.h"
@@ -671,6 +672,7 @@ cudaError_t launch_step(sbn_program *P, const StepDesc &st, const SbnStep &q, cu
     P->launches++;
     if (st.kind == 1 && q.tile_off != nullptr && sbn_tma_eligible(P, st))
         return sbn_tma_launch(P, st, q.ev, q.ld_ev, q.n_rows, stream);
+    if (st.kind == 1 && q.tile_off != nullptr && sbn_join_rows(P, st, q) > 0) return sbn_join_launch(P, st, q, stream);
     if (st.kind == 1 && q.tile_off != nullptr) {
         const int64_t chunks = (q.n_tiles + q.tiles_per_cta - 1) / q.tiles_per_cta;
         const int64_t grid = chunks * q.n_bblocks;
@@ -1016,6 +1018,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
             SBN_CUDA_P(set_tiled_attrs());
             SBN_CUDA_P(sbn_chain_set_attrs());
             SBN_CUDA_P(sbn_tma_set_attrs());
+            SBN_CUDA_P(sbn_join_set_attrs());
             done[device] = true;
         }
     }

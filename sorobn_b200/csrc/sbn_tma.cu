@@ -290,6 +290,17 @@ cudaError_t set_attr() {
 
 }  // namespace
 
+bool sbn_tma_encode_rows(CUtensorMap *map, const float *base, int64_t ld, int64_t n_rows, int64_t entries, int box_rows, int e_lo) {
+    if (!encode_fn() || e_lo <= 0 || entries % e_lo != 0) return false;
+    const cuuint64_t dims[3] = {static_cast<cuuint64_t>(n_rows), static_cast<cuuint64_t>(e_lo), static_cast<cuuint64_t>(entries / e_lo)};
+    const cuuint64_t strides[2] = {static_cast<cuuint64_t>(ld) * 4, static_cast<cuuint64_t>(ld) * 4 * e_lo};
+    const cuuint32_t box[3] = {static_cast<cuuint32_t>(box_rows), static_cast<cuuint32_t>(e_lo), static_cast<cuuint32_t>(entries / e_lo)};
+    const cuuint32_t estr[3] = {1, 1, 1};
+    return encode_fn()(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float *>(base), dims, strides, box, estr,
+                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
 cudaError_t sbn_tma_set_attrs() {
     cudaError_t e = set_attr<5, 5>();
     if (e == cudaSuccess) e = set_attr<4, 4>();

@@ -79,3 +79,8 @@ bool sbn_tma_eligible(const sbn_program *P, const StepDesc &st);
 cudaError_t sbn_tma_launch(sbn_program *P, const StepDesc &st, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows,
                            cudaStream_t stream);
 cudaError_t sbn_tma_set_attrs();
+// Tensor map of the first n_rows rows of a batched factor [entries][ld] as the 3-D view
+// (row, entry % e_lo, entry / e_lo), box = (box_rows, e_lo, entries / e_lo): one instruction copies the whole
+// factor for box_rows rows, entry-major in shared memory.  Rows past n_rows arrive as zeros.  false when the
+// driver has no encoder or refuses the view.
+bool sbn_tma_encode_rows(CUtensorMap *map, const float *base, int64_t ld, int64_t n_rows, int64_t entries, int box_rows, int e_lo);
