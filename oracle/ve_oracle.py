@@ -344,3 +344,18 @@ def gibbs_conditional(net: DenseNet, node):
     with np.errstate(invalid="ignore", divide="ignore"):
         table = vals / vals.sum(axis=-1, keepdims=True)
     return boundary, table
+
+
+def gibbs_conditional_at(net: DenseNet, node, state: dict):
+    """One row of `gibbs_conditional`: P(node | Markov boundary) for the boundary values in
+    `state` (node -> state value; other entries are ignored), without building the table over the
+    whole boundary, which a variable with many children cannot afford.  NaN when every state of
+    `node` has probability zero."""
+    children = [c for c in net.nodes if node in net.parents.get(c, ())]
+    dom = net.domains[node]
+    w = np.ones(len(dom))
+    for n in [node, *children]:
+        index = tuple(slice(None) if v == node else net.domains[v].index(state[v]) for v in net.scope(n))
+        w = w * net.cpt[n][index]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        return w / w.sum()

@@ -1573,11 +1573,28 @@ int sbn_gibbs_create(int device, int32_t n_vars, const int32_t *card, const int3
     // the straight-line variant (sbn_gibbs_flat_kernel): fixed-size records, when the network is small enough
     std::vector<int32_t> flat;
     bool flat_ok = max_card <= 8 && n_query <= 4 && n_vars < 0xffff;
+    // The straight-line kernel multiplies its <= 5 factors without the rescaling of sbn_gibbs_weights.
+    // It takes a cycle position only when the product of the smallest non-zero entries of those
+    // tables stays far above float32's smallest normal, so that no weight can underflow and both
+    // kernels pick the same states.
+    std::vector<double> min_entry(n_vars, 1.0);
+    if (flat_ok)
+        for (int v = 0; v < n_vars; ++v) {
+            int64_t size = card[v];
+            for (int k = par_ptr[v]; k < par_ptr[v + 1]; ++k) size *= card[par_idx[k]];
+            for (int64_t e = 0; e < size; ++e) {
+                const float t = tables[cpt_off[v] + e];
+                if (t > 0.f) min_entry[v] = std::min(min_entry[v], static_cast<double>(t));
+            }
+        }
     const int32_t ones_off = static_cast<int32_t>(n_table_floats);  // a 1.0f appended to the table blob
     for (int i = 0; i < n_cycle && flat_ok; ++i) {
         const int v = cycle[i];
         const int np = par_ptr[v + 1] - par_ptr[v], nc = chi_ptr[v + 1] - chi_ptr[v];
         if (np > SBN_GF_TERMS || nc > SBN_GF_GROUPS - 1) { flat_ok = false; break; }
+        double smallest = min_entry[v];
+        for (int k = chi_ptr[v]; k < chi_ptr[v + 1]; ++k) smallest *= min_entry[chi_idx[k]];
+        if (smallest < 1e-30) { flat_ok = false; break; }
         std::vector<int32_t> rec(SBN_GF_WORDS, 0);
         rec[0] = v | card[v] << 16;
         auto group = [&](int g) { return rec.data() + 2 + g * (2 + 2 * SBN_GF_TERMS); };
@@ -1777,7 +1794,8 @@ static int sampler_run(sbn_sampler *S, int algo, const uint8_t *ev, int64_t ld_e
         else sbn_gibbs_kernel<SBN_GIBBS_MAX_CARD><<<static_cast<unsigned>(grid), SBN_GIBBS_CHAINS, smem, S->stream>>>(g);
     } else {
         // one CTA per evidence row; its threads share the row's n_iterations samples
-        const size_t smem = ((static_cast<size_t>(S->n_vars) * (SBN_GIBBS_THREADS + 1) + 15) / 16) * 16 + static_cast<size_t>(S->Q) * 8;
+        // (per joint query state: a double sum and a uint32 count)
+        const size_t smem = ((static_cast<size_t>(S->n_vars) * (SBN_GIBBS_THREADS + 1) + 15) / 16) * 16 + static_cast<size_t>(S->Q) * 12;
         if (smem > 200 * 1024) return fail(SBN_E_INVALID, "sampler state needs %zu bytes of shared memory", smem);
         sbn_forward_kernel<<<static_cast<unsigned>(n_chains), SBN_GIBBS_THREADS, smem, S->stream>>>(g, algo);
     }

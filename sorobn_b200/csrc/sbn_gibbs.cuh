@@ -115,6 +115,13 @@ struct SbnRng {
 //              n_other x (other parent variable, stride)
 // Un-normalised P(v = x | Markov blanket) for x < card into w[] (bayes_net.py:699-712 computes the
 // same table ahead of time with pandas; here it is evaluated for the current state only).
+// The product runs over every child in float32, so a variable with many children (a naive-Bayes
+// class variable) would underflow to all zeros.  After each child's factor, weights whose largest
+// entry fell below SBN_GIBBS_TINY are all multiplied by SBN_GIBBS_RESCALE.  A power of two scales
+// every weight, every prefix sum and u * total exactly, so no comparison of the draw changes where
+// nothing underflowed; weights stay below 2^32 (the CPT row gives a largest entry >= 1 / card).
+#define SBN_GIBBS_TINY 0x1p-32f
+#define SBN_GIBBS_RESCALE 0x1p64f
 template <int MAXC, typename StateFn, typename TableFn>
 __device__ __forceinline__ int sbn_gibbs_weights(const int32_t *__restrict__ r, StateFn state, TableFn table, float (&w)[MAXC]) {
     const int v_c = r[0];
@@ -130,9 +137,17 @@ __device__ __forceinline__ int sbn_gibbs_weights(const int32_t *__restrict__ r, 
         const int sv = r[2], no = r[3];
         r += 4;
         for (int k = 0; k < no; ++k, r += 2) cb += state(r[0]) * r[1];
+        float m = 0.f;
 #pragma unroll
         for (int x = 0; x < MAXC; ++x)
-            if (x < c) w[x] *= table(cb + x * sv);
+            if (x < c) {
+                w[x] *= table(cb + x * sv);
+                m = fmaxf(m, w[x]);
+            }
+        if (m < SBN_GIBBS_TINY) {
+#pragma unroll
+            for (int x = 0; x < MAXC; ++x) w[x] *= SBN_GIBBS_RESCALE;
+        }
     }
     return v_c;
 }
@@ -212,8 +227,10 @@ __global__ void __launch_bounds__(SBN_GIBBS_CHAINS) sbn_gibbs_kernel(const __gri
             total += w[x];
             cum[x] = total;
         }
+        // one draw per update, used or not, as in sbn_gibbs_flat_kernel: the two kernels' streams stay aligned
+        const float u01 = rng.uniform();
         if (total > 0.f) {  // an all-zero conditional (deterministic CPTs) keeps the current value
-            const float u = rng.uniform() * total;
+            const float u = u01 * total;
             // first x with u <= cum[x] == number of x with cum[x] < u (cum is flat, = total >= u,
             // beyond the cardinality; a zero-weight state repeats its predecessor's cum and is never picked)
             int pick = 0;
@@ -384,19 +401,21 @@ __global__ void sbn_gibbs_conditional_kernel(const SbnGibbs p, int pos, const ui
 //           contradict the event are dropped; the answer is the frequency of each query state
 //           among the kept ones (NaN when none is kept: the reference returns an empty Series).
 // One CTA per evidence row, its threads share the row's samples; per-state sums live in
-// shared memory (atomics, low contention).
+// shared memory (atomics, low contention).  A sample's likelihood is a product over every
+// variable: on the 100-node benchmark grid it is around 1e-60, below float32's range, so the
+// likelihood, the per-state sums and the normalisation are kept in double.
 __global__ void __launch_bounds__(SBN_GIBBS_THREADS) sbn_forward_kernel(const __grid_constant__ SbnGibbs p, int algo) {
-    extern __shared__ uint8_t s_raw[];
+    extern __shared__ __align__(16) uint8_t s_raw[];
     const int T = SBN_GIBBS_THREADS;
     uint8_t *state = s_raw + threadIdx.x;                                             // [n_vars][T]
     uint8_t *evcode = s_raw + static_cast<size_t>(p.n_vars) * T;                      // [n_vars], 0xff = free
-    float *acc_sum = reinterpret_cast<float *>(s_raw + ((static_cast<size_t>(p.n_vars) * (T + 1) + 15) / 16) * 16);  // [Q]
+    double *acc_sum = reinterpret_cast<double *>(s_raw + ((static_cast<size_t>(p.n_vars) * (T + 1) + 15) / 16) * 16);  // [Q]
     uint32_t *acc_cnt = reinterpret_cast<uint32_t *>(acc_sum + p.Q);                  // [Q]
     const int64_t row = blockIdx.x;
 
     for (int v = threadIdx.x; v < p.n_vars; v += T) evcode[v] = 0xff;
     for (int q = threadIdx.x; q < p.Q; q += T) {
-        acc_sum[q] = 0.f;
+        acc_sum[q] = 0.0;
         acc_cnt[q] = 0;
     }
     __syncthreads();
@@ -409,7 +428,7 @@ __global__ void __launch_bounds__(SBN_GIBBS_THREADS) sbn_forward_kernel(const __
     for (int64_t it = threadIdx.x; it < p.n_iterations; it += T) {
         SbnRng rng;
         rng.init(p.seed, static_cast<uint64_t>(row) * static_cast<uint64_t>(p.n_iterations) + static_cast<uint64_t>(it));
-        float lik = 1.f;
+        double lik = 1.0;
         bool keep = true;
         for (int v = 0; v < p.n_vars; ++v) {
             int base = p.cpt_off[v];
@@ -431,7 +450,7 @@ __global__ void __launch_bounds__(SBN_GIBBS_THREADS) sbn_forward_kernel(const __
                 }
                 if (algo == 2 && evcode[v] != 0xff && x != evcode[v]) keep = false;
             }
-            lik *= __ldg(p.tables + base + x);
+            lik *= static_cast<double>(__ldg(p.tables + base + x));
             state[v * T] = static_cast<uint8_t>(x);
         }
         int qi = 0;
@@ -446,17 +465,27 @@ __global__ void __launch_bounds__(SBN_GIBBS_THREADS) sbn_forward_kernel(const __
     __syncthreads();
     // normalise: likelihood -> per-state mean, then over the states; rejection -> frequency
     __shared__ float s_total;
+    __shared__ double s_total64;
     if (threadIdx.x == 0) {
-        float total = 0.f;
-        for (int q = 0; q < p.Q; ++q) {
-            const float v = algo == 1 ? (acc_cnt[q] ? acc_sum[q] / static_cast<float>(acc_cnt[q]) : 0.f)
-                                      : static_cast<float>(acc_cnt[q]);
-            acc_sum[q] = v;
-            total += v;
+        if (algo == 1) {
+            double total = 0.0;
+            for (int q = 0; q < p.Q; ++q) {
+                const double v = acc_cnt[q] ? acc_sum[q] / static_cast<double>(acc_cnt[q]) : 0.0;
+                acc_sum[q] = v;
+                total += v;
+            }
+            s_total64 = total;
+        } else {
+            float total = 0.f;
+            for (int q = 0; q < p.Q; ++q) total += static_cast<float>(acc_cnt[q]);
+            s_total = total;
         }
-        s_total = total;
     }
     __syncthreads();
-    for (int q = threadIdx.x; q < p.Q; q += T)
-        p.out[static_cast<int64_t>(q) * p.ld_out + row] = s_total > 0.f ? acc_sum[q] / s_total : __int_as_float(0x7fc00000);
+    for (int q = threadIdx.x; q < p.Q; q += T) {
+        float f;
+        if (algo == 1) f = s_total64 > 0.0 ? static_cast<float>(acc_sum[q] / s_total64) : __int_as_float(0x7fc00000);
+        else f = s_total > 0.f ? static_cast<float>(acc_cnt[q]) / s_total : __int_as_float(0x7fc00000);
+        p.out[static_cast<int64_t>(q) * p.ld_out + row] = f;
+    }
 }

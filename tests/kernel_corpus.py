@@ -114,6 +114,22 @@ def evidence_rows(spec, evidence, n_rows, seed=0):
     return np.ascontiguousarray(joint[:, :n_rows])
 
 
+def naive_bayes(n_children=60, root_states=5, child_states=17, seed=0):
+    """A class variable `c` with `n_children` children `f00`, `f01`, ... and no other edge: the shape
+    where the product over a variable's children in the Gibbs conditional underflows float32.  The
+    CPT entries are float32 values (rows sum to 1 within float32 rounding), so the float64 oracle
+    and the device's float32 tables hold the same numbers."""
+    rng = np.random.default_rng(seed)
+    kids = [f"f{k:02d}" for k in range(n_children)]
+    nodes = ["c", *kids]
+    cpt = {"c": rng.dirichlet(np.ones(root_states))}
+    for k in kids:
+        cpt[k] = rng.dirichlet(np.ones(child_states), size=root_states)
+    cpt = {n: np.asarray(a, dtype=np.float32).astype(np.float64) for n, a in cpt.items()}
+    return synthetic.NetSpec(f"naive{n_children}s{root_states}x{child_states}", nodes, {k: ["c"] for k in kids},
+                             {"c": root_states, **{k: child_states for k in kids}}, cpt)
+
+
 def case_id(case):
     return case["name"]
 

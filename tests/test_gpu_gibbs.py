@@ -111,38 +111,6 @@ def test_gibbs_conditionals_match_the_reference_tables():
     assert checked > 200
 
 
-def _lw_reference_estimator(bn, query, event):
-    """Exact expectation of the reference's likelihood-weighting estimator
-    (bayes_net.py:621-663), by enumeration: samples are drawn from g(s) = prod over non-event
-    variables of P(v | parents) with the event clamped, each is weighted by the JOINT
-    probability P(s) (bayes_net.py:546 multiplies over all variables), the per-state MEAN
-    weight is taken (:660) and normalised (:661)."""
-    import itertools
-
-    net = bn._compiled
-    names = net.names
-    doms = [range(int(c)) for c in net.card]
-    qids = sorted((net.index[q] for q in query), key=lambda v: names[v])
-    ev = {net.index[k]: net.domains[net.index[k]].index(v) for k, v in event.items()}
-    num = {}
-    den = {}
-    for s in itertools.product(*doms):
-        if any(s[v] != x for v, x in ev.items()):
-            continue
-        joint, g = 1.0, 1.0
-        for v in range(len(names)):
-            p = net.cpt[v][tuple(s[u] for u in net.parents[v]) + (s[v],)]
-            joint *= p
-            if v not in ev:
-                g *= p
-        key = tuple(s[v] for v in qids)
-        num[key] = num.get(key, 0.0) + g * joint
-        den[key] = den.get(key, 0.0) + g
-    means = {k: num[k] / den[k] for k in num if den[k] > 0}
-    total = sum(means.values())
-    return {k: v / total for k, v in means.items()}
-
-
 def test_rejection_sampling_converges_to_exact_posterior():
     from sorobn_b200 import examples
 
@@ -162,13 +130,14 @@ def test_rejection_sampling_converges_to_exact_posterior():
 
 
 def test_likelihood_weighting_matches_the_reference_estimator():
+    from oracle.sampler_replay import lw_expectation
     from sorobn_b200 import examples
 
     for make, query, event in ((examples.sprinkler, ("Rain",), {"Sprinkler": True}),
                                (examples.alarm, ("Burglary",), {"John calls": True, "Mary calls": True}),
                                (examples.grades, ("Letter", "SAT"), {"Intelligence": "Smart"})):
         bn = make(seed=5)
-        want = _lw_reference_estimator(bn, query, event)
+        want = lw_expectation(bn._compiled, query, event)
         got = bn.query(*query, event=event, algorithm="likelihood", n_iterations=2_000_000)
         net = bn._compiled
         assert np.isclose(got.sum(), 1.0, atol=1e-5)
