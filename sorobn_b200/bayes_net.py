@@ -342,27 +342,34 @@ class BayesNet:
         return frame if n > 1 else frame.iloc[0]
 
     # ---------------------------------------------------------------------- query
-    def _plan(self, query, evidence_vars, mode, robust=False, device=None):
+    def _plan(self, query, evidence_vars, mode, robust=False, device=None, marginals=False):
+        """(plan, program) of P(query | evidence vars), cached.  marginals=True: `query` are the targets of
+        a marginals program (planner.build_marginals_plan), cached under its own mode key."""
         with self._cache_lock:
-            return self._plan_locked(query, evidence_vars, mode, robust, device)
+            return self._plan_locked(query, evidence_vars, mode, robust, device, marginals)
 
-    def _plan_locked(self, query, evidence_vars, mode, robust, device):
+    def _plan_locked(self, query, evidence_vars, mode, robust, device, marginals=False):
         if self._compiled is None:
             self._compile()
             if self._compiled is None:
                 raise ValueError("every node needs a CPT in P before querying; call prepare()")
         net = self._compiled
         device = self.device if device is None else device
-        key = (tuple(query), tuple(evidence_vars), mode, robust, device)
+        key = (tuple(query), tuple(evidence_vars), ("marginals", mode) if marginals else mode, robust, device)
         hit = self._engine_cache.get(key)
         if hit is None:
             for name in (*query, *evidence_vars):
                 if name not in net.index:
                     raise KeyError(name)
             twin = next((v for k, v in self._engine_cache.items() if isinstance(v, tuple) and k[:4] == key[:4]), None)
-            plan = twin[0] if twin else _planner.build_plan(
-                net, [net.index[q] for q in query], [net.index[e] for e in evidence_vars],
-                mode=mode, allow_empty_query=True)  # the same plan serves every device
+            if twin:
+                plan = twin[0]  # the same plan serves every device
+            elif marginals:
+                plan = _planner.build_marginals_plan(net, [net.index[e] for e in evidence_vars],
+                                                     targets=[net.index[q] for q in query], mode=mode)
+            else:
+                plan = _planner.build_plan(net, [net.index[q] for q in query], [net.index[e] for e in evidence_vars],
+                                           mode=mode, allow_empty_query=True)
             from . import engine  # raises if libsorobn_b200.so cannot be loaded
 
             # single-event programs run in float64 (latency-bound anyway); batches in float32,
@@ -533,24 +540,96 @@ class BayesNet:
             out.loc[events.index[bad]] = np.nan
         return out
 
-    def _posterior_codes(self, query, ev_vars, codes, bad, device=None):
+    def _posterior_codes(self, query, ev_vars, codes, bad, device=None, marginals=False):
         """Posterior float64 [Q, n] for uint8 evidence codes [n_ev, n] on one device.  Rows the
         float32 program flags (NaN: impossible evidence, or an entry below the float32 range)
         are settled in float64 -- a few one by one with the single-event program, many as one
-        batch with the batched float64 program; a row that is still NaN there is impossible."""
+        batch with the batched float64 program; a row that is still NaN there is impossible.
+        marginals=True: `query` are the targets of a marginals program (every segment normalised)."""
         n = codes.shape[1] if len(ev_vars) else len(bad)
-        _, program = self._plan(query, ev_vars, _planner.MODE_BATCHED, device=device)
+        _, program = self._plan(query, ev_vars, _planner.MODE_BATCHED, device=device, marginals=marginals)
         post = self._run_evicting(program, codes, n).astype(np.float64)  # [Q, n]
         suspect = np.isnan(post).any(axis=0) & ~bad
         rows = np.nonzero(suspect)[0]
         if len(rows) > 8:
-            _, robust = self._plan(query, ev_vars, _planner.MODE_BATCHED, robust=True, device=device)
+            _, robust = self._plan(query, ev_vars, _planner.MODE_BATCHED, robust=True, device=device, marginals=marginals)
             post[:, rows] = robust.run(np.ascontiguousarray(codes[:, rows]), len(rows))
         elif len(rows):
-            _, flat = self._plan(query, ev_vars, _planner.MODE_FLAT, device=device)
+            _, flat = self._plan(query, ev_vars, _planner.MODE_FLAT, device=device, marginals=marginals)
             for b in rows:
                 post[:, b] = flat.run(np.ascontiguousarray(codes[:, b:b + 1]), 1)[:, 0]
         return post
+
+    def _targets(self, variables, ev_vars):
+        """Target names of a marginals query, sorted: `variables`, or every variable that is not evidence."""
+        if self._compiled is None:
+            self._compile()
+            if self._compiled is None:
+                raise ValueError("every node needs a CPT in P before querying; call prepare()")
+        if variables is None:
+            variables = [n for n in self.nodes if n not in set(ev_vars)]
+        variables = list(variables)
+        for v in variables:
+            if v in ev_vars:
+                raise ValueError("A query variable cannot be part of the event")
+            if v not in self._compiled.index:
+                raise KeyError(v)
+        if not variables:
+            raise ValueError("At least one query variable has to be specified")
+        return tuple(sorted(set(variables)))
+
+    def marginals_many(self, events: pd.DataFrame, variables=None) -> pd.DataFrame:
+        """The posterior marginal of every variable in `variables` (default: every variable that is not
+        a column of `events`), for every row of `events`, from ONE device program: an upward and a
+        downward pass over the bucket tree of the elimination, then one readout per variable
+        (planner.build_marginals_plan).  Equals `query_many(v, events=events)` for each v.
+
+        Returns one row per evidence row; the columns are a MultiIndex of (variable, state), variables
+        sorted by name, states sorted.  Zero-probability states stay (as 0.0); impossible rows and rows
+        with a value outside its variable's domain are NaN."""
+        ev_vars = tuple(events.columns)
+        targets = self._targets(variables, ev_vars)
+        net = self._compiled
+        columns = pd.MultiIndex.from_tuples([(t, s) for t in targets for s in net.domains[net.index[t]]],
+                                            names=["variable", "state"])
+        n = len(events.index)
+        if n == 0:
+            return pd.DataFrame(np.zeros((0, len(columns))), index=events.index, columns=columns)
+        codes, bad = self._encode_events(ev_vars, [events[v].to_numpy() for v in ev_vars])
+        if not ev_vars:
+            bad = np.zeros(n, dtype=bool)
+        post = self._posterior_codes(targets, ev_vars, codes, bad, marginals=True)
+        out = pd.DataFrame(post.T, index=events.index, columns=columns)
+        if bad.any():
+            out.loc[events.index[bad]] = np.nan
+        return out
+
+    def marginals(self, event: dict, variables=None) -> dict:
+        """`marginals_many` for one event, in float64 (as `query`): {variable: Series}, each Series equal to
+        `query(variable, event=event)` -- named "P(variable)", zero states left out, empty for evidence of
+        probability zero."""
+        ev_vars = tuple(event)
+        targets = self._targets(variables, ev_vars)
+        net = self._compiled
+        plan, program = self._plan(targets, ev_vars, _planner.MODE_FLAT, marginals=True)
+        codes = np.empty((len(ev_vars), 1), dtype=np.uint8)
+        bad = False
+        for i, v in enumerate(ev_vars):
+            code = self._code_of(net.index[v]).get(event[v], -1)
+            bad |= code < 0
+            codes[i, 0] = max(code, 0)
+        post = None if bad else program.run(codes, 1)[:, 0].astype(np.float64)
+        out, q = {}, 0
+        for t in targets:
+            index = pd.Index(net.domains[net.index[t]], name=t)
+            seg = None if post is None else post[q:q + len(index)]
+            q += len(index)
+            if seg is None or np.isnan(seg).any():
+                out[t] = pd.Series([], index=index[:0], name=f"P({t})", dtype=np.float64)
+            else:
+                keep = seg > 0
+                out[t] = pd.Series(seg[keep], index=index[keep], name=f"P({t})")
+        return out
 
     def _run_evicting(self, program, codes, n):
         """`program.run`, retried once after closing every OTHER cached device object when the device

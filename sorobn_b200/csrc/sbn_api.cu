@@ -21,6 +21,7 @@
 #include "sbn_join.h"
 #include "sbn_kernels.cuh"
 #include "sbn_launch.h"
+#include "sbn_marginal.cuh"
 #include "sbn_pair.h"
 #include "sbn_tma.h"
 
@@ -48,6 +49,8 @@ int fail(int code, const char *fmt, ...) {
 
 constexpr int32_t kMagic = 0x53424E31;
 constexpr int kVersion = 4;
+constexpr int kVersionMarginals = 5;  // planner.build_marginals_plan: kind-2 readouts, no posterior slot
+constexpr int64_t kMarginalZoffMax = 1 << 24;  // int32 words of one readout's joint-state offset table
 constexpr int kMaxElim = 3;
 constexpr int kMaxZ = 256;
 constexpr int kHeaderWords = 12;
@@ -59,7 +62,9 @@ namespace {
 int parse(sbn_program *P, const int32_t *w, int64_t n) {
     if (n < kHeaderWords) return fail(SBN_E_INVALID, "program shorter than its header");
     if (w[0] != kMagic) return fail(SBN_E_INVALID, "bad program magic 0x%x", w[0]);
-    if (w[1] != kVersion) return fail(SBN_E_INVALID, "program version %d, engine expects %d", w[1], kVersion);
+    if (w[1] != kVersion && w[1] != kVersionMarginals)
+        return fail(SBN_E_INVALID, "program version %d, engine expects %d or %d", w[1], kVersion, kVersionMarginals);
+    P->marginals = w[1] == kVersionMarginals;
     P->mode = w[2];
     P->n_ev = w[3];
     const int n_tables = w[4], n_slots = w[5], n_steps = w[6];
@@ -69,7 +74,8 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
     if (P->mode != 0 && P->mode != 1) return fail(SBN_E_INVALID, "bad mode %d", P->mode);
     if (P->n_ev < 0 || n_tables < 0 || n_slots <= 0 || n_steps <= 0 || P->Q <= 0)
         return fail(SBN_E_INVALID, "bad header counts");
-    if (P->post_slot < 0 || P->post_slot >= n_slots) return fail(SBN_E_INVALID, "post slot out of range");
+    if (P->marginals ? (P->post_slot != -1 || P->post_batched != 0) : (P->post_slot < 0 || P->post_slot >= n_slots))
+        return fail(SBN_E_INVALID, "post slot out of range");
     int64_t p = kHeaderWords;
     auto need = [&](int64_t k) { return p + k <= n; };
     if (!need(2LL * n_tables + 2LL * n_slots)) return fail(SBN_E_INVALID, "truncated table/slot section");
@@ -88,8 +94,9 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         if (batched && P->mode == 0) return fail(SBN_E_INVALID, "batched slot in a flat program");
         P->slots.push_back({batched != 0, size, round_up(size, 4), nullptr});
     }
-    if ((P->slots[P->post_slot].batched ? 1 : 0) != P->post_batched || P->slots[P->post_slot].size < P->Q)
+    if (!P->marginals && ((P->slots[P->post_slot].batched ? 1 : 0) != P->post_batched || P->slots[P->post_slot].size < P->Q))
         return fail(SBN_E_INVALID, "posterior slot mismatch");
+    std::vector<int> written(P->marginals ? P->Q : 0, 0);  // posterior entries written by the readouts
     for (int s = 0; s < n_steps; ++s) {
         if (!need(5)) return fail(SBN_E_INVALID, "truncated step %d", s);
         StepDesc st;
@@ -100,12 +107,20 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         const int n_elim = w[p + 4];
         st.cx = 1;
         p += 5;
-        if (st.kind != 0 && st.kind != 1) return fail(SBN_E_INVALID, "step %d: bad kind", s);
+        const bool readout = st.kind == 2;
+        if (st.kind != 0 && st.kind != 1 && !(readout && P->marginals)) return fail(SBN_E_INVALID, "step %d: bad kind", s);
+        if (readout) {
+            // one output axis (the target), written at posterior rows q_offset .. q_offset + card - 1
+            if (!need(1)) return fail(SBN_E_INVALID, "truncated step %d", s);
+            st.q_offset = w[p++];
+            if (st.out_slot != -1 || n_axes != 1 || n_elim < 0 || n_elim > 64)
+                return fail(SBN_E_INVALID, "step %d: bad readout step", s);
+        }
         if (st.kind == 1 && P->mode == 0) return fail(SBN_E_INVALID, "step %d: batched step in a flat program", s);
         if (n_in < 1 || n_in > SBN_MAX_IN) return fail(SBN_E_INVALID, "step %d: %d inputs", s, n_in);
         if (n_axes < 0 || n_axes > SBN_MAX_AXES) return fail(SBN_E_INVALID, "step %d: %d axes", s, n_axes);
-        if (n_elim < 0 || n_elim > kMaxElim) return fail(SBN_E_INVALID, "step %d: %d eliminated axes", s, n_elim);
-        if (st.out_slot < 0 || st.out_slot >= n_slots) return fail(SBN_E_INVALID, "step %d: out slot", s);
+        if (!readout && (n_elim < 0 || n_elim > kMaxElim)) return fail(SBN_E_INVALID, "step %d: %d eliminated axes", s, n_elim);
+        if (!readout && (st.out_slot < 0 || st.out_slot >= n_slots)) return fail(SBN_E_INVALID, "step %d: out slot", s);
         if (!need(n_axes + n_elim)) return fail(SBN_E_INVALID, "truncated step %d", s);
         st.n_out = 1;
         for (int j = 0; j < n_axes; ++j) {
@@ -119,14 +134,21 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         for (int k = 0; k < n_elim; ++k) {
             const int c = w[p + k];
             if (c < 1) return fail(SBN_E_INVALID, "step %d: eliminated card %d", s, c);
-            if (static_cast<int64_t>(st.cx) * c > kMaxZ) return fail(SBN_E_INVALID, "step %d: too many eliminated states", s);
+            if (static_cast<int64_t>(st.cx) * c > (readout ? kMarginalZoffMax / SBN_MAX_IN : kMaxZ))
+                return fail(SBN_E_INVALID, "step %d: too many eliminated states", s);
             st.cx *= c;
             st.ecards.push_back(c);
         }
         p += n_elim;
-        const Slot &os = P->slots[st.out_slot];
-        if (os.batched != (st.kind == 1)) return fail(SBN_E_INVALID, "step %d: out slot kind mismatch", s);
-        if (os.size < st.n_out) return fail(SBN_E_INVALID, "step %d: out slot too small", s);
+        if (readout) {
+            if (st.q_offset < 0 || st.q_offset + st.n_out > P->Q) return fail(SBN_E_INVALID, "step %d: segment outside the posterior", s);
+            for (int64_t q = st.q_offset; q < st.q_offset + st.n_out; ++q) written[q]++;
+        } else {
+            const Slot &os = P->slots[st.out_slot];
+            if (os.batched != (st.kind == 1)) return fail(SBN_E_INVALID, "step %d: out slot kind mismatch", s);
+            if (os.size < st.n_out) return fail(SBN_E_INVALID, "step %d: out slot too small", s);
+        }
+        const bool per_row = st.kind == 1 || (readout && P->mode == 1);  // batched operands allowed
         for (int i = 0; i < n_in; ++i) {
             if (!need(4)) return fail(SBN_E_INVALID, "truncated step %d input %d", s, i);
             InDesc in;
@@ -150,9 +172,9 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
                 if (in.batched) return fail(SBN_E_INVALID, "step %d input %d: batched table", s, i);
                 size = P->tables[in.id].second;
             }
-            if (in.batched && st.kind != 1) return fail(SBN_E_INVALID, "step %d: batched input in flat step", s);
+            if (in.batched && !per_row) return fail(SBN_E_INVALID, "step %d: batched input in flat step", s);
             if (in.batched && n_ev) return fail(SBN_E_INVALID, "step %d input %d: batched input with ev axes", s, i);
-            if (n_ev && st.kind != 1 && P->mode != 0)
+            if (n_ev && !per_row && P->mode != 0)
                 return fail(SBN_E_INVALID, "step %d input %d: evidence axes in an unbatched step", s, i);
             int64_t max_off = 0;
             for (int k = 0; k < n_ev; ++k) {
@@ -181,6 +203,10 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             if (max_off >= size) return fail(SBN_E_INVALID, "step %d input %d: reads past its buffer", s, i);
             st.in.push_back(std::move(in));
         }
+        if (readout) {
+            std::stable_partition(st.in.begin(), st.in.end(), [](const InDesc &in) { return in.strides[0] == 0; });
+            st.n_common = static_cast<int>(std::count_if(st.in.begin(), st.in.end(), [](const InDesc &in) { return in.strides[0] == 0; }));
+        }
         P->steps.push_back(std::move(st));
     }
     if (p != n) return fail(SBN_E_INVALID, "trailing words in program");
@@ -192,7 +218,12 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             if (st.kind == 0 && ++writes[st.out_slot] > 1)
                 return fail(SBN_E_INVALID, "unbatched slot %d is written twice in a batched program", st.out_slot);
     }
-    if (P->steps.back().out_slot != P->post_slot) return fail(SBN_E_INVALID, "last step does not write the posterior");
+    if (P->marginals) {
+        for (int q = 0; q < P->Q; ++q)
+            if (written[q] != 1) return fail(SBN_E_INVALID, "posterior entry %d is written %d times", q, written[q]);
+    } else if (P->steps.back().out_slot != P->post_slot) {
+        return fail(SBN_E_INVALID, "last step does not write the posterior");
+    }
     return SBN_OK;
 }
 
@@ -379,7 +410,7 @@ void plan_tiles(sbn_program *P, std::vector<int32_t> *words) {
     // zoff[i][z] = sum_k digit_k(z) * estride_i[k], first eliminated variable fastest
     for (StepDesc &st : P->steps) {
         st.zoff_pos = -1;
-        if (st.ecards.size() < 2) continue;
+        if (st.ecards.size() < 2 && st.kind != 2) continue;
         st.zoff_pos = static_cast<int64_t>(words->size());
         for (const InDesc &in : st.in) {
             for (int z = 0; z < st.cx; ++z) {
@@ -670,7 +701,7 @@ cudaError_t set_tiled_attrs() {
 
 cudaError_t launch_step(sbn_program *P, const StepDesc &st, const SbnStep &q, cudaStream_t stream) {
     P->launches++;
-    if (st.kind == 1 && q.tile_off != nullptr && sbn_tma_eligible(P, st))
+    if (st.kind == 1 && q.tile_off != nullptr && !P->marginals && sbn_tma_eligible(P, st))
         return sbn_tma_launch(P, st, q.ev, q.ld_ev, q.n_rows, stream);
     if (st.kind == 1 && q.tile_off != nullptr && sbn_join_rows(P, st, q) > 0) return sbn_join_launch(P, st, q, stream);
     if (st.kind == 1 && q.tile_off != nullptr) {
@@ -705,6 +736,58 @@ cudaError_t launch_step(sbn_program *P, const StepDesc &st, const SbnStep &q, cu
         return cudaGetLastError();
     }
     return sbn_batched_launch(q, grid, stream);
+}
+
+// Readout of one target (kind 2): its segment of the posterior, normalised, for rows 0 .. n_rows - 1.
+cudaError_t launch_marginal(sbn_program *P, const StepDesc &st, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, float *d_out,
+                            int64_t ld_out, cudaStream_t stream) {
+    P->launches++;
+    SbnMarginal m;
+    memset(&m, 0, sizeof m);
+    const size_t elem = P->f64 ? 8 : 4;
+    m.out = reinterpret_cast<char *>(d_out) + st.q_offset * ld_out * static_cast<int64_t>(elem);
+    m.ld_out = ld_out;
+    m.ev = ev;
+    m.ld_ev = ld_ev;
+    m.ld = P->ld;
+    m.zoff = P->d_tile_off + st.zoff_pos;
+    m.min_total = P->f64 ? 1e-290 : static_cast<double>(SBN_MIN_TOTAL_F32);
+    m.n_rows = static_cast<int32_t>(n_rows);
+    m.n_in = static_cast<int32_t>(st.in.size());
+    m.n_common = st.n_common;
+    m.card = st.cards[0];
+    m.cz = st.cx;
+    int64_t smem = 0;
+    for (size_t i = 0; i < st.in.size(); ++i) {
+        const InDesc &in = st.in[i];
+        SbnMargIn &d = m.in[i];
+        int64_t padded;
+        if (in.is_slot) {
+            d.ptr = P->slots[in.id].ptr;
+            padded = P->slots[in.id].padded;
+        } else {
+            d.ptr = reinterpret_cast<const char *>(P->d_tables) + P->tables[in.id].first * static_cast<int64_t>(elem);
+            padded = P->table_padded[in.id];
+        }
+        d.batched = in.batched ? 1 : 0;
+        d.ts = in.strides[0];
+        d.n_ev = static_cast<int32_t>(in.ev.size());
+        for (size_t k = 0; k < in.ev.size(); ++k) {
+            d.ev_col[k] = in.ev[k].col;
+            d.ev_stride[k] = in.ev[k].stride;
+            d.ev_card[k] = in.ev[k].card;
+        }
+        d.smem_off = -1;
+        // tables are staged like the step kernels' (bulk-TMA, 16-byte aligned and sized); float programs only
+        if (!P->f64 && !in.batched && (smem + padded) * 4 <= SBN_SMEM_BUDGET) {
+            d.smem_off = static_cast<int32_t>(smem);
+            d.stage_floats = static_cast<int32_t>(padded);
+            smem += padded;
+        }
+    }
+    m.smem_floats = static_cast<int32_t>(smem);
+    if (P->f64) return sbn_marginal_launch<double>(m, 0, stream);
+    return sbn_marginal_launch<float>(m, static_cast<size_t>(smem) * 4, stream);
 }
 
 cudaError_t launch_normalise(sbn_program *P, float *d_out, int64_t ld_out, int64_t n_rows, cudaStream_t stream) {
@@ -782,6 +865,10 @@ int issue_all(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows
         if (events) SBN_CUDA(cudaEventRecord(events[k], stream));
         ++k;
         if (hoisted(P, st)) continue;  // computed once, when the program was created
+        if (st.kind == 2) {
+            SBN_CUDA(launch_marginal(P, st, d_ev, ld_ev, n_rows, d_out, ld_out, stream));
+            continue;
+        }
         const int seg = chain_on(P) ? P->seg_first[k - 1] : -1;
         if (seg == -2) continue;       // runs inside the segment launched at its first step
         if (seg >= 0) {
@@ -812,7 +899,7 @@ int issue_all(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows
         SBN_CUDA(launch_step(P, st, q, stream));
     }
     if (events) SBN_CUDA(cudaEventRecord(events[k], stream));
-    if (!folded && !(chain_on(P) && !P->segments.empty() && P->segments.back()->ends_in_posterior))
+    if (!P->marginals && !folded && !(chain_on(P) && !P->segments.empty() && P->segments.back()->ends_in_posterior))
         SBN_CUDA(launch_normalise(P, d_out, ld_out, n_rows, stream));
     if (events) SBN_CUDA(cudaEventRecord(events[k + 1], stream));
     return SBN_OK;
@@ -854,8 +941,10 @@ int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n
                 }
             }
         }
-        if (last_writer[st.out_slot] >= 0) deps.push_back(last_writer[st.out_slot]);
-        for (int r : readers[st.out_slot]) deps.push_back(r);
+        const bool readout = st.kind == 2;  // writes the posterior, no slot
+        if (!readout && last_writer[st.out_slot] >= 0) deps.push_back(last_writer[st.out_slot]);
+        if (!readout)
+            for (int r : readers[st.out_slot]) deps.push_back(r);
         const int k = home >= 0 ? home : (rr++ % sbn_program::kBranches);
         stream_of[s] = k;
         cudaStream_t stream = P->branch[k];
@@ -867,11 +956,16 @@ int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n
         deps.erase(std::unique(deps.begin(), deps.end()), deps.end());
         for (int d : deps)
             if (stream_of[d] != k) SBN_CUDA(cudaStreamWaitEvent(stream, P->step_done[d], 0));
-        build_params(P, st, d_ev, ld_ev, n_rows, &q);
-        SBN_CUDA(launch_step(P, st, q, stream));
+        if (readout) {
+            SBN_CUDA(launch_marginal(P, st, d_ev, ld_ev, n_rows, d_out, ld_out, stream));
+        } else {
+            build_params(P, st, d_ev, ld_ev, n_rows, &q);
+            SBN_CUDA(launch_step(P, st, q, stream));
+        }
         SBN_CUDA(cudaEventRecord(P->step_done[s], stream));
         for (const InDesc &in : st.in)
             if (in.is_slot) readers[in.id].push_back(s);
+        if (readout) continue;
         last_writer[st.out_slot] = s;
         readers[st.out_slot].clear();
     }
@@ -881,7 +975,7 @@ int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n
         if (!hoisted(P, P->steps[s])) tail[stream_of[s]] = s;
     for (int k = 0; k < sbn_program::kBranches; ++k)
         if (tail[k] >= 0) SBN_CUDA(cudaStreamWaitEvent(origin, P->step_done[tail[k]], 0));
-    SBN_CUDA(launch_normalise(P, d_out, ld_out, n_rows, origin));
+    if (!P->marginals) SBN_CUDA(launch_normalise(P, d_out, ld_out, n_rows, origin));
     return SBN_OK;
 }
 
@@ -1007,7 +1101,9 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
                                        cudaMemcpyHostToDevice, P->stream));
         }
         SBN_CUDA_P(cudaStreamSynchronize(P->stream));
-        sbn_chain_plan(P);
+        // The on-chip segments and paired steps assume every intermediate has ONE consumer; the factors of a
+        // marginals program feed several launches, so it runs on the classic per-step launches.
+        if (!P->marginals) sbn_chain_plan(P);
     }
     {
         // opt every step-kernel instantiation into SBN_SMEM_BUDGET of dynamic shared memory
@@ -1019,6 +1115,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
             SBN_CUDA_P(sbn_chain_set_attrs());
             SBN_CUDA_P(sbn_tma_set_attrs());
             SBN_CUDA_P(sbn_join_set_attrs());
+            SBN_CUDA_P(sbn_marginal_set_attrs());
             done[device] = true;
         }
     }
@@ -1027,7 +1124,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
     if (rc != SBN_OK) return bail(rc);
     {
         // pairs multiply the tables of two steps on the host: needs the outputs of the table steps above
-        cudaError_t e = sbn_pair_plan(P);
+        cudaError_t e = P->marginals ? cudaSuccess : sbn_pair_plan(P);
         if (e != cudaSuccess) return bail(fail(SBN_E_CUDA, "planning the paired steps failed: %s", cudaGetErrorString(e)));
     }
     *out = P;
@@ -1169,6 +1266,8 @@ static int run_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int
     int rc = check_run_args(P, ev, ld_ev, n_rows, out_, want_totals ? n_rows : ld_out);
     if (rc != SBN_OK) return rc;
     if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the run call");
+    if (want_totals && P->marginals)
+        return fail(SBN_E_INVALID, "a marginals program has no single normaliser; P(event) comes from a program without targets");
     const size_t elem = f64 ? 8 : 4;
     char *out = static_cast<char *>(out_);
     SBN_CUDA(cudaSetDevice(P->device));

@@ -50,6 +50,10 @@ struct StepDesc {
     int64_t slice_pos = -1;
     int64_t slice_tpc = 0;
     int64_t slice_smem = 0;      // floats of shared memory of the largest chunk
+    // readout of a marginals program (kind 2, sbn_marginal.cuh): first posterior row of the target's segment;
+    // `in` is reordered so that the n_common inputs without the target axis come first
+    int64_t q_offset = -1;
+    int n_common = 0;
 };
 struct Slot {
     bool batched;
@@ -68,6 +72,7 @@ struct sbn_program {
     int n_sms = 1;     // multiprocessors of `device`: the grid-size heuristics count waves in them
     bool f64 = false;  // single-event programs computed and returned in double
     int mode = 0, n_ev = 0, Q = 0, post_slot = 0, post_batched = 0;
+    bool marginals = false;  // version-5 program: kind-2 readouts write the posterior, already normalised
     std::vector<std::pair<int64_t, int64_t>> tables;  // (offset, size) in floats
     std::vector<int64_t> table_padded;
     float *d_tables = nullptr;

@@ -44,6 +44,19 @@ input that spans both tile axes.
 `mode` 0 = flat (one evidence row, nothing batched: evidence offsets are uniform),
 1 = batched.  The posterior is produced by the last step into `post_slot`
 (`[Q]` or `[Q, B]`, unnormalised) and normalised per row by the engine.
+
+Marginals programs (`build_marginals_plan`, VERSION 5) answer P(t | e) for many targets t at
+once.  They use the same words, with two differences:
+
+    header : MAGIC 5 mode n_ev n_tables n_slots n_steps Q -1 0 0 0     -- no posterior slot
+    kind 2 : 2 n_in -1 1 n_elim q_offset | card_t | ecards[n_elim] | inputs as above
+
+A kind-2 step (KIND_MARGINAL, the readout of target t from its bucket) has one output axis, the
+target, and sums out the `n_elim` other variables of the bucket, with no MAX_ELIM / MAX_Z limit.
+It writes the target's `card_t` posterior entries, already normalised per row, at rows
+`q_offset ..` of the run's output.  Targets are sorted by name and Q = sum of their cards.
+Intermediates of a version-5 program may have several consumers; `build_plan`'s version-4
+programs are unchanged.
 """
 from __future__ import annotations
 
@@ -68,6 +81,8 @@ SLICE_MIN_BYTES = 64 * 1024  # tables of one launch beyond this are laid out for
 PRELOAD_MAX_IN = 3  # the tiled kernel's preload schedule (all operands of a block in registers)
 MODE_FLAT, MODE_BATCHED = 0, 1
 KIND_FLAT, KIND_BATCHED = 0, 1
+KIND_MARGINAL = 2  # readout of one target's marginal from a bucket (marginals programs only)
+VERSION_MARGINALS = 5
 HEADER_WORDS = 12
 
 
@@ -126,6 +141,7 @@ class Step:
     elims: tuple  # variables summed out by this launch
     ecards: tuple
     out_slot: int = -1
+    q_offset: int = -1  # KIND_MARGINAL: first posterior entry of the target's segment
 
     @property
     def cx(self):
@@ -147,6 +163,8 @@ class Plan:
     table_blob: np.ndarray = None
     table_blob64: np.ndarray = None
     table_offsets: list = None
+    version: int = VERSION
+    targets: tuple = ()  # marginals plans: target var ids, sorted by name (== posterior segment order)
 
     # ---- cost model (DESIGN.md "algorithmic bytes") -------------------------------
     def bytes_per_row(self):
@@ -155,21 +173,23 @@ class Plan:
         codes in and the posterior out."""
         total = 0
         for st in self.steps:
-            if st.kind != KIND_BATCHED:
+            if st.kind not in (KIND_BATCHED, KIND_MARGINAL):
                 continue
             for f, _, _ in st.inputs:
                 if f.batched:
                     total += 4 * int(np.prod([self._card[v] for v in f.vars], dtype=np.int64))
             total += 4 * int(np.prod(st.cards, dtype=np.int64))
-        # normalise: read unnormalised posterior, write posterior
-        total += 8 * self.Q
+        if self.version == VERSION:
+            # normalise: read unnormalised posterior, write posterior (a marginals program's
+            # readouts write their segments normalised, counted above)
+            total += 8 * self.Q
         total += len(self.evidence)  # uint8 codes
         return total
 
     def step_bytes_per_row(self):
         out = []
         for st in self.steps:
-            if st.kind != KIND_BATCHED:
+            if st.kind not in (KIND_BATCHED, KIND_MARGINAL):
                 out.append(0)
                 continue
             t = 4 * int(np.prod(st.cards, dtype=np.int64))
@@ -239,6 +259,31 @@ def build_plan(net: CompiledNet, query, evidence, mode=MODE_BATCHED, order=None,
     query / evidence are sequences of var ids.  `evidence` fixes the evidence
     *columns*; their values arrive at run time.
     """
+    return _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evidence, allow_empty_query,
+                  fuse_elims, None)
+
+
+def build_marginals_plan(net: CompiledNet, evidence, targets=None, mode=MODE_BATCHED, order=None, max_in=MAX_IN,
+                         lift_evidence=True, fuse_elims=None) -> Plan:
+    """Plan P(t | evidence) for every target t at once (a version-5 program, see the module docstring).
+
+    `targets` defaults to every variable that is not evidence.  The posterior is the
+    concatenation of the targets' marginals, targets sorted by name, states in domain order."""
+    evidence = tuple(evidence)
+    if targets is None:
+        targets = [v for v in range(len(net.names)) if v not in set(evidence)]
+    targets = tuple(targets)
+    if not targets:
+        raise ValueError("no target variable: every variable is evidence")
+    if set(targets) & set(evidence):
+        raise ValueError("A query variable cannot be part of the event")
+    if len(set(targets)) != len(targets):
+        raise ValueError("duplicate target variable")
+    return _build(net, (), evidence, mode, order, max_in, False, lift_evidence, True, fuse_elims, targets)
+
+
+def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evidence, allow_empty_query, fuse_elims,
+           targets):
     if merge_sum_outs is None:
         merge_sum_outs = os.environ.get("SOROBN_B200_MERGE", "0") == "1"
     if fuse_elims is None:
@@ -248,7 +293,7 @@ def build_plan(net: CompiledNet, query, evidence, mode=MODE_BATCHED, order=None,
     if not query and not allow_empty_query:
         # bayes_net.py:840-841
         raise ValueError("At least one query variable has to be specified")
-    if not query and not evidence:
+    if not query and not evidence and targets is None:
         raise ValueError("nothing to compute: no query variable and no evidence")
     if set(query) & set(evidence):
         # bayes_net.py:843-845
@@ -261,7 +306,7 @@ def build_plan(net: CompiledNet, query, evidence, mode=MODE_BATCHED, order=None,
             raise ValueError(f"evidence variable {net.names[v]!r} has {card[v]} states; state codes are uint8")
 
     # bayes_net.py:763-766
-    relevant = {*query, *evidence}
+    relevant = {*query, *evidence, *(targets or ())}
     for v in list(relevant):
         relevant |= net.ancestors(v)
     hidden = relevant - set(query) - set(evidence)
@@ -458,6 +503,7 @@ def build_plan(net: CompiledNet, query, evidence, mode=MODE_BATCHED, order=None,
     # separate launches walk, but the intermediate over w is never written and read back, and
     # the tile axes are chosen for the launch's real output.
     gone = set()
+    buckets = []  # marginals plans: (F_k, eliminated variables, U_k, lambda_k) per launch of the loop below
     for k, x in enumerate(order):
         if x in gone:
             continue
@@ -482,7 +528,14 @@ def build_plan(net: CompiledNet, query, evidence, mode=MODE_BATCHED, order=None,
                 elims.append(w)
                 z *= int(card[w])
         gone.update(elims)
+        bucket_factors = list(touching)
         factors.append(product_chain(touching, tuple(elims)))
+        if targets is not None:
+            buckets.append((bucket_factors, tuple(elims), set().union(*[f.vars for f in bucket_factors]), factors[-1]))
+
+    if targets is not None:
+        return _marginals_passes(net, evidence, mode, order, max_in, targets, buckets, factors, steps, tables,
+                                 table_arrays, emit, combine_tables, axis_order, fsize)
 
     # bayes_net.py:788-794: product of what is left; the answer's levels are sorted
     # by name (bayes_net.py:872-873) and rows by state (sort_index, :875)
@@ -502,6 +555,174 @@ def build_plan(net: CompiledNet, query, evidence, mode=MODE_BATCHED, order=None,
     plan._card = card
     _serialise(plan, table_arrays)
     return plan
+
+
+def _marginals_passes(net, evidence, mode, order, max_in, targets, buckets, leftovers, steps, tables, table_arrays,
+                      emit, combine_tables, axis_order, fsize):
+    """Downward pass and readouts of a marginals plan (DESIGN.md "Marginals of every variable").
+
+    `buckets` are the launches of the upward pass: (F_k, eliminated variables, U_k, lambda_k).
+    Bucket j's parent is the bucket whose F contains lambda_j.  The message to a child is
+        pi_j(S_j) = sum_{U_p - S_j} pi_p * prod_{f in F_p, f != lambda_j} f,
+    and a target t is read from the smallest bucket k with t in U_k:
+        M_t(t) = sum_{U_k - {t}} pi_k * prod_{f in F_k} f.
+    What is left after the upward pass are per-row scalars (the root buckets' messages and the
+    tables of evidence-only variables); a root bucket's pi is the product of the others, so that
+    every bucket belief is P(U_k, e) and a row of probability zero stays NaN as in `build_plan`."""
+    card = net.card
+    n = len(buckets)
+    owner = {id(lam): k for k, (_, _, _, lam) in enumerate(buckets)}
+    parent = [None] * n
+    for k, (F, _, _, _) in enumerate(buckets):
+        for f in F:
+            j = owner.get(id(f))
+            if j is not None:
+                parent[j] = k
+
+    def joint(vs):
+        return int(np.prod([card[v] for v in vs], dtype=np.int64)) if vs else 1
+
+    t_sorted = tuple(sorted(targets, key=lambda v: net.names[v]))
+    read = {t: min((joint(U), k) for k, (_, _, U, _) in enumerate(buckets) if t in U)[1] for t in t_sorted}
+    need = [False] * n
+    for k in read.values():
+        while k is not None and not need[k]:
+            need[k] = True
+            k = parent[k]
+
+    def fold(inputs):
+        """At most max_in factors per launch: multiply the smallest ones first (as product_chain)."""
+        inputs = list(inputs)
+        while len(inputs) > max_in:
+            inputs.sort(key=fsize)
+            head, inputs = inputs[:max_in], inputs[max_in:]
+            union = set().union(*[f.vars for f in head])
+            inputs.append(emit(head, None, axis_order(head, union)))
+        return inputs
+
+    def message(inputs, out_vars, elims):
+        """sum_{elims} prod(inputs) over out_vars, at most MAX_ELIM variables / MAX_Z joint states per launch:
+        the first launch multiplies and sums out the first group, each later one sums out the next group."""
+        groups, cur, z = [], [], 1
+        for v in sorted(elims, key=lambda v: (-int(card[v]), v)):
+            if cur and (len(cur) >= MAX_ELIM or z * int(card[v]) > MAX_Z):
+                groups.append(cur)
+                cur, z = [], 1
+            cur.append(v)
+            z *= int(card[v])
+        if cur:
+            groups.append(cur)
+        inputs = combine_tables(inputs, PRELOAD_MAX_IN if groups and len(groups[0]) > 1 else TILED_MAX_IN)
+        inputs = fold(inputs)
+        rest = [v for g in groups for v in g]
+        if not groups:
+            return emit(inputs, None, axis_order(inputs, set(out_vars)))
+        f = None
+        for g in groups:
+            rest = [v for v in rest if v not in g]
+            keep = set(out_vars) | set(rest)
+            src = inputs if f is None else [f]
+            f = emit(src, tuple(g), axis_order(src, keep))
+        return f
+
+    pi = {}
+    for k in reversed(range(n)):  # a parent is eliminated after its children
+        if not need[k]:
+            continue
+        lam_k = buckets[k][3]
+        if parent[k] is None:
+            others = [f for f in leftovers if f is not lam_k]
+            pi[k] = emit(fold(others), None, [], may_lift=False) if others else None
+            continue
+        p = parent[k]
+        F_p, _, U_p, _ = buckets[p]
+        inputs = ([pi[p]] if pi[p] is not None else []) + [f for f in F_p if f is not lam_k]
+        S_k = set(lam_k.vars)
+        pi[k] = message(inputs, S_k, U_p - S_k) if inputs else None
+
+    offsets, q = {}, 0
+    for t in t_sorted:
+        offsets[t] = q
+        q += int(card[t])
+    for t in t_sorted:
+        k = read[t]
+        F_k, _, U_k, _ = buckets[k]
+        inputs = fold(([pi[k]] if pi[k] is not None else []) + list(F_k))
+        # joint states of the summed-out variables are walked first-variable fastest: the variables the
+        # largest batched operand lacks go first, so each of its entries is read in one stretch
+        big = max(inputs, key=lambda f: (f.batched, fsize(f)))
+        pos_big = dict(zip(big.vars, big.strides))
+        elims = sorted(U_k - {t}, key=lambda v: (v in pos_big, pos_big.get(v, 0), v))
+        if joint(elims) * int(card[t]) >= 2**31:
+            raise ValueError(f"the bucket read for {net.names[t]!r} has more than 2^31 joint states")
+        ins = []
+        for f in inputs:
+            pos = dict(zip(f.vars, f.strides))
+            ins.append((f, tuple(pos.get(e, 0) for e in elims), (pos.get(t, 0),)))
+        steps.append(Step(KIND_MARGINAL, ins, -1, (t,), (int(card[t]),), tuple(elims),
+                          tuple(int(card[e]) for e in elims), q_offset=offsets[t]))
+
+    steps[:] = _prune_dead(steps)
+    slots = _assign_slots_shared(steps, keep_unbatched=(mode == MODE_BATCHED))
+    plan = Plan(mode=mode, query=(), evidence=evidence, order=list(order), tables=tables, slots=slots, steps=steps,
+                post_slot=-1, Q=q, version=VERSION_MARGINALS, targets=t_sorted)
+    plan._card = card
+    _serialise(plan, table_arrays)
+    return plan
+
+
+def _prune_dead(steps):
+    """Drop the launches nothing reads (the root buckets' own messages when no other root needs them)."""
+    used, keep = set(), []
+    for st in reversed(steps):
+        if st.kind == KIND_MARGINAL or st.out_id in used:
+            keep.append(st)
+            used.update(f.buf for f, _, _ in st.inputs if f.is_slot)
+    return keep[::-1]
+
+
+def _assign_slots_shared(steps, keep_unbatched):
+    """`_assign_slots` for plans whose intermediates have several consumers (the factors of a
+    bucket feed its upward message, its downward messages and its readouts): a slot is released
+    after its last consumer.  The output slot is taken before the inputs are released, so a launch
+    never writes a buffer it reads.  Readouts write the posterior, not a slot."""
+    remaining = {}
+    for st in steps:
+        for f, _, _ in st.inputs:
+            if f.is_slot:
+                remaining[f.buf] = remaining.get(f.buf, 0) + 1
+    slots, where = [], {}
+
+    def alloc(batched, size):
+        best = None
+        for i, (b, sz, free) in enumerate(slots):
+            if free and b == batched and sz >= size and (best is None or sz < slots[best][1]):
+                best = i
+        if best is None:
+            slots.append([batched, size, False])
+            return len(slots) - 1
+        slots[best][2] = False
+        return best
+
+    for st in steps:
+        if st.kind != KIND_MARGINAL:
+            size = int(np.prod(st.cards, dtype=np.int64)) if st.cards else 1
+            st.out_slot = alloc(st.kind == KIND_BATCHED, size)
+        new_inputs = []
+        for f, es, ss in st.inputs:
+            if f.is_slot:
+                phys = where[f.buf]
+                remaining[f.buf] -= 1
+                if remaining[f.buf] == 0:
+                    slots[phys][2] = not (keep_unbatched and not slots[phys][0])
+                f = _Factor(True, phys, f.vars, f.strides, f.ev, f.batched)
+            new_inputs.append((f, es, ss))
+        st.inputs = new_inputs
+        if st.kind != KIND_MARGINAL:
+            where[st.out_id] = st.out_slot
+    if not slots:  # every operand is a CPT: the engine still expects one scratch slot
+        slots.append([False, 1, True])
+    return [(bool(b), int(sz)) for b, sz, _ in slots]
 
 
 def _relayout_big_tables(steps, table_arrays, table_axes, evidence, card):
@@ -700,8 +921,12 @@ def _serialise(plan: Plan, table_arrays):
     plan.table_blob = plan.table_blob64.astype(np.float32)
     plan.table_offsets = offsets
 
-    w = [MAGIC, VERSION, plan.mode, len(plan.evidence), len(plan.tables), len(plan.slots), len(plan.steps),
-         plan.Q, plan.post_slot, int(plan.slots[plan.post_slot][0]), 0, 0]
+    if plan.version == VERSION:
+        post = [plan.post_slot, int(plan.slots[plan.post_slot][0])]
+    else:
+        post = [-1, 0]  # the readouts write the posterior themselves
+    w = [MAGIC, plan.version, plan.mode, len(plan.evidence), len(plan.tables), len(plan.slots), len(plan.steps),
+         plan.Q, *post, 0, 0]
     assert len(w) == HEADER_WORDS
     for o, s in offsets:
         w += [o, s]
@@ -709,6 +934,8 @@ def _serialise(plan: Plan, table_arrays):
         w += [int(b), s]
     for st in plan.steps:
         w += [st.kind, len(st.inputs), st.out_slot, len(st.cards), len(st.ecards)]
+        if st.kind == KIND_MARGINAL:
+            w.append(st.q_offset)
         w += list(st.cards)
         w += list(st.ecards)
         for f, estrides, strides in st.inputs:
