@@ -16,6 +16,14 @@
 //     others once per (z, s);
 //   * C accumulators per thread, one per target state; a target with more than C states is done
 //     in passes of C states (the raw values are written, then re-read and normalised);
+//   * a readout sums cz joint states per entry with no MAX_Z bound (625 on the benchmark grid, up to
+//     2^21), and a float32 running sum of that many terms misses the 1e-6 relative promise.  So the
+//     products are summed in T over runs of SBN_MARG_PART joint states, and those partial sums in
+//     double; the segment total, the range rule and the division are double too, and each entry is
+//     rounded to T once (a raw value of a multi-pass target twice: when it is written, and after the
+//     division).  A double add per product would need a float->double conversion per product, a
+//     low-throughput instruction on sm_90: that variant made the benchmark grid's marginals program
+//     4.5 % slower (100k rows, H100 80GB HBM3 at a 400 W power limit);
 //   * tables (CPTs, evidence-independent factors) are staged in shared memory by bulk-TMA when
 //     they fit SBN_SMEM_BUDGET (float only), otherwise gathered through L1;
 //   * the range rule of sbn_normalise: a row whose segment total, or smallest non-zero entry, is
@@ -24,6 +32,7 @@
 #include "sbn_kernels.cuh"
 
 #define SBN_MARG_THREADS 128
+#define SBN_MARG_PART 32  // joint states summed in T before the double accumulator takes the partial sum
 
 struct SbnMargIn {
     const void *ptr;                 // table / slot base (device), float or double
@@ -111,53 +120,60 @@ __global__ void __launch_bounds__(SBN_MARG_THREADS) sbn_marginal_step(const __gr
 
     T *const out = static_cast<T *>(p.out) + b;
     const int n_in = p.n_in, n_common = p.n_common, cz = p.cz, card = p.card;
-    T total = T(0), lo = static_cast<T>(p.min_total);
-    T keep[C];
+    // float: runs of SBN_MARG_PART joint states; double: one run (the partial sum is the sum)
+    constexpr int kRun = std::is_same<T, float>::value ? SBN_MARG_PART : (1 << 30);
+    double total = 0.0, lo = p.min_total;
+    double acc[C];  // after the last pass: its sums (all of them when card <= C)
     for (int s0 = 0; s0 < card; s0 += C) {
-        T acc[C];
 #pragma unroll
-        for (int s = 0; s < C; ++s) acc[s] = T(0);
-        for (int z = 0; z < cz; ++z) {
-            int e[SBN_MAX_IN];
+        for (int s = 0; s < C; ++s) acc[s] = 0.0;
+        for (int z0 = 0; z0 < cz; z0 += kRun) {
+            T part[C];
 #pragma unroll
-            for (int i = 0; i < SBN_MAX_IN; ++i)
-                if (i < n_in) e[i] = __ldg(p.zoff + static_cast<int64_t>(i) * cz + z) + s0 * p.in[i].ts;
-            T common = T(1);
+            for (int s = 0; s < C; ++s) part[s] = T(0);
+            const int z1 = z0 + min(kRun, cz - z0);
+            for (int z = z0; z < z1; ++z) {
+                int e[SBN_MAX_IN];
 #pragma unroll
-            for (int i = 0; i < SBN_MAX_IN; ++i)
-                if (i < n_common) common *= src[i][e[i] * mul[i]];
+                for (int i = 0; i < SBN_MAX_IN; ++i)
+                    if (i < n_in) e[i] = __ldg(p.zoff + static_cast<int64_t>(i) * cz + z) + s0 * p.in[i].ts;
+                T common = T(1);
 #pragma unroll
-            for (int s = 0; s < C; ++s) {
-                if (s0 + s < card) {
-                    T v = common;
+                for (int i = 0; i < SBN_MAX_IN; ++i)
+                    if (i < n_common) common *= src[i][e[i] * mul[i]];
 #pragma unroll
-                    for (int i = 0; i < SBN_MAX_IN; ++i)
-                        if (i >= n_common && i < n_in) v *= src[i][static_cast<int64_t>(e[i] + s * p.in[i].ts) * mul[i]];
-                    acc[s] += v;
+                for (int s = 0; s < C; ++s) {
+                    if (s0 + s < card) {
+                        T v = common;
+#pragma unroll
+                        for (int i = 0; i < SBN_MAX_IN; ++i)
+                            if (i >= n_common && i < n_in) v *= src[i][static_cast<int64_t>(e[i] + s * p.in[i].ts) * mul[i]];
+                        part[s] += v;
+                    }
                 }
             }
+#pragma unroll
+            for (int s = 0; s < C; ++s) acc[s] += static_cast<double>(part[s]);
         }
 #pragma unroll
         for (int s = 0; s < C; ++s) {
             if (s0 + s < card) {
                 total += acc[s];
-                if (acc[s] > T(0) && acc[s] < lo) lo = acc[s];
-                if (card > C) out[static_cast<int64_t>(s0 + s) * p.ld_out] = acc[s];
-                keep[s] = acc[s];
+                if (acc[s] > 0.0 && acc[s] < lo) lo = acc[s];
+                if (card > C) out[static_cast<int64_t>(s0 + s) * p.ld_out] = static_cast<T>(acc[s]);
             }
         }
     }
-    const T mt = static_cast<T>(p.min_total);
-    const bool ok = total >= mt && lo >= mt;  // false for NaN too
+    const bool ok = total >= p.min_total && lo >= p.min_total;  // false for NaN too
     const T nan = static_cast<T>(__int_as_float(0x7fc00000));
     if (card <= C) {
 #pragma unroll
         for (int s = 0; s < C; ++s)
-            if (s < card) out[static_cast<int64_t>(s) * p.ld_out] = ok ? keep[s] / total : nan;
+            if (s < card) out[static_cast<int64_t>(s) * p.ld_out] = ok ? static_cast<T>(acc[s] / total) : nan;
     } else {
         for (int s = 0; s < card; ++s) {
             T *o = out + static_cast<int64_t>(s) * p.ld_out;
-            *o = ok ? *o / total : nan;
+            *o = ok ? static_cast<T>(static_cast<double>(*o) / total) : nan;
         }
     }
 }

@@ -82,6 +82,9 @@ PRELOAD_MAX_IN = 3  # the tiled kernel's preload schedule (all operands of a blo
 MODE_FLAT, MODE_BATCHED = 0, 1
 KIND_FLAT, KIND_BATCHED = 0, 1
 KIND_MARGINAL = 2  # readout of one target's marginal from a bucket (marginals programs only)
+# Joint states one readout sums out: its offset table, [SBN_MAX_IN][cz] int32 words, is capped at 2^24
+# words (csrc/sbn_api.cu: kMarginalZoffMax / SBN_MAX_IN)
+MARGINAL_MAX_Z = 2**21
 VERSION_MARGINALS = 5
 HEADER_WORDS = 12
 
@@ -653,8 +656,9 @@ def _marginals_passes(net, evidence, mode, order, max_in, targets, buckets, left
         big = max(inputs, key=lambda f: (f.batched, fsize(f)))
         pos_big = dict(zip(big.vars, big.strides))
         elims = sorted(U_k - {t}, key=lambda v: (v in pos_big, pos_big.get(v, 0), v))
-        if joint(elims) * int(card[t]) >= 2**31:
-            raise ValueError(f"the bucket read for {net.names[t]!r} has more than 2^31 joint states")
+        if joint(elims) > MARGINAL_MAX_Z or joint(elims) * int(card[t]) >= 2**31:
+            raise ValueError(f"the bucket read for {net.names[t]!r} is too large for a readout: {joint(elims)} joint "
+                             f"states summed out (at most {MARGINAL_MAX_Z}) x {int(card[t])} target states (below 2^31)")
         ins = []
         for f in inputs:
             pos = dict(zip(f.vars, f.strides))

@@ -72,7 +72,9 @@ def _targs(s):
 def variants(launches):
     """Coverage items (strings) of a census.  Tiled: the input combination, tile edge, preload
     width, slab and several-eliminated-variables flags; batched: inputs and preload width; pairs:
-    the two coefficient modes; triples: the group axis (the CTA's second block dimension)."""
+    the two coefficient modes; triples: the group axis (the CTA's second block dimension); the join
+    kernel: its input combination; the readout of marginals programs: element type and accumulator
+    count, `marginal<float,2>` ... `marginal<double,8>`."""
     out = set()
     for name, block_y in launches:
         m = re.match(r"(\w+)(?:<(.*)>)?$", name)
@@ -104,4 +106,8 @@ def variants(launches):
             out.add(f"pair ({targs[0]},{targs[1]})")
         elif kernel == "sbn_triple_kernel":
             out.add(f"triple group={block_y}")
+        elif kernel == "sbn_join_kernel":
+            out.add("join ({},{},{})".format(*targs))
+        elif kernel == "sbn_marginal_step":
+            out.add(f"marginal<{targs[0]},{targs[1]}>")
     return out

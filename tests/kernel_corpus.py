@@ -155,6 +155,53 @@ def plan_items(plan):
     return {"tiled sliced staging"} if big else set()
 
 
+READOUT_C_MAX = 8  # the widest accumulator set of the readout kernel (csrc/sbn_marginal.cuh)
+
+
+def readout_items(plan):
+    """Coverage items of a marginals plan's readouts (kind-2 steps), read from the plan: a target with
+    more states than the widest accumulator set (read in passes), float tables of one readout beyond
+    the shared-memory budget (some are gathered from global memory), a readout with no batched
+    operand, and a single-state target."""
+    size = [n for _, n in plan.table_offsets]
+    out = set()
+    for st in plan.steps:
+        if st.kind != planner.KIND_MARGINAL:
+            continue
+        if st.cards[0] > READOUT_C_MAX:
+            out.add("readout multi-pass")
+        if sum(size[f.buf] for f, _, _ in st.inputs if not f.is_slot) * 4 > planner.SLICE_MIN_BYTES:
+            out.add("readout unstaged tables")
+        if not any(f.batched for f, _, _ in st.inputs):
+            out.add("readout tables only")
+        if st.cards[0] == 1:
+            out.add("readout card 1")
+    return out
+
+
+READOUT_ITEMS = ("readout multi-pass", "readout unstaged tables", "readout tables only", "readout card 1")
+NAIVE_BAYES_12 = "naive12s5x17_e6"
+
+
+def build_marginals(name, mode=planner.MODE_BATCHED):
+    """(spec, CompiledNet, DenseNet, marginals plan, evidence names) of a corpus network: a case's
+    network and evidence, or (NAIVE_BAYES_12) `naive_bayes` with 12 children, every other one observed.
+    The plan targets every variable that is not evidence."""
+    if name == NAIVE_BAYES_12:
+        spec = naive_bayes(n_children=12)
+        # rows that sum to 1 in float64: a hidden child's table then sums out to exactly 1, as the
+        # oracle, which drops hidden leaves, assumes
+        spec.cpt = {n: a / a.sum(axis=-1, keepdims=True) for n, a in spec.cpt.items()}
+        evidence = spec.nodes[1::2]
+    else:
+        case = next(c for c in CASES if c["name"] == name)
+        spec = make_spec(case)
+        evidence = [spec.nodes[k] for k in case["evidence"]]
+    net = compiled_net(spec)
+    plan = planner.build_marginals_plan(net, [net.index[e] for e in evidence], mode=mode)
+    return spec, net, dense_net(spec), plan, evidence
+
+
 CASES = [
     {'name': 'dag9p2s4x1x4x4_seed54_q1-8_e2', 'gen': 'random_dag', 'args': [9, 2, [4, 1, 4, 4]], 'seed': 54, 'kwargs': {'window': 6}, 'query': [1, 8], 'evidence': [3, 0], 'claims': ['batched CX=1', 'batched N_IN=4', 'tiled (1,1,2,0)', 'tiled T=2 CX=0']},
     {'name': 'dag16p4s5x8_seed63_single8-0_q14_e3', 'gen': 'random_dag', 'args': [16, 4, [5, 8]], 'seed': 63, 'kwargs': {'window': 4}, 'query': [14], 'evidence': [15, 8, 13], 'single': [8, 0], 'claims': ['batched CX=1', 'batched N_IN=4', 'tiled (2,2,0,0)', 'tiled T=5 CX=0']},
@@ -246,3 +293,8 @@ def required_items():
     req.add("triple group=5")
     req.update({"flat<float>", "flat<double>", "batched_f64"})
     return req
+
+
+# The networks the marginals tests run (build_marginals): every case, plus a naive Bayes network whose
+# 17-state targets take the readout's multi-pass path next to a 5-state one.
+MARGINALS_CASES = [c["name"] for c in CASES] + [NAIVE_BAYES_12]

@@ -13,6 +13,7 @@ import numpy as np
 
 MAGIC = 0x53424E31
 HEADER_WORDS = 12
+READOUT_RUN = 32  # joint states a readout sums in the program's type before a float64 add (SBN_MARG_PART)
 
 
 def parse(words):
@@ -54,12 +55,22 @@ def parse(words):
     return hdr, tables, slots, steps
 
 
-def run(words, table_blob, ev_codes, n_rows=None, dtype=np.float64, min_total=None):
+def run(words, table_blob, ev_codes, n_rows=None, dtype=np.float64, min_total=None, readout_acc=None):
     """Execute the program.  ev_codes: uint8 [n_ev, B].  Returns the posterior [Q, B], every target's
-    segment normalised per row (NaN for a row whose segment is out of range)."""
+    segment normalised per row (NaN for a row whose segment is out of range).
+
+    `readout_acc` is the accumulator type of the readouts (kind 2), which sum joint states without the
+    MAX_Z bound of the other steps.  By default it is float64, as in the readout kernel
+    (sbn_marginal.cuh): the products are summed in `dtype` over runs of READOUT_RUN joint states, the
+    partial sums in float64; the segment total, the range rule and the division are float64, and the
+    result is rounded once to `dtype` (a target of more than 8 states, which the kernel reads in passes,
+    has its raw sums rounded to `dtype` before the division too).  `readout_acc=np.float32` is a single
+    float32 accumulator throughout, in the kernel's summation order."""
     hdr, tables, slots, steps = parse(words)
     if min_total is None:
         min_total = 1e-30 if dtype == np.float32 else 1e-290
+    if readout_acc is None:
+        readout_acc = np.float64
     ev_codes = np.asarray(ev_codes, dtype=np.uint8)
     if hdr["n_ev"]:
         ev_codes = ev_codes.reshape(hdr["n_ev"], -1)
@@ -84,7 +95,8 @@ def run(words, table_blob, ev_codes, n_rows=None, dtype=np.float64, min_total=No
         assert all(not (i["is_slot"] and i["buf"] == st["out_slot"]) for i in st["inputs"]), "output aliases an input"
         per_row = st["kind"] in (1, 2) or hdr["mode"] == 0
         rows = B if per_row else 1
-        acc = np.zeros((n_out, rows), dtype=dtype)
+        acc_t = readout_acc if st["kind"] == 2 else dtype
+        acc = np.zeros((n_out, rows), dtype=acc_t)
         cx = int(np.prod(st["ecards"], dtype=np.int64)) if st["ecards"] else 1
         for x in range(cx):
             xd, rem_x = [], x
@@ -107,15 +119,23 @@ def run(words, table_blob, ev_codes, n_rows=None, dtype=np.float64, min_total=No
                 else:
                     vals = src.reshape(-1)[off[:, None] + evoff[None, :]]
                 prod = (prod * vals).astype(dtype)
-            acc = (acc + prod).astype(dtype)
+            if acc_t == dtype:
+                acc = (acc + prod).astype(acc_t)
+            else:  # partial sums in dtype over runs of READOUT_RUN joint states
+                part = prod if x % READOUT_RUN == 0 else (part + prod).astype(dtype)
+                if x % READOUT_RUN == READOUT_RUN - 1 or x == cx - 1:
+                    acc = acc + part.astype(acc_t)
         if st["kind"] == 2:
             if acc.shape[1] != B:
                 acc = np.repeat(acc, B, axis=1)
-            total = acc.sum(axis=0, dtype=dtype)
+            total = np.zeros(B, dtype=acc_t)
+            for s in range(n_out):  # in state order, as the kernel
+                total = (total + acc[s]).astype(acc_t)
             lo = np.where(acc > 0, acc, np.inf).min(axis=0)
+            raw = acc.astype(dtype).astype(acc_t) if n_out > 8 else acc
             with np.errstate(invalid="ignore", divide="ignore"):
                 ok = (total >= min_total) & (lo >= min_total)
-                seg = np.where(ok[None, :], acc / total[None, :], np.nan).astype(dtype)
+                seg = np.where(ok[None, :], raw / total[None, :], np.nan).astype(dtype)
             q0 = st["q_offset"]
             post[q0:q0 + n_out] = seg
             assert not written[q0:q0 + n_out].any(), "two readouts write one posterior entry"
@@ -127,3 +147,51 @@ def run(words, table_blob, ev_codes, n_rows=None, dtype=np.float64, min_total=No
             bufs[st["out_slot"]] = acc.reshape(-1)
     assert written.all(), "a posterior entry is never written"
     return post
+
+
+# A float32 readout writes NaN for a row whose total P(e), or smallest non-zero entry P(e) * p, is below
+# min_total = 1e-30 (the engine re-runs such rows in float64).  A NaN segment is put down to that rule
+# where the float64 answer puts either below 1e-29, a margin for float32 rounding on the way.
+RANGE_RULE_F32 = 1e-29
+
+
+def segment_starts(plan):
+    """First posterior entry of every target's segment (targets in plan order)."""
+    return np.cumsum([0] + [int(plan._card[t]) for t in plan.targets[:-1]])
+
+
+def check_posterior(got, want, starts, p_event=None):
+    """A marginals posterior `got` [Q, B] against the float64 answer `want`, target segment by segment
+    (`starts`: segment_starts): rows `want` gives NaN (impossible evidence) must be NaN throughout;
+    elsewhere every entry is finite, and exact zeros stay exactly 0.  With `p_event` ([B], the float64
+    P(e) of every row: float32 runs), a segment that is NaN throughout is accepted where the float32
+    range rule explains it; any other NaN fails.  Returns (worst relative error of the non-zero
+    entries, number of segments accepted as NaN)."""
+    got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
+    assert got.shape == want.shape, (got.shape, want.shape)
+    impossible = np.isnan(want).all(axis=0)
+    assert np.isnan(got[:, impossible]).all(), f"rows {np.flatnonzero(impossible)}: impossible evidence, not NaN"
+    got, want = got[:, ~impossible], want[:, ~impossible]
+    rows = np.flatnonzero(~impossible)
+    assert np.isfinite(want).all(), "the reference has a NaN on a possible row"
+    nan_got = np.isnan(got)
+    all_nan = np.logical_and.reduceat(nan_got, starts, axis=0)  # [n_segments, B]
+    any_nan = np.logical_or.reduceat(nan_got, starts, axis=0)
+    bad = np.argwhere(any_nan & ~all_nan)
+    assert not len(bad), f"(segment, row) {[(int(s), int(rows[b])) for s, b in bad[:5]]}: partly NaN"
+    flagged = 0
+    if all_nan.any():
+        assert p_event is not None, f"(segment, row) {[(int(s), int(rows[b])) for s, b in np.argwhere(all_nan)[:5]]}: NaN"
+        p_e = np.asarray(p_event, dtype=np.float64)[~impossible]
+        lo = np.minimum.reduceat(np.where(want > 0, want, np.inf), starts, axis=0) * p_e[None, :]
+        unexplained = all_nan & ~((p_e[None, :] < RANGE_RULE_F32) | (lo < RANGE_RULE_F32))
+        assert not unexplained.any(), \
+            f"(segment, row) {[(int(s), int(rows[b])) for s, b in np.argwhere(unexplained)[:5]]}: NaN within float32 range"
+        flagged = int(all_nan.sum())
+    keep = ~np.repeat(all_nan, np.diff(np.append(starts, got.shape[0])), axis=0)
+    zero = keep & (want == 0)
+    assert (got[zero] == 0).all(), f"entries (q, row) {[(int(q), int(rows[b])) for q, b in np.argwhere(zero & (got != 0))[:5]]}: not 0"
+    pos = keep & (want > 0)
+    err = np.zeros_like(want)
+    err[pos] = np.abs(got[pos] - want[pos]) / want[pos]
+    return float(err.max(initial=0.0)), flagged

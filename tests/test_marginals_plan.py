@@ -93,13 +93,14 @@ def test_float32_interpretation_on_the_benchmark_grid():
     wl = workloads.grid10x10()
     bn = wl.build()
     net = bn._compiled
-    codes = wl.codes(bn, 8, seed=3)
+    n = 256  # a float32 readout accumulator is off by 1.8e-6 on one of these rows: the check must see that
+    codes = wl.codes(bn, n, seed=3)
     plan = planner.build_marginals_plan(net, [net.index[e] for e in wl.evidence])
     got64 = marginals_interp.run(plan.words, plan.table_blob64, codes)
     got32 = marginals_interp.run(plan.words, plan.table_blob, codes, dtype=np.float32)
     assert np.isfinite(got32).all()
     assert np.max(np.abs(got32 - got64) / np.maximum(got64, 1e-300) * (got64 > 1e-12)) < 1e-6
-    assert np.allclose(got32.reshape(-1, 8).sum(axis=0), 70, rtol=1e-5)
+    assert np.allclose(got32.sum(axis=0), 70, rtol=1e-5)
     # every targetless grid variable's marginal equals its own query plan
     for t in (net.names[plan.targets[0]], net.names[plan.targets[35]], net.names[plan.targets[-1]]):
         p4 = planner.build_plan(net, [net.index[t]], [net.index[e] for e in wl.evidence])
