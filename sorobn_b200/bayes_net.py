@@ -342,20 +342,23 @@ class BayesNet:
         return frame if n > 1 else frame.iloc[0]
 
     # ---------------------------------------------------------------------- query
-    def _plan(self, query, evidence_vars, mode, robust=False, device=None, marginals=False):
+    def _plan(self, query, evidence_vars, mode, robust=False, device=None, marginals=False, replica=0):
         """(plan, program) of P(query | evidence vars), cached.  marginals=True: `query` are the targets of
-        a marginals program (planner.build_marginals_plan), cached under its own mode key."""
+        a marginals program (planner.build_marginals_plan), cached under its own mode key.  replica=k > 0:
+        a separate program on the same device, for the k-th other thread that runs this query there at the
+        same time (a program's scratch, staging buffers and graph capture serve one caller at a time)."""
         with self._cache_lock:
-            return self._plan_locked(query, evidence_vars, mode, robust, device, marginals)
+            return self._plan_locked(query, evidence_vars, mode, robust, device, marginals, replica)
 
-    def _plan_locked(self, query, evidence_vars, mode, robust, device, marginals=False):
+    def _plan_locked(self, query, evidence_vars, mode, robust, device, marginals=False, replica=0):
         if self._compiled is None:
             self._compile()
             if self._compiled is None:
                 raise ValueError("every node needs a CPT in P before querying; call prepare()")
         net = self._compiled
         device = self.device if device is None else device
-        key = (tuple(query), tuple(evidence_vars), ("marginals", mode) if marginals else mode, robust, device)
+        key = (tuple(query), tuple(evidence_vars), ("marginals", mode) if marginals else mode, robust,
+               (device, replica) if replica else device)
         hit = self._engine_cache.get(key)
         if hit is None:
             for name in (*query, *evidence_vars):
@@ -540,22 +543,23 @@ class BayesNet:
             out.loc[events.index[bad]] = np.nan
         return out
 
-    def _posterior_codes(self, query, ev_vars, codes, bad, device=None, marginals=False):
+    def _posterior_codes(self, query, ev_vars, codes, bad, device=None, marginals=False, replica=0):
         """Posterior float64 [Q, n] for uint8 evidence codes [n_ev, n] on one device.  Rows the
         float32 program flags (NaN: impossible evidence, or an entry below the float32 range)
         are settled in float64 -- a few one by one with the single-event program, many as one
         batch with the batched float64 program; a row that is still NaN there is impossible.
         marginals=True: `query` are the targets of a marginals program (every segment normalised)."""
         n = codes.shape[1] if len(ev_vars) else len(bad)
-        _, program = self._plan(query, ev_vars, _planner.MODE_BATCHED, device=device, marginals=marginals)
+        _, program = self._plan(query, ev_vars, _planner.MODE_BATCHED, device=device, marginals=marginals, replica=replica)
         post = self._run_evicting(program, codes, n).astype(np.float64)  # [Q, n]
         suspect = np.isnan(post).any(axis=0) & ~bad
         rows = np.nonzero(suspect)[0]
         if len(rows) > 8:
-            _, robust = self._plan(query, ev_vars, _planner.MODE_BATCHED, robust=True, device=device, marginals=marginals)
+            _, robust = self._plan(query, ev_vars, _planner.MODE_BATCHED, robust=True, device=device, marginals=marginals,
+                                   replica=replica)
             post[:, rows] = robust.run(np.ascontiguousarray(codes[:, rows]), len(rows))
         elif len(rows):
-            _, flat = self._plan(query, ev_vars, _planner.MODE_FLAT, device=device, marginals=marginals)
+            _, flat = self._plan(query, ev_vars, _planner.MODE_FLAT, device=device, marginals=marginals, replica=replica)
             for b in rows:
                 post[:, b] = flat.run(np.ascontiguousarray(codes[:, b:b + 1]), 1)[:, 0]
         return post
@@ -652,7 +656,8 @@ class BayesNet:
 
     def _posterior_codes_multi(self, query, ev_vars, codes, bad, devices):
         """Row-shard `_posterior_codes` over several GPUs of this process: contiguous balanced
-        slices (sharding.row_shard), one thread per device."""
+        slices (sharding.row_shard), one thread per listed device.  A device listed several times
+        gets one set of programs per listing: no program is run by two threads at once."""
         import threading
 
         from .sharding import row_shard
@@ -660,8 +665,9 @@ class BayesNet:
         n = len(bad)
         world = len(devices)
         # programs are created up front, on this thread (the cache is not thread-safe)
-        for d in devices:
-            self._plan(query, ev_vars, _planner.MODE_BATCHED, device=d)
+        replicas = [devices[:r].count(d) for r, d in enumerate(devices)]
+        for d, k in zip(devices, replicas):
+            self._plan(query, ev_vars, _planner.MODE_BATCHED, device=d, replica=k)
         plan, _ = self._plan(query, ev_vars, _planner.MODE_BATCHED, device=devices[0])
         post = np.empty((plan.Q, n), dtype=np.float64)
         errors = []
@@ -672,7 +678,7 @@ class BayesNet:
                 return
             try:
                 post[:, sl] = self._posterior_codes(query, ev_vars, np.ascontiguousarray(codes[:, sl]), bad[sl],
-                                                    device=devices[r])
+                                                    device=devices[r], replica=replicas[r])
             except Exception as exc:  # surfaced on the calling thread
                 errors.append(exc)
 

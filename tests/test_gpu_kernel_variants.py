@@ -6,7 +6,14 @@ slab (128), pair (256) and triple (32 / 128) kernels; the batch run in 128-row p
 equal the single run bit for bit; the plain kernel and the unpaired program within 3e-6; the float32
 and float64 single-event programs and the float64 batch; and the kernel census, which must show the
 variants the case claims.  The coverage test checks the census of all cases against the required set.
+The census of every case is taken once, in a fresh interpreter: after many profiler sessions in one
+process the profiler stops recording some launches.
 """
+import json
+import os
+import subprocess
+import sys
+
 import numpy as np
 import pytest
 
@@ -68,8 +75,26 @@ def items_of(cases):
             for i, c in enumerate(cases)]
 
 
+_CENSUS_SCRIPT = """
+import json, sys
+import kernel_corpus, test_gpu_kernel_variants as T
+json.dump([sorted(s) for s in T.items_of([T.Case(case) for case in kernel_corpus.CASES])], sys.stdout)
+"""
+
+
+@pytest.fixture(scope="module")
+def corpus_items():
+    """Coverage items of every corpus case (`items_of`), taken in a fresh interpreter."""
+    here = os.path.dirname(os.path.abspath(__file__))
+    env = dict(os.environ, PYTHONPATH=os.pathsep.join([here, os.path.dirname(here), os.environ.get("PYTHONPATH", "")]))
+    res = subprocess.run([sys.executable, "-c", _CENSUS_SCRIPT], capture_output=True, text=True, env=env, cwd=here,
+                         timeout=1800)
+    assert res.returncode == 0, res.stderr[-3000:]
+    return {case["name"]: set(items) for case, items in zip(kernel_corpus.CASES, json.loads(res.stdout))}
+
+
 @pytest.mark.parametrize("case", kernel_corpus.CASES, ids=kernel_corpus.case_id)
-def test_variant_case_matches_oracle(case):
+def test_variant_case_matches_oracle(case, corpus_items):
     c = Case(case)
     order = [c.net.names[v] for v in c.plan.order]
     codes = c.codes
@@ -111,16 +136,15 @@ def test_variant_case_matches_oracle(case):
     for b in range(N_MAX):
         check_row(out64[:, b], want(b)[0], 1e-12)
 
-    seen = items_of([c])[0]
+    seen = corpus_items[case["name"]]
     assert set(case["claims"]) <= seen, sorted(set(case["claims"]) - seen)
     assert not seen & set(kernel_corpus.UNREACHABLE), sorted(seen & set(kernel_corpus.UNREACHABLE))
 
 
-def test_variant_corpus_covers_the_required_items():
-    """The census of every corpus case, taken here: each required item is reached by some case, or
-    listed in UNREACHABLE (a reason from the dispatch code) or OPEN, which no case may reach."""
-    names = [case["name"] for case in kernel_corpus.CASES]
-    seen = dict(zip(names, items_of([Case(case) for case in kernel_corpus.CASES])))
+def test_variant_corpus_covers_the_required_items(corpus_items):
+    """The census of every corpus case: each required item is reached by some case, or listed in
+    UNREACHABLE (a reason from the dispatch code) or OPEN, which no case may reach."""
+    seen = corpus_items
     union = set().union(*seen.values())
     lines = []
     for item in sorted(kernel_corpus.required_items()):

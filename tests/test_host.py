@@ -309,3 +309,33 @@ def test_out_of_memory_evicts_other_cached_programs_and_retries():
 
     with pytest.raises(engine.EngineError):
         bn._run_evicting(Broken(False), np.zeros((1, 4), dtype=np.uint8), 4)
+
+
+def test_a_device_listed_twice_gets_a_program_per_listing(monkeypatch):
+    """`query_many(devices=[0, 0, 0])` runs three threads on one GPU.  A program's scratch arena,
+    staging buffers and graph capture serve one caller at a time, so each listing must get its own
+    programs; one shared program let the threads free and capture each other's buffers and streams."""
+    import threading
+
+    users = {}  # program -> threads that ran it
+
+    class FakeProgram:
+        def __init__(self, plan, device=None, f64=False):
+            self.Q = plan.Q
+
+        def run(self, codes, n):
+            users.setdefault(id(self), set()).add(threading.get_ident())
+            return np.full((self.Q, n), 1.0 / self.Q, dtype=np.float32)
+
+        def close(self):
+            pass
+
+    monkeypatch.setattr(engine, "Program", FakeProgram)
+    bn = examples.build(examples.NETWORKS["asia"])
+    ev_vars = ("Smoker", "Dispnea")
+    codes = np.zeros((2, 9), dtype=np.uint8)
+    post = bn._posterior_codes_multi(("Lung cancer",), ev_vars, codes, np.zeros(9, dtype=bool), [0, 0, 0])
+    assert post.shape == (2, 9) and np.allclose(post, 0.5)
+    assert len(users) == 3 and all(len(t) == 1 for t in users.values()), users
+    keys = [k for k in bn._engine_cache if k[2] == 1 and not k[3]]
+    assert len(keys) == 3 and {k[4] for k in keys} == {0, (0, 1), (0, 2)}, keys
