@@ -572,6 +572,7 @@ SbnPair *plan_triple(sbn_program *P, int i1, int i2, std::vector<int32_t> *tiles
             dig[k] = 0;
         }
     }
+    sbn_triple_rows_plan(q, tiles->data() + pr->tile_off_pos, &pr->rows);
     return pr;
 }
 
@@ -790,6 +791,7 @@ static cudaError_t triple_launch(sbn_program *P, const SbnPair &pr, int64_t n_ro
     q.ld = P->ld;
     q.n_rows = static_cast<int32_t>(n_rows);
     q.tile_off = P->d_pair_tiles + pr.tile_off_pos;
+    if (sbn_triple_rows_launch(P, pr.rows, q, stream)) return cudaGetLastError();
     // with a group axis: 32 rows x T group digits per CTA; without: 128 rows
     const int rows_per_cta = q.group > 1 ? 32 : 128;
     const int64_t n_rblocks = (n_rows + rows_per_cta - 1) / rows_per_cta;

@@ -101,6 +101,25 @@ struct SbnTripleParams {
     int32_t a_g, o_g;             // ... with these entry strides in A and in the output
 };
 
+// Row-block variant of the expanding product (sbn_triple_rows.cu), for batches with enough blocks of
+// SBN_TRIPLE_ROWS_R rows to fill every SM.  A persistent CTA walks the row blocks and, per block, the T values of
+// p: the entries of A, B and C that one p needs for the block's rows (T x T per combination of the untouched axes)
+// arrive in shared memory as one tensor-map TMA box per operand, into a ring of full / empty mbarriers.  Each
+// operand is then read from HBM once instead of once per combination it lacks.  Thread = (row, combination c):
+// the same fp32 operations in the same order as sbn_triple_kernel, so the two kernels give bitwise equal results.
+// A combination c = tile t + n_tiles x group digit g must select, in each operand, one digit of (at most) one
+// axis beside p and the two loop axes: the box is (R rows) x T x T x (that axis' digits).
+#define SBN_TRIPLE_ROWS_R 16          // evidence rows per block: 64 B per entry
+#define SBN_TRIPLE_ROWS_COMBOS 25     // combinations per row at most (R x 25 = 400 consumer threads)
+#define SBN_TRIPLE_ROWS_MIN_COMBOS 8  // fewer leave the SM short of threads (R x 8 = 128)
+struct SbnTripleRows {
+    int ok;                                     // 0: shape not covered, sbn_triple_kernel runs at every batch size
+    int n_combos;                               // n_tiles x group
+    int32_t u_card[3], u_stride[3];             // A, B, C: digits and entry stride of the axis the combinations walk
+    int32_t u_dig[3][SBN_TRIPLE_ROWS_COMBOS];   // ... and its digit for each combination
+    int32_t o_off[SBN_TRIPLE_ROWS_COMBOS];      // output entry of each combination at z = s = 0
+};
+
 // One planned pair (host side).
 struct SbnPair {
     int kind;                     // 0: two table x frontier steps (SbnPairParams); 1: expanding product + contraction (SbnTripleParams)
@@ -110,6 +129,7 @@ struct SbnPair {
     int m1, m2;                   // SbnPairMode of the two steps
     SbnPairParams q;              // everything but the run-time pointers
     SbnTripleParams t;
+    SbnTripleRows rows;           // kind 1: the row-block variant's view of the operands
     int a_in, b_in, c_in;         // kind 1: operand indices (A, B among step1's inputs, C among step2's)
     int64_t tile_off_pos;         // int32 offset into the pair tile table
     int64_t canon_pos;            // float offset into the canonical coefficient buffer
@@ -125,3 +145,10 @@ cudaError_t sbn_pair_launch(sbn_program *P, const SbnPair &pr, const uint8_t *d_
 bool sbn_pair_fits(const sbn_program *P, const SbnPair &pr);
 cudaError_t sbn_pair_set_attrs();
 void sbn_pair_free(sbn_program *P);
+
+// sbn_triple_rows.cu.  Plan: fills `rows` from a triple's parameters and its tile table ([n_tiles][4] words).
+void sbn_triple_rows_plan(const SbnTripleParams &q, const int32_t *tiles, SbnTripleRows *rows);
+// Launch: `q` with its run-time pointers set.  false (nothing launched) when the shape is not covered, the batch has
+// fewer than 2 x SMs row blocks, or SOROBN_B200_TRIPLE_ROWS=0: sbn_triple_kernel runs the triple then.
+bool sbn_triple_rows_launch(const sbn_program *P, const SbnTripleRows &rows, const SbnTripleParams &q, cudaStream_t stream);
+cudaError_t sbn_triple_rows_set_attrs();

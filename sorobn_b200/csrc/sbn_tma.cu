@@ -301,6 +301,25 @@ bool sbn_tma_encode_rows(CUtensorMap *map, const float *base, int64_t ld, int64_
                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+bool sbn_tma_encode_view(CUtensorMap *map, const float *base, int64_t ld, int64_t n_rows, int rank, const int64_t *dims,
+                         const int64_t *strides, const int *box, int box_rows) {
+    if (!encode_fn() || rank < 1 || rank > 4) return false;
+    cuuint64_t gdim[5], gstride[4];
+    cuuint32_t gbox[5], estr[5];
+    gdim[0] = static_cast<cuuint64_t>(n_rows);
+    gbox[0] = static_cast<cuuint32_t>(box_rows);
+    estr[0] = 1;
+    for (int k = 0; k < rank; ++k) {
+        gdim[k + 1] = static_cast<cuuint64_t>(dims[k]);
+        gstride[k] = static_cast<cuuint64_t>(dims[k] > 1 ? strides[k] : 1) * static_cast<cuuint64_t>(ld) * 4;
+        gbox[k + 1] = static_cast<cuuint32_t>(box[k]);
+        estr[k + 1] = 1;
+    }
+    return encode_fn()(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, static_cast<cuuint32_t>(rank + 1), const_cast<float *>(base), gdim, gstride,
+                       gbox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
 cudaError_t sbn_tma_set_attrs() {
     cudaError_t e = set_attr<5, 5>();
     if (e == cudaSuccess) e = set_attr<4, 4>();

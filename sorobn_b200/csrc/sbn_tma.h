@@ -84,3 +84,9 @@ cudaError_t sbn_tma_set_attrs();
 // factor for box_rows rows, entry-major in shared memory.  Rows past n_rows arrive as zeros.  false when the
 // driver has no encoder or refuses the view.
 bool sbn_tma_encode_rows(CUtensorMap *map, const float *base, int64_t ld, int64_t n_rows, int64_t entries, int box_rows, int e_lo);
+// Tensor map of the first n_rows rows of a batched factor [entries][ld] seen through `rank` (<= 4) entry axes of
+// extents dims[] and entry strides strides[] (any order; an axis of extent 1 may have any stride): the view
+// (row, axis 0, .., axis rank-1), box (box_rows, box[0], .., box[rank-1]), row-major in shared memory with the row
+// fastest.  Rows past n_rows arrive as zeros.  false when the driver has no encoder or refuses the view.
+bool sbn_tma_encode_view(CUtensorMap *map, const float *base, int64_t ld, int64_t n_rows, int rank, const int64_t *dims,
+                         const int64_t *strides, const int *box, int box_rows);
