@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SBN_ABI_VERSION 9
+#define SBN_ABI_VERSION 10
 
 #define SBN_OK 0
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
@@ -99,6 +99,26 @@ int sbn_program_run_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev
  * a row below the float32 range (re-run it with a float64 program). */
 int sbn_program_evidence_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, float *prob);
 int sbn_program_evidence_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *prob);
+
+/* Expected counts (the E-step of expectation-maximisation) of a counts program
+ * (planner.build_counts_plan, version 6; the run and evidence calls refuse it, and these calls refuse
+ * every other program).  For every row b and every node v, P(v, parents(v) | the row's observed cells)
+ * is ADDED into counts[c_offset(v) + ...]: the dense [*parents, v] arrays of the CPTs in the network's
+ * order, concatenated, n_counts entries in all.  prob[b] = P(observed cells of b), or NaN for a row below
+ * the float32 range (1e-30; 1e-290 for the float64 twin) or of probability zero: such a row adds nothing,
+ * re-run it with a float64 program.  The rows are reduced without floating-point atomics: two calls on
+ * the same device and batch give bitwise the same counts.  Large batches run in chunks. */
+int sbn_program_counts_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts,
+                            int64_t n_counts, float *prob);
+int sbn_program_counts_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts,
+                                int64_t n_counts, double *prob);
+
+/* Replace a counts program's table blob in place (same size and layout: planner.refresh_tables) and
+ * re-run its evidence-independent launches; later runs, graph replays included, use the new values.
+ * An EM loop plans once and calls this every iteration.  Other programs are refused: their paired
+ * steps fold table products into coefficients built on the host. */
+int sbn_program_set_tables(sbn_program *prog, const float *tables, int64_t n_table_floats);
+int sbn_program_set_tables_f64(sbn_program *prog, const double *tables, int64_t n_table_doubles);
 
 /* Same with DEVICE buffers, asynchronous on `stream` (a cudaStream_t; NULL = default
  * stream).  n_rows must not exceed the reserved chunk size. */

@@ -20,6 +20,10 @@ The approximate algorithms run on the device too (csrc/sbn_gibbs.cuh): `algorith
 (bayes_net.py:665-737) one chain per evidence row, `"likelihood"` (:621-663) and `"rejection"`
 (:577-619) n_iterations forward samples per row.  `fit` / `partial_fit` / `sample`
 (:467-575) stay on the host (pandas / numpy), as in the reference.
+
+`expected_counts` / `fit_em` learn from incomplete data (missing cells, latent nodes) by
+expectation-maximisation; the E-step runs on the device as one counts program per missingness
+pattern (planner.build_counts_plan, csrc/sbn_count.cuh).
 """
 from __future__ import annotations
 
@@ -39,6 +43,39 @@ __all__ = ["BayesNet"]
 
 def _as_list(obj):
     return obj if isinstance(obj, list) else [obj]
+
+
+class _CountsRunner:
+    """The device programs of one missingness pattern: the float32 counts program, and the float64 one
+    for the rows it flags (created when first needed).  `set_cpts` gives both new tables in place."""
+
+    def __init__(self, plan, device):
+        from . import engine  # raises if libsorobn_b200.so cannot be loaded
+
+        self.plan, self.device = plan, device
+        self.f32 = engine.Program(plan, device=device)
+        self._f64 = None
+        self._blob64 = None
+
+    def set_cpts(self, cpts):
+        blob32, self._blob64 = _planner.refresh_tables(self.plan, cpts)
+        self.f32.set_tables(blob32)
+        if self._f64 is not None:
+            self._f64.set_tables(self._blob64)
+
+    def f64(self):
+        if self._f64 is None:
+            from . import engine
+
+            self._f64 = engine.Program(self.plan, device=self.device, f64=True)
+            if self._blob64 is not None:
+                self._f64.set_tables(self._blob64)
+        return self._f64
+
+    def close(self):
+        self.f32.close()
+        if self._f64 is not None:
+            self._f64.close()
 
 
 class BayesNet:
@@ -312,6 +349,181 @@ class BayesNet:
         self.P = {}
         self._P_sizes = {}
         return self.partial_fit(X)
+
+    # ------------------------------------------------------- expected counts / EM
+    def expected_counts(self, X: pd.DataFrame) -> dict:
+        """The E-step of expectation-maximisation: for every node v, the sum over the rows of `X` of
+        P(v, parents(v) | the row's observed cells), computed on the GPU.
+
+        A missing cell is None or NaN; a node without a column in `X` is latent (unobserved in every
+        row).  Returns {node: float64 Series} indexed like the densified CPT -- levels [*parents, v],
+        every combination of the compiled domains, zeros kept.  Raises ValueError for a value outside
+        its variable's domain and for rows whose observed cells have probability zero.
+
+        Rows are grouped by missingness pattern (the set of observed columns); each pattern is one
+        counts program (planner.build_counts_plan), so the cost grows with the number of distinct
+        patterns as well as with the rows."""
+        groups = self._count_patterns(X)
+        net = self._compiled
+        offsets, n_counts = _planner.count_layout(net)
+        # each pattern's programs are fetched right before they run: with more patterns than the cache holds,
+        # fetching one may close the least recently used ones, which have run by then
+        counts, _ = self._e_step(X, groups, lambda k, ev: self._counts_runner(ev), n_counts)
+        out = {}
+        for v, name in enumerate(net.names):
+            size = int(np.prod(net.cpt[v].shape))
+            out[name] = pd.Series(counts[offsets[v]:offsets[v] + size], index=self._family_index(v), name=name)
+        return out
+
+    def fit_em(self, X: pd.DataFrame, max_iter: int = 100, tol: float = 1e-6) -> "BayesNet":
+        """Fit the CPTs to `X` by expectation-maximisation, when cells are missing (None / NaN) or nodes
+        are latent (no column in `X`).
+
+        Start: the current CPTs if every node has one; otherwise, if every node is a column of `X`, the
+        available-case `fit(X)`; otherwise ValueError (a latent variable's domain, and a start that
+        breaks its symmetry, must come from the user).  Each iteration runs `expected_counts` (the
+        programs are planned once per call; only their tables change) and normalises the counts per
+        parent configuration, after one pseudo-observation per entry with `prior_count`.  Entries of
+        zero expected count are left out of the Series, as `fit` leaves out unseen combinations.
+        Iteration stops when the observed-data log-likelihood sum_b log P(observed cells of b) rises by
+        less than `tol` per row, or after `max_iter` iterations.  The log-likelihood of every iteration
+        is kept in `em_log_likelihood_`; `_P_sizes` holds the final expected counts, so a later
+        `partial_fit` continues from them."""
+        if int(max_iter) < 1:
+            raise ValueError(f"max_iter must be at least 1, not {max_iter}")
+        if all(n in self.P for n in self.nodes):
+            if self._compiled is None:
+                self.prepare()
+        elif all(n in X.columns for n in self.nodes):
+            self.fit(X)
+        else:
+            latent = [n for n in self.nodes if n not in X.columns]
+            raise ValueError(f"fit_em needs initial CPTs in P when nodes have no column in X ({latent[:5]}): a latent "
+                             "variable's states and a start that breaks its symmetry must come from the user")
+        groups = self._count_patterns(X)
+        net = self._compiled
+        offsets, n_counts = _planner.count_layout(net)
+        n_rows = len(X.index)
+        runners = [_CountsRunner(_planner.build_counts_plan(net, ev), self.device) for ev, _, _ in groups]
+        cpts = [np.array(c, dtype=np.float64) for c in net.cpt]
+        lls = []
+        try:
+            for it in range(int(max_iter)):
+                if it:
+                    for r in runners:
+                        r.set_cpts(cpts)
+                counts, ll = self._e_step(X, groups, lambda k, ev: runners[k], n_counts)
+                lls.append(ll)
+                fam = [counts[offsets[v]:offsets[v] + c.size].reshape(c.shape) for v, c in enumerate(cpts)]
+                if self.prior_count:
+                    fam = [f + 1.0 for f in fam]
+                totals = [f.sum(axis=-1) for f in fam]
+                with np.errstate(invalid="ignore", divide="ignore"):
+                    cpts = [np.where(t[..., None] > 0, f / t[..., None], 0.0) for f, t in zip(fam, totals)]
+                if it and ll - lls[-2] < tol * n_rows:
+                    break
+        finally:
+            for r in runners:
+                r.close()
+        self.em_log_likelihood_ = lls
+        for v, node in enumerate(net.names):
+            table = pd.Series(cpts[v].reshape(-1), index=self._family_index(v))
+            self.P[node] = table[fam[v].reshape(-1) > 0]
+            parents = self.parents.get(node)
+            if parents:
+                tot = totals[v].reshape(-1)
+                index = self._family_index(v, parents_only=True)
+                self._P_sizes[node] = pd.Series(tot, index=index)[tot > 0]
+            else:
+                self._P_sizes[node] = float(totals[v])
+        self.prepare()
+        return self
+
+    def _family_index(self, v, parents_only=False):
+        """Index of every combination of the compiled domains of [*parents, v] (or of the parents alone)."""
+        net = self._compiled
+        scope = list(net.scope(v))[:-1] if parents_only else list(net.scope(v))
+        names = [net.names[u] for u in scope]
+        if len(scope) == 1:
+            return pd.Index(net.domains[scope[0]], name=names[0])
+        return pd.MultiIndex.from_product([net.domains[u] for u in scope], names=names)
+
+    def _count_patterns(self, X):
+        """[(observed var ids, sorted; positions of the rows; uint8 codes [n_observed, n_rows])] per
+        missingness pattern of `X`."""
+        if self._compiled is None:
+            self._compile()
+            if self._compiled is None:
+                raise ValueError("every node needs a CPT in P before computing expected counts; call prepare()")
+        net = self._compiled
+        cols = list(X.columns)
+        for c in cols:
+            if c not in net.index:
+                raise KeyError(c)
+        n = len(X.index)
+        missing = X.isna().to_numpy().reshape(n, len(cols))
+        codes = np.zeros((len(cols), n), dtype=np.uint8)
+        for i, c in enumerate(cols):
+            v = net.index[c]
+            idx = pd.Index(net.domains[v]).get_indexer(pd.Index(X[c].to_numpy()))
+            bad = (idx < 0) & ~missing[:, i]
+            if bad.any():
+                b = int(np.flatnonzero(bad)[0])
+                raise ValueError(f"column {c!r}: {X[c].iloc[b]!r} (row {X.index[b]!r}) is not a state of the variable")
+            codes[i] = np.where(idx < 0, 0, idx).astype(np.uint8)
+        if n == 0:
+            return []
+        # group the rows by their observed-column bitmask, packed into 64-bit words (np.unique(axis=0) on the
+        # boolean matrix sorts structured rows: seconds for a million rows)
+        bits = np.packbits(~missing, axis=1)
+        width = max(8, -(-bits.shape[1] // 8) * 8)  # bytes per row: whole 64-bit words, at least one
+        bits = np.pad(bits, ((0, 0), (0, width - bits.shape[1])))
+        words = np.ascontiguousarray(bits).view(np.uint64)
+        order = np.lexsort(words.T[::-1]) if words.shape[1] > 1 else np.argsort(words[:, 0], kind="stable")
+        ordered = words[order]
+        starts = np.flatnonzero(np.r_[True, (ordered[1:] != ordered[:-1]).any(axis=1)])
+        groups = []
+        for s, e in zip(starts, np.r_[starts[1:], n]):
+            rows = np.sort(order[s:e])
+            observed = ~missing[rows[0]]
+            col_of = {net.index[cols[i]]: i for i in range(len(cols)) if observed[i]}
+            ev = tuple(sorted(col_of))
+            groups.append((ev, rows, np.ascontiguousarray(codes[[col_of[v] for v in ev]][:, rows])))
+        return groups
+
+    def _counts_runner(self, ev):
+        """The cached programs of one missingness pattern (dropped by `prepare()`, as every program)."""
+        with self._cache_lock:
+            key = ("counts", ev, self.device)
+            hit = self._engine_cache.get(key)
+            if hit is None:
+                hit = self._engine_cache[key] = _CountsRunner(_planner.build_counts_plan(self._compiled, ev), self.device)
+                self._evict()
+            else:
+                self._engine_cache.move_to_end(key)
+            return hit
+
+    def _e_step(self, X, groups, runner_of, n_counts):
+        """(expected counts [n_counts], observed-data log-likelihood) of every pattern's rows;
+        `runner_of(k, observed var ids)` gives the programs of pattern k.  Rows the float32 program flags
+        are settled by the float64 one; rows still without a probability raise."""
+        counts = np.zeros(n_counts, dtype=np.float64)
+        ll = 0.0
+        for k, (ev, rows, codes) in enumerate(groups):
+            runner = runner_of(k, ev)
+            c, prob = runner.f32.counts(codes, len(rows))
+            counts += c
+            prob = prob.astype(np.float64)
+            flagged = np.flatnonzero(np.isnan(prob))
+            if len(flagged):
+                c, prob[flagged] = runner.f64().counts(np.ascontiguousarray(codes[:, flagged]), len(flagged))
+                counts += c
+            impossible = np.isnan(prob)
+            if impossible.any():
+                raise ValueError(f"{int(impossible.sum())} row(s) have observed cells of probability zero "
+                                 f"(first: {X.index[rows[impossible][0]]!r}); their expected counts are undefined")
+            ll += float(np.log(prob).sum())
+        return counts, ll
 
     def sample(self, n=1, init: dict | None = None, method="forward"):
         """Forward (ancestral) samples (bayes_net.py:550-575): a Series for n == 1, otherwise a

@@ -16,6 +16,7 @@
 #include <vector>
 
 #include "sbn_chain.h"
+#include "sbn_count.cuh"
 #include "sbn_gibbs.cuh"
 #include "sbn_internal.h"
 #include "sbn_join.h"
@@ -50,6 +51,7 @@ int fail(int code, const char *fmt, ...) {
 constexpr int32_t kMagic = 0x53424E31;
 constexpr int kVersion = 4;
 constexpr int kVersionMarginals = 5;  // planner.build_marginals_plan: kind-2 readouts, no posterior slot
+constexpr int kVersionCounts = 6;     // planner.build_counts_plan: kind-3 count steps, P(observed) in the posterior slot
 constexpr int64_t kMarginalZoffMax = 1 << 24;  // int32 words of one readout's joint-state offset table
 constexpr int kMaxElim = 3;
 constexpr int kMaxZ = 256;
@@ -62,9 +64,11 @@ namespace {
 int parse(sbn_program *P, const int32_t *w, int64_t n) {
     if (n < kHeaderWords) return fail(SBN_E_INVALID, "program shorter than its header");
     if (w[0] != kMagic) return fail(SBN_E_INVALID, "bad program magic 0x%x", w[0]);
-    if (w[1] != kVersion && w[1] != kVersionMarginals)
-        return fail(SBN_E_INVALID, "program version %d, engine expects %d or %d", w[1], kVersion, kVersionMarginals);
+    if (w[1] != kVersion && w[1] != kVersionMarginals && w[1] != kVersionCounts)
+        return fail(SBN_E_INVALID, "program version %d, engine expects %d, %d or %d", w[1], kVersion, kVersionMarginals,
+                    kVersionCounts);
     P->marginals = w[1] == kVersionMarginals;
+    P->counts = w[1] == kVersionCounts;
     P->mode = w[2];
     P->n_ev = w[3];
     const int n_tables = w[4], n_slots = w[5], n_steps = w[6];
@@ -74,6 +78,10 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
     if (P->mode != 0 && P->mode != 1) return fail(SBN_E_INVALID, "bad mode %d", P->mode);
     if (P->n_ev < 0 || n_tables < 0 || n_slots <= 0 || n_steps <= 0 || P->Q <= 0)
         return fail(SBN_E_INVALID, "bad header counts");
+    if (P->counts) {
+        P->n_counts = w[10];
+        if (P->Q != 1 || P->n_counts <= 0) return fail(SBN_E_INVALID, "bad counts header");
+    }
     if (P->marginals ? (P->post_slot != -1 || P->post_batched != 0) : (P->post_slot < 0 || P->post_slot >= n_slots))
         return fail(SBN_E_INVALID, "post slot out of range");
     int64_t p = kHeaderWords;
@@ -108,7 +116,42 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         st.cx = 1;
         p += 5;
         const bool readout = st.kind == 2;
-        if (st.kind != 0 && st.kind != 1 && !(readout && P->marginals)) return fail(SBN_E_INVALID, "step %d: bad kind", s);
+        const bool count = st.kind == 3;
+        if (st.kind != 0 && st.kind != 1 && !(readout && P->marginals) && !(count && P->counts))
+            return fail(SBN_E_INVALID, "step %d: bad kind", s);
+        if (count) {
+            // c_offset, the observed members' gathers and the count-table strides of the output axes
+            if (!need(2)) return fail(SBN_E_INVALID, "truncated step %d", s);
+            st.q_offset = w[p];
+            const int n_key = w[p + 1];
+            p += 2;
+            if (st.out_slot != -1 || n_axes < 0 || n_axes > SBN_MAX_AXES || n_elim < 0 || n_elim > 64 || n_key < 0 ||
+                n_key > SBN_MAX_EV || (n_in == 0 && (n_axes != 0 || n_elim != 0)))
+                return fail(SBN_E_INVALID, "step %d: bad count step", s);
+            if (!need(3LL * n_key + n_axes)) return fail(SBN_E_INVALID, "truncated step %d", s);
+            int64_t span = 1;
+            for (int k = 0; k < n_key; ++k) {
+                EvAxis a{w[p], w[p + 1], w[p + 2]};
+                p += 3;
+                if (a.col < 0 || a.col >= P->n_ev || a.stride < 0 || a.card < 1 || a.card > 256)
+                    return fail(SBN_E_INVALID, "step %d: bad key axis", s);
+                span += static_cast<int64_t>(a.card - 1) * a.stride;
+                st.key.push_back(a);
+            }
+            for (int j = 0; j < n_axes; ++j) {
+                if (w[p + j] < 0) return fail(SBN_E_INVALID, "step %d: negative count stride", s);
+                st.cstrides.push_back(w[p + j]);
+            }
+            p += n_axes;
+            if (!need(n_axes)) return fail(SBN_E_INVALID, "truncated step %d", s);
+            for (int j = 0; j < n_axes; ++j) {
+                if (w[p + j] < 1) return fail(SBN_E_INVALID, "step %d: axis card %d", s, w[p + j]);
+                span += static_cast<int64_t>(w[p + j] - 1) * st.cstrides[j];
+            }
+            if (st.q_offset < 0 || span >= (1LL << 31) || st.q_offset + span > P->n_counts)
+                return fail(SBN_E_INVALID, "step %d: count-table entries outside the table", s);
+            st.span = span;
+        }
         if (readout) {
             // one output axis (the target), written at posterior rows q_offset .. q_offset + card - 1
             if (!need(1)) return fail(SBN_E_INVALID, "truncated step %d", s);
@@ -117,24 +160,26 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
                 return fail(SBN_E_INVALID, "step %d: bad readout step", s);
         }
         if (st.kind == 1 && P->mode == 0) return fail(SBN_E_INVALID, "step %d: batched step in a flat program", s);
-        if (n_in < 1 || n_in > SBN_MAX_IN) return fail(SBN_E_INVALID, "step %d: %d inputs", s, n_in);
+        if (n_in < (count ? 0 : 1) || n_in > SBN_MAX_IN) return fail(SBN_E_INVALID, "step %d: %d inputs", s, n_in);
         if (n_axes < 0 || n_axes > SBN_MAX_AXES) return fail(SBN_E_INVALID, "step %d: %d axes", s, n_axes);
-        if (!readout && (n_elim < 0 || n_elim > kMaxElim)) return fail(SBN_E_INVALID, "step %d: %d eliminated axes", s, n_elim);
-        if (!readout && (st.out_slot < 0 || st.out_slot >= n_slots)) return fail(SBN_E_INVALID, "step %d: out slot", s);
+        const bool writes_slot = !readout && !count;
+        if (writes_slot && (n_elim < 0 || n_elim > kMaxElim)) return fail(SBN_E_INVALID, "step %d: %d eliminated axes", s, n_elim);
+        if (writes_slot && (st.out_slot < 0 || st.out_slot >= n_slots)) return fail(SBN_E_INVALID, "step %d: out slot", s);
         if (!need(n_axes + n_elim)) return fail(SBN_E_INVALID, "truncated step %d", s);
         st.n_out = 1;
         for (int j = 0; j < n_axes; ++j) {
             const int c = w[p + j];
             if (c < 1) return fail(SBN_E_INVALID, "step %d: axis card %d", s, c);
             st.n_out *= c;
-            if (st.n_out >= (1LL << 31)) return fail(SBN_E_INVALID, "step %d: output too large", s);
+            if (st.n_out >= (1LL << 31) || (count && st.n_out > kMarginalZoffMax / SBN_MAX_IN))
+                return fail(SBN_E_INVALID, "step %d: output too large", s);
             st.cards.push_back(c);
         }
         p += n_axes;
         for (int k = 0; k < n_elim; ++k) {
             const int c = w[p + k];
             if (c < 1) return fail(SBN_E_INVALID, "step %d: eliminated card %d", s, c);
-            if (static_cast<int64_t>(st.cx) * c > (readout ? kMarginalZoffMax / SBN_MAX_IN : kMaxZ))
+            if (static_cast<int64_t>(st.cx) * c > (readout || count ? kMarginalZoffMax / SBN_MAX_IN : kMaxZ))
                 return fail(SBN_E_INVALID, "step %d: too many eliminated states", s);
             st.cx *= c;
             st.ecards.push_back(c);
@@ -143,12 +188,14 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         if (readout) {
             if (st.q_offset < 0 || st.q_offset + st.n_out > P->Q) return fail(SBN_E_INVALID, "step %d: segment outside the posterior", s);
             for (int64_t q = st.q_offset; q < st.q_offset + st.n_out; ++q) written[q]++;
+        } else if (count) {
+            if (static_cast<int64_t>(st.cx) * st.n_out >= (1LL << 31)) return fail(SBN_E_INVALID, "step %d: count step too large", s);
         } else {
             const Slot &os = P->slots[st.out_slot];
             if (os.batched != (st.kind == 1)) return fail(SBN_E_INVALID, "step %d: out slot kind mismatch", s);
             if (os.size < st.n_out) return fail(SBN_E_INVALID, "step %d: out slot too small", s);
         }
-        const bool per_row = st.kind == 1 || (readout && P->mode == 1);  // batched operands allowed
+        const bool per_row = st.kind == 1 || ((readout || count) && P->mode == 1);  // batched operands allowed
         for (int i = 0; i < n_in; ++i) {
             if (!need(4)) return fail(SBN_E_INVALID, "truncated step %d input %d", s, i);
             InDesc in;
@@ -203,6 +250,11 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             if (max_off >= size) return fail(SBN_E_INVALID, "step %d input %d: reads past its buffer", s, i);
             st.in.push_back(std::move(in));
         }
+        if (count) {  // inputs without any family axis first: loaded once per joint state z
+            auto no_axis = [](const InDesc &in) { return std::all_of(in.strides.begin(), in.strides.end(), [](int v) { return v == 0; }); };
+            std::stable_partition(st.in.begin(), st.in.end(), no_axis);
+            st.n_common = static_cast<int>(std::count_if(st.in.begin(), st.in.end(), no_axis));
+        }
         if (readout) {
             std::stable_partition(st.in.begin(), st.in.end(), [](const InDesc &in) { return in.strides[0] == 0; });
             st.n_common = static_cast<int>(std::count_if(st.in.begin(), st.in.end(), [](const InDesc &in) { return in.strides[0] == 0; }));
@@ -221,6 +273,21 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
     if (P->marginals) {
         for (int q = 0; q < P->Q; ++q)
             if (written[q] != 1) return fail(SBN_E_INVALID, "posterior entry %d is written %d times", q, written[q]);
+    } else if (P->counts) {
+        // P(observed) is written before the first count step and not overwritten before the last one
+        int first = -1, last = -1, writer = -1;
+        for (size_t i = 0; i < P->steps.size(); ++i) {
+            if (P->steps[i].kind == 3) {
+                if (first < 0) first = static_cast<int>(i);
+                last = static_cast<int>(i);
+            } else if (P->steps[i].out_slot == P->post_slot) {
+                writer = static_cast<int>(i);
+            }
+        }
+        if (first < 0) return fail(SBN_E_INVALID, "a counts program without a count step");
+        if (writer < 0 || writer > first) return fail(SBN_E_INVALID, "P(observed) is not written before the count steps");
+        for (int i = first; i <= last; ++i)
+            if (P->steps[i].kind != 3) return fail(SBN_E_INVALID, "step %d comes between the count steps", i);
     } else if (P->steps.back().out_slot != P->post_slot) {
         return fail(SBN_E_INVALID, "last step does not write the posterior");
     }
@@ -410,7 +477,29 @@ void plan_tiles(sbn_program *P, std::vector<int32_t> *words) {
     // zoff[i][z] = sum_k digit_k(z) * estride_i[k], first eliminated variable fastest
     for (StepDesc &st : P->steps) {
         st.zoff_pos = -1;
-        if (st.ecards.size() < 2 && st.kind != 2) continue;
+        if (st.kind == 3) {
+            // count step: soff[i][s] = sum_j digit_j(s) * strides_i[j], coff[s] = sum_j digit_j(s) * cstrides[j]
+            st.soff_pos = static_cast<int64_t>(words->size());
+            for (const InDesc &in : st.in)
+                for (int64_t s = 0; s < st.n_out; ++s) {
+                    int64_t r = s, off = 0;
+                    for (size_t j = 0; j < st.cards.size(); ++j) {
+                        off += (r % st.cards[j]) * in.strides[j];
+                        r /= st.cards[j];
+                    }
+                    words->push_back(static_cast<int32_t>(off));
+                }
+            st.coff_pos = static_cast<int64_t>(words->size());
+            for (int64_t s = 0; s < st.n_out; ++s) {
+                int64_t r = s, off = 0;
+                for (size_t j = 0; j < st.cards.size(); ++j) {
+                    off += (r % st.cards[j]) * st.cstrides[j];
+                    r /= st.cards[j];
+                }
+                words->push_back(static_cast<int32_t>(off));
+            }
+        }
+        if (st.ecards.size() < 2 && st.kind != 2 && st.kind != 3) continue;
         st.zoff_pos = static_cast<int64_t>(words->size());
         for (const InDesc &in : st.in) {
             for (int z = 0; z < st.cx; ++z) {
@@ -790,6 +879,103 @@ cudaError_t launch_marginal(sbn_program *P, const StepDesc &st, const uint8_t *e
     return sbn_marginal_launch<float>(m, static_cast<size_t>(smem) * 4, stream);
 }
 
+// Persistent CTAs of one count step: enough for 4 per SM, fewer when the per-warp partial tables of a large
+// family would pass kCountPartialBytes.  Depends on the step, the device and n_rows only.
+constexpr int64_t kCountPartialBytes = 64LL << 20;
+int64_t count_grid(const sbn_program *P, const StepDesc &st, int64_t n_rows) {
+    const int64_t blocks = (n_rows + SBN_COUNT_THREADS - 1) / SBN_COUNT_THREADS;
+    const int64_t cap = std::max<int64_t>(1, kCountPartialBytes / (8 * SBN_COUNT_WARPS * st.span));
+    return std::max<int64_t>(1, std::min<int64_t>({blocks, 4LL * P->n_sms, cap}));
+}
+
+// Count step (kind 3): adds the family's expected counts of rows 0 .. n_rows - 1 into P->d_counts.
+cudaError_t launch_count(sbn_program *P, const StepDesc &st, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, cudaStream_t stream) {
+    P->launches += 2;
+    SbnCount c;
+    memset(&c, 0, sizeof c);
+    const size_t elem = P->f64 ? 8 : 4;
+    const int64_t grid = count_grid(P, st, n_rows);
+    c.partial = P->d_partial;
+    c.ev = ev;
+    c.ld_ev = ld_ev;
+    c.ld = P->ld;
+    const Slot &ps = P->slots[P->post_slot];
+    c.prob = ps.ptr;
+    c.prob_batched = ps.batched ? 1 : 0;
+    c.zoff = st.zoff_pos >= 0 ? P->d_tile_off + st.zoff_pos : nullptr;
+    c.soff = P->d_tile_off + st.soff_pos;
+    c.coff = P->d_tile_off + st.coff_pos;
+    c.min_total = P->f64 ? 1e-290 : static_cast<double>(SBN_MIN_TOTAL_F32);
+    c.n_rows = static_cast<int32_t>(n_rows);
+    c.n_in = static_cast<int32_t>(st.in.size());
+    c.n_common = st.n_common;
+    c.cs = static_cast<int32_t>(st.n_out);
+    c.cz = st.cx;
+    c.n_entries = static_cast<int32_t>(st.span);
+    c.n_key = static_cast<int32_t>(st.key.size());
+    for (size_t k = 0; k < st.key.size(); ++k) {
+        c.key_col[k] = st.key[k].col;
+        c.key_stride[k] = st.key[k].stride;
+        c.key_card[k] = st.key[k].card;
+    }
+    int64_t smem = 0;
+    for (size_t i = 0; i < st.in.size(); ++i) {
+        const InDesc &in = st.in[i];
+        SbnCountIn &d = c.in[i];
+        int64_t padded;
+        if (in.is_slot) {
+            d.ptr = P->slots[in.id].ptr;
+            padded = P->slots[in.id].padded;
+        } else {
+            d.ptr = reinterpret_cast<const char *>(P->d_tables) + P->tables[in.id].first * static_cast<int64_t>(elem);
+            padded = P->table_padded[in.id];
+        }
+        d.batched = in.batched ? 1 : 0;
+        d.n_ev = static_cast<int32_t>(in.ev.size());
+        for (size_t k = 0; k < in.ev.size(); ++k) {
+            d.ev_col[k] = in.ev[k].col;
+            d.ev_stride[k] = in.ev[k].stride;
+            d.ev_card[k] = in.ev[k].card;
+        }
+        d.smem_off = -1;
+        if (!P->f64 && !in.batched && (smem + padded) * 4 <= SBN_SMEM_BUDGET) {
+            d.smem_off = static_cast<int32_t>(smem);
+            d.stage_floats = static_cast<int32_t>(padded);
+            smem += padded;
+        }
+    }
+    c.smem_floats = static_cast<int32_t>(smem);
+    double *counts = P->d_counts + st.q_offset;
+    if (P->f64) return sbn_count_launch<double>(c, grid, 0, counts, stream);
+    return sbn_count_launch<float>(c, grid, static_cast<size_t>(smem) * 4, counts, stream);
+}
+
+// Every launch of one run of a counts program: the upward / downward passes, the count steps and P(observed) out.
+int issue_counts(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, void *d_prob, cudaStream_t stream) {
+    SbnStep q;
+    for (const StepDesc &st : P->steps) {
+        if (P->mode == 1 && st.kind == 0) continue;  // computed once, when the program was created
+        if (st.kind == 3) {
+            SBN_CUDA(launch_count(P, st, d_ev, ld_ev, n_rows, stream));
+            continue;
+        }
+        build_params(P, st, d_ev, ld_ev, n_rows, &q);
+        SBN_CUDA(launch_step(P, st, q, stream));
+    }
+    P->launches++;
+    const Slot &ps = P->slots[P->post_slot];
+    const int threads = 256;
+    const unsigned grid = static_cast<unsigned>((n_rows + threads - 1) / threads);
+    if (P->f64)
+        sbn_count_prob<double><<<grid, threads, 0, stream>>>(reinterpret_cast<const double *>(ps.ptr), ps.batched ? 1 : 0,
+                                                             static_cast<int32_t>(n_rows), 1e-290, static_cast<double *>(d_prob));
+    else
+        sbn_count_prob<float><<<grid, threads, 0, stream>>>(ps.ptr, ps.batched ? 1 : 0, static_cast<int32_t>(n_rows),
+                                                            static_cast<double>(SBN_MIN_TOTAL_F32), static_cast<float *>(d_prob));
+    SBN_CUDA(cudaGetLastError());
+    return SBN_OK;
+}
+
 cudaError_t launch_normalise(sbn_program *P, float *d_out, int64_t ld_out, int64_t n_rows, cudaStream_t stream) {
     P->launches++;
     const int threads = 256;
@@ -987,6 +1173,7 @@ int check_run_args(sbn_program *P, const void *ev, int64_t ld_ev, int64_t n_rows
     if (P->n_ev > 1 && ld_ev < n_rows) return fail(SBN_E_INVALID, "ld_ev < n_rows");
     if (P->Q > 1 && ld_out < n_rows) return fail(SBN_E_INVALID, "ld_out < n_rows");
     if (P->mode == 0 && n_rows != 1) return fail(SBN_E_INVALID, "a flat program answers exactly one row");
+    if (P->counts) return fail(SBN_E_INVALID, "a counts program runs through sbn_program_counts_host");
     return SBN_OK;
 }
 
@@ -1017,6 +1204,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
     sbn_program *P = new sbn_program();
     P->device = device;
     P->f64 = f64;
+    P->n_table_floats = n_table_floats;
     {
         const char *e = getenv("SOROBN_B200_CHAIN");
         P->use_chain = e && atoi(e) != 0;  // on-chip segments are opt-in (see sbn_chain.cu)
@@ -1103,7 +1291,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
         SBN_CUDA_P(cudaStreamSynchronize(P->stream));
         // The on-chip segments and paired steps assume every intermediate has ONE consumer; the factors of a
         // marginals program feed several launches, so it runs on the classic per-step launches.
-        if (!P->marginals) sbn_chain_plan(P);
+        if (!P->marginals && !P->counts) sbn_chain_plan(P);
     }
     {
         // opt every step-kernel instantiation into SBN_SMEM_BUDGET of dynamic shared memory
@@ -1117,15 +1305,24 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
             SBN_CUDA_P(sbn_join_set_attrs());
             SBN_CUDA_P(sbn_triple_rows_set_attrs());
             SBN_CUDA_P(sbn_marginal_set_attrs());
+            SBN_CUDA_P(sbn_count_set_attrs());
             done[device] = true;
         }
+    }
+    if (P->counts) {
+        // the count table; the largest step's per-warp partial tables (count_grid caps them) are sized here and
+        // allocated by each counts call only for its duration, so idle programs hold no partial tables
+        for (const StepDesc &st : P->steps)
+            if (st.kind == 3)
+                P->partial_doubles = std::max<int64_t>(P->partial_doubles, count_grid(P, st, INT32_MAX) * SBN_COUNT_WARPS * st.span);
+        SBN_CUDA_P(cudaMalloc(&P->d_counts, static_cast<size_t>(P->n_counts) * 8));
     }
 #undef SBN_CUDA_P
     rc = run_table_steps(P);
     if (rc != SBN_OK) return bail(rc);
     {
         // pairs multiply the tables of two steps on the host: needs the outputs of the table steps above
-        cudaError_t e = P->marginals ? cudaSuccess : sbn_pair_plan(P);
+        cudaError_t e = P->marginals || P->counts ? cudaSuccess : sbn_pair_plan(P);
         if (e != cudaSuccess) return bail(fail(SBN_E_CUDA, "planning the paired steps failed: %s", cudaGetErrorString(e)));
     }
     *out = P;
@@ -1149,6 +1346,8 @@ void sbn_program_destroy(sbn_program *P) {
     sbn_chain_free(P);
     sbn_pair_free(P);
     cudaFree(P->d_shared);
+    cudaFree(P->d_counts);
+    cudaFree(P->d_partial);
     cudaFree(P->d_tile_off);
     cudaFree(P->d_tables);
     if (P->stream) cudaStreamDestroy(P->stream);
@@ -1430,6 +1629,133 @@ int sbn_program_evidence_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, 
 
 int sbn_program_evidence_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *prob) {
     return run_host_common(P, ev, ld_ev, n_rows, prob, n_rows, true, true);
+}
+
+static int counts_chunks(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, void *prob,
+                         size_t elem);
+
+static int counts_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, int64_t n_counts,
+                              void *prob, bool f64) {
+    if (!P) return fail(SBN_E_INVALID, "null program");
+    if (!P->counts) return fail(SBN_E_INVALID, "not a counts program (planner.build_counts_plan)");
+    if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the counts call");
+    if (n_rows <= 0) return fail(SBN_E_INVALID, "n_rows must be positive");
+    if (!counts || !prob) return fail(SBN_E_INVALID, "null output");
+    if (n_counts != P->n_counts) return fail(SBN_E_INVALID, "the count table has %lld entries, not %lld", (long long)P->n_counts, (long long)n_counts);
+    if (P->n_ev > 0 && !ev) return fail(SBN_E_INVALID, "null evidence");
+    if (P->n_ev > 1 && ld_ev < n_rows) return fail(SBN_E_INVALID, "ld_ev < n_rows");
+    if (P->mode == 0 && n_rows != 1) return fail(SBN_E_INVALID, "a flat program answers exactly one row");
+    SBN_CUDA(cudaSetDevice(P->device));
+    if (n_rows > P->reserved_rows) {
+        const int rc = sbn_program_reserve(P, n_rows);
+        if (rc != SBN_OK) return rc;
+    }
+    // the per-warp partial tables live for this call only: a program that is not running holds none of them
+    {
+        const cudaError_t e = cudaMalloc(&P->d_partial, static_cast<size_t>(std::max<int64_t>(1, P->partial_doubles)) * 8);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            P->d_partial = nullptr;
+            return fail(SBN_E_NOMEM, "cudaMalloc of %lld bytes of partial count tables failed: %s",
+                        (long long)(P->partial_doubles * 8), cudaGetErrorString(e));
+        }
+    }
+    const int rc = counts_chunks(P, ev, ld_ev, n_rows, counts, prob, f64 ? 8 : 4);
+    cudaStreamSynchronize(P->stream);  // nothing may still read the partial tables
+    cudaFree(P->d_partial);
+    P->d_partial = nullptr;
+    return rc;
+}
+
+static int counts_chunks(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, void *prob,
+                         size_t elem) {
+    const int64_t cap = P->reserved_rows;
+    SBN_CUDA(cudaMemsetAsync(P->d_counts, 0, static_cast<size_t>(P->n_counts) * 8, P->stream));
+    for (int64_t r0 = 0; r0 < n_rows; r0 += cap) {
+        const int64_t rows = std::min(cap, n_rows - r0);
+        if (P->n_ev > 0)
+            SBN_CUDA(cudaMemcpy2DAsync(P->d_ev, static_cast<size_t>(P->ld), ev + r0, static_cast<size_t>(ld_ev),
+                                       static_cast<size_t>(rows), static_cast<size_t>(P->n_ev), cudaMemcpyHostToDevice, P->stream));
+        if (!P->use_graph) {
+            const int rc = issue_counts(P, P->d_ev, P->ld, rows, P->d_out, P->stream);
+            if (rc != SBN_OK) return rc;
+        } else {
+            // one graph per chunk size; it reads the tables and the count table by address, so it replays the
+            // values sbn_program_set_tables uploads
+            auto &k = P->graph_key;
+            if (!P->exec || k.ev != P->d_ev || k.n_rows != rows || k.out != reinterpret_cast<float *>(P->d_counts) ||
+                P->graph_partial != P->d_partial) {
+                if (P->exec) {
+                    cudaGraphExecDestroy(P->exec);
+                    P->exec = nullptr;
+                }
+                SBN_CUDA(cudaStreamBeginCapture(P->stream, cudaStreamCaptureModeRelaxed));
+                const int64_t before = P->launches;
+                const int rc = issue_counts(P, P->d_ev, P->ld, rows, P->d_out, P->stream);
+                cudaGraph_t graph = nullptr;
+                cudaError_t e = cudaStreamEndCapture(P->stream, &graph);
+                P->graph_launches = P->launches - before;
+                P->launches = before;
+                if (rc != SBN_OK) {
+                    if (graph) cudaGraphDestroy(graph);
+                    return rc;
+                }
+                if (e != cudaSuccess) return fail(SBN_E_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
+                e = cudaGraphInstantiate(&P->exec, graph, 0);
+                cudaGraphDestroy(graph);
+                if (e != cudaSuccess) return fail(SBN_E_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
+                k = {P->d_ev, P->ld, rows, reinterpret_cast<float *>(P->d_counts), P->ld};
+                P->graph_partial = P->d_partial;
+            }
+            SBN_CUDA(cudaGraphLaunch(P->exec, P->stream));
+            P->launches += P->graph_launches;
+        }
+        SBN_CUDA(cudaMemcpyAsync(static_cast<char *>(prob) + r0 * elem, P->d_out, static_cast<size_t>(rows) * elem,
+                                 cudaMemcpyDeviceToHost, P->stream));
+    }
+    std::vector<double> h(static_cast<size_t>(P->n_counts));
+    SBN_CUDA(cudaMemcpyAsync(h.data(), P->d_counts, h.size() * 8, cudaMemcpyDeviceToHost, P->stream));
+    SBN_CUDA(cudaStreamSynchronize(P->stream));
+    for (int64_t i = 0; i < P->n_counts; ++i) counts[i] += h[static_cast<size_t>(i)];
+    return SBN_OK;
+}
+
+int sbn_program_counts_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, int64_t n_counts,
+                            float *prob) {
+    return counts_host_common(P, ev, ld_ev, n_rows, counts, n_counts, prob, false);
+}
+
+int sbn_program_counts_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts,
+                                int64_t n_counts, double *prob) {
+    return counts_host_common(P, ev, ld_ev, n_rows, counts, n_counts, prob, true);
+}
+
+static int set_tables_common(sbn_program *P, const void *tables, int64_t n, bool f64) {
+    if (!P) return fail(SBN_E_INVALID, "null program");
+    if (!P->counts)
+        return fail(SBN_E_INVALID, "only counts programs take new tables (other programs fold table products into their launches)");
+    if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the table call");
+    if (n != P->n_table_floats || (n > 0 && !tables))
+        return fail(SBN_E_INVALID, "the table blob has %lld entries, not %lld", (long long)P->n_table_floats, (long long)n);
+    SBN_CUDA(cudaSetDevice(P->device));
+    if (n > 0)
+        SBN_CUDA(cudaMemcpyAsync(P->d_tables, tables, static_cast<size_t>(n) * (f64 ? 8 : 4), cudaMemcpyHostToDevice, P->stream));
+    // the evidence-independent launches read the tables once, at creation: run them again
+    const int64_t launches = P->launches, setup = P->setup_launches;
+    const int rc = run_table_steps(P);
+    P->setup_launches += setup;
+    P->launches = launches;
+    if (rc != SBN_OK) return rc;
+    SBN_CUDA(cudaStreamSynchronize(P->stream));
+    return SBN_OK;
+}
+
+int sbn_program_set_tables(sbn_program *P, const float *tables, int64_t n_table_floats) {
+    return set_tables_common(P, tables, n_table_floats, false);
+}
+
+int sbn_program_set_tables_f64(sbn_program *P, const double *tables, int64_t n_table_doubles) {
+    return set_tables_common(P, tables, n_table_doubles, true);
 }
 
 int sbn_program_profile(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out,

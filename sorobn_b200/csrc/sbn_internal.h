@@ -54,6 +54,12 @@ struct StepDesc {
     // `in` is reordered so that the n_common inputs without the target axis come first
     int64_t q_offset = -1;
     int n_common = 0;
+    // count step of a counts program (kind 3, sbn_count.cuh): q_offset is the family's first count-table entry,
+    // `key` gathers the observed members, `cstrides` place the unobserved ones; [n_in][cs] / [cs] offset tables
+    std::vector<EvAxis> key;
+    std::vector<int> cstrides;
+    int64_t span = 0;          // entries of the family's count table
+    int64_t soff_pos = -1, coff_pos = -1;
 };
 struct Slot {
     bool batched;
@@ -73,6 +79,13 @@ struct sbn_program {
     bool f64 = false;  // single-event programs computed and returned in double
     int mode = 0, n_ev = 0, Q = 0, post_slot = 0, post_batched = 0;
     bool marginals = false;  // version-5 program: kind-2 readouts write the posterior, already normalised
+    bool counts = false;     // version-6 program: kind-3 steps add expected counts, post_slot holds P(observed)
+    int64_t n_counts = 0;    // counts program: entries of the count table
+    int64_t n_table_floats = 0;  // size of the table blob (sbn_program_set_tables replaces it in place)
+    double *d_counts = nullptr;   // counts program: the run's count table [n_counts]
+    double *d_partial = nullptr;  // counts program: per-warp partial tables of one count step (during a counts call only)
+    const double *graph_partial = nullptr;  // the partial tables the captured counts graph writes
+    int64_t partial_doubles = 0;
     std::vector<std::pair<int64_t, int64_t>> tables;  // (offset, size) in floats
     std::vector<int64_t> table_padded;
     float *d_tables = nullptr;

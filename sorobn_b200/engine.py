@@ -16,7 +16,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libsorobn_
 _lib = None
 
 SBN_OK = 0
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 
 class EngineError(RuntimeError):
@@ -64,6 +64,12 @@ def load():
     lib.sbn_program_evidence_host.argtypes = [vp, vp, i64, i64, vp]
     lib.sbn_program_evidence_host_f64.restype = i32
     lib.sbn_program_evidence_host_f64.argtypes = [vp, vp, i64, i64, vp]
+    for name in ("sbn_program_counts_host", "sbn_program_counts_host_f64"):
+        getattr(lib, name).restype = i32
+        getattr(lib, name).argtypes = [vp, vp, i64, i64, vp, i64, vp]
+    for name in ("sbn_program_set_tables", "sbn_program_set_tables_f64"):
+        getattr(lib, name).restype = i32
+        getattr(lib, name).argtypes = [vp, vp, i64]
     lib.sbn_program_destroy.restype = None
     lib.sbn_program_destroy.argtypes = [vp]
     lib.sbn_program_reserve.restype = i32
@@ -106,7 +112,8 @@ EXPORTS = (
     "sbn_abi_version", "sbn_last_error", "sbn_device_count", "sbn_program_create", "sbn_program_create_f64",
     "sbn_program_run_host_f64", "sbn_program_evidence_host", "sbn_program_evidence_host_f64", "sbn_program_destroy",
     "sbn_program_reserve", "sbn_program_run_host", "sbn_program_run_device", "sbn_program_profile",
-    "sbn_program_step_roles",
+    "sbn_program_step_roles", "sbn_program_counts_host", "sbn_program_counts_host_f64", "sbn_program_set_tables",
+    "sbn_program_set_tables_f64",
     "sbn_program_info", "sbn_program_set_graph", "sbn_program_set_tiled", "sbn_gibbs_create", "sbn_gibbs_run_host",
     "sbn_sampler_run_host", "sbn_gibbs_conditional", "sbn_gibbs_destroy", "sbn_host_alloc", "sbn_host_free",
 )
@@ -243,6 +250,26 @@ class Program:
         fn = load().sbn_program_evidence_host_f64 if self.f64 else load().sbn_program_evidence_host
         _check(fn(self._h, codes.ctypes.data if self.n_ev else None, n_rows, n_rows, out.ctypes.data))
         return out
+
+    def counts(self, codes: np.ndarray, n_rows: int):
+        """Counts programs (planner.build_counts_plan): (expected counts float64 [n_counts] summed over the
+        rows, P(observed) [n_rows], NaN for a row the float32 range rule flags), host path."""
+        n_rows = int(n_rows)
+        codes = np.ascontiguousarray(codes, dtype=np.uint8)
+        if self.n_ev and codes.shape != (self.n_ev, n_rows):
+            raise ValueError(f"evidence codes have shape {codes.shape}, expected {(self.n_ev, n_rows)}")
+        counts = np.zeros(int(self.plan.n_counts), dtype=np.float64)
+        prob = np.empty(n_rows, dtype=np.float64 if self.f64 else np.float32)
+        fn = load().sbn_program_counts_host_f64 if self.f64 else load().sbn_program_counts_host
+        _check(fn(self._h, codes.ctypes.data if self.n_ev else None, n_rows, n_rows, counts.ctypes.data, counts.size,
+                  prob.ctypes.data))
+        return counts, prob
+
+    def set_tables(self, blob: np.ndarray):
+        """Replace a counts program's tables (planner.refresh_tables gives the blob of new CPTs)."""
+        blob = np.ascontiguousarray(blob, dtype=np.float64 if self.f64 else np.float32)
+        fn = load().sbn_program_set_tables_f64 if self.f64 else load().sbn_program_set_tables
+        _check(fn(self._h, blob.ctypes.data, blob.size))
 
     def run_device(self, d_ev: int, ld_ev: int, n_rows: int, d_out: int, ld_out: int, stream: int = 0):
         """Device path: raw device pointers, asynchronous on `stream`."""

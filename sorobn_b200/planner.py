@@ -57,6 +57,28 @@ It writes the target's `card_t` posterior entries, already normalised per row, a
 `q_offset ..` of the run's output.  Targets are sorted by name and Q = sum of their cards.
 Intermediates of a version-5 program may have several consumers; `build_plan`'s version-4
 programs are unchanged.
+
+Counts programs (`build_counts_plan`, VERSION 6) compute the E-step of expectation-maximisation:
+for every CPT family (v, parents(v)), sum over the rows of P(family | the row's observed cells).
+They reuse the version-5 upward and downward passes and add a count step (kind 3):
+
+    header : MAGIC 6 mode n_ev n_tables n_slots n_steps 1 p_slot p_batched n_counts 0
+    kind 3 : 3 n_in -1 n_axes n_elim c_offset n_key (col stride card)*n_key cstrides[n_axes] |
+             cards[n_axes] | ecards[n_elim] | inputs as above
+
+`p_slot` holds P(observed cells) of every row (`[1]` or `[1, B]`): the product of the upward
+pass's leftover scalars, computed once per run.  The run's per-row output is that probability, NaN
+where it is below the float range rule (1e-30 in float32, 1e-290 in float64, or zero / NaN); such
+a row adds nothing to the counts.  The count table (`n_counts` float64 entries) is every CPT's
+dense `[*parents, v]` array in CompiledNet order, concatenated.  A kind-3 step for node v has the
+unobserved members M_v of v's family as output axes.  It reads the smallest bucket whose scope
+holds M_v and, per row, adds
+
+    sum_{elims} prod_i in_i[...] / P(observed)     (n_in = 0, M_v empty: 1)
+
+at `c_offset + key(row) + sum_m state_m * cstrides[m]`, with key(row) = sum_k ev[col_k] * stride_k
+over the observed family members.  No step writes a slot that a later one still needs: a kind-3
+step writes only the count table.
 """
 from __future__ import annotations
 
@@ -86,6 +108,8 @@ KIND_MARGINAL = 2  # readout of one target's marginal from a bucket (marginals p
 # words (csrc/sbn_api.cu: kMarginalZoffMax / SBN_MAX_IN)
 MARGINAL_MAX_Z = 2**21
 VERSION_MARGINALS = 5
+KIND_COUNT = 3  # expected counts of one CPT family, summed over the rows (counts programs only)
+VERSION_COUNTS = 6
 HEADER_WORDS = 12
 
 
@@ -144,7 +168,10 @@ class Step:
     elims: tuple  # variables summed out by this launch
     ecards: tuple
     out_slot: int = -1
-    q_offset: int = -1  # KIND_MARGINAL: first posterior entry of the target's segment
+    q_offset: int = -1  # KIND_MARGINAL: first posterior entry of the target's segment; KIND_COUNT: c_offset
+    key: tuple = ()  # KIND_COUNT: ((ev_col, stride, card), ...) of the observed family members
+    cstrides: tuple = ()  # KIND_COUNT: count-table stride of every output axis
+    norm: object = None  # KIND_COUNT: the factor holding P(observed) (read through the header's p_slot)
 
     @property
     def cx(self):
@@ -168,6 +195,10 @@ class Plan:
     table_offsets: list = None
     version: int = VERSION
     targets: tuple = ()  # marginals plans: target var ids, sorted by name (== posterior segment order)
+    n_counts: int = 0  # counts plans: entries of the count table
+    count_offsets: list = None  # counts plans: first count-table entry of every var id's family
+    table_axes: list = None  # var ids of every shipped table's axes, outermost first (refresh_tables)
+    table_scopes: list = None  # the CPT scope [*parents, v] every table was transposed from
 
     # ---- cost model (DESIGN.md "algorithmic bytes") -------------------------------
     def bytes_per_row(self):
@@ -176,16 +207,21 @@ class Plan:
         codes in and the posterior out."""
         total = 0
         for st in self.steps:
-            if st.kind not in (KIND_BATCHED, KIND_MARGINAL):
+            if st.kind not in (KIND_BATCHED, KIND_MARGINAL, KIND_COUNT):
                 continue
             for f, _, _ in st.inputs:
                 if f.batched:
                     total += 4 * int(np.prod([self._card[v] for v in f.vars], dtype=np.int64))
+            if st.kind == KIND_COUNT:
+                total += 4  # P(observed); the count table is per program, not per row
+                continue
             total += 4 * int(np.prod(st.cards, dtype=np.int64))
         if self.version == VERSION:
             # normalise: read unnormalised posterior, write posterior (a marginals program's
             # readouts write their segments normalised, counted above)
             total += 8 * self.Q
+        elif self.version == VERSION_COUNTS:
+            total += 4  # P(observed) out
         total += len(self.evidence)  # uint8 codes
         return total
 
@@ -285,8 +321,43 @@ def build_marginals_plan(net: CompiledNet, evidence, targets=None, mode=MODE_BAT
     return _build(net, (), evidence, mode, order, max_in, False, lift_evidence, True, fuse_elims, targets)
 
 
+def build_counts_plan(net: CompiledNet, evidence, mode=MODE_BATCHED, order=None, max_in=MAX_IN, lift_evidence=True,
+                      fuse_elims=None) -> Plan:
+    """Plan the expected counts of every CPT family given the observed columns `evidence` (a version-6
+    program, see the module docstring): one program serves every row of one missingness pattern.
+    Its count table is laid out by `count_layout`."""
+    evidence = tuple(evidence)
+    hidden = tuple(v for v in range(len(net.names)) if v not in set(evidence))
+    return _build(net, (), evidence, mode, order, max_in, False, lift_evidence, True, fuse_elims, hidden, counts=True)
+
+
+def count_layout(net: CompiledNet):
+    """(first count-table entry of every var id's family, total entries): the dense `[*parents, v]`
+    arrays of the CPTs in CompiledNet order, concatenated."""
+    offsets, off = [], 0
+    for v in range(len(net.names)):
+        offsets.append(off)
+        off += int(np.prod([int(net.card[u]) for u in net.scope(v)], dtype=np.int64))
+    return offsets, off
+
+
+def refresh_tables(plan: Plan, cpts):
+    """The (float32, float64) table blobs of `plan` for new CPT values `cpts` (var id -> ndarray
+    [*parents, v], the same domains): the layout of the planned tables (axis permutations, relayouts,
+    offsets) is kept, so a program can take them in place of its own (engine.Program.set_tables)."""
+    arrays = []
+    for t, v in enumerate(plan.tables):
+        scope = list(plan.table_scopes[t])
+        arr = np.asarray(cpts[v], dtype=np.float64)
+        if arr.shape != tuple(int(plan._card[u]) for u in scope):
+            raise ValueError(f"the CPT of var {v} has shape {arr.shape}; the plan has {[int(plan._card[u]) for u in scope]}")
+        arrays.append(np.ascontiguousarray(np.transpose(arr, [scope.index(u) for u in plan.table_axes[t]])))
+    blob64, _ = _blobs(arrays)
+    return blob64.astype(np.float32), blob64
+
+
 def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evidence, allow_empty_query, fuse_elims,
-           targets):
+           targets, counts=False):
     if merge_sum_outs is None:
         merge_sum_outs = os.environ.get("SOROBN_B200_MERGE", "0") == "1"
     if fuse_elims is None:
@@ -536,6 +607,9 @@ def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evide
         if targets is not None:
             buckets.append((bucket_factors, tuple(elims), set().union(*[f.vars for f in bucket_factors]), factors[-1]))
 
+    if counts:
+        return _counts_passes(net, evidence, mode, order, max_in, buckets, factors, steps, tables, table_arrays,
+                              table_axes, emit, combine_tables, axis_order, fsize)
     if targets is not None:
         return _marginals_passes(net, evidence, mode, order, max_in, targets, buckets, factors, steps, tables,
                                  table_arrays, emit, combine_tables, axis_order, fsize)
@@ -554,7 +628,8 @@ def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evide
     slots, post_slot = _assign_slots(steps, post.buf, keep_unbatched=(mode == MODE_BATCHED))
 
     plan = Plan(mode=mode, query=q_sorted, evidence=evidence, order=list(order), tables=tables,
-                slots=slots, steps=steps, post_slot=post_slot, Q=Q)
+                slots=slots, steps=steps, post_slot=post_slot, Q=Q,
+                table_axes=[list(a) for a in table_axes], table_scopes=[net.scope(v) for v in tables])
     plan._card = card
     _serialise(plan, table_arrays)
     return plan
@@ -573,6 +648,117 @@ def _marginals_passes(net, evidence, mode, order, max_in, targets, buckets, left
     tables of evidence-only variables); a root bucket's pi is the product of the others, so that
     every bucket belief is P(U_k, e) and a row of probability zero stays NaN as in `build_plan`."""
     card = net.card
+
+    def joint(vs):
+        return int(np.prod([card[v] for v in vs], dtype=np.int64)) if vs else 1
+
+    t_sorted = tuple(sorted(targets, key=lambda v: net.names[v]))
+    read = {t: min((joint(U), k) for k, (_, _, U, _) in enumerate(buckets) if t in U)[1] for t in t_sorted}
+    pi, fold = _downward(net, max_in, buckets, leftovers, read.values(), emit, combine_tables, axis_order, fsize)
+
+    offsets, q = {}, 0
+    for t in t_sorted:
+        offsets[t] = q
+        q += int(card[t])
+    for t in t_sorted:
+        k = read[t]
+        F_k, _, U_k, _ = buckets[k]
+        inputs = fold(([pi[k]] if pi[k] is not None else []) + list(F_k))
+        # joint states of the summed-out variables are walked first-variable fastest: the variables the
+        # largest batched operand lacks go first, so each of its entries is read in one stretch
+        big = max(inputs, key=lambda f: (f.batched, fsize(f)))
+        pos_big = dict(zip(big.vars, big.strides))
+        elims = sorted(U_k - {t}, key=lambda v: (v in pos_big, pos_big.get(v, 0), v))
+        if joint(elims) > MARGINAL_MAX_Z or joint(elims) * int(card[t]) >= 2**31:
+            raise ValueError(f"the bucket read for {net.names[t]!r} is too large for a readout: {joint(elims)} joint "
+                             f"states summed out (at most {MARGINAL_MAX_Z}) x {int(card[t])} target states (below 2^31)")
+        ins = []
+        for f in inputs:
+            pos = dict(zip(f.vars, f.strides))
+            ins.append((f, tuple(pos.get(e, 0) for e in elims), (pos.get(t, 0),)))
+        steps.append(Step(KIND_MARGINAL, ins, -1, (t,), (int(card[t]),), tuple(elims),
+                          tuple(int(card[e]) for e in elims), q_offset=offsets[t]))
+
+    steps[:] = _prune_dead(steps)
+    slots = _assign_slots_shared(steps, keep_unbatched=(mode == MODE_BATCHED))[0]
+    plan = Plan(mode=mode, query=(), evidence=evidence, order=list(order), tables=tables, slots=slots, steps=steps,
+                post_slot=-1, Q=q, version=VERSION_MARGINALS, targets=t_sorted)
+    plan._card = card
+    _serialise(plan, table_arrays)
+    return plan
+
+
+def _counts_passes(net, evidence, mode, order, max_in, buckets, leftovers, steps, tables, table_arrays, table_axes,
+                   emit, combine_tables, axis_order, fsize):
+    """Downward pass and count steps of a counts plan (DESIGN.md "Expected counts and EM").
+
+    The unobserved members M_v of v's family are read from the smallest bucket k with M_v in U_k (the
+    bucket the CPT of v entered has them all):
+        counts_v(M_v; key(row)) += sum_{U_k - M_v} pi_k * prod_{f in F_k} f / P(observed),
+    where P(observed) is the product of every leftover scalar of the upward pass, computed once."""
+    card = net.card
+    ev_col = {v: i for i, v in enumerate(evidence)}
+
+    def joint(vs):
+        return int(np.prod([card[v] for v in vs], dtype=np.int64)) if vs else 1
+
+    n_vars = len(net.names)
+    members = {v: [u for u in net.scope(v) if u not in ev_col] for v in range(n_vars)}
+    read = {}
+    for v in range(n_vars):
+        if members[v]:
+            M = set(members[v])
+            read[v] = min((joint(U), k) for k, (_, _, U, _) in enumerate(buckets) if M <= U)[1]
+    pi, fold = _downward(net, max_in, buckets, leftovers, read.values(), emit, combine_tables, axis_order, fsize)
+    prob = emit(fold(list(leftovers)), None, [], may_lift=False)
+
+    c_offsets, n_counts = count_layout(net)
+    for v in range(n_vars):
+        scope = net.scope(v)
+        shape = [int(card[u]) for u in scope]
+        stride = {u: int(np.prod(shape[i + 1:], dtype=np.int64)) for i, u in enumerate(scope)}
+        key = tuple((ev_col[u], stride[u], int(card[u])) for u in scope if u in ev_col)
+        if len(key) > MAX_EV:
+            raise ValueError(f"the family of {net.names[v]!r} has {len(key)} observed members; the kernel gathers {MAX_EV}")
+        M = members[v]
+        if not M:  # fully observed family: a histogram of the rows' keys
+            steps.append(Step(KIND_COUNT, [], -1, (), (), (), (), q_offset=c_offsets[v], key=key, norm=prob))
+            continue
+        k = read[v]
+        F_k, _, U_k, _ = buckets[k]
+        inputs = fold(([pi[k]] if pi[k] is not None else []) + list(F_k))
+        big = max(inputs, key=lambda f: (f.batched, fsize(f)))
+        pos_big = dict(zip(big.vars, big.strides))
+        elims = sorted(U_k - set(M), key=lambda u: (u in pos_big, pos_big.get(u, 0), u))
+        out_vars = tuple(reversed(M))  # v (count-table stride 1) is the fastest output axis
+        cs = joint(out_vars)
+        if joint(elims) > MARGINAL_MAX_Z or cs > MARGINAL_MAX_Z or joint(elims) * cs >= 2**31:
+            raise ValueError(f"the bucket read for the family of {net.names[v]!r} is too large for a count step: "
+                             f"{joint(elims)} joint states summed out and {cs} family states (each at most "
+                             f"{MARGINAL_MAX_Z}, their product below 2^31)")
+        ins = []
+        for f in inputs:
+            pos = dict(zip(f.vars, f.strides))
+            ins.append((f, tuple(pos.get(e, 0) for e in elims), tuple(pos.get(u, 0) for u in out_vars)))
+        steps.append(Step(KIND_COUNT, ins, -1, out_vars, tuple(int(card[u]) for u in out_vars), tuple(elims),
+                          tuple(int(card[e]) for e in elims), q_offset=c_offsets[v], key=key,
+                          cstrides=tuple(stride[u] for u in out_vars), norm=prob))
+
+    steps[:] = _prune_dead(steps)
+    slots, where = _assign_slots_shared(steps, keep_unbatched=(mode == MODE_BATCHED))
+    p_slot = where[prob.buf]
+    plan = Plan(mode=mode, query=(), evidence=evidence, order=list(order), tables=tables, slots=slots, steps=steps,
+                post_slot=p_slot, Q=1, version=VERSION_COUNTS, n_counts=n_counts, count_offsets=c_offsets,
+                table_axes=[list(a) for a in table_axes], table_scopes=[net.scope(v) for v in tables])
+    plan._card = card
+    _serialise(plan, table_arrays)
+    return plan
+
+
+def _downward(net, max_in, buckets, leftovers, reads, emit, combine_tables, axis_order, fsize):
+    """Downward messages pi_k of the buckets on the way from a root to every bucket in `reads`
+    (`_marginals_passes`).  Returns (pi, fold)."""
+    card = net.card
     n = len(buckets)
     owner = {id(lam): k for k, (_, _, _, lam) in enumerate(buckets)}
     parent = [None] * n
@@ -582,13 +768,8 @@ def _marginals_passes(net, evidence, mode, order, max_in, targets, buckets, left
             if j is not None:
                 parent[j] = k
 
-    def joint(vs):
-        return int(np.prod([card[v] for v in vs], dtype=np.int64)) if vs else 1
-
-    t_sorted = tuple(sorted(targets, key=lambda v: net.names[v]))
-    read = {t: min((joint(U), k) for k, (_, _, U, _) in enumerate(buckets) if t in U)[1] for t in t_sorted}
     need = [False] * n
-    for k in read.values():
+    for k in reads:
         while k is not None and not need[k]:
             need[k] = True
             k = parent[k]
@@ -642,46 +823,18 @@ def _marginals_passes(net, evidence, mode, order, max_in, targets, buckets, left
         inputs = ([pi[p]] if pi[p] is not None else []) + [f for f in F_p if f is not lam_k]
         S_k = set(lam_k.vars)
         pi[k] = message(inputs, S_k, U_p - S_k) if inputs else None
-
-    offsets, q = {}, 0
-    for t in t_sorted:
-        offsets[t] = q
-        q += int(card[t])
-    for t in t_sorted:
-        k = read[t]
-        F_k, _, U_k, _ = buckets[k]
-        inputs = fold(([pi[k]] if pi[k] is not None else []) + list(F_k))
-        # joint states of the summed-out variables are walked first-variable fastest: the variables the
-        # largest batched operand lacks go first, so each of its entries is read in one stretch
-        big = max(inputs, key=lambda f: (f.batched, fsize(f)))
-        pos_big = dict(zip(big.vars, big.strides))
-        elims = sorted(U_k - {t}, key=lambda v: (v in pos_big, pos_big.get(v, 0), v))
-        if joint(elims) > MARGINAL_MAX_Z or joint(elims) * int(card[t]) >= 2**31:
-            raise ValueError(f"the bucket read for {net.names[t]!r} is too large for a readout: {joint(elims)} joint "
-                             f"states summed out (at most {MARGINAL_MAX_Z}) x {int(card[t])} target states (below 2^31)")
-        ins = []
-        for f in inputs:
-            pos = dict(zip(f.vars, f.strides))
-            ins.append((f, tuple(pos.get(e, 0) for e in elims), (pos.get(t, 0),)))
-        steps.append(Step(KIND_MARGINAL, ins, -1, (t,), (int(card[t]),), tuple(elims),
-                          tuple(int(card[e]) for e in elims), q_offset=offsets[t]))
-
-    steps[:] = _prune_dead(steps)
-    slots = _assign_slots_shared(steps, keep_unbatched=(mode == MODE_BATCHED))
-    plan = Plan(mode=mode, query=(), evidence=evidence, order=list(order), tables=tables, slots=slots, steps=steps,
-                post_slot=-1, Q=q, version=VERSION_MARGINALS, targets=t_sorted)
-    plan._card = card
-    _serialise(plan, table_arrays)
-    return plan
+    return pi, fold
 
 
 def _prune_dead(steps):
     """Drop the launches nothing reads (the root buckets' own messages when no other root needs them)."""
     used, keep = set(), []
     for st in reversed(steps):
-        if st.kind == KIND_MARGINAL or st.out_id in used:
+        if st.kind in (KIND_MARGINAL, KIND_COUNT) or st.out_id in used:
             keep.append(st)
             used.update(f.buf for f, _, _ in st.inputs if f.is_slot)
+            if st.norm is not None:
+                used.add(st.norm.buf)
     return keep[::-1]
 
 
@@ -689,12 +842,15 @@ def _assign_slots_shared(steps, keep_unbatched):
     """`_assign_slots` for plans whose intermediates have several consumers (the factors of a
     bucket feed its upward message, its downward messages and its readouts): a slot is released
     after its last consumer.  The output slot is taken before the inputs are released, so a launch
-    never writes a buffer it reads.  Readouts write the posterior, not a slot."""
+    never writes a buffer it reads.  Readouts write the posterior, not a slot; count steps write the
+    count table and also read P(observed) (`Step.norm`).  Returns (slots, logical id -> slot)."""
     remaining = {}
     for st in steps:
         for f, _, _ in st.inputs:
             if f.is_slot:
                 remaining[f.buf] = remaining.get(f.buf, 0) + 1
+        if st.norm is not None:
+            remaining[st.norm.buf] = remaining.get(st.norm.buf, 0) + 1
     slots, where = [], {}
 
     def alloc(batched, size):
@@ -708,25 +864,32 @@ def _assign_slots_shared(steps, keep_unbatched):
         slots[best][2] = False
         return best
 
+    def release(buf):
+        remaining[buf] -= 1
+        if remaining[buf] == 0:
+            phys = where[buf]
+            slots[phys][2] = not (keep_unbatched and not slots[phys][0])
+
     for st in steps:
-        if st.kind != KIND_MARGINAL:
+        writes_slot = st.kind not in (KIND_MARGINAL, KIND_COUNT)
+        if writes_slot:
             size = int(np.prod(st.cards, dtype=np.int64)) if st.cards else 1
             st.out_slot = alloc(st.kind == KIND_BATCHED, size)
         new_inputs = []
         for f, es, ss in st.inputs:
             if f.is_slot:
                 phys = where[f.buf]
-                remaining[f.buf] -= 1
-                if remaining[f.buf] == 0:
-                    slots[phys][2] = not (keep_unbatched and not slots[phys][0])
+                release(f.buf)
                 f = _Factor(True, phys, f.vars, f.strides, f.ev, f.batched)
             new_inputs.append((f, es, ss))
         st.inputs = new_inputs
-        if st.kind != KIND_MARGINAL:
+        if st.norm is not None:
+            release(st.norm.buf)
+        if writes_slot:
             where[st.out_id] = st.out_slot
     if not slots:  # every operand is a CPT: the engine still expects one scratch slot
         slots.append([False, 1, True])
-    return [(bool(b), int(sz)) for b, sz, _ in slots]
+    return [(bool(b), int(sz)) for b, sz, _ in slots], where
 
 
 def _relayout_big_tables(steps, table_arrays, table_axes, evidence, card):
@@ -905,7 +1068,8 @@ def _assign_slots(steps, post_id, keep_unbatched=False):
     return [(bool(b), int(sz)) for b, sz, _ in slots], where[post_id]
 
 
-def _serialise(plan: Plan, table_arrays):
+def _blobs(table_arrays):
+    """(float64 table blob, [(offset, size)] per table)."""
     blob = []
     offsets = []
     off = 0
@@ -919,18 +1083,25 @@ def _serialise(plan: Plan, table_arrays):
         if pad:
             blob.append(np.zeros(pad, dtype=np.float64))
         off += t.size + pad
+    return (np.concatenate(blob) if blob else np.zeros(0, dtype=np.float64)), offsets
+
+
+def _serialise(plan: Plan, table_arrays):
     # float64 copy: only the CPU checker (oracle/program_interp.py) reads it, to
     # separate planner errors from fp32 rounding; the device gets the fp32 blob
-    plan.table_blob64 = np.concatenate(blob) if blob else np.zeros(0, dtype=np.float64)
+    plan.table_blob64, offsets = _blobs(table_arrays)
     plan.table_blob = plan.table_blob64.astype(np.float32)
     plan.table_offsets = offsets
 
-    if plan.version == VERSION:
+    extra = [0, 0]
+    if plan.version in (VERSION, VERSION_COUNTS):
         post = [plan.post_slot, int(plan.slots[plan.post_slot][0])]
+        if plan.version == VERSION_COUNTS:
+            extra = [plan.n_counts, 0]
     else:
         post = [-1, 0]  # the readouts write the posterior themselves
     w = [MAGIC, plan.version, plan.mode, len(plan.evidence), len(plan.tables), len(plan.slots), len(plan.steps),
-         plan.Q, *post, 0, 0]
+         plan.Q, *post, *extra]
     assert len(w) == HEADER_WORDS
     for o, s in offsets:
         w += [o, s]
@@ -940,6 +1111,11 @@ def _serialise(plan: Plan, table_arrays):
         w += [st.kind, len(st.inputs), st.out_slot, len(st.cards), len(st.ecards)]
         if st.kind == KIND_MARGINAL:
             w.append(st.q_offset)
+        elif st.kind == KIND_COUNT:
+            w += [st.q_offset, len(st.key)]
+            for col, s, c in st.key:
+                w += [col, s, c]
+            w += list(st.cstrides)
         w += list(st.cards)
         w += list(st.ecards)
         for f, estrides, strides in st.inputs:
