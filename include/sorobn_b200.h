@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SBN_ABI_VERSION 10
+#define SBN_ABI_VERSION 11
 
 #define SBN_OK 0
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
@@ -119,6 +119,20 @@ int sbn_program_counts_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld
  * steps fold table products into coefficients built on the host. */
 int sbn_program_set_tables(sbn_program *prog, const float *tables, int64_t n_table_floats);
 int sbn_program_set_tables_f64(sbn_program *prog, const double *tables, int64_t n_table_doubles);
+
+/* Exact posterior draws of a sample program (planner.build_sample_plan, version 7; the run, evidence and
+ * counts calls refuse it, and these calls refuse every other program).  For every row b and draw d,
+ * out[(j * n_draws + d) * n_rows + b] is the code of the j-th sampled variable (Plan.sampled), drawn from
+ * P(unobserved | the row's observed cells) by backward sampling over the bucket tree.  The draws depend only
+ * on (seed, row_base + b, d): Philox-4x32-10, key (seed lo, seed hi), counter (sample step, d, row lo, row hi),
+ * so a batch cut into pieces run with their row_base gives the same draws, and so do two calls.
+ * prob[b] = P(observed cells of b), or NaN for a row below the float32 range (1e-30; 1e-290 for the float64
+ * twin) or of probability zero: its draws are meaningless, re-run it with a float64 program and the same
+ * row_base + b.  Large batches run in chunks. */
+int sbn_program_sample_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws,
+                            uint64_t seed, int64_t row_base, uint8_t *out, float *prob);
+int sbn_program_sample_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws,
+                                uint64_t seed, int64_t row_base, uint8_t *out, double *prob);
 
 /* Same with DEVICE buffers, asynchronous on `stream` (a cudaStream_t; NULL = default
  * stream).  n_rows must not exceed the reserved chunk size. */

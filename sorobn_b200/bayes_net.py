@@ -23,7 +23,9 @@ The approximate algorithms run on the device too (csrc/sbn_gibbs.cuh): `algorith
 
 `expected_counts` / `fit_em` learn from incomplete data (missing cells, latent nodes) by
 expectation-maximisation; the E-step runs on the device as one counts program per missingness
-pattern (planner.build_counts_plan, csrc/sbn_count.cuh).
+pattern (planner.build_counts_plan, csrc/sbn_count.cuh).  `sample_many` draws exact posterior
+samples of the missing cells and latent nodes, one sample program per pattern
+(planner.build_sample_plan, csrc/sbn_sample.cuh).
 """
 from __future__ import annotations
 
@@ -45,9 +47,10 @@ def _as_list(obj):
     return obj if isinstance(obj, list) else [obj]
 
 
-class _CountsRunner:
-    """The device programs of one missingness pattern: the float32 counts program, and the float64 one
-    for the rows it flags (created when first needed).  `set_cpts` gives both new tables in place."""
+class _PatternRunner:
+    """The device programs of one missingness pattern (a counts or a sample plan): the float32 program, and
+    the float64 one for the rows it flags (created when first needed).  `set_cpts` gives both new tables in
+    place (counts programs)."""
 
     def __init__(self, plan, device):
         from . import engine  # raises if libsorobn_b200.so cannot be loaded
@@ -404,7 +407,7 @@ class BayesNet:
         net = self._compiled
         offsets, n_counts = _planner.count_layout(net)
         n_rows = len(X.index)
-        runners = [_CountsRunner(_planner.build_counts_plan(net, ev), self.device) for ev, _, _ in groups]
+        runners = [_PatternRunner(_planner.build_counts_plan(net, ev), self.device) for ev, _, _ in groups]
         cpts = [np.array(c, dtype=np.float64) for c in net.cpt]
         lls = []
         try:
@@ -492,12 +495,22 @@ class BayesNet:
         return groups
 
     def _counts_runner(self, ev):
-        """The cached programs of one missingness pattern (dropped by `prepare()`, as every program)."""
+        """The cached counts programs of one missingness pattern."""
+        return self._pattern_runner("counts", ev)
+
+    def _sample_runner(self, ev):
+        """The cached sample programs of one missingness pattern."""
+        return self._pattern_runner("sample", ev)
+
+    def _pattern_runner(self, kind, ev):
+        """The cached programs of one missingness pattern, `kind` "counts" or "sample" (dropped by `prepare()`,
+        as every program)."""
         with self._cache_lock:
-            key = ("counts", ev, self.device)
+            key = (kind, ev, self.device)
             hit = self._engine_cache.get(key)
             if hit is None:
-                hit = self._engine_cache[key] = _CountsRunner(_planner.build_counts_plan(self._compiled, ev), self.device)
+                build = _planner.build_counts_plan if kind == "counts" else _planner.build_sample_plan
+                hit = self._engine_cache[key] = _PatternRunner(build(self._compiled, ev), self.device)
                 self._evict()
             else:
                 self._engine_cache.move_to_end(key)
@@ -524,6 +537,62 @@ class BayesNet:
                                  f"(first: {X.index[rows[impossible][0]]!r}); their expected counts are undefined")
             ll += float(np.log(prob).sum())
         return counts, ll
+
+    def sample_many(self, events: pd.DataFrame, n: int = 1, seed: int | None = None) -> pd.DataFrame:
+        """`n` exact draws of every unobserved variable from P(unobserved | the row's observed cells), for
+        every row of `events`, computed on the GPU.
+
+        A missing cell is None or NaN; a node without a column is latent.  Both are sampled; observed
+        cells are copied through.  Returns `len(events) * n` rows indexed by (the events label, `draw`
+        0 .. n - 1), the draws of a row adjacent and the rows in `events` order, with one column per node
+        (sorted, dtypes inferred, as `sample`).  `seed=None` takes 64 bits from the network's stream.  The
+        draws of a row depend only on the seed, its position in `events`, the draw index and its
+        missingness pattern.  Raises ValueError for a value outside its variable's domain, for rows whose
+        observed cells have probability zero and for `n < 1`.
+
+        Rows are grouped by missingness pattern; each pattern is one sample program
+        (planner.build_sample_plan): the upward pass of variable elimination, then one draw per bucket
+        of the elimination, top-down (csrc/sbn_sample.cuh)."""
+        if int(n) < 1:
+            raise ValueError(f"n must be at least 1, not {n}")
+        n = int(n)
+        groups = self._count_patterns(events)
+        net = self._compiled
+        seed = self._rng.getrandbits(64) if seed is None else int(seed) & (2**64 - 1)
+        n_rows = len(events.index)
+        codes = np.zeros((len(net.names), n_rows, n), dtype=np.uint8)
+        for ev, rows, ev_codes in groups:
+            # fetched right before it runs: with more patterns than the cache holds, fetching one may close
+            # the least recently used programs, which have run by then
+            runner = self._sample_runner(ev)
+            drawn, prob = self._draw(runner.f32, ev_codes, rows, n, seed)
+            flagged = np.flatnonzero(np.isnan(prob))
+            if len(flagged):
+                drawn[:, :, flagged], prob[flagged] = self._draw(runner.f64(), np.ascontiguousarray(ev_codes[:, flagged]),
+                                                                 rows[flagged], n, seed)
+            impossible = np.isnan(prob)
+            if impossible.any():
+                raise ValueError(f"{int(impossible.sum())} row(s) have observed cells of probability zero "
+                                 f"(first: {events.index[rows[impossible][0]]!r}); they have no posterior to sample from")
+            for i, v in enumerate(ev):
+                codes[v][rows] = ev_codes[i][:, None]
+            for j, v in enumerate(runner.plan.sampled):
+                codes[v][rows] = drawn[j].T
+        index = pd.MultiIndex.from_arrays([np.repeat(events.index.to_numpy(), n), np.tile(np.arange(n), n_rows)],
+                                          names=[events.index.name, "draw"])
+        frame = pd.DataFrame({name: np.asarray(net.domains[v], dtype=object)[codes[v].reshape(-1)]
+                              for v, name in enumerate(net.names)}, index=index)
+        return frame.infer_objects().sort_index(axis="columns")
+
+    @staticmethod
+    def _draw(program, ev_codes, rows, n, seed):
+        """(drawn codes [n_sampled, n, len(rows)], P(observed) float64) of the rows at positions `rows`
+        (sorted): one call per run of consecutive positions, whose first position is the call's row_base,
+        so that a row's random stream is its position whatever the grouping."""
+        starts = np.flatnonzero(np.r_[True, np.diff(rows) != 1])
+        parts = [program.sample(np.ascontiguousarray(ev_codes[:, a:b]), b - a, n, seed, row_base=int(rows[a]))
+                 for a, b in zip(starts, np.r_[starts[1:], len(rows)])]
+        return np.concatenate([d for d, _ in parts], axis=2), np.concatenate([p for _, p in parts]).astype(np.float64)
 
     def sample(self, n=1, init: dict | None = None, method="forward"):
         """Forward (ancestral) samples (bayes_net.py:550-575): a Series for n == 1, otherwise a

@@ -24,6 +24,7 @@
 #include "sbn_launch.h"
 #include "sbn_marginal.cuh"
 #include "sbn_pair.h"
+#include "sbn_sample.cuh"
 #include "sbn_tma.h"
 
 namespace {
@@ -52,6 +53,7 @@ constexpr int32_t kMagic = 0x53424E31;
 constexpr int kVersion = 4;
 constexpr int kVersionMarginals = 5;  // planner.build_marginals_plan: kind-2 readouts, no posterior slot
 constexpr int kVersionCounts = 6;     // planner.build_counts_plan: kind-3 count steps, P(observed) in the posterior slot
+constexpr int kVersionSample = 7;     // planner.build_sample_plan: kind-4 sample steps, P(observed) in the posterior slot
 constexpr int64_t kMarginalZoffMax = 1 << 24;  // int32 words of one readout's joint-state offset table
 constexpr int kMaxElim = 3;
 constexpr int kMaxZ = 256;
@@ -64,11 +66,12 @@ namespace {
 int parse(sbn_program *P, const int32_t *w, int64_t n) {
     if (n < kHeaderWords) return fail(SBN_E_INVALID, "program shorter than its header");
     if (w[0] != kMagic) return fail(SBN_E_INVALID, "bad program magic 0x%x", w[0]);
-    if (w[1] != kVersion && w[1] != kVersionMarginals && w[1] != kVersionCounts)
-        return fail(SBN_E_INVALID, "program version %d, engine expects %d, %d or %d", w[1], kVersion, kVersionMarginals,
-                    kVersionCounts);
+    if (w[1] != kVersion && w[1] != kVersionMarginals && w[1] != kVersionCounts && w[1] != kVersionSample)
+        return fail(SBN_E_INVALID, "program version %d, engine expects %d, %d, %d or %d", w[1], kVersion, kVersionMarginals,
+                    kVersionCounts, kVersionSample);
     P->marginals = w[1] == kVersionMarginals;
     P->counts = w[1] == kVersionCounts;
+    P->sample = w[1] == kVersionSample;
     P->mode = w[2];
     P->n_ev = w[3];
     const int n_tables = w[4], n_slots = w[5], n_steps = w[6];
@@ -82,6 +85,11 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         P->n_counts = w[10];
         if (P->Q != 1 || P->n_counts <= 0) return fail(SBN_E_INVALID, "bad counts header");
     }
+    if (P->sample) {
+        P->n_sampled = w[10];
+        if (P->Q != 1 || P->mode != 1 || P->n_sampled < 0) return fail(SBN_E_INVALID, "bad sample header");
+    }
+    int n_drawn = 0;  // sample program: drawn-code rows written by the sample steps so far
     if (P->marginals ? (P->post_slot != -1 || P->post_batched != 0) : (P->post_slot < 0 || P->post_slot >= n_slots))
         return fail(SBN_E_INVALID, "post slot out of range");
     int64_t p = kHeaderWords;
@@ -117,8 +125,17 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         p += 5;
         const bool readout = st.kind == 2;
         const bool count = st.kind == 3;
-        if (st.kind != 0 && st.kind != 1 && !(readout && P->marginals) && !(count && P->counts))
+        const bool draw = st.kind == 4;
+        if (st.kind != 0 && st.kind != 1 && !(readout && P->marginals) && !(count && P->counts) && !(draw && P->sample))
             return fail(SBN_E_INVALID, "step %d: bad kind", s);
+        if (draw) {
+            // the drawn variables are the step's `n_elim` axes; they fill the next drawn-code rows
+            if (!need(1)) return fail(SBN_E_INVALID, "truncated step %d", s);
+            st.q_offset = w[p++];
+            if (st.out_slot != -1 || n_axes != 0 || n_elim < 1 || n_elim > SBN_SAMPLE_MAX_X || st.q_offset != n_drawn ||
+                n_drawn + n_elim > P->n_sampled)
+                return fail(SBN_E_INVALID, "step %d: bad sample step", s);
+        }
         if (count) {
             // c_offset, the observed members' gathers and the count-table strides of the output axes
             if (!need(2)) return fail(SBN_E_INVALID, "truncated step %d", s);
@@ -162,7 +179,7 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         if (st.kind == 1 && P->mode == 0) return fail(SBN_E_INVALID, "step %d: batched step in a flat program", s);
         if (n_in < (count ? 0 : 1) || n_in > SBN_MAX_IN) return fail(SBN_E_INVALID, "step %d: %d inputs", s, n_in);
         if (n_axes < 0 || n_axes > SBN_MAX_AXES) return fail(SBN_E_INVALID, "step %d: %d axes", s, n_axes);
-        const bool writes_slot = !readout && !count;
+        const bool writes_slot = !readout && !count && !draw;
         if (writes_slot && (n_elim < 0 || n_elim > kMaxElim)) return fail(SBN_E_INVALID, "step %d: %d eliminated axes", s, n_elim);
         if (writes_slot && (st.out_slot < 0 || st.out_slot >= n_slots)) return fail(SBN_E_INVALID, "step %d: out slot", s);
         if (!need(n_axes + n_elim)) return fail(SBN_E_INVALID, "truncated step %d", s);
@@ -178,7 +195,7 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         p += n_axes;
         for (int k = 0; k < n_elim; ++k) {
             const int c = w[p + k];
-            if (c < 1) return fail(SBN_E_INVALID, "step %d: eliminated card %d", s, c);
+            if (c < 1 || (draw && c > 256)) return fail(SBN_E_INVALID, "step %d: eliminated card %d", s, c);
             if (static_cast<int64_t>(st.cx) * c > (readout || count ? kMarginalZoffMax / SBN_MAX_IN : kMaxZ))
                 return fail(SBN_E_INVALID, "step %d: too many eliminated states", s);
             st.cx *= c;
@@ -190,12 +207,12 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             for (int64_t q = st.q_offset; q < st.q_offset + st.n_out; ++q) written[q]++;
         } else if (count) {
             if (static_cast<int64_t>(st.cx) * st.n_out >= (1LL << 31)) return fail(SBN_E_INVALID, "step %d: count step too large", s);
-        } else {
+        } else if (!draw) {
             const Slot &os = P->slots[st.out_slot];
             if (os.batched != (st.kind == 1)) return fail(SBN_E_INVALID, "step %d: out slot kind mismatch", s);
             if (os.size < st.n_out) return fail(SBN_E_INVALID, "step %d: out slot too small", s);
         }
-        const bool per_row = st.kind == 1 || ((readout || count) && P->mode == 1);  // batched operands allowed
+        const bool per_row = st.kind == 1 || ((readout || count || draw) && P->mode == 1);  // batched operands allowed
         for (int i = 0; i < n_in; ++i) {
             if (!need(4)) return fail(SBN_E_INVALID, "truncated step %d input %d", s, i);
             InDesc in;
@@ -205,7 +222,8 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             in.sx = 0;
             const int n_ev = w[p + 3];
             p += 4;
-            if (n_ev < 0 || n_ev > SBN_MAX_EV) return fail(SBN_E_INVALID, "step %d input %d: %d ev axes", s, i, n_ev);
+            if (n_ev < 0 || n_ev > (draw ? SBN_SAMPLE_MAX_TERMS : SBN_MAX_EV))
+                return fail(SBN_E_INVALID, "step %d input %d: %d ev axes", s, i, n_ev);
             if (!need(3LL * n_ev + n_elim + n_axes)) return fail(SBN_E_INVALID, "truncated step %d input %d", s, i);
             int64_t size;
             if (in.is_slot) {
@@ -220,14 +238,17 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
                 size = P->tables[in.id].second;
             }
             if (in.batched && !per_row) return fail(SBN_E_INVALID, "step %d: batched input in flat step", s);
-            if (in.batched && n_ev) return fail(SBN_E_INVALID, "step %d input %d: batched input with ev axes", s, i);
+            if (in.batched && n_ev && !draw) return fail(SBN_E_INVALID, "step %d input %d: batched input with ev axes", s, i);
             if (n_ev && !per_row && P->mode != 0)
                 return fail(SBN_E_INVALID, "step %d input %d: evidence axes in an unbatched step", s, i);
             int64_t max_off = 0;
             for (int k = 0; k < n_ev; ++k) {
                 EvAxis a{w[p], w[p + 1], w[p + 2]};
                 p += 3;
-                if (a.col < 0 || a.col >= P->n_ev || a.stride < 0 || a.card < 1 || a.card > 256)
+                // a sample step also gathers the codes drawn by the steps before it (col >= n_ev); a batched
+                // operand only those: its observed columns are part of its rows already
+                const int n_cols = draw ? P->n_ev + n_drawn : P->n_ev;
+                if (a.col < 0 || a.col >= n_cols || (in.batched && a.col < P->n_ev) || a.stride < 0 || a.card < 1 || a.card > 256)
                     return fail(SBN_E_INVALID, "step %d input %d: bad ev axis", s, i);
                 max_off += static_cast<int64_t>(a.card - 1) * a.stride;
                 in.ev.push_back(a);
@@ -255,6 +276,7 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             std::stable_partition(st.in.begin(), st.in.end(), no_axis);
             st.n_common = static_cast<int>(std::count_if(st.in.begin(), st.in.end(), no_axis));
         }
+        if (draw) n_drawn += n_elim;  // at most kMaxZ joint states: checked with the eliminated cards
         if (readout) {
             std::stable_partition(st.in.begin(), st.in.end(), [](const InDesc &in) { return in.strides[0] == 0; });
             st.n_common = static_cast<int>(std::count_if(st.in.begin(), st.in.end(), [](const InDesc &in) { return in.strides[0] == 0; }));
@@ -270,7 +292,20 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             if (st.kind == 0 && ++writes[st.out_slot] > 1)
                 return fail(SBN_E_INVALID, "unbatched slot %d is written twice in a batched program", st.out_slot);
     }
-    if (P->marginals) {
+    if (P->sample) {
+        // every drawn-code row is written; the sample steps run last, after the last write of P(observed)
+        if (n_drawn != P->n_sampled) return fail(SBN_E_INVALID, "%d of %d drawn-code rows are written", n_drawn, P->n_sampled);
+        int writer = -1, first = static_cast<int>(P->steps.size());
+        for (size_t i = 0; i < P->steps.size(); ++i) {
+            if (P->steps[i].kind == 4) {
+                if (first > static_cast<int>(i)) first = static_cast<int>(i);
+            } else {
+                if (first < static_cast<int>(i)) return fail(SBN_E_INVALID, "step %zu comes after a sample step", i);
+                if (P->steps[i].out_slot == P->post_slot) writer = static_cast<int>(i);
+            }
+        }
+        if (writer < 0) return fail(SBN_E_INVALID, "P(observed) is not written before the sample steps");
+    } else if (P->marginals) {
         for (int q = 0; q < P->Q; ++q)
             if (written[q] != 1) return fail(SBN_E_INVALID, "posterior entry %d is written %d times", q, written[q]);
     } else if (P->counts) {
@@ -499,7 +534,7 @@ void plan_tiles(sbn_program *P, std::vector<int32_t> *words) {
                 words->push_back(static_cast<int32_t>(off));
             }
         }
-        if (st.ecards.size() < 2 && st.kind != 2 && st.kind != 3) continue;
+        if (st.ecards.size() < 2 && st.kind != 2 && st.kind != 3 && st.kind != 4) continue;
         st.zoff_pos = static_cast<int64_t>(words->size());
         for (const InDesc &in : st.in) {
             for (int z = 0; z < st.cx; ++z) {
@@ -976,6 +1011,93 @@ int issue_counts(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_r
     return SBN_OK;
 }
 
+// Sample step (kind 4): draws its variables for rows 0 .. n_rows - 1 and draws 0 .. n_draws - 1 (`k`: its index
+// among the sample steps).
+cudaError_t launch_sample(sbn_program *P, const StepDesc &st, int k, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
+                          int64_t n_draws, int64_t ld_drawn, cudaStream_t stream) {
+    P->launches++;
+    SbnSample m;
+    memset(&m, 0, sizeof m);
+    const size_t elem = P->f64 ? 8 : 4;
+    m.ev = ev;
+    m.ld_ev = ld_ev;
+    m.drawn = P->d_drawn;
+    m.ld_drawn = ld_drawn;
+    m.ld = P->ld;
+    m.zoff = P->d_tile_off + st.zoff_pos;
+    m.args = P->d_sample_args;
+    m.flag = P->d_drawn + static_cast<int64_t>(P->n_sampled) * n_draws * ld_drawn;
+    m.min_total = P->f64 ? 1e-290 : static_cast<double>(SBN_MIN_TOTAL_F32);
+    m.n_rows = static_cast<int32_t>(n_rows);
+    m.n_draws = static_cast<int32_t>(n_draws);
+    m.n_ev = P->n_ev;
+    m.n_in = static_cast<int32_t>(st.in.size());
+    m.cz = st.cx;
+    m.n_x = static_cast<int32_t>(st.ecards.size());
+    m.d_first = static_cast<int32_t>(st.q_offset);
+    m.step = k;
+    for (size_t j = 0; j < st.ecards.size(); ++j) m.x_card[j] = st.ecards[j];
+    int64_t smem = 0;
+    for (size_t i = 0; i < st.in.size(); ++i) {
+        const InDesc &in = st.in[i];
+        SbnSampleIn &d = m.in[i];
+        int64_t padded;
+        if (in.is_slot) {
+            d.ptr = P->slots[in.id].ptr;
+            padded = P->slots[in.id].padded;
+        } else {
+            d.ptr = reinterpret_cast<const char *>(P->d_tables) + P->tables[in.id].first * static_cast<int64_t>(elem);
+            padded = P->table_padded[in.id];
+        }
+        d.batched = in.batched ? 1 : 0;
+        d.n_terms = static_cast<int32_t>(in.ev.size());
+        for (size_t t = 0; t < in.ev.size(); ++t) {
+            d.t_col[t] = in.ev[t].col;
+            d.t_stride[t] = in.ev[t].stride;
+            d.t_card[t] = in.ev[t].card;
+        }
+        d.smem_off = -1;
+        if (!P->f64 && !in.batched && (smem + padded) * 4 <= SBN_SMEM_BUDGET) {
+            d.smem_off = static_cast<int32_t>(smem);
+            d.stage_floats = static_cast<int32_t>(padded);
+            smem += padded;
+        }
+    }
+    m.smem_floats = static_cast<int32_t>(smem);
+    if (P->f64) return sbn_sample_launch<double>(m, 0, stream);
+    return sbn_sample_launch<float>(m, static_cast<size_t>(smem) * 4, stream);
+}
+
+// Every launch of one run of a sample program: the upward pass, the sample steps and P(observed) out.
+int issue_sample(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws, int64_t ld_drawn,
+                 void *d_prob, cudaStream_t stream) {
+    uint8_t *flag = P->d_drawn + static_cast<int64_t>(P->n_sampled) * n_draws * ld_drawn;
+    SBN_CUDA(cudaMemsetAsync(flag, 0, static_cast<size_t>(n_rows), stream));
+    SbnStep q;
+    int k = 0;
+    for (const StepDesc &st : P->steps) {
+        if (st.kind == 0) continue;  // computed once, when the program was created (sample programs are batched)
+        if (st.kind == 4) {
+            SBN_CUDA(launch_sample(P, st, k++, d_ev, ld_ev, n_rows, n_draws, ld_drawn, stream));
+            continue;
+        }
+        build_params(P, st, d_ev, ld_ev, n_rows, &q);
+        SBN_CUDA(launch_step(P, st, q, stream));
+    }
+    P->launches++;
+    const Slot &ps = P->slots[P->post_slot];
+    const int threads = 256;
+    const unsigned grid = static_cast<unsigned>((n_rows + threads - 1) / threads);
+    if (P->f64)
+        sbn_sample_prob<double><<<grid, threads, 0, stream>>>(reinterpret_cast<const double *>(ps.ptr), ps.batched ? 1 : 0, flag,
+                                                              static_cast<int32_t>(n_rows), 1e-290, static_cast<double *>(d_prob));
+    else
+        sbn_sample_prob<float><<<grid, threads, 0, stream>>>(ps.ptr, ps.batched ? 1 : 0, flag, static_cast<int32_t>(n_rows),
+                                                             static_cast<double>(SBN_MIN_TOTAL_F32), static_cast<float *>(d_prob));
+    SBN_CUDA(cudaGetLastError());
+    return SBN_OK;
+}
+
 cudaError_t launch_normalise(sbn_program *P, float *d_out, int64_t ld_out, int64_t n_rows, cudaStream_t stream) {
     P->launches++;
     const int threads = 256;
@@ -1174,6 +1296,7 @@ int check_run_args(sbn_program *P, const void *ev, int64_t ld_ev, int64_t n_rows
     if (P->Q > 1 && ld_out < n_rows) return fail(SBN_E_INVALID, "ld_out < n_rows");
     if (P->mode == 0 && n_rows != 1) return fail(SBN_E_INVALID, "a flat program answers exactly one row");
     if (P->counts) return fail(SBN_E_INVALID, "a counts program runs through sbn_program_counts_host");
+    if (P->sample) return fail(SBN_E_INVALID, "a sample program runs through sbn_program_sample_host");
     return SBN_OK;
 }
 
@@ -1291,7 +1414,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
         SBN_CUDA_P(cudaStreamSynchronize(P->stream));
         // The on-chip segments and paired steps assume every intermediate has ONE consumer; the factors of a
         // marginals program feed several launches, so it runs on the classic per-step launches.
-        if (!P->marginals && !P->counts) sbn_chain_plan(P);
+        if (!P->marginals && !P->counts && !P->sample) sbn_chain_plan(P);
     }
     {
         // opt every step-kernel instantiation into SBN_SMEM_BUDGET of dynamic shared memory
@@ -1306,6 +1429,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
             SBN_CUDA_P(sbn_triple_rows_set_attrs());
             SBN_CUDA_P(sbn_marginal_set_attrs());
             SBN_CUDA_P(sbn_count_set_attrs());
+            SBN_CUDA_P(sbn_sample_set_attrs());
             done[device] = true;
         }
     }
@@ -1322,7 +1446,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
     if (rc != SBN_OK) return bail(rc);
     {
         // pairs multiply the tables of two steps on the host: needs the outputs of the table steps above
-        cudaError_t e = P->marginals || P->counts ? cudaSuccess : sbn_pair_plan(P);
+        cudaError_t e = P->marginals || P->counts || P->sample ? cudaSuccess : sbn_pair_plan(P);
         if (e != cudaSuccess) return bail(fail(SBN_E_CUDA, "planning the paired steps failed: %s", cudaGetErrorString(e)));
     }
     *out = P;
@@ -1348,6 +1472,8 @@ void sbn_program_destroy(sbn_program *P) {
     cudaFree(P->d_shared);
     cudaFree(P->d_counts);
     cudaFree(P->d_partial);
+    cudaFree(P->d_drawn);
+    cudaFree(P->d_sample_args);
     cudaFree(P->d_tile_off);
     cudaFree(P->d_tables);
     if (P->stream) cudaStreamDestroy(P->stream);
@@ -1756,6 +1882,117 @@ int sbn_program_set_tables(sbn_program *P, const float *tables, int64_t n_table_
 
 int sbn_program_set_tables_f64(sbn_program *P, const double *tables, int64_t n_table_doubles) {
     return set_tables_common(P, tables, n_table_doubles, true);
+}
+
+constexpr int64_t kSampleGraphMinRows = 4096;
+
+static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws, uint64_t seed,
+                              int64_t row_base, uint8_t *out, void *prob, bool f64) {
+    if (!P) return fail(SBN_E_INVALID, "null program");
+    if (!P->sample) return fail(SBN_E_INVALID, "not a sample program (planner.build_sample_plan)");
+    if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the sample call");
+    if (n_rows <= 0) return fail(SBN_E_INVALID, "n_rows must be positive");
+    if (n_draws <= 0 || n_draws > INT32_MAX) return fail(SBN_E_INVALID, "n_draws must be in 1 .. 2^31 - 1");
+    if (row_base < 0) return fail(SBN_E_INVALID, "row_base must not be negative");
+    if ((P->n_sampled > 0 && !out) || !prob) return fail(SBN_E_INVALID, "null output");
+    if (P->n_ev > 0 && !ev) return fail(SBN_E_INVALID, "null evidence");
+    if (P->n_ev > 1 && ld_ev < n_rows) return fail(SBN_E_INVALID, "ld_ev < n_rows");
+    SBN_CUDA(cudaSetDevice(P->device));
+    if (n_rows > P->reserved_rows) {
+        const int rc = sbn_program_reserve(P, n_rows);
+        if (rc != SBN_OK) return rc;
+    }
+    // the drawn codes of a chunk ([n_sampled][n_draws] bytes + one flag byte per row) take at most half of the
+    // free device memory: larger batches run in more chunks
+    const int64_t per_row = static_cast<int64_t>(P->n_sampled) * n_draws + 1;
+    int64_t cap = P->reserved_rows;
+    if (round_up(std::min(cap, n_rows), 32) * per_row > P->drawn_bytes) {  // the buffer of an earlier call may do
+        size_t free_b = 0, total_b = 0;
+        SBN_CUDA(cudaMemGetInfo(&free_b, &total_b));
+        const int64_t budget = static_cast<int64_t>(free_b / 2) + P->drawn_bytes;
+        if (round_up(cap, 32) * per_row > budget) cap = std::max<int64_t>(32, budget / per_row / 32 * 32);
+    }
+    const int64_t ld_drawn = round_up(std::min(cap, n_rows), 32);
+    const int64_t bytes = ld_drawn * per_row;
+    if (bytes > P->drawn_bytes) {
+        SBN_CUDA(cudaStreamSynchronize(P->stream));
+        cudaFree(P->d_drawn);
+        P->d_drawn = nullptr;
+        P->drawn_bytes = 0;
+        const cudaError_t e = cudaMalloc(&P->d_drawn, static_cast<size_t>(bytes));
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            P->d_drawn = nullptr;
+            return fail(SBN_E_NOMEM, "cudaMalloc of %lld bytes of drawn codes failed: %s", (long long)bytes, cudaGetErrorString(e));
+        }
+        P->drawn_bytes = bytes;
+    }
+    if (!P->d_sample_args) SBN_CUDA(cudaMalloc(&P->d_sample_args, 4 * sizeof(uint32_t)));
+    const size_t elem = f64 ? 8 : 4;
+    for (int64_t r0 = 0; r0 < n_rows; r0 += cap) {
+        const int64_t rows = std::min(cap, n_rows - r0);
+        if (P->n_ev > 0)
+            SBN_CUDA(cudaMemcpy2DAsync(P->d_ev, static_cast<size_t>(P->ld), ev + r0, static_cast<size_t>(ld_ev),
+                                       static_cast<size_t>(rows), static_cast<size_t>(P->n_ev), cudaMemcpyHostToDevice, P->stream));
+        // read by the sample steps at run time, so that one captured graph serves every seed and chunk
+        const uint64_t first = static_cast<uint64_t>(row_base + r0);
+        const uint32_t args[4] = {static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32), static_cast<uint32_t>(first),
+                                  static_cast<uint32_t>(first >> 32)};
+        SBN_CUDA(cudaMemcpyAsync(P->d_sample_args, args, sizeof args, cudaMemcpyHostToDevice, P->stream));
+        // a short chunk runs as plain launches: capturing and instantiating a graph costs more than it saves, and
+        // the short runs of a pattern whose rows are scattered through a frame come in many lengths
+        if (!P->use_graph || rows < kSampleGraphMinRows) {
+            const int rc = issue_sample(P, P->d_ev, P->ld, rows, n_draws, ld_drawn, P->d_out, P->stream);
+            if (rc != SBN_OK) return rc;
+        } else {
+            // one graph per (chunk size, n_draws, drawn-code buffer)
+            auto &k = P->graph_key;
+            if (!P->exec || k.ev != P->d_ev || k.n_rows != rows || k.out != reinterpret_cast<float *>(P->d_drawn) ||
+                k.ld_out != ld_drawn || P->graph_draws != n_draws) {
+                if (P->exec) {
+                    cudaGraphExecDestroy(P->exec);
+                    P->exec = nullptr;
+                }
+                SBN_CUDA(cudaStreamBeginCapture(P->stream, cudaStreamCaptureModeRelaxed));
+                const int64_t before = P->launches;
+                const int rc = issue_sample(P, P->d_ev, P->ld, rows, n_draws, ld_drawn, P->d_out, P->stream);
+                cudaGraph_t graph = nullptr;
+                cudaError_t e = cudaStreamEndCapture(P->stream, &graph);
+                P->graph_launches = P->launches - before;
+                P->launches = before;
+                if (rc != SBN_OK) {
+                    if (graph) cudaGraphDestroy(graph);
+                    return rc;
+                }
+                if (e != cudaSuccess) return fail(SBN_E_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
+                e = cudaGraphInstantiate(&P->exec, graph, 0);
+                cudaGraphDestroy(graph);
+                if (e != cudaSuccess) return fail(SBN_E_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
+                k = {P->d_ev, P->ld, rows, reinterpret_cast<float *>(P->d_drawn), ld_drawn};
+                P->graph_draws = n_draws;
+            }
+            SBN_CUDA(cudaGraphLaunch(P->exec, P->stream));
+            P->launches += P->graph_launches;
+        }
+        if (P->n_sampled > 0)
+            SBN_CUDA(cudaMemcpy2DAsync(out + r0, static_cast<size_t>(n_rows), P->d_drawn, static_cast<size_t>(ld_drawn),
+                                       static_cast<size_t>(rows), static_cast<size_t>(P->n_sampled * n_draws),
+                                       cudaMemcpyDeviceToHost, P->stream));
+        SBN_CUDA(cudaMemcpyAsync(static_cast<char *>(prob) + r0 * elem, P->d_out, static_cast<size_t>(rows) * elem,
+                                 cudaMemcpyDeviceToHost, P->stream));
+    }
+    SBN_CUDA(cudaStreamSynchronize(P->stream));
+    return SBN_OK;
+}
+
+int sbn_program_sample_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws, uint64_t seed,
+                            int64_t row_base, uint8_t *out, float *prob) {
+    return sample_host_common(P, ev, ld_ev, n_rows, n_draws, seed, row_base, out, prob, false);
+}
+
+int sbn_program_sample_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws,
+                                uint64_t seed, int64_t row_base, uint8_t *out, double *prob) {
+    return sample_host_common(P, ev, ld_ev, n_rows, n_draws, seed, row_base, out, prob, true);
 }
 
 int sbn_program_profile(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out,

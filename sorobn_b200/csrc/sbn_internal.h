@@ -60,6 +60,8 @@ struct StepDesc {
     std::vector<int> cstrides;
     int64_t span = 0;          // entries of the family's count table
     int64_t soff_pos = -1, coff_pos = -1;
+    // sample step of a sample program (kind 4, sbn_sample.cuh): the `ecards` variables are drawn (not summed
+    // out) into drawn-code rows q_offset ..; an input's `ev` terms may name drawn rows (col >= n_ev)
 };
 struct Slot {
     bool batched;
@@ -86,6 +88,12 @@ struct sbn_program {
     double *d_partial = nullptr;  // counts program: per-warp partial tables of one count step (during a counts call only)
     const double *graph_partial = nullptr;  // the partial tables the captured counts graph writes
     int64_t partial_doubles = 0;
+    bool sample = false;          // version-7 program: kind-4 steps draw codes, post_slot holds P(observed)
+    int n_sampled = 0;            // sample program: drawn-code rows (one per unobserved variable)
+    uint8_t *d_drawn = nullptr;   // sample program: drawn codes [n_sampled][n_draws][ld_drawn], then flags [ld_drawn]
+    int64_t drawn_bytes = 0;
+    uint32_t *d_sample_args = nullptr;  // seed lo, seed hi, row_base lo, row_base hi of the current chunk
+    int64_t graph_draws = 0;      // n_draws of the captured sample graph
     std::vector<std::pair<int64_t, int64_t>> tables;  // (offset, size) in floats
     std::vector<int64_t> table_padded;
     float *d_tables = nullptr;

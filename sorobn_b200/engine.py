@@ -16,7 +16,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libsorobn_
 _lib = None
 
 SBN_OK = 0
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 
 class EngineError(RuntimeError):
@@ -70,6 +70,9 @@ def load():
     for name in ("sbn_program_set_tables", "sbn_program_set_tables_f64"):
         getattr(lib, name).restype = i32
         getattr(lib, name).argtypes = [vp, vp, i64]
+    for name in ("sbn_program_sample_host", "sbn_program_sample_host_f64"):
+        getattr(lib, name).restype = i32
+        getattr(lib, name).argtypes = [vp, vp, i64, i64, i64, c.c_uint64, i64, vp, vp]
     lib.sbn_program_destroy.restype = None
     lib.sbn_program_destroy.argtypes = [vp]
     lib.sbn_program_reserve.restype = i32
@@ -113,7 +116,7 @@ EXPORTS = (
     "sbn_program_run_host_f64", "sbn_program_evidence_host", "sbn_program_evidence_host_f64", "sbn_program_destroy",
     "sbn_program_reserve", "sbn_program_run_host", "sbn_program_run_device", "sbn_program_profile",
     "sbn_program_step_roles", "sbn_program_counts_host", "sbn_program_counts_host_f64", "sbn_program_set_tables",
-    "sbn_program_set_tables_f64",
+    "sbn_program_set_tables_f64", "sbn_program_sample_host", "sbn_program_sample_host_f64",
     "sbn_program_info", "sbn_program_set_graph", "sbn_program_set_tiled", "sbn_gibbs_create", "sbn_gibbs_run_host",
     "sbn_sampler_run_host", "sbn_gibbs_conditional", "sbn_gibbs_destroy", "sbn_host_alloc", "sbn_host_free",
 )
@@ -270,6 +273,21 @@ class Program:
         blob = np.ascontiguousarray(blob, dtype=np.float64 if self.f64 else np.float32)
         fn = load().sbn_program_set_tables_f64 if self.f64 else load().sbn_program_set_tables
         _check(fn(self._h, blob.ctypes.data, blob.size))
+
+    def sample(self, codes: np.ndarray, n_rows: int, n_draws: int, seed: int, row_base: int = 0):
+        """Sample programs (planner.build_sample_plan): (drawn codes uint8 [n_sampled, n_draws, n_rows] in
+        the order of `plan.sampled`, P(observed) [n_rows], NaN for a row the float32 range rule flags), host
+        path.  Row b's draws depend only on (seed, row_base + b, draw index)."""
+        n_rows, n_draws = int(n_rows), int(n_draws)
+        codes = np.ascontiguousarray(codes, dtype=np.uint8)
+        if self.n_ev and codes.shape != (self.n_ev, n_rows):
+            raise ValueError(f"evidence codes have shape {codes.shape}, expected {(self.n_ev, n_rows)}")
+        out = np.empty((len(self.plan.sampled), n_draws, n_rows), dtype=np.uint8)
+        prob = np.empty(n_rows, dtype=np.float64 if self.f64 else np.float32)
+        fn = load().sbn_program_sample_host_f64 if self.f64 else load().sbn_program_sample_host
+        _check(fn(self._h, codes.ctypes.data if self.n_ev else None, n_rows, n_rows, n_draws,
+                  int(seed) & (2**64 - 1), int(row_base), out.ctypes.data, prob.ctypes.data))
+        return out, prob
 
     def run_device(self, d_ev: int, ld_ev: int, n_rows: int, d_out: int, ld_out: int, stream: int = 0):
         """Device path: raw device pointers, asynchronous on `stream`."""

@@ -79,6 +79,27 @@ holds M_v and, per row, adds
 at `c_offset + key(row) + sum_m state_m * cstrides[m]`, with key(row) = sum_k ev[col_k] * stride_k
 over the observed family members.  No step writes a slot that a later one still needs: a kind-3
 step writes only the count table.
+
+Sample programs (`build_sample_plan`, VERSION 7) draw exact posterior samples of every unobserved
+variable: the version-5 upward pass (no downward pass), then one sample step (kind 4) per bucket in
+reverse elimination order (forward filtering, backward sampling):
+
+    header : MAGIC 7 1 n_ev n_tables n_slots n_steps 1 p_slot p_batched n_sampled 0
+    kind 4 : 4 n_in -1 0 n_x d_first | cards[n_x] |
+             per input: is_slot id batched n_terms (col stride card)*n_terms strides[n_x]
+
+`p_slot` holds P(observed cells) of every row, as in version 6.  The drawn codes are extra code
+rows: row `n_ev + j` is the j-th sampled variable, `[n_sampled][n_draws][ld]` uint8.  A kind-4 step
+draws the joint state X of its bucket's eliminated variables (`n_x` of them, first one fastest,
+at most MAX_Z joint states) with probability proportional to
+
+    w(X) = prod_i in_i[ sum_x X_x * strides_i[x] + sum_t code_t(row, draw) * stride_t ]
+
+where the terms `(col stride card)` gather observed columns (col < n_ev) or variables drawn by an
+earlier step (col >= n_ev): the bucket's separator, which lies above it in the bucket tree.  A
+batched input's gathered offset is multiplied by the row pitch.  The step writes the codes of its
+variables to drawn rows `d_first .. d_first + n_x - 1`; steps write consecutive rows, so the
+sampled variables are numbered in drawing order.  A sample step writes no slot.
 """
 from __future__ import annotations
 
@@ -110,6 +131,10 @@ MARGINAL_MAX_Z = 2**21
 VERSION_MARGINALS = 5
 KIND_COUNT = 3  # expected counts of one CPT family, summed over the rows (counts programs only)
 VERSION_COUNTS = 6
+KIND_SAMPLE = 4  # draw one bucket's eliminated variables given the drawn separator (sample programs only)
+VERSION_SAMPLE = 7
+SAMPLE_MAX_CARD = 255  # a sampled variable's states (its codes are uint8)
+SAMPLE_MAX_TERMS = 16  # gathered (col stride card) terms per input of a sample step (csrc: SBN_SAMPLE_MAX_TERMS)
 HEADER_WORDS = 12
 
 
@@ -168,10 +193,11 @@ class Step:
     elims: tuple  # variables summed out by this launch
     ecards: tuple
     out_slot: int = -1
-    q_offset: int = -1  # KIND_MARGINAL: first posterior entry of the target's segment; KIND_COUNT: c_offset
+    q_offset: int = -1  # KIND_MARGINAL: first posterior entry of the target's segment; KIND_COUNT: c_offset;
+    # KIND_SAMPLE: first drawn-code row it writes
     key: tuple = ()  # KIND_COUNT: ((ev_col, stride, card), ...) of the observed family members
     cstrides: tuple = ()  # KIND_COUNT: count-table stride of every output axis
-    norm: object = None  # KIND_COUNT: the factor holding P(observed) (read through the header's p_slot)
+    norm: object = None  # KIND_COUNT / KIND_SAMPLE: the factor holding P(observed) (the header's p_slot)
 
     @property
     def cx(self):
@@ -199,14 +225,22 @@ class Plan:
     count_offsets: list = None  # counts plans: first count-table entry of every var id's family
     table_axes: list = None  # var ids of every shipped table's axes, outermost first (refresh_tables)
     table_scopes: list = None  # the CPT scope [*parents, v] every table was transposed from
+    sampled: tuple = ()  # sample plans: the var id of every drawn-code row, in drawing order
 
     # ---- cost model (DESIGN.md "algorithmic bytes") -------------------------------
-    def bytes_per_row(self):
+    def bytes_per_row(self, n_draws=1):
         """Algorithmic HBM bytes per evidence row: every batched step reads each
         batched input once and writes its output once (fp32), plus the evidence
-        codes in and the posterior out."""
+        codes in and the posterior out.  A sample step reads, per draw, the part of each
+        batched input its drawn separator selects and writes its codes (`n_draws` draws)."""
         total = 0
         for st in self.steps:
+            if st.kind == KIND_SAMPLE:
+                for f, es, _ in st.inputs:
+                    if f.batched:
+                        total += 4 * n_draws * int(np.prod([c for c, s in zip(st.ecards, es) if s], dtype=np.int64))
+                total += n_draws * len(st.elims)
+                continue
             if st.kind not in (KIND_BATCHED, KIND_MARGINAL, KIND_COUNT):
                 continue
             for f, _, _ in st.inputs:
@@ -220,7 +254,7 @@ class Plan:
             # normalise: read unnormalised posterior, write posterior (a marginals program's
             # readouts write their segments normalised, counted above)
             total += 8 * self.Q
-        elif self.version == VERSION_COUNTS:
+        elif self.version in (VERSION_COUNTS, VERSION_SAMPLE):
             total += 4  # P(observed) out
         total += len(self.evidence)  # uint8 codes
         return total
@@ -331,6 +365,16 @@ def build_counts_plan(net: CompiledNet, evidence, mode=MODE_BATCHED, order=None,
     return _build(net, (), evidence, mode, order, max_in, False, lift_evidence, True, fuse_elims, hidden, counts=True)
 
 
+def build_sample_plan(net: CompiledNet, evidence, order=None, max_in=MAX_IN, lift_evidence=True, fuse_elims=None) -> Plan:
+    """Plan exact posterior draws of every variable that is not in `evidence` (a version-7 program, see
+    the module docstring): the upward pass of variable elimination, then one sample step per bucket,
+    top-down.  `Plan.sampled` names the variable of every drawn-code row."""
+    evidence = tuple(evidence)
+    hidden = tuple(v for v in range(len(net.names)) if v not in set(evidence))
+    return _build(net, (), evidence, MODE_BATCHED, order, max_in, False, lift_evidence, True, fuse_elims, hidden,
+                  sample=True)
+
+
 def count_layout(net: CompiledNet):
     """(first count-table entry of every var id's family, total entries): the dense `[*parents, v]`
     arrays of the CPTs in CompiledNet order, concatenated."""
@@ -357,7 +401,7 @@ def refresh_tables(plan: Plan, cpts):
 
 
 def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evidence, allow_empty_query, fuse_elims,
-           targets, counts=False):
+           targets, counts=False, sample=False):
     if merge_sum_outs is None:
         merge_sum_outs = os.environ.get("SOROBN_B200_MERGE", "0") == "1"
     if fuse_elims is None:
@@ -607,6 +651,9 @@ def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evide
         if targets is not None:
             buckets.append((bucket_factors, tuple(elims), set().union(*[f.vars for f in bucket_factors]), factors[-1]))
 
+    if sample:
+        return _sample_passes(net, evidence, order, max_in, buckets, factors, steps, tables, table_arrays, table_axes,
+                              emit, combine_tables, axis_order, fsize)
     if counts:
         return _counts_passes(net, evidence, mode, order, max_in, buckets, factors, steps, tables, table_arrays,
                               table_axes, emit, combine_tables, axis_order, fsize)
@@ -755,6 +802,57 @@ def _counts_passes(net, evidence, mode, order, max_in, buckets, leftovers, steps
     return plan
 
 
+def _sample_passes(net, evidence, order, max_in, buckets, leftovers, steps, tables, table_arrays, table_axes, emit,
+                   combine_tables, axis_order, fsize):
+    """Sample steps of a sample plan (DESIGN.md "Posterior samples").
+
+    Bucket k eliminated X_k and sent lambda_k(S_k) to a later bucket.  Walking the buckets in reverse
+    elimination order, every variable of S_k has been drawn when bucket k is reached, and
+        P(X_k | S_k = drawn, e) is proportional to prod_{f in F_k} f(X_k, S_k = drawn, e).
+    P(observed) is the product of the upward pass's leftover scalars, as in a counts plan."""
+    card = net.card
+    n_ev = len(evidence)
+    _, fold = _downward(net, max_in, buckets, leftovers, (), emit, combine_tables, axis_order, fsize)
+    # the folds (products of the factors beyond max_in) do not depend on the draws: they all run before
+    # the sample steps, which then form one contiguous run at the end of the program
+    inputs_of = [fold(list(buckets[k][0])) for k in range(len(buckets))]
+    prob = emit(fold(list(leftovers)), None, [], may_lift=False)
+
+    drawn = {}  # var id -> drawn-code row
+    for k in reversed(range(len(buckets))):
+        _, X, _, _ = buckets[k]
+        for x in X:
+            if int(card[x]) > SAMPLE_MAX_CARD:
+                raise ValueError(f"{net.names[x]!r} has {int(card[x])} states; drawn codes are uint8 (at most "
+                                 f"{SAMPLE_MAX_CARD} states)")
+        cz = int(np.prod([int(card[x]) for x in X], dtype=np.int64))
+        if cz > MAX_Z:
+            raise ValueError(f"the bucket of {[net.names[x] for x in X]} has {cz} joint states; a sample step draws "
+                             f"from at most {MAX_Z}")
+        ins = []
+        for f in inputs_of[k]:
+            pos = dict(zip(f.vars, f.strides))
+            terms = tuple(f.ev) + tuple((n_ev + drawn[u], pos[u], int(card[u])) for u in f.vars if u not in X)
+            if len(terms) > SAMPLE_MAX_TERMS:
+                raise ValueError(f"a factor of the bucket of {[net.names[x] for x in X]} gathers {len(terms)} observed "
+                                 f"or drawn variables; a sample step gathers at most {SAMPLE_MAX_TERMS}")
+            g = _Factor(f.is_slot, f.buf, f.vars, f.strides, terms, f.batched)
+            ins.append((g, tuple(pos.get(x, 0) for x in X), ()))
+        steps.append(Step(KIND_SAMPLE, ins, -1, (), (), tuple(X), tuple(int(card[x]) for x in X),
+                          q_offset=len(drawn), norm=prob))
+        for x in X:
+            drawn[x] = len(drawn)
+
+    slots, where = _assign_slots_shared(steps, keep_unbatched=True)
+    plan = Plan(mode=MODE_BATCHED, query=(), evidence=evidence, order=list(order), tables=tables, slots=slots,
+                steps=steps, post_slot=where[prob.buf], Q=1, version=VERSION_SAMPLE,
+                table_axes=[list(a) for a in table_axes], table_scopes=[net.scope(v) for v in tables],
+                sampled=tuple(sorted(drawn, key=drawn.get)))
+    plan._card = card
+    _serialise(plan, table_arrays)
+    return plan
+
+
 def _downward(net, max_in, buckets, leftovers, reads, emit, combine_tables, axis_order, fsize):
     """Downward messages pi_k of the buckets on the way from a root to every bucket in `reads`
     (`_marginals_passes`).  Returns (pi, fold)."""
@@ -871,7 +969,7 @@ def _assign_slots_shared(steps, keep_unbatched):
             slots[phys][2] = not (keep_unbatched and not slots[phys][0])
 
     for st in steps:
-        writes_slot = st.kind not in (KIND_MARGINAL, KIND_COUNT)
+        writes_slot = st.kind not in (KIND_MARGINAL, KIND_COUNT, KIND_SAMPLE)
         if writes_slot:
             size = int(np.prod(st.cards, dtype=np.int64)) if st.cards else 1
             st.out_slot = alloc(st.kind == KIND_BATCHED, size)
@@ -1094,10 +1192,12 @@ def _serialise(plan: Plan, table_arrays):
     plan.table_offsets = offsets
 
     extra = [0, 0]
-    if plan.version in (VERSION, VERSION_COUNTS):
+    if plan.version in (VERSION, VERSION_COUNTS, VERSION_SAMPLE):
         post = [plan.post_slot, int(plan.slots[plan.post_slot][0])]
         if plan.version == VERSION_COUNTS:
             extra = [plan.n_counts, 0]
+        elif plan.version == VERSION_SAMPLE:
+            extra = [len(plan.sampled), 0]
     else:
         post = [-1, 0]  # the readouts write the posterior themselves
     w = [MAGIC, plan.version, plan.mode, len(plan.evidence), len(plan.tables), len(plan.slots), len(plan.steps),
@@ -1116,6 +1216,8 @@ def _serialise(plan: Plan, table_arrays):
             for col, s, c in st.key:
                 w += [col, s, c]
             w += list(st.cstrides)
+        elif st.kind == KIND_SAMPLE:
+            w.append(st.q_offset)
         w += list(st.cards)
         w += list(st.ecards)
         for f, estrides, strides in st.inputs:
