@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SBN_ABI_VERSION 11
+#define SBN_ABI_VERSION 12
 
 #define SBN_OK 0
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
@@ -133,6 +133,16 @@ int sbn_program_sample_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev,
                             uint64_t seed, int64_t row_base, uint8_t *out, float *prob);
 int sbn_program_sample_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws,
                                 uint64_t seed, int64_t row_base, uint8_t *out, double *prob);
+
+/* Most probable explanation of an MPE program (planner.build_mpe_plan, version 8; the run, evidence, counts
+ * and sample calls refuse it, this call refuses every other program, and it is created in float32 only).
+ * For every row b, codes[j * n_rows + b] is the code of the j-th decoded variable (Plan.sampled) in the
+ * argmax over every unobserved variable jointly of P(unobserved, the row's observed cells); ties go to the
+ * first joint state of a bucket (first variable fastest).  log_prob[b] = that maximum, log P(x*, e), or
+ * -inf for a row whose observed cells have probability zero (its codes are meaningless).  Large batches
+ * run in chunks. */
+int sbn_program_mpe_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
+                         uint8_t *codes /* [n_decoded][n_rows] */, float *log_prob /* [n_rows] */);
 
 /* Same with DEVICE buffers, asynchronous on `stream` (a cudaStream_t; NULL = default
  * stream).  n_rows must not exceed the reserved chunk size. */

@@ -25,7 +25,8 @@ The approximate algorithms run on the device too (csrc/sbn_gibbs.cuh): `algorith
 expectation-maximisation; the E-step runs on the device as one counts program per missingness
 pattern (planner.build_counts_plan, csrc/sbn_count.cuh).  `sample_many` draws exact posterior
 samples of the missing cells and latent nodes, one sample program per pattern
-(planner.build_sample_plan, csrc/sbn_sample.cuh).
+(planner.build_sample_plan, csrc/sbn_sample.cuh).  `mpe_many` / `mpe` find their most probable
+explanation, one log-domain max-sum program per pattern (planner.build_mpe_plan, csrc/sbn_mpe.cuh).
 """
 from __future__ import annotations
 
@@ -48,9 +49,9 @@ def _as_list(obj):
 
 
 class _PatternRunner:
-    """The device programs of one missingness pattern (a counts or a sample plan): the float32 program, and
-    the float64 one for the rows it flags (created when first needed).  `set_cpts` gives both new tables in
-    place (counts programs)."""
+    """The device programs of one missingness pattern (a counts, sample or MPE plan): the float32 program,
+    and the float64 one for the rows it flags (created when first needed; never for an MPE plan, whose logs
+    do not underflow).  `set_cpts` gives both new tables in place (counts programs)."""
 
     def __init__(self, plan, device):
         from . import engine  # raises if libsorobn_b200.so cannot be loaded
@@ -502,14 +503,19 @@ class BayesNet:
         """The cached sample programs of one missingness pattern."""
         return self._pattern_runner("sample", ev)
 
+    def _mpe_runner(self, ev):
+        """The cached MPE program of one missingness pattern."""
+        return self._pattern_runner("mpe", ev)
+
     def _pattern_runner(self, kind, ev):
-        """The cached programs of one missingness pattern, `kind` "counts" or "sample" (dropped by `prepare()`,
-        as every program)."""
+        """The cached programs of one missingness pattern, `kind` "counts", "sample" or "mpe" (dropped by
+        `prepare()`, as every program)."""
         with self._cache_lock:
             key = (kind, ev, self.device)
             hit = self._engine_cache.get(key)
             if hit is None:
-                build = _planner.build_counts_plan if kind == "counts" else _planner.build_sample_plan
+                build = {"counts": _planner.build_counts_plan, "sample": _planner.build_sample_plan,
+                         "mpe": _planner.build_mpe_plan}[kind]
                 hit = self._engine_cache[key] = _PatternRunner(build(self._compiled, ev), self.device)
                 self._evict()
             else:
@@ -583,6 +589,53 @@ class BayesNet:
         frame = pd.DataFrame({name: np.asarray(net.domains[v], dtype=object)[codes[v].reshape(-1)]
                               for v, name in enumerate(net.names)}, index=index)
         return frame.infer_objects().sort_index(axis="columns")
+
+    def mpe_many(self, events: pd.DataFrame, return_log_proba: bool = False):
+        """The most probable explanation of every row of `events`, computed on the GPU: the joint state of
+        every unobserved variable that maximises P(unobserved, the row's observed cells).
+
+        A missing cell is None or NaN; a node without a column is latent.  Both are decoded; observed
+        cells are copied through.  Returns one row per row of `events` (same index) with one column per
+        node (sorted, dtypes inferred, as `sample_many`).  With `return_log_proba=True` returns (frame,
+        Series of log P(explanation, observed cells) in float64, same index); a row with every cell
+        observed decodes nothing and gets log P(row).  Ties go to the first joint state of a bucket of
+        the elimination (first variable fastest).  Raises ValueError for a value outside its variable's
+        domain and for rows whose observed cells have probability zero.
+
+        Unlike `impute_many`, which takes the mode of the dense posterior over the joint of the missing
+        columns, the cost grows with the number of variables, not with their joint.  Rows are grouped by
+        missingness pattern; each pattern is one MPE program (planner.build_mpe_plan): the upward pass of
+        variable elimination in the log domain with max in place of sum, then one argmax per bucket,
+        top-down (csrc/sbn_mpe.cuh)."""
+        groups = self._count_patterns(events)
+        net = self._compiled
+        n_rows = len(events.index)
+        codes = np.zeros((len(net.names), n_rows), dtype=np.uint8)
+        log_p = np.zeros(n_rows, dtype=np.float64)
+        for ev, rows, ev_codes in groups:
+            # fetched right before it runs, as in `sample_many`
+            runner = self._mpe_runner(ev)
+            decoded, lp = runner.f32.mpe(ev_codes, len(rows))
+            impossible = ~(lp > -np.inf)
+            if impossible.any():
+                raise ValueError(f"{int(impossible.sum())} row(s) have observed cells of probability zero "
+                                 f"(first: {events.index[rows[impossible][0]]!r}); they have nothing to explain")
+            for i, v in enumerate(ev):
+                codes[v][rows] = ev_codes[i]
+            for j, v in enumerate(runner.plan.sampled):
+                codes[v][rows] = decoded[j]
+            log_p[rows] = lp
+        frame = pd.DataFrame({name: np.asarray(net.domains[v], dtype=object)[codes[v]]
+                              for v, name in enumerate(net.names)}, index=events.index)
+        frame = frame.infer_objects().sort_index(axis="columns")
+        if return_log_proba:
+            return frame, pd.Series(log_p, index=events.index)
+        return frame
+
+    def mpe(self, event: dict) -> pd.Series:
+        """The most probable explanation of one event: `mpe_many(pd.DataFrame([event])).iloc[0]`, a Series
+        indexed by node name."""
+        return self.mpe_many(pd.DataFrame([event])).iloc[0]
 
     @staticmethod
     def _draw(program, ev_codes, rows, n, seed):

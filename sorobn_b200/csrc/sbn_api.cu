@@ -23,6 +23,7 @@
 #include "sbn_kernels.cuh"
 #include "sbn_launch.h"
 #include "sbn_marginal.cuh"
+#include "sbn_mpe.cuh"
 #include "sbn_pair.h"
 #include "sbn_sample.cuh"
 #include "sbn_tma.h"
@@ -54,6 +55,8 @@ constexpr int kVersion = 4;
 constexpr int kVersionMarginals = 5;  // planner.build_marginals_plan: kind-2 readouts, no posterior slot
 constexpr int kVersionCounts = 6;     // planner.build_counts_plan: kind-3 count steps, P(observed) in the posterior slot
 constexpr int kVersionSample = 7;     // planner.build_sample_plan: kind-4 sample steps, P(observed) in the posterior slot
+constexpr int kVersionMpe = 8;        // planner.build_mpe_plan: log tables, max-sum steps, kind-5 argmax steps,
+                                      // max log P(x, e) in the posterior slot
 constexpr int64_t kMarginalZoffMax = 1 << 24;  // int32 words of one readout's joint-state offset table
 constexpr int kMaxElim = 3;
 constexpr int kMaxZ = 256;
@@ -66,12 +69,14 @@ namespace {
 int parse(sbn_program *P, const int32_t *w, int64_t n) {
     if (n < kHeaderWords) return fail(SBN_E_INVALID, "program shorter than its header");
     if (w[0] != kMagic) return fail(SBN_E_INVALID, "bad program magic 0x%x", w[0]);
-    if (w[1] != kVersion && w[1] != kVersionMarginals && w[1] != kVersionCounts && w[1] != kVersionSample)
-        return fail(SBN_E_INVALID, "program version %d, engine expects %d, %d, %d or %d", w[1], kVersion, kVersionMarginals,
-                    kVersionCounts, kVersionSample);
+    if (w[1] != kVersion && w[1] != kVersionMarginals && w[1] != kVersionCounts && w[1] != kVersionSample &&
+        w[1] != kVersionMpe)
+        return fail(SBN_E_INVALID, "program version %d, engine expects %d, %d, %d, %d or %d", w[1], kVersion,
+                    kVersionMarginals, kVersionCounts, kVersionSample, kVersionMpe);
     P->marginals = w[1] == kVersionMarginals;
     P->counts = w[1] == kVersionCounts;
     P->sample = w[1] == kVersionSample;
+    P->mpe = w[1] == kVersionMpe;
     P->mode = w[2];
     P->n_ev = w[3];
     const int n_tables = w[4], n_slots = w[5], n_steps = w[6];
@@ -85,11 +90,14 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         P->n_counts = w[10];
         if (P->Q != 1 || P->n_counts <= 0) return fail(SBN_E_INVALID, "bad counts header");
     }
-    if (P->sample) {
+    if (P->sample || P->mpe) {
         P->n_sampled = w[10];
-        if (P->Q != 1 || P->mode != 1 || P->n_sampled < 0) return fail(SBN_E_INVALID, "bad sample header");
+        if (P->Q != 1 || P->mode != 1 || P->n_sampled < 0)
+            return fail(SBN_E_INVALID, P->mpe ? "bad MPE header" : "bad sample header");
     }
-    int n_drawn = 0;  // sample program: drawn-code rows written by the sample steps so far
+    // sample program: kind-4 steps draw codes; MPE program: kind-5 steps decode them (same words)
+    const int decode_kind = P->mpe ? 5 : 4;
+    int n_drawn = 0;  // sample / MPE program: drawn-code rows written by the sample / argmax steps so far
     if (P->marginals ? (P->post_slot != -1 || P->post_batched != 0) : (P->post_slot < 0 || P->post_slot >= n_slots))
         return fail(SBN_E_INVALID, "post slot out of range");
     int64_t p = kHeaderWords;
@@ -125,8 +133,8 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         p += 5;
         const bool readout = st.kind == 2;
         const bool count = st.kind == 3;
-        const bool draw = st.kind == 4;
-        if (st.kind != 0 && st.kind != 1 && !(readout && P->marginals) && !(count && P->counts) && !(draw && P->sample))
+        const bool draw = (st.kind == 4 && P->sample) || (st.kind == 5 && P->mpe);
+        if (st.kind != 0 && st.kind != 1 && !(readout && P->marginals) && !(count && P->counts) && !draw)
             return fail(SBN_E_INVALID, "step %d: bad kind", s);
         if (draw) {
             // the drawn variables are the step's `n_elim` axes; they fill the next drawn-code rows
@@ -134,7 +142,7 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             st.q_offset = w[p++];
             if (st.out_slot != -1 || n_axes != 0 || n_elim < 1 || n_elim > SBN_SAMPLE_MAX_X || st.q_offset != n_drawn ||
                 n_drawn + n_elim > P->n_sampled)
-                return fail(SBN_E_INVALID, "step %d: bad sample step", s);
+                return fail(SBN_E_INVALID, P->mpe ? "step %d: bad argmax step" : "step %d: bad sample step", s);
         }
         if (count) {
             // c_offset, the observed members' gathers and the count-table strides of the output axes
@@ -292,12 +300,13 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             if (st.kind == 0 && ++writes[st.out_slot] > 1)
                 return fail(SBN_E_INVALID, "unbatched slot %d is written twice in a batched program", st.out_slot);
     }
-    if (P->sample) {
-        // every drawn-code row is written; the sample steps run last, after the last write of P(observed)
+    if (P->sample || P->mpe) {
+        // every drawn-code row is written; the sample / argmax steps run last, after the last write of the
+        // posterior slot (P(observed), or max log P(x, e))
         if (n_drawn != P->n_sampled) return fail(SBN_E_INVALID, "%d of %d drawn-code rows are written", n_drawn, P->n_sampled);
         int writer = -1, first = static_cast<int>(P->steps.size());
         for (size_t i = 0; i < P->steps.size(); ++i) {
-            if (P->steps[i].kind == 4) {
+            if (P->steps[i].kind == decode_kind) {
                 if (first > static_cast<int>(i)) first = static_cast<int>(i);
             } else {
                 if (first < static_cast<int>(i)) return fail(SBN_E_INVALID, "step %zu comes after a sample step", i);
@@ -534,7 +543,7 @@ void plan_tiles(sbn_program *P, std::vector<int32_t> *words) {
                 words->push_back(static_cast<int32_t>(off));
             }
         }
-        if (st.ecards.size() < 2 && st.kind != 2 && st.kind != 3 && st.kind != 4) continue;
+        if (st.ecards.size() < 2 && st.kind != 2 && st.kind != 3 && st.kind != 4 && st.kind != 5) continue;
         st.zoff_pos = static_cast<int64_t>(words->size());
         for (const InDesc &in : st.in) {
             for (int z = 0; z < st.cx; ++z) {
@@ -550,7 +559,8 @@ void plan_tiles(sbn_program *P, std::vector<int32_t> *words) {
     }
     for (StepDesc &st : P->steps) {
         st.tile = 0;
-        if (st.kind != 1 || st.in.size() > static_cast<size_t>(kTiledMaxIn)) continue;
+        // an MPE program's steps run on the max-sum kernels only (launch_step), which have no tiled variant
+        if (st.kind != 1 || P->mpe || st.in.size() > static_cast<size_t>(kTiledMaxIn)) continue;
 
         int64_t smem = 0;
         for (const InDesc &in : st.in)
@@ -823,8 +833,25 @@ cudaError_t set_tiled_attrs() {
     return e;
 }
 
+// A step of an MPE program (log tables): the max-sum instantiations of the flat and the plain batched kernel,
+// whatever the program's switches say -- the tiled, paired, TMA, join and on-chip kernels are sum-product only.
+cudaError_t launch_maxsum(const StepDesc &st, const SbnStep &q, cudaStream_t stream) {
+    if (st.kind == 0) {
+        const int threads = 256;
+        const int64_t grid = (st.n_out + threads - 1) / threads;
+        sbn_launch(sbn_step_flat<float, SbnMaxSum>, dim3(static_cast<unsigned>(grid)), dim3(threads), 0, stream, q);
+        return cudaGetLastError();
+    }
+    if (st.kind != 1 || q.tile_off != nullptr) return cudaErrorInvalidValue;
+    const int64_t rest = st.n_out / (static_cast<int64_t>(q.n_axes > 0 ? q.card[0] : 1) * (q.n_axes > 1 ? q.card[1] : 1));
+    const int64_t grid = static_cast<int64_t>(q.n_bblocks) * q.n_tile1 * rest;
+    if (grid >= (1LL << 31)) return cudaErrorInvalidConfiguration;
+    return sbn_batched_maxsum_launch(q, grid, stream);
+}
+
 cudaError_t launch_step(sbn_program *P, const StepDesc &st, const SbnStep &q, cudaStream_t stream) {
     P->launches++;
+    if (P->mpe) return launch_maxsum(st, q, stream);
     if (st.kind == 1 && q.tile_off != nullptr && !P->marginals && sbn_tma_eligible(P, st))
         return sbn_tma_launch(P, st, q.ev, q.ld_ev, q.n_rows, stream);
     if (st.kind == 1 && q.tile_off != nullptr && sbn_join_rows(P, st, q) > 0) return sbn_join_launch(P, st, q, stream);
@@ -1012,7 +1039,7 @@ int issue_counts(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_r
 }
 
 // Sample step (kind 4): draws its variables for rows 0 .. n_rows - 1 and draws 0 .. n_draws - 1 (`k`: its index
-// among the sample steps).
+// among the sample steps).  Argmax step of an MPE program (kind 5, n_draws = 1): decodes them.
 cudaError_t launch_sample(sbn_program *P, const StepDesc &st, int k, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
                           int64_t n_draws, int64_t ld_drawn, cudaStream_t stream) {
     P->launches++;
@@ -1064,6 +1091,7 @@ cudaError_t launch_sample(sbn_program *P, const StepDesc &st, int k, const uint8
         }
     }
     m.smem_floats = static_cast<int32_t>(smem);
+    if (P->mpe) return sbn_argmax_launch(m, static_cast<size_t>(smem) * 4, stream);
     if (P->f64) return sbn_sample_launch<double>(m, 0, stream);
     return sbn_sample_launch<float>(m, static_cast<size_t>(smem) * 4, stream);
 }
@@ -1095,6 +1123,22 @@ int issue_sample(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_r
         sbn_sample_prob<float><<<grid, threads, 0, stream>>>(ps.ptr, ps.batched ? 1 : 0, flag, static_cast<int32_t>(n_rows),
                                                              static_cast<double>(SBN_MIN_TOTAL_F32), static_cast<float *>(d_prob));
     SBN_CUDA(cudaGetLastError());
+    return SBN_OK;
+}
+
+// Every launch of one run of an MPE program: the max-sum upward pass, which leaves max log P(x, e) in the
+// posterior slot, and the argmax steps.
+int issue_mpe(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, int64_t ld_drawn, cudaStream_t stream) {
+    SbnStep q;
+    for (const StepDesc &st : P->steps) {
+        if (st.kind == 0) continue;  // computed once, when the program was created (MPE programs are batched)
+        if (st.kind == 5) {
+            SBN_CUDA(launch_sample(P, st, 0, d_ev, ld_ev, n_rows, 1, ld_drawn, stream));
+            continue;
+        }
+        build_params(P, st, d_ev, ld_ev, n_rows, &q);
+        SBN_CUDA(launch_step(P, st, q, stream));
+    }
     return SBN_OK;
 }
 
@@ -1297,6 +1341,7 @@ int check_run_args(sbn_program *P, const void *ev, int64_t ld_ev, int64_t n_rows
     if (P->mode == 0 && n_rows != 1) return fail(SBN_E_INVALID, "a flat program answers exactly one row");
     if (P->counts) return fail(SBN_E_INVALID, "a counts program runs through sbn_program_counts_host");
     if (P->sample) return fail(SBN_E_INVALID, "a sample program runs through sbn_program_sample_host");
+    if (P->mpe) return fail(SBN_E_INVALID, "an MPE program runs through sbn_program_mpe_host");
     return SBN_OK;
 }
 
@@ -1342,6 +1387,10 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
     if (rc != SBN_OK) {
         delete P;
         return rc;
+    }
+    if (P->mpe && f64) {
+        delete P;
+        return fail(SBN_E_INVALID, "an MPE program runs in float32 only (its tables are logs: nothing underflows)");
     }
     for (size_t t = 0; t < P->tables.size(); ++t) {
         if (P->tables[t].first + P->table_padded[t] > n_table_floats) {
@@ -1414,7 +1463,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
         SBN_CUDA_P(cudaStreamSynchronize(P->stream));
         // The on-chip segments and paired steps assume every intermediate has ONE consumer; the factors of a
         // marginals program feed several launches, so it runs on the classic per-step launches.
-        if (!P->marginals && !P->counts && !P->sample) sbn_chain_plan(P);
+        if (!P->marginals && !P->counts && !P->sample && !P->mpe) sbn_chain_plan(P);
     }
     {
         // opt every step-kernel instantiation into SBN_SMEM_BUDGET of dynamic shared memory
@@ -1430,6 +1479,8 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
             SBN_CUDA_P(sbn_marginal_set_attrs());
             SBN_CUDA_P(sbn_count_set_attrs());
             SBN_CUDA_P(sbn_sample_set_attrs());
+            SBN_CUDA_P(sbn_argmax_set_attrs());
+            SBN_CUDA_P(sbn_batched_maxsum_set_attrs());
             done[device] = true;
         }
     }
@@ -1446,7 +1497,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
     if (rc != SBN_OK) return bail(rc);
     {
         // pairs multiply the tables of two steps on the host: needs the outputs of the table steps above
-        cudaError_t e = P->marginals || P->counts || P->sample ? cudaSuccess : sbn_pair_plan(P);
+        cudaError_t e = P->marginals || P->counts || P->sample || P->mpe ? cudaSuccess : sbn_pair_plan(P);
         if (e != cudaSuccess) return bail(fail(SBN_E_CUDA, "planning the paired steps failed: %s", cudaGetErrorString(e)));
     }
     *out = P;
@@ -1886,10 +1937,13 @@ int sbn_program_set_tables_f64(sbn_program *P, const double *tables, int64_t n_t
 
 constexpr int64_t kSampleGraphMinRows = 4096;
 
+// The host path of sample programs and (mpe = true, one draw, no seed) of MPE programs: the decoded codes of a
+// chunk are the drawn-code buffer, the per-row output is P(observed) (sample) or max log P(x, e) (MPE).
 static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws, uint64_t seed,
-                              int64_t row_base, uint8_t *out, void *prob, bool f64) {
+                              int64_t row_base, uint8_t *out, void *prob, bool f64, bool mpe = false) {
     if (!P) return fail(SBN_E_INVALID, "null program");
-    if (!P->sample) return fail(SBN_E_INVALID, "not a sample program (planner.build_sample_plan)");
+    if (mpe && !P->mpe) return fail(SBN_E_INVALID, "not an MPE program (planner.build_mpe_plan)");
+    if (!mpe && !P->sample) return fail(SBN_E_INVALID, "not a sample program (planner.build_sample_plan)");
     if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the sample call");
     if (n_rows <= 0) return fail(SBN_E_INVALID, "n_rows must be positive");
     if (n_draws <= 0 || n_draws > INT32_MAX) return fail(SBN_E_INVALID, "n_draws must be in 1 .. 2^31 - 1");
@@ -1927,8 +1981,13 @@ static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, 
         }
         P->drawn_bytes = bytes;
     }
-    if (!P->d_sample_args) SBN_CUDA(cudaMalloc(&P->d_sample_args, 4 * sizeof(uint32_t)));
+    if (!mpe && !P->d_sample_args) SBN_CUDA(cudaMalloc(&P->d_sample_args, 4 * sizeof(uint32_t)));
     const size_t elem = f64 ? 8 : 4;
+    const Slot &ps = P->slots[P->post_slot];  // MPE program: max log P(x, e), [1][ld] or one value for every row
+    auto issue = [&](int64_t rows) {
+        return mpe ? issue_mpe(P, P->d_ev, P->ld, rows, ld_drawn, P->stream)
+                   : issue_sample(P, P->d_ev, P->ld, rows, n_draws, ld_drawn, P->d_out, P->stream);
+    };
     for (int64_t r0 = 0; r0 < n_rows; r0 += cap) {
         const int64_t rows = std::min(cap, n_rows - r0);
         if (P->n_ev > 0)
@@ -1938,11 +1997,11 @@ static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, 
         const uint64_t first = static_cast<uint64_t>(row_base + r0);
         const uint32_t args[4] = {static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32), static_cast<uint32_t>(first),
                                   static_cast<uint32_t>(first >> 32)};
-        SBN_CUDA(cudaMemcpyAsync(P->d_sample_args, args, sizeof args, cudaMemcpyHostToDevice, P->stream));
+        if (!mpe) SBN_CUDA(cudaMemcpyAsync(P->d_sample_args, args, sizeof args, cudaMemcpyHostToDevice, P->stream));
         // a short chunk runs as plain launches: capturing and instantiating a graph costs more than it saves, and
         // the short runs of a pattern whose rows are scattered through a frame come in many lengths
         if (!P->use_graph || rows < kSampleGraphMinRows) {
-            const int rc = issue_sample(P, P->d_ev, P->ld, rows, n_draws, ld_drawn, P->d_out, P->stream);
+            const int rc = issue(rows);
             if (rc != SBN_OK) return rc;
         } else {
             // one graph per (chunk size, n_draws, drawn-code buffer)
@@ -1955,7 +2014,7 @@ static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, 
                 }
                 SBN_CUDA(cudaStreamBeginCapture(P->stream, cudaStreamCaptureModeRelaxed));
                 const int64_t before = P->launches;
-                const int rc = issue_sample(P, P->d_ev, P->ld, rows, n_draws, ld_drawn, P->d_out, P->stream);
+                const int rc = issue(rows);
                 cudaGraph_t graph = nullptr;
                 cudaError_t e = cudaStreamEndCapture(P->stream, &graph);
                 P->graph_launches = P->launches - before;
@@ -1978,10 +2037,14 @@ static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, 
             SBN_CUDA(cudaMemcpy2DAsync(out + r0, static_cast<size_t>(n_rows), P->d_drawn, static_cast<size_t>(ld_drawn),
                                        static_cast<size_t>(rows), static_cast<size_t>(P->n_sampled * n_draws),
                                        cudaMemcpyDeviceToHost, P->stream));
-        SBN_CUDA(cudaMemcpyAsync(static_cast<char *>(prob) + r0 * elem, P->d_out, static_cast<size_t>(rows) * elem,
-                                 cudaMemcpyDeviceToHost, P->stream));
+        if (!mpe || ps.batched)
+            SBN_CUDA(cudaMemcpyAsync(static_cast<char *>(prob) + r0 * elem, mpe ? ps.ptr : P->d_out,
+                                     static_cast<size_t>(rows) * elem, cudaMemcpyDeviceToHost, P->stream));
+        else if (r0 == 0)
+            SBN_CUDA(cudaMemcpyAsync(prob, ps.ptr, elem, cudaMemcpyDeviceToHost, P->stream));
     }
     SBN_CUDA(cudaStreamSynchronize(P->stream));
+    if (mpe && !ps.batched) std::fill(static_cast<float *>(prob) + 1, static_cast<float *>(prob) + n_rows, *static_cast<float *>(prob));
     return SBN_OK;
 }
 
@@ -1993,6 +2056,10 @@ int sbn_program_sample_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, in
 int sbn_program_sample_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws,
                                 uint64_t seed, int64_t row_base, uint8_t *out, double *prob) {
     return sample_host_common(P, ev, ld_ev, n_rows, n_draws, seed, row_base, out, prob, true);
+}
+
+int sbn_program_mpe_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, uint8_t *codes, float *log_prob) {
+    return sample_host_common(P, ev, ld_ev, n_rows, 1, 0, 0, codes, log_prob, false, true);
 }
 
 int sbn_program_profile(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out,

@@ -61,7 +61,8 @@ struct StepDesc {
     int64_t span = 0;          // entries of the family's count table
     int64_t soff_pos = -1, coff_pos = -1;
     // sample step of a sample program (kind 4, sbn_sample.cuh): the `ecards` variables are drawn (not summed
-    // out) into drawn-code rows q_offset ..; an input's `ev` terms may name drawn rows (col >= n_ev)
+    // out) into drawn-code rows q_offset ..; an input's `ev` terms may name drawn rows (col >= n_ev).
+    // An argmax step of an MPE program (kind 5, sbn_mpe.cuh) has the same layout and decodes instead.
 };
 struct Slot {
     bool batched;
@@ -89,7 +90,9 @@ struct sbn_program {
     const double *graph_partial = nullptr;  // the partial tables the captured counts graph writes
     int64_t partial_doubles = 0;
     bool sample = false;          // version-7 program: kind-4 steps draw codes, post_slot holds P(observed)
-    int n_sampled = 0;            // sample program: drawn-code rows (one per unobserved variable)
+    bool mpe = false;             // version-8 program: log tables, max-sum upward pass, kind-5 argmax steps,
+                                  // post_slot holds max log P(x, e); also uses n_sampled / d_drawn with one draw
+    int n_sampled = 0;            // sample / MPE program: drawn-code rows (one per unobserved variable)
     uint8_t *d_drawn = nullptr;   // sample program: drawn codes [n_sampled][n_draws][ld_drawn], then flags [ld_drawn]
     int64_t drawn_bytes = 0;
     uint32_t *d_sample_args = nullptr;  // seed lo, seed hi, row_base lo, row_base hi of the current chunk

@@ -145,6 +145,41 @@ __device__ __forceinline__ float4 sbn_mul4(float4 a, float4 b) {
     return make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w);
 }
 
+// Reduction policy of the batched and flat step kernels: how the inputs of one term combine (`times`,
+// starting from `one`) and how the terms of the eliminated states reduce (`plus`, starting from `zero`).
+// Sum-product is the default of every instantiation.  The policy is an optional trailing template argument
+// (SbnPolicy below), so that the sum-product kernels keep their names -- `sbn_step_batched<2, 4>`, as
+// profiles and tests/kernel_census.py read them -- and their code.  Max-sum (`out = max_x sum_i in_i`) runs the
+// log-domain programs of the most probable explanation (planner.build_mpe_plan): additions and maxima
+// only, so there is no FMA to contract and a CPU replay in float32 is bitwise equal.
+struct SbnSumProduct {
+    template <typename T> static __device__ __forceinline__ T one() { return T(1); }
+    template <typename T> static __device__ __forceinline__ T zero() { return T(0); }
+    template <typename T> static __device__ __forceinline__ T times(T a, T b) { return a * b; }
+    template <typename T> static __device__ __forceinline__ T plus(T a, T b) { return a + b; }
+    static __device__ __forceinline__ float4 times4(float4 a, float4 b) { return sbn_mul4(a, b); }
+};
+struct SbnMaxSum {
+    template <typename T> static __device__ __forceinline__ T one() { return T(0); }
+    template <typename T> static __device__ __forceinline__ T zero() { return static_cast<T>(__int_as_float(0xff800000)); }
+    template <typename T> static __device__ __forceinline__ T times(T a, T b) { return a + b; }
+    template <typename T> static __device__ __forceinline__ T plus(T a, T b) {
+        if constexpr (std::is_same<T, float>::value) return fmaxf(a, b);
+        else return fmax(a, b);
+    }
+    static __device__ __forceinline__ float4 times4(float4 a, float4 b) {
+        return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+    }
+};
+template <typename... R>
+struct SbnPolicy {
+    using type = SbnSumProduct;
+};
+template <typename R>
+struct SbnPolicy<R> {
+    using type = R;
+};
+
 // ------------------------------------------------------------- batched step kernel
 // The general fallback (more than 4 inputs, two inputs spanning the tile, tables too
 // large for shared memory, tile table too large): no limits beyond SBN_MAX_IN / SBN_MAX_AXES.
@@ -156,8 +191,10 @@ __device__ __forceinline__ float4 sbn_mul4(float4 a, float4 b) {
 // Thread = 4 consecutive rows (one float4) looping over the tile, one output per
 // iteration; the eliminated axis is reduced in-thread (strided float4 loads, each fully
 // coalesced across the warp); operands shared by consecutive outputs are L1 hits.
-template <int N_IN, int CX>
+// Policy: none (sum-product), or SbnMaxSum for the log-domain MPE programs.
+template <int N_IN, int CX, typename... Policy>
 __global__ void __launch_bounds__(SBN_THREADS) sbn_step_batched(const __grid_constant__ SbnStep p) {
+    using R = typename SbnPolicy<Policy...>::type;
     extern __shared__ __align__(16) float s_tab[];
     __shared__ __align__(8) uint64_t s_bar;
     sbn_pdl_entry();
@@ -236,9 +273,10 @@ __global__ void __launch_bounds__(SBN_THREADS) sbn_step_batched(const __grid_con
 #pragma unroll
         for (int i = 0; i < N_IN; ++i) e0[i] = off[i] + d1 * (p.n_axes > 1 ? p.in[i].stride[1] : 0);
         for (int d0 = 0; d0 < c0; ++d0) {
-            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+            const float z0 = R::template zero<float>(), o1 = R::template one<float>();
+            float4 acc = make_float4(z0, z0, z0, z0);
             auto term = [&](int x) {
-                float4 prod = make_float4(1.f, 1.f, 1.f, 1.f);
+                float4 prod = make_float4(o1, o1, o1, o1);
 #pragma unroll
                 for (int i = 0; i < N_IN; ++i) {
                     const int e = e0[i] + (p.zoff ? __ldg(p.zoff + i * cx + x) : x * p.in[i].sx);
@@ -253,12 +291,12 @@ __global__ void __launch_bounds__(SBN_THREADS) sbn_step_batched(const __grid_con
                         v = make_float4(__ldg(t + evo[i][0]), __ldg(t + evo[i][1]), __ldg(t + evo[i][2]),
                                         __ldg(t + evo[i][3]));
                     }
-                    prod = sbn_mul4(prod, v);
+                    prod = R::times4(prod, v);
                 }
-                acc.x += prod.x;
-                acc.y += prod.y;
-                acc.z += prod.z;
-                acc.w += prod.w;
+                acc.x = R::plus(acc.x, prod.x);
+                acc.y = R::plus(acc.y, prod.y);
+                acc.z = R::plus(acc.z, prod.z);
+                acc.w = R::plus(acc.w, prod.w);
             };
             if constexpr (CX > 0) {
 #pragma unroll
@@ -818,8 +856,10 @@ __global__ void __launch_bounds__(SBN_TILED_THREADS, (CX > 0 ? ((MX && (NU + NA 
 // eliminated axis reduced in-thread.  Evidence offsets are uniform (row 0).
 // T = float inside batched programs, double for single-event programs (those are
 // launch-latency bound, so they get the reference's own precision and range for free).
-template <typename T>
+// Policy: the reduction policy, as for sbn_step_batched.
+template <typename T, typename... Policy>
 __global__ void __launch_bounds__(256) sbn_step_flat(const __grid_constant__ SbnStep p) {
+    using R = typename SbnPolicy<Policy...>::type;
     sbn_pdl_entry();
     const int64_t o = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (o >= p.n_out) return;
@@ -843,15 +883,15 @@ __global__ void __launch_bounds__(256) sbn_step_flat(const __grid_constant__ Sbn
         for (int i = 0; i < SBN_MAX_IN; ++i)
             if (i < p.n_in) off[i] += d * p.in[i].stride[j];
     }
-    T acc = T(0);
+    T acc = R::template zero<T>();
     for (int x = 0; x < p.cx; ++x) {
-        T prod = T(1);
+        T prod = R::template one<T>();
 #pragma unroll
         for (int i = 0; i < SBN_MAX_IN; ++i)
             if (i < p.n_in)
-                prod *= __ldg(reinterpret_cast<const T *>(p.in[i].ptr) + off[i] +
-                              (p.zoff ? __ldg(p.zoff + i * p.cx + x) : x * p.in[i].sx));
-        acc += prod;
+                prod = R::times(prod, __ldg(reinterpret_cast<const T *>(p.in[i].ptr) + off[i] +
+                                            (p.zoff ? __ldg(p.zoff + i * p.cx + x) : x * p.in[i].sx)));
+        acc = R::plus(acc, prod);
     }
     reinterpret_cast<T *>(p.out)[o] = acc;
 }

@@ -65,12 +65,11 @@ struct SbnSample {
     SbnSampleIn in[SBN_MAX_IN];
 };
 
-// One (row b, draw d) of the launch below
+// The operands of one (row b, draw d) of a sample or argmax step (sbn_mpe.cuh): entry e of operand i is
+// src[i][e * mul[i]], the row's observed codes and the codes decoded before this step already gathered.
 template <typename T>
-__device__ __forceinline__ void sbn_sample_draw(const SbnSample &p, const float *s_tab, int64_t b, int d) {
-    // operand i, entry e, this (row, draw):  src[i][e * mul[i]]
-    const T *src[SBN_MAX_IN];
-    int64_t mul[SBN_MAX_IN];
+__device__ __forceinline__ void sbn_decode_operands(const SbnSample &p, const float *s_tab, int64_t b, int d,
+                                                    const T *(&src)[SBN_MAX_IN], int64_t (&mul)[SBN_MAX_IN]) {
 #pragma unroll
     for (int i = 0; i < SBN_MAX_IN; ++i) {
         src[i] = nullptr;
@@ -94,6 +93,35 @@ __device__ __forceinline__ void sbn_sample_draw(const SbnSample &p, const float 
             }
         }
     }
+}
+
+// Stage the launch's tables in shared memory by bulk-TMA (sample and argmax steps).  Returns whether the
+// CTA has to wait on `bar` before it reads them.
+__device__ __forceinline__ bool sbn_decode_stage(const SbnSample &p, float *s_tab, uint64_t *bar) {
+    const bool staged = p.smem_floats > 0;
+    if (staged) {
+        if (threadIdx.x == 0) {
+            sbn_mbar_init(bar, 1);
+            sbn_fence_mbar_init();
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            sbn_mbar_expect_tx(bar, static_cast<uint32_t>(p.smem_floats) * 4u);
+            for (int i = 0; i < p.n_in; ++i)
+                if (p.in[i].smem_off >= 0)
+                    sbn_tma_bulk_g2s(s_tab + p.in[i].smem_off, p.in[i].ptr, static_cast<uint32_t>(p.in[i].stage_floats) * 4u,
+                                     bar);
+        }
+    }
+    return staged;
+}
+
+// One (row b, draw d) of the launch below
+template <typename T>
+__device__ __forceinline__ void sbn_sample_draw(const SbnSample &p, const float *s_tab, int64_t b, int d) {
+    const T *src[SBN_MAX_IN];
+    int64_t mul[SBN_MAX_IN];
+    sbn_decode_operands<T>(p, s_tab, b, d, src, mul);
     const int n_in = p.n_in, cz = p.cz;
     auto weight = [&](int z) {
         T w = T(1);
@@ -139,22 +167,7 @@ __global__ void __launch_bounds__(SBN_SAMPLE_THREADS) sbn_sample_step(const __gr
     extern __shared__ __align__(16) float s_tab[];
     __shared__ __align__(8) uint64_t s_bar;
     sbn_pdl_entry();
-
-    const bool staged = p.smem_floats > 0;
-    if (staged) {
-        if (threadIdx.x == 0) {
-            sbn_mbar_init(&s_bar, 1);
-            sbn_fence_mbar_init();
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            sbn_mbar_expect_tx(&s_bar, static_cast<uint32_t>(p.smem_floats) * 4u);
-            for (int i = 0; i < p.n_in; ++i)
-                if (p.in[i].smem_off >= 0)
-                    sbn_tma_bulk_g2s(s_tab + p.in[i].smem_off, p.in[i].ptr, static_cast<uint32_t>(p.in[i].stage_floats) * 4u,
-                                     &s_bar);
-        }
-    }
+    const bool staged = sbn_decode_stage(p, s_tab, &s_bar);
 
     const int64_t b = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     const bool live = b < p.n_rows;

@@ -43,6 +43,41 @@ cudaError_t sbn_batched_launch(const SbnStep &q, int64_t grid, cudaStream_t stre
     return cudaErrorInvalidValue;
 }
 
+// The max-sum instantiations (MPE programs): the generic eliminated-state loop only
+namespace {
+template <int N_IN>
+cudaError_t launch_batched_maxsum_n(const SbnStep &q, int64_t grid, cudaStream_t stream) {
+    sbn_launch(sbn_step_batched<N_IN, 0, SbnMaxSum>, dim3(static_cast<unsigned>(grid)), dim3(SBN_THREADS),
+               static_cast<size_t>(q.smem_floats) * 4, stream, q);
+    return cudaGetLastError();
+}
+}  // namespace
+
+cudaError_t sbn_batched_maxsum_launch(const SbnStep &q, int64_t grid, cudaStream_t stream) {
+    switch (q.n_in) {
+        case 1: return launch_batched_maxsum_n<1>(q, grid, stream);
+        case 2: return launch_batched_maxsum_n<2>(q, grid, stream);
+        case 3: return launch_batched_maxsum_n<3>(q, grid, stream);
+        case 4: return launch_batched_maxsum_n<4>(q, grid, stream);
+        case 5: return launch_batched_maxsum_n<5>(q, grid, stream);
+        case 6: return launch_batched_maxsum_n<6>(q, grid, stream);
+        case 7: return launch_batched_maxsum_n<7>(q, grid, stream);
+        case 8: return launch_batched_maxsum_n<8>(q, grid, stream);
+    }
+    return cudaErrorInvalidValue;
+}
+
+cudaError_t sbn_batched_maxsum_set_attrs() {
+    cudaError_t e = cudaSuccess;
+#define SBN_M(N)                                                                                                   \
+    if (e == cudaSuccess)                                                                                          \
+        e = cudaFuncSetAttribute(sbn_step_batched<N, 0, SbnMaxSum>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                 SBN_SMEM_BUDGET);
+    SBN_M(1) SBN_M(2) SBN_M(3) SBN_M(4) SBN_M(5) SBN_M(6) SBN_M(7) SBN_M(8)
+#undef SBN_M
+    return e;
+}
+
 cudaError_t sbn_batched_set_attrs() {
     cudaError_t e = set_smem_attr_n<1>();
     if (e == cudaSuccess) e = set_smem_attr_n<2>();

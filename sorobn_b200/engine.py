@@ -16,7 +16,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libsorobn_
 _lib = None
 
 SBN_OK = 0
-ABI_VERSION = 11
+ABI_VERSION = 12
 
 
 class EngineError(RuntimeError):
@@ -73,6 +73,8 @@ def load():
     for name in ("sbn_program_sample_host", "sbn_program_sample_host_f64"):
         getattr(lib, name).restype = i32
         getattr(lib, name).argtypes = [vp, vp, i64, i64, i64, c.c_uint64, i64, vp, vp]
+    lib.sbn_program_mpe_host.restype = i32
+    lib.sbn_program_mpe_host.argtypes = [vp, vp, i64, i64, vp, vp]
     lib.sbn_program_destroy.restype = None
     lib.sbn_program_destroy.argtypes = [vp]
     lib.sbn_program_reserve.restype = i32
@@ -116,7 +118,7 @@ EXPORTS = (
     "sbn_program_run_host_f64", "sbn_program_evidence_host", "sbn_program_evidence_host_f64", "sbn_program_destroy",
     "sbn_program_reserve", "sbn_program_run_host", "sbn_program_run_device", "sbn_program_profile",
     "sbn_program_step_roles", "sbn_program_counts_host", "sbn_program_counts_host_f64", "sbn_program_set_tables",
-    "sbn_program_set_tables_f64", "sbn_program_sample_host", "sbn_program_sample_host_f64",
+    "sbn_program_set_tables_f64", "sbn_program_sample_host", "sbn_program_sample_host_f64", "sbn_program_mpe_host",
     "sbn_program_info", "sbn_program_set_graph", "sbn_program_set_tiled", "sbn_gibbs_create", "sbn_gibbs_run_host",
     "sbn_sampler_run_host", "sbn_gibbs_conditional", "sbn_gibbs_destroy", "sbn_host_alloc", "sbn_host_free",
 )
@@ -288,6 +290,19 @@ class Program:
         _check(fn(self._h, codes.ctypes.data if self.n_ev else None, n_rows, n_rows, n_draws,
                   int(seed) & (2**64 - 1), int(row_base), out.ctypes.data, prob.ctypes.data))
         return out, prob
+
+    def mpe(self, codes: np.ndarray, n_rows: int):
+        """MPE programs (planner.build_mpe_plan): (decoded codes uint8 [n_decoded, n_rows] in the order of
+        `plan.sampled`, max log P(x, e) float32 [n_rows], -inf for a row of probability zero), host path."""
+        n_rows = int(n_rows)
+        codes = np.ascontiguousarray(codes, dtype=np.uint8)
+        if self.n_ev and codes.shape != (self.n_ev, n_rows):
+            raise ValueError(f"evidence codes have shape {codes.shape}, expected {(self.n_ev, n_rows)}")
+        out = np.empty((len(self.plan.sampled), n_rows), dtype=np.uint8)
+        log_prob = np.empty(n_rows, dtype=np.float32)
+        _check(load().sbn_program_mpe_host(self._h, codes.ctypes.data if self.n_ev else None, n_rows, n_rows,
+                                           out.ctypes.data, log_prob.ctypes.data))
+        return out, log_prob
 
     def run_device(self, d_ev: int, ld_ev: int, n_rows: int, d_out: int, ld_out: int, stream: int = 0):
         """Device path: raw device pointers, asynchronous on `stream`."""

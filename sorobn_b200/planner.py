@@ -100,6 +100,24 @@ earlier step (col >= n_ev): the bucket's separator, which lies above it in the b
 batched input's gathered offset is multiplied by the row pitch.  The step writes the codes of its
 variables to drawn rows `d_first .. d_first + n_x - 1`; steps write consecutive rows, so the
 sampled variables are numbered in drawing order.  A sample step writes no slot.
+
+MPE programs (`build_mpe_plan`, VERSION 8) find the most probable explanation of every row: the joint
+state x* of every unobserved variable that maximises P(x, e).  They are sample programs in the log
+domain, with an argmax step (kind 5) in place of every sample step:
+
+    header : MAGIC 8 1 n_ev n_tables n_slots n_steps 1 p_slot p_batched n_decoded 0
+    kind 5 : the words of kind 4
+
+The table blob holds log(table) (the float64 logs cast to float32; a zero entry is -inf), and every
+kind-0 / kind-1 step means max-sum: `out = max_x sum_i in_i[...]`, or `sum_i in_i[...]` for a
+product-only step.  `p_slot` holds max log P(x, e) of every row, the sum of the upward pass's leftover
+scalars (-inf: the observed cells are impossible).  A kind-5 step decodes its bucket's variables given
+the decoded separator: the first joint state z (first variable fastest) with the largest
+
+    w(z) = sum_i in_i[ sum_x X_x * strides_i[x] + sum_t code_t(row) * stride_t ].
+
+Logs, because the maximum is a product of one entry of every CPT: it shrinks with the network and with
+every observed cell, past the float32 range of the sum-product programs, where its log cannot underflow.
 """
 from __future__ import annotations
 
@@ -135,6 +153,8 @@ KIND_SAMPLE = 4  # draw one bucket's eliminated variables given the drawn separa
 VERSION_SAMPLE = 7
 SAMPLE_MAX_CARD = 255  # a sampled variable's states (its codes are uint8)
 SAMPLE_MAX_TERMS = 16  # gathered (col stride card) terms per input of a sample step (csrc: SBN_SAMPLE_MAX_TERMS)
+KIND_ARGMAX = 5  # decode one bucket's eliminated variables given the decoded separator (MPE programs only)
+VERSION_MPE = 8
 HEADER_WORDS = 12
 
 
@@ -194,10 +214,10 @@ class Step:
     ecards: tuple
     out_slot: int = -1
     q_offset: int = -1  # KIND_MARGINAL: first posterior entry of the target's segment; KIND_COUNT: c_offset;
-    # KIND_SAMPLE: first drawn-code row it writes
+    # KIND_SAMPLE / KIND_ARGMAX: first drawn-code row it writes
     key: tuple = ()  # KIND_COUNT: ((ev_col, stride, card), ...) of the observed family members
     cstrides: tuple = ()  # KIND_COUNT: count-table stride of every output axis
-    norm: object = None  # KIND_COUNT / KIND_SAMPLE: the factor holding P(observed) (the header's p_slot)
+    norm: object = None  # KIND_COUNT / KIND_SAMPLE / KIND_ARGMAX: the factor in the header's p_slot
 
     @property
     def cx(self):
@@ -225,21 +245,23 @@ class Plan:
     count_offsets: list = None  # counts plans: first count-table entry of every var id's family
     table_axes: list = None  # var ids of every shipped table's axes, outermost first (refresh_tables)
     table_scopes: list = None  # the CPT scope [*parents, v] every table was transposed from
-    sampled: tuple = ()  # sample plans: the var id of every drawn-code row, in drawing order
+    sampled: tuple = ()  # sample / MPE plans: the var id of every drawn (decoded) code row, in drawing order
 
     # ---- cost model (DESIGN.md "algorithmic bytes") -------------------------------
     def bytes_per_row(self, n_draws=1):
         """Algorithmic HBM bytes per evidence row: every batched step reads each
         batched input once and writes its output once (fp32), plus the evidence
         codes in and the posterior out.  A sample step reads, per draw, the part of each
-        batched input its drawn separator selects and writes its codes (`n_draws` draws)."""
+        batched input its drawn separator selects and writes its codes (`n_draws` draws); an
+        argmax step counts as a sample step with one draw."""
         total = 0
         for st in self.steps:
-            if st.kind == KIND_SAMPLE:
+            if st.kind in (KIND_SAMPLE, KIND_ARGMAX):
+                nd = n_draws if st.kind == KIND_SAMPLE else 1
                 for f, es, _ in st.inputs:
                     if f.batched:
-                        total += 4 * n_draws * int(np.prod([c for c, s in zip(st.ecards, es) if s], dtype=np.int64))
-                total += n_draws * len(st.elims)
+                        total += 4 * nd * int(np.prod([c for c, s in zip(st.ecards, es) if s], dtype=np.int64))
+                total += nd * len(st.elims)
                 continue
             if st.kind not in (KIND_BATCHED, KIND_MARGINAL, KIND_COUNT):
                 continue
@@ -254,8 +276,8 @@ class Plan:
             # normalise: read unnormalised posterior, write posterior (a marginals program's
             # readouts write their segments normalised, counted above)
             total += 8 * self.Q
-        elif self.version in (VERSION_COUNTS, VERSION_SAMPLE):
-            total += 4  # P(observed) out
+        elif self.version in (VERSION_COUNTS, VERSION_SAMPLE, VERSION_MPE):
+            total += 4  # P(observed) (max log P(x, e)) out
         total += len(self.evidence)  # uint8 codes
         return total
 
@@ -372,7 +394,18 @@ def build_sample_plan(net: CompiledNet, evidence, order=None, max_in=MAX_IN, lif
     evidence = tuple(evidence)
     hidden = tuple(v for v in range(len(net.names)) if v not in set(evidence))
     return _build(net, (), evidence, MODE_BATCHED, order, max_in, False, lift_evidence, True, fuse_elims, hidden,
-                  sample=True)
+                  sample=KIND_SAMPLE)
+
+
+def build_mpe_plan(net: CompiledNet, evidence, order=None, max_in=MAX_IN, lift_evidence=True, fuse_elims=None) -> Plan:
+    """Plan the most probable explanation of every row (a version-8 program, see the module docstring):
+    the sample plan's steps in the log domain, the upward pass max-sum, then one argmax step per bucket,
+    top-down.  Every variable that is not in `evidence` is decoded -- barren nodes too: their CPT rows
+    do not max to 1 -- and `Plan.sampled` names the variable of every decoded-code row."""
+    evidence = tuple(evidence)
+    hidden = tuple(v for v in range(len(net.names)) if v not in set(evidence))
+    return _build(net, (), evidence, MODE_BATCHED, order, max_in, False, lift_evidence, True, fuse_elims, hidden,
+                  sample=KIND_ARGMAX)
 
 
 def count_layout(net: CompiledNet):
@@ -401,7 +434,7 @@ def refresh_tables(plan: Plan, cpts):
 
 
 def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evidence, allow_empty_query, fuse_elims,
-           targets, counts=False, sample=False):
+           targets, counts=False, sample=None):
     if merge_sum_outs is None:
         merge_sum_outs = os.environ.get("SOROBN_B200_MERGE", "0") == "1"
     if fuse_elims is None:
@@ -651,9 +684,9 @@ def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evide
         if targets is not None:
             buckets.append((bucket_factors, tuple(elims), set().union(*[f.vars for f in bucket_factors]), factors[-1]))
 
-    if sample:
+    if sample is not None:
         return _sample_passes(net, evidence, order, max_in, buckets, factors, steps, tables, table_arrays, table_axes,
-                              emit, combine_tables, axis_order, fsize)
+                              emit, combine_tables, axis_order, fsize, sample)
     if counts:
         return _counts_passes(net, evidence, mode, order, max_in, buckets, factors, steps, tables, table_arrays,
                               table_axes, emit, combine_tables, axis_order, fsize)
@@ -803,13 +836,17 @@ def _counts_passes(net, evidence, mode, order, max_in, buckets, leftovers, steps
 
 
 def _sample_passes(net, evidence, order, max_in, buckets, leftovers, steps, tables, table_arrays, table_axes, emit,
-                   combine_tables, axis_order, fsize):
-    """Sample steps of a sample plan (DESIGN.md "Posterior samples").
+                   combine_tables, axis_order, fsize, kind=KIND_SAMPLE):
+    """Sample steps of a sample plan (DESIGN.md "Posterior samples"), or argmax steps of an MPE plan
+    (`kind` KIND_ARGMAX, DESIGN.md "Most probable explanation").
 
     Bucket k eliminated X_k and sent lambda_k(S_k) to a later bucket.  Walking the buckets in reverse
     elimination order, every variable of S_k has been drawn when bucket k is reached, and
         P(X_k | S_k = drawn, e) is proportional to prod_{f in F_k} f(X_k, S_k = drawn, e).
-    P(observed) is the product of the upward pass's leftover scalars, as in a counts plan."""
+    P(observed) is the product of the upward pass's leftover scalars, as in a counts plan.  In the log
+    domain of an MPE plan the same steps mean max-sum: lambda_k(S_k) = max_{X_k} sum_{f in F_k} log f,
+    the leftovers sum to max log P(x, e), and the argmax of sum_{f in F_k} log f(X_k, S_k = decoded, e)
+    is X_k's state in the maximising assignment."""
     card = net.card
     n_ev = len(evidence)
     _, fold = _downward(net, max_in, buckets, leftovers, (), emit, combine_tables, axis_order, fsize)
@@ -838,14 +875,15 @@ def _sample_passes(net, evidence, order, max_in, buckets, leftovers, steps, tabl
                                  f"or drawn variables; a sample step gathers at most {SAMPLE_MAX_TERMS}")
             g = _Factor(f.is_slot, f.buf, f.vars, f.strides, terms, f.batched)
             ins.append((g, tuple(pos.get(x, 0) for x in X), ()))
-        steps.append(Step(KIND_SAMPLE, ins, -1, (), (), tuple(X), tuple(int(card[x]) for x in X),
+        steps.append(Step(kind, ins, -1, (), (), tuple(X), tuple(int(card[x]) for x in X),
                           q_offset=len(drawn), norm=prob))
         for x in X:
             drawn[x] = len(drawn)
 
     slots, where = _assign_slots_shared(steps, keep_unbatched=True)
     plan = Plan(mode=MODE_BATCHED, query=(), evidence=evidence, order=list(order), tables=tables, slots=slots,
-                steps=steps, post_slot=where[prob.buf], Q=1, version=VERSION_SAMPLE,
+                steps=steps, post_slot=where[prob.buf], Q=1,
+                version=VERSION_SAMPLE if kind == KIND_SAMPLE else VERSION_MPE,
                 table_axes=[list(a) for a in table_axes], table_scopes=[net.scope(v) for v in tables],
                 sampled=tuple(sorted(drawn, key=drawn.get)))
     plan._card = card
@@ -969,7 +1007,7 @@ def _assign_slots_shared(steps, keep_unbatched):
             slots[phys][2] = not (keep_unbatched and not slots[phys][0])
 
     for st in steps:
-        writes_slot = st.kind not in (KIND_MARGINAL, KIND_COUNT, KIND_SAMPLE)
+        writes_slot = st.kind not in (KIND_MARGINAL, KIND_COUNT, KIND_SAMPLE, KIND_ARGMAX)
         if writes_slot:
             size = int(np.prod(st.cards, dtype=np.int64)) if st.cards else 1
             st.out_slot = alloc(st.kind == KIND_BATCHED, size)
@@ -1188,15 +1226,19 @@ def _serialise(plan: Plan, table_arrays):
     # float64 copy: only the CPU checker (oracle/program_interp.py) reads it, to
     # separate planner errors from fp32 rounding; the device gets the fp32 blob
     plan.table_blob64, offsets = _blobs(table_arrays)
+    if plan.version == VERSION_MPE:
+        # max-sum programs work on logs; a zero entry (and the padding) is -inf
+        with np.errstate(divide="ignore"):
+            plan.table_blob64 = np.log(plan.table_blob64)
     plan.table_blob = plan.table_blob64.astype(np.float32)
     plan.table_offsets = offsets
 
     extra = [0, 0]
-    if plan.version in (VERSION, VERSION_COUNTS, VERSION_SAMPLE):
+    if plan.version in (VERSION, VERSION_COUNTS, VERSION_SAMPLE, VERSION_MPE):
         post = [plan.post_slot, int(plan.slots[plan.post_slot][0])]
         if plan.version == VERSION_COUNTS:
             extra = [plan.n_counts, 0]
-        elif plan.version == VERSION_SAMPLE:
+        elif plan.version in (VERSION_SAMPLE, VERSION_MPE):
             extra = [len(plan.sampled), 0]
     else:
         post = [-1, 0]  # the readouts write the posterior themselves
@@ -1216,7 +1258,7 @@ def _serialise(plan: Plan, table_arrays):
             for col, s, c in st.key:
                 w += [col, s, c]
             w += list(st.cstrides)
-        elif st.kind == KIND_SAMPLE:
+        elif st.kind in (KIND_SAMPLE, KIND_ARGMAX):
             w.append(st.q_offset)
         w += list(st.cards)
         w += list(st.ecards)
