@@ -57,6 +57,7 @@ constexpr int kVersionCounts = 6;     // planner.build_counts_plan: kind-3 count
 constexpr int kVersionSample = 7;     // planner.build_sample_plan: kind-4 sample steps, P(observed) in the posterior slot
 constexpr int kVersionMpe = 8;        // planner.build_mpe_plan: log tables, max-sum steps, kind-5 argmax steps,
                                       // max log P(x, e) in the posterior slot
+static_assert(kVersionMpe - kVersion == kMpe, "one program kind per header version, in order");
 constexpr int64_t kMarginalZoffMax = 1 << 24;  // int32 words of one readout's joint-state offset table
 constexpr int kMaxElim = 3;
 constexpr int kMaxZ = 256;
@@ -69,14 +70,12 @@ namespace {
 int parse(sbn_program *P, const int32_t *w, int64_t n) {
     if (n < kHeaderWords) return fail(SBN_E_INVALID, "program shorter than its header");
     if (w[0] != kMagic) return fail(SBN_E_INVALID, "bad program magic 0x%x", w[0]);
-    if (w[1] != kVersion && w[1] != kVersionMarginals && w[1] != kVersionCounts && w[1] != kVersionSample &&
-        w[1] != kVersionMpe)
+    if (w[1] < kVersion || w[1] > kVersionMpe)
         return fail(SBN_E_INVALID, "program version %d, engine expects %d, %d, %d, %d or %d", w[1], kVersion,
                     kVersionMarginals, kVersionCounts, kVersionSample, kVersionMpe);
-    P->marginals = w[1] == kVersionMarginals;
-    P->counts = w[1] == kVersionCounts;
-    P->sample = w[1] == kVersionSample;
-    P->mpe = w[1] == kVersionMpe;
+    P->kind = static_cast<ProgramKind>(w[1] - kVersion);
+    const bool marginals = P->kind == kMarginals, counts = P->kind == kCounts, mpe = P->kind == kMpe;
+    const bool decodes = P->kind == kSample || mpe;  // sample and MPE programs share the words of their last steps
     P->mode = w[2];
     P->n_ev = w[3];
     const int n_tables = w[4], n_slots = w[5], n_steps = w[6];
@@ -86,19 +85,19 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
     if (P->mode != 0 && P->mode != 1) return fail(SBN_E_INVALID, "bad mode %d", P->mode);
     if (P->n_ev < 0 || n_tables < 0 || n_slots <= 0 || n_steps <= 0 || P->Q <= 0)
         return fail(SBN_E_INVALID, "bad header counts");
-    if (P->counts) {
+    if (counts) {
         P->n_counts = w[10];
         if (P->Q != 1 || P->n_counts <= 0) return fail(SBN_E_INVALID, "bad counts header");
     }
-    if (P->sample || P->mpe) {
+    if (decodes) {
         P->n_sampled = w[10];
         if (P->Q != 1 || P->mode != 1 || P->n_sampled < 0)
-            return fail(SBN_E_INVALID, P->mpe ? "bad MPE header" : "bad sample header");
+            return fail(SBN_E_INVALID, mpe ? "bad MPE header" : "bad sample header");
     }
     // sample program: kind-4 steps draw codes; MPE program: kind-5 steps decode them (same words)
-    const int decode_kind = P->mpe ? 5 : 4;
+    const int decode_kind = mpe ? 5 : 4;
     int n_drawn = 0;  // sample / MPE program: drawn-code rows written by the sample / argmax steps so far
-    if (P->marginals ? (P->post_slot != -1 || P->post_batched != 0) : (P->post_slot < 0 || P->post_slot >= n_slots))
+    if (marginals ? (P->post_slot != -1 || P->post_batched != 0) : (P->post_slot < 0 || P->post_slot >= n_slots))
         return fail(SBN_E_INVALID, "post slot out of range");
     int64_t p = kHeaderWords;
     auto need = [&](int64_t k) { return p + k <= n; };
@@ -118,9 +117,9 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         if (batched && P->mode == 0) return fail(SBN_E_INVALID, "batched slot in a flat program");
         P->slots.push_back({batched != 0, size, round_up(size, 4), nullptr});
     }
-    if (!P->marginals && ((P->slots[P->post_slot].batched ? 1 : 0) != P->post_batched || P->slots[P->post_slot].size < P->Q))
+    if (!marginals && ((P->slots[P->post_slot].batched ? 1 : 0) != P->post_batched || P->slots[P->post_slot].size < P->Q))
         return fail(SBN_E_INVALID, "posterior slot mismatch");
-    std::vector<int> written(P->marginals ? P->Q : 0, 0);  // posterior entries written by the readouts
+    std::vector<int> written(marginals ? P->Q : 0, 0);  // posterior entries written by the readouts
     for (int s = 0; s < n_steps; ++s) {
         if (!need(5)) return fail(SBN_E_INVALID, "truncated step %d", s);
         StepDesc st;
@@ -133,8 +132,8 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         p += 5;
         const bool readout = st.kind == 2;
         const bool count = st.kind == 3;
-        const bool draw = (st.kind == 4 && P->sample) || (st.kind == 5 && P->mpe);
-        if (st.kind != 0 && st.kind != 1 && !(readout && P->marginals) && !(count && P->counts) && !draw)
+        const bool draw = decodes && st.kind == decode_kind;
+        if (st.kind != 0 && st.kind != 1 && !(readout && marginals) && !(count && counts) && !draw)
             return fail(SBN_E_INVALID, "step %d: bad kind", s);
         if (draw) {
             // the drawn variables are the step's `n_elim` axes; they fill the next drawn-code rows
@@ -142,7 +141,7 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             st.q_offset = w[p++];
             if (st.out_slot != -1 || n_axes != 0 || n_elim < 1 || n_elim > SBN_SAMPLE_MAX_X || st.q_offset != n_drawn ||
                 n_drawn + n_elim > P->n_sampled)
-                return fail(SBN_E_INVALID, P->mpe ? "step %d: bad argmax step" : "step %d: bad sample step", s);
+                return fail(SBN_E_INVALID, mpe ? "step %d: bad argmax step" : "step %d: bad sample step", s);
         }
         if (count) {
             // c_offset, the observed members' gathers and the count-table strides of the output axes
@@ -300,7 +299,7 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             if (st.kind == 0 && ++writes[st.out_slot] > 1)
                 return fail(SBN_E_INVALID, "unbatched slot %d is written twice in a batched program", st.out_slot);
     }
-    if (P->sample || P->mpe) {
+    if (decodes) {
         // every drawn-code row is written; the sample / argmax steps run last, after the last write of the
         // posterior slot (P(observed), or max log P(x, e))
         if (n_drawn != P->n_sampled) return fail(SBN_E_INVALID, "%d of %d drawn-code rows are written", n_drawn, P->n_sampled);
@@ -314,10 +313,10 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             }
         }
         if (writer < 0) return fail(SBN_E_INVALID, "P(observed) is not written before the sample steps");
-    } else if (P->marginals) {
+    } else if (marginals) {
         for (int q = 0; q < P->Q; ++q)
             if (written[q] != 1) return fail(SBN_E_INVALID, "posterior entry %d is written %d times", q, written[q]);
-    } else if (P->counts) {
+    } else if (counts) {
         // P(observed) is written before the first count step and not overwritten before the last one
         int first = -1, last = -1, writer = -1;
         for (size_t i = 0; i < P->steps.size(); ++i) {
@@ -560,7 +559,7 @@ void plan_tiles(sbn_program *P, std::vector<int32_t> *words) {
     for (StepDesc &st : P->steps) {
         st.tile = 0;
         // an MPE program's steps run on the max-sum kernels only (launch_step), which have no tiled variant
-        if (st.kind != 1 || P->mpe || st.in.size() > static_cast<size_t>(kTiledMaxIn)) continue;
+        if (st.kind != 1 || P->kind == kMpe || st.in.size() > static_cast<size_t>(kTiledMaxIn)) continue;
 
         int64_t smem = 0;
         for (const InDesc &in : st.in)
@@ -664,15 +663,19 @@ void plan_tiles(sbn_program *P, std::vector<int32_t> *words) {
     }
 }
 
+void drop_graph(CachedGraph &g) {
+    if (g.exec) cudaGraphExecDestroy(g.exec);
+    g.exec = nullptr;
+}
+
+void drop_graphs(sbn_program *P) {
+    // captured launches embed the kernel variants and pointers of the moment they were captured
+    drop_graph(P->graph);
+    drop_graph(P->pipe_graph);
+}
+
 void free_scratch(sbn_program *P) {
-    if (P->exec) {
-        cudaGraphExecDestroy(P->exec);
-        P->exec = nullptr;
-    }
-    if (P->pipe_exec) {
-        cudaGraphExecDestroy(P->pipe_exec);
-        P->pipe_exec = nullptr;
-    }
+    drop_graphs(P);
     cudaFree(P->d_arena);
     cudaFree(P->d_ev);
     cudaFree(P->d_out);
@@ -851,8 +854,8 @@ cudaError_t launch_maxsum(const StepDesc &st, const SbnStep &q, cudaStream_t str
 
 cudaError_t launch_step(sbn_program *P, const StepDesc &st, const SbnStep &q, cudaStream_t stream) {
     P->launches++;
-    if (P->mpe) return launch_maxsum(st, q, stream);
-    if (st.kind == 1 && q.tile_off != nullptr && !P->marginals && sbn_tma_eligible(P, st))
+    if (P->kind == kMpe) return launch_maxsum(st, q, stream);
+    if (st.kind == 1 && q.tile_off != nullptr && P->kind != kMarginals && sbn_tma_eligible(P, st))
         return sbn_tma_launch(P, st, q.ev, q.ld_ev, q.n_rows, stream);
     if (st.kind == 1 && q.tile_off != nullptr && sbn_join_rows(P, st, q) > 0) return sbn_join_launch(P, st, q, stream);
     if (st.kind == 1 && q.tile_off != nullptr) {
@@ -889,6 +892,41 @@ cudaError_t launch_step(sbn_program *P, const StepDesc &st, const SbnStep &q, cu
     return sbn_batched_launch(q, grid, stream);
 }
 
+// The operands of a readout, count, sample or argmax step (SbnMargIn, SbnCountIn, SbnSampleIn): pointer, batched
+// flag and (col stride card) gathers.  Tables are staged like the step kernels' (bulk-TMA, 16-byte aligned and
+// sized), float programs only.  Returns the floats of shared memory they take.
+template <typename In>
+int64_t bind_operands(const sbn_program *P, const StepDesc &st, In *ins) {
+    const int64_t elem = P->f64 ? 8 : 4;
+    int64_t smem = 0;
+    for (size_t i = 0; i < st.in.size(); ++i) {
+        const InDesc &in = st.in[i];
+        In &d = ins[i];
+        int64_t padded;
+        if (in.is_slot) {
+            d.ptr = P->slots[in.id].ptr;
+            padded = P->slots[in.id].padded;
+        } else {
+            d.ptr = reinterpret_cast<const char *>(P->d_tables) + P->tables[in.id].first * elem;
+            padded = P->table_padded[in.id];
+        }
+        d.batched = in.batched ? 1 : 0;
+        d.n_ev = static_cast<int32_t>(in.ev.size());
+        for (size_t k = 0; k < in.ev.size(); ++k) {
+            d.ev_col[k] = in.ev[k].col;
+            d.ev_stride[k] = in.ev[k].stride;
+            d.ev_card[k] = in.ev[k].card;
+        }
+        d.smem_off = -1;
+        if (!P->f64 && !in.batched && (smem + padded) * 4 <= SBN_SMEM_BUDGET) {
+            d.smem_off = static_cast<int32_t>(smem);
+            d.stage_floats = static_cast<int32_t>(padded);
+            smem += padded;
+        }
+    }
+    return smem;
+}
+
 // Readout of one target (kind 2): its segment of the posterior, normalised, for rows 0 .. n_rows - 1.
 cudaError_t launch_marginal(sbn_program *P, const StepDesc &st, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, float *d_out,
                             int64_t ld_out, cudaStream_t stream) {
@@ -908,34 +946,8 @@ cudaError_t launch_marginal(sbn_program *P, const StepDesc &st, const uint8_t *e
     m.n_common = st.n_common;
     m.card = st.cards[0];
     m.cz = st.cx;
-    int64_t smem = 0;
-    for (size_t i = 0; i < st.in.size(); ++i) {
-        const InDesc &in = st.in[i];
-        SbnMargIn &d = m.in[i];
-        int64_t padded;
-        if (in.is_slot) {
-            d.ptr = P->slots[in.id].ptr;
-            padded = P->slots[in.id].padded;
-        } else {
-            d.ptr = reinterpret_cast<const char *>(P->d_tables) + P->tables[in.id].first * static_cast<int64_t>(elem);
-            padded = P->table_padded[in.id];
-        }
-        d.batched = in.batched ? 1 : 0;
-        d.ts = in.strides[0];
-        d.n_ev = static_cast<int32_t>(in.ev.size());
-        for (size_t k = 0; k < in.ev.size(); ++k) {
-            d.ev_col[k] = in.ev[k].col;
-            d.ev_stride[k] = in.ev[k].stride;
-            d.ev_card[k] = in.ev[k].card;
-        }
-        d.smem_off = -1;
-        // tables are staged like the step kernels' (bulk-TMA, 16-byte aligned and sized); float programs only
-        if (!P->f64 && !in.batched && (smem + padded) * 4 <= SBN_SMEM_BUDGET) {
-            d.smem_off = static_cast<int32_t>(smem);
-            d.stage_floats = static_cast<int32_t>(padded);
-            smem += padded;
-        }
-    }
+    const int64_t smem = bind_operands(P, st, m.in);
+    for (size_t i = 0; i < st.in.size(); ++i) m.in[i].ts = st.in[i].strides[0];
     m.smem_floats = static_cast<int32_t>(smem);
     if (P->f64) return sbn_marginal_launch<double>(m, 0, stream);
     return sbn_marginal_launch<float>(m, static_cast<size_t>(smem) * 4, stream);
@@ -955,7 +967,6 @@ cudaError_t launch_count(sbn_program *P, const StepDesc &st, const uint8_t *ev, 
     P->launches += 2;
     SbnCount c;
     memset(&c, 0, sizeof c);
-    const size_t elem = P->f64 ? 8 : 4;
     const int64_t grid = count_grid(P, st, n_rows);
     c.partial = P->d_partial;
     c.ev = ev;
@@ -980,83 +991,38 @@ cudaError_t launch_count(sbn_program *P, const StepDesc &st, const uint8_t *ev, 
         c.key_stride[k] = st.key[k].stride;
         c.key_card[k] = st.key[k].card;
     }
-    int64_t smem = 0;
-    for (size_t i = 0; i < st.in.size(); ++i) {
-        const InDesc &in = st.in[i];
-        SbnCountIn &d = c.in[i];
-        int64_t padded;
-        if (in.is_slot) {
-            d.ptr = P->slots[in.id].ptr;
-            padded = P->slots[in.id].padded;
-        } else {
-            d.ptr = reinterpret_cast<const char *>(P->d_tables) + P->tables[in.id].first * static_cast<int64_t>(elem);
-            padded = P->table_padded[in.id];
-        }
-        d.batched = in.batched ? 1 : 0;
-        d.n_ev = static_cast<int32_t>(in.ev.size());
-        for (size_t k = 0; k < in.ev.size(); ++k) {
-            d.ev_col[k] = in.ev[k].col;
-            d.ev_stride[k] = in.ev[k].stride;
-            d.ev_card[k] = in.ev[k].card;
-        }
-        d.smem_off = -1;
-        if (!P->f64 && !in.batched && (smem + padded) * 4 <= SBN_SMEM_BUDGET) {
-            d.smem_off = static_cast<int32_t>(smem);
-            d.stage_floats = static_cast<int32_t>(padded);
-            smem += padded;
-        }
-    }
+    const int64_t smem = bind_operands(P, st, c.in);
     c.smem_floats = static_cast<int32_t>(smem);
     double *counts = P->d_counts + st.q_offset;
     if (P->f64) return sbn_count_launch<double>(c, grid, 0, counts, stream);
     return sbn_count_launch<float>(c, grid, static_cast<size_t>(smem) * 4, counts, stream);
 }
 
-// Every launch of one run of a counts program: the upward / downward passes, the count steps and P(observed) out.
-int issue_counts(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, void *d_prob, cudaStream_t stream) {
-    SbnStep q;
-    for (const StepDesc &st : P->steps) {
-        if (P->mode == 1 && st.kind == 0) continue;  // computed once, when the program was created
-        if (st.kind == 3) {
-            SBN_CUDA(launch_count(P, st, d_ev, ld_ev, n_rows, stream));
-            continue;
-        }
-        build_params(P, st, d_ev, ld_ev, n_rows, &q);
-        SBN_CUDA(launch_step(P, st, q, stream));
-    }
-    P->launches++;
-    const Slot &ps = P->slots[P->post_slot];
-    const int threads = 256;
-    const unsigned grid = static_cast<unsigned>((n_rows + threads - 1) / threads);
-    if (P->f64)
-        sbn_count_prob<double><<<grid, threads, 0, stream>>>(reinterpret_cast<const double *>(ps.ptr), ps.batched ? 1 : 0,
-                                                             static_cast<int32_t>(n_rows), 1e-290, static_cast<double *>(d_prob));
-    else
-        sbn_count_prob<float><<<grid, threads, 0, stream>>>(ps.ptr, ps.batched ? 1 : 0, static_cast<int32_t>(n_rows),
-                                                            static_cast<double>(SBN_MIN_TOTAL_F32), static_cast<float *>(d_prob));
-    SBN_CUDA(cudaGetLastError());
-    return SBN_OK;
-}
+// The drawn-code buffer of a sample / MPE run (P->d_drawn): codes [n_sampled][n_draws][ld_drawn] (one draw for
+// MPE), then one flag byte per row
+struct DrawnCodes {
+    int64_t n_draws = 1, ld_drawn = 0;
+    uint8_t *flags(const sbn_program *P) const { return P->d_drawn + static_cast<int64_t>(P->n_sampled) * n_draws * ld_drawn; }
+};
 
 // Sample step (kind 4): draws its variables for rows 0 .. n_rows - 1 and draws 0 .. n_draws - 1 (`k`: its index
 // among the sample steps).  Argmax step of an MPE program (kind 5, n_draws = 1): decodes them.
 cudaError_t launch_sample(sbn_program *P, const StepDesc &st, int k, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
-                          int64_t n_draws, int64_t ld_drawn, cudaStream_t stream) {
+                          const DrawnCodes &dc, cudaStream_t stream) {
     P->launches++;
     SbnSample m;
     memset(&m, 0, sizeof m);
-    const size_t elem = P->f64 ? 8 : 4;
     m.ev = ev;
     m.ld_ev = ld_ev;
     m.drawn = P->d_drawn;
-    m.ld_drawn = ld_drawn;
+    m.ld_drawn = dc.ld_drawn;
     m.ld = P->ld;
     m.zoff = P->d_tile_off + st.zoff_pos;
     m.args = P->d_sample_args;
-    m.flag = P->d_drawn + static_cast<int64_t>(P->n_sampled) * n_draws * ld_drawn;
+    m.flag = dc.flags(P);
     m.min_total = P->f64 ? 1e-290 : static_cast<double>(SBN_MIN_TOTAL_F32);
     m.n_rows = static_cast<int32_t>(n_rows);
-    m.n_draws = static_cast<int32_t>(n_draws);
+    m.n_draws = static_cast<int32_t>(dc.n_draws);
     m.n_ev = P->n_ev;
     m.n_in = static_cast<int32_t>(st.in.size());
     m.cz = st.cx;
@@ -1064,82 +1030,42 @@ cudaError_t launch_sample(sbn_program *P, const StepDesc &st, int k, const uint8
     m.d_first = static_cast<int32_t>(st.q_offset);
     m.step = k;
     for (size_t j = 0; j < st.ecards.size(); ++j) m.x_card[j] = st.ecards[j];
-    int64_t smem = 0;
-    for (size_t i = 0; i < st.in.size(); ++i) {
-        const InDesc &in = st.in[i];
-        SbnSampleIn &d = m.in[i];
-        int64_t padded;
-        if (in.is_slot) {
-            d.ptr = P->slots[in.id].ptr;
-            padded = P->slots[in.id].padded;
-        } else {
-            d.ptr = reinterpret_cast<const char *>(P->d_tables) + P->tables[in.id].first * static_cast<int64_t>(elem);
-            padded = P->table_padded[in.id];
-        }
-        d.batched = in.batched ? 1 : 0;
-        d.n_terms = static_cast<int32_t>(in.ev.size());
-        for (size_t t = 0; t < in.ev.size(); ++t) {
-            d.t_col[t] = in.ev[t].col;
-            d.t_stride[t] = in.ev[t].stride;
-            d.t_card[t] = in.ev[t].card;
-        }
-        d.smem_off = -1;
-        if (!P->f64 && !in.batched && (smem + padded) * 4 <= SBN_SMEM_BUDGET) {
-            d.smem_off = static_cast<int32_t>(smem);
-            d.stage_floats = static_cast<int32_t>(padded);
-            smem += padded;
-        }
-    }
+    const int64_t smem = bind_operands(P, st, m.in);
     m.smem_floats = static_cast<int32_t>(smem);
-    if (P->mpe) return sbn_argmax_launch(m, static_cast<size_t>(smem) * 4, stream);
+    if (P->kind == kMpe) return sbn_argmax_launch(m, static_cast<size_t>(smem) * 4, stream);
     if (P->f64) return sbn_sample_launch<double>(m, 0, stream);
     return sbn_sample_launch<float>(m, static_cast<size_t>(smem) * 4, stream);
 }
 
-// Every launch of one run of a sample program: the upward pass, the sample steps and P(observed) out.
-int issue_sample(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws, int64_t ld_drawn,
-                 void *d_prob, cudaStream_t stream) {
-    uint8_t *flag = P->d_drawn + static_cast<int64_t>(P->n_sampled) * n_draws * ld_drawn;
-    SBN_CUDA(cudaMemsetAsync(flag, 0, static_cast<size_t>(n_rows), stream));
-    SbnStep q;
-    int k = 0;
-    for (const StepDesc &st : P->steps) {
-        if (st.kind == 0) continue;  // computed once, when the program was created (sample programs are batched)
-        if (st.kind == 4) {
-            SBN_CUDA(launch_sample(P, st, k++, d_ev, ld_ev, n_rows, n_draws, ld_drawn, stream));
-            continue;
-        }
-        build_params(P, st, d_ev, ld_ev, n_rows, &q);
-        SBN_CUDA(launch_step(P, st, q, stream));
-    }
+// A readout, count, sample or argmax step (kinds 2 .. 5) on its own launch; `k`: its index among the sample /
+// argmax steps (Philox counter word 0 of a sample step)
+cudaError_t launch_kind_step(sbn_program *P, const StepDesc &st, int k, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
+                             float *d_out, int64_t ld_out, const DrawnCodes &dc, cudaStream_t stream) {
+    if (st.kind == 2) return launch_marginal(P, st, ev, ld_ev, n_rows, d_out, ld_out, stream);
+    if (st.kind == 3) return launch_count(P, st, ev, ld_ev, n_rows, stream);
+    return launch_sample(P, st, k, ev, ld_ev, n_rows, dc, stream);
+}
+
+// The per-row output of a counts or sample run: P(observed) out of the posterior slot, NaN where it is out of
+// range (and, sample run, where a sample step flagged the row)
+cudaError_t launch_prob(sbn_program *P, int64_t n_rows, void *d_prob, const uint8_t *flag, cudaStream_t stream) {
     P->launches++;
     const Slot &ps = P->slots[P->post_slot];
     const int threads = 256;
     const unsigned grid = static_cast<unsigned>((n_rows + threads - 1) / threads);
-    if (P->f64)
-        sbn_sample_prob<double><<<grid, threads, 0, stream>>>(reinterpret_cast<const double *>(ps.ptr), ps.batched ? 1 : 0, flag,
-                                                              static_cast<int32_t>(n_rows), 1e-290, static_cast<double *>(d_prob));
+    const int32_t rows = static_cast<int32_t>(n_rows), batched = ps.batched ? 1 : 0;
+    const double *p64 = reinterpret_cast<const double *>(ps.ptr);
+    if (!flag && P->f64)
+        sbn_count_prob<double><<<grid, threads, 0, stream>>>(p64, batched, rows, 1e-290, static_cast<double *>(d_prob));
+    else if (!flag)
+        sbn_count_prob<float><<<grid, threads, 0, stream>>>(ps.ptr, batched, rows, static_cast<double>(SBN_MIN_TOTAL_F32),
+                                                            static_cast<float *>(d_prob));
+    else if (P->f64)
+        sbn_sample_prob<double><<<grid, threads, 0, stream>>>(p64, batched, flag, rows, 1e-290, static_cast<double *>(d_prob));
     else
-        sbn_sample_prob<float><<<grid, threads, 0, stream>>>(ps.ptr, ps.batched ? 1 : 0, flag, static_cast<int32_t>(n_rows),
-                                                             static_cast<double>(SBN_MIN_TOTAL_F32), static_cast<float *>(d_prob));
-    SBN_CUDA(cudaGetLastError());
-    return SBN_OK;
-}
-
-// Every launch of one run of an MPE program: the max-sum upward pass, which leaves max log P(x, e) in the
-// posterior slot, and the argmax steps.
-int issue_mpe(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, int64_t ld_drawn, cudaStream_t stream) {
-    SbnStep q;
-    for (const StepDesc &st : P->steps) {
-        if (st.kind == 0) continue;  // computed once, when the program was created (MPE programs are batched)
-        if (st.kind == 5) {
-            SBN_CUDA(launch_sample(P, st, 0, d_ev, ld_ev, n_rows, 1, ld_drawn, stream));
-            continue;
-        }
-        build_params(P, st, d_ev, ld_ev, n_rows, &q);
-        SBN_CUDA(launch_step(P, st, q, stream));
-    }
-    return SBN_OK;
+        sbn_sample_prob<float><<<grid, threads, 0, stream>>>(ps.ptr, batched, flag, rows, static_cast<double>(SBN_MIN_TOTAL_F32),
+                                                             static_cast<float *>(d_prob));
+    return cudaGetLastError();
 }
 
 cudaError_t launch_normalise(sbn_program *P, float *d_out, int64_t ld_out, int64_t n_rows, cudaStream_t stream) {
@@ -1172,8 +1098,6 @@ inline bool pair_on(const sbn_program *P) {
     return P->use_pair && P->use_tiled && !P->use_branches && (!chain_on(P) || P->pairs_avoid_segments) && !P->pairs.empty();
 }
 
-inline bool graph_allowed(const sbn_program *P) { return P->use_graph; }
-
 int run_table_steps(sbn_program *P) {
     if (P->mode != 1) return SBN_OK;
     SbnStep q;
@@ -1203,22 +1127,30 @@ inline bool fold_normalise(const sbn_program *P, const StepDesc &st, const SbnSt
         const char *e = getenv("SOROBN_B200_FOLD_NORMALISE");
         return e ? atoi(e) != 0 : true;
     }();
-    return enabled && !P->f64 && P->post_batched && st.kind == 1 && q.tile_off != nullptr && q.slab_off == nullptr && st.n_tiles == 1 &&
-           st.n_out == P->Q && !sbn_tma_eligible(P, st);
+    return enabled && P->kind == kPosterior && !P->f64 && P->post_batched && st.kind == 1 && q.tile_off != nullptr &&
+           q.slab_off == nullptr && st.n_tiles == 1 && st.n_out == P->Q && !sbn_tma_eligible(P, st);
 }
 
+// Every launch of one run of rows 0 .. n_rows - 1, whatever the program's kind: its steps, then its epilogue.
+// d_out is the posterior [Q][ld_out] of a posterior or marginals run, P(observed) [n_rows] of a counts or sample
+// run; an MPE run leaves max log P(x, e) in the posterior slot.  `events` (profiling): one record per step, one
+// after the steps, one after the epilogue.
 int issue_all(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out, int64_t ld_out,
-              cudaStream_t stream, cudaEvent_t *events) {
+              cudaStream_t stream, cudaEvent_t *events, const DrawnCodes &dc = {}) {
+    // the flags of the sample steps start clear in every run, captured graph or not
+    if (P->kind == kSample) SBN_CUDA(cudaMemsetAsync(dc.flags(P), 0, static_cast<size_t>(n_rows), stream));
     SbnStep q;
     int k = 0;
+    int n_decoded = 0;  // sample / argmax steps issued so far
     bool folded = false;
     bool skip_second = false;  // the pair launched last covers the next launched step
     for (const StepDesc &st : P->steps) {
         if (events) SBN_CUDA(cudaEventRecord(events[k], stream));
         ++k;
         if (hoisted(P, st)) continue;  // computed once, when the program was created
-        if (st.kind == 2) {
-            SBN_CUDA(launch_marginal(P, st, d_ev, ld_ev, n_rows, d_out, ld_out, stream));
+        if (st.kind >= 2) {
+            const int decoded = st.kind >= 4 ? n_decoded++ : 0;
+            SBN_CUDA(launch_kind_step(P, st, decoded, d_ev, ld_ev, n_rows, d_out, ld_out, dc, stream));
             continue;
         }
         const int seg = chain_on(P) ? P->seg_first[k - 1] : -1;
@@ -1251,8 +1183,16 @@ int issue_all(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows
         SBN_CUDA(launch_step(P, st, q, stream));
     }
     if (events) SBN_CUDA(cudaEventRecord(events[k], stream));
-    if (!P->marginals && !folded && !(chain_on(P) && !P->segments.empty() && P->segments.back()->ends_in_posterior))
-        SBN_CUDA(launch_normalise(P, d_out, ld_out, n_rows, stream));
+    switch (P->kind) {
+        case kPosterior:
+            if (!folded && !(chain_on(P) && P->segments.back()->ends_in_posterior))
+                SBN_CUDA(launch_normalise(P, d_out, ld_out, n_rows, stream));
+            break;
+        case kCounts: SBN_CUDA(launch_prob(P, n_rows, d_out, nullptr, stream)); break;
+        case kSample: SBN_CUDA(launch_prob(P, n_rows, d_out, dc.flags(P), stream)); break;
+        case kMarginals:  // the readouts normalise
+        case kMpe: break;
+    }
     if (events) SBN_CUDA(cudaEventRecord(events[k + 1], stream));
     return SBN_OK;
 }
@@ -1293,7 +1233,7 @@ int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n
                 }
             }
         }
-        const bool readout = st.kind == 2;  // writes the posterior, no slot
+        const bool readout = st.kind >= 2;  // writes the posterior (marginals program), no slot
         if (!readout && last_writer[st.out_slot] >= 0) deps.push_back(last_writer[st.out_slot]);
         if (!readout)
             for (int r : readers[st.out_slot]) deps.push_back(r);
@@ -1309,7 +1249,7 @@ int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n
         for (int d : deps)
             if (stream_of[d] != k) SBN_CUDA(cudaStreamWaitEvent(stream, P->step_done[d], 0));
         if (readout) {
-            SBN_CUDA(launch_marginal(P, st, d_ev, ld_ev, n_rows, d_out, ld_out, stream));
+            SBN_CUDA(launch_kind_step(P, st, 0, d_ev, ld_ev, n_rows, d_out, ld_out, {}, stream));
         } else {
             build_params(P, st, d_ev, ld_ev, n_rows, &q);
             SBN_CUDA(launch_step(P, st, q, stream));
@@ -1327,21 +1267,101 @@ int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n
         if (!hoisted(P, P->steps[s])) tail[stream_of[s]] = s;
     for (int k = 0; k < sbn_program::kBranches; ++k)
         if (tail[k] >= 0) SBN_CUDA(cudaStreamWaitEvent(origin, P->step_done[tail[k]], 0));
-    if (!P->marginals) SBN_CUDA(launch_normalise(P, d_out, ld_out, n_rows, origin));
+    if (P->kind == kPosterior) SBN_CUDA(launch_normalise(P, d_out, ld_out, n_rows, origin));
     return SBN_OK;
 }
 
-int check_run_args(sbn_program *P, const void *ev, int64_t ld_ev, int64_t n_rows, const void *out, int64_t ld_out) {
+// The checks every run shares: the program is of the kind the entry point runs (kPosterior: the run, evidence
+// and profile calls, which take posterior and marginals programs), and the rows and their evidence are well formed
+int check_rows(const sbn_program *P, ProgramKind kind, const void *ev, int64_t ld_ev, int64_t n_rows) {
+    static const char *const name[] = {"posterior", "marginals", "counts", "sample", "MPE"};
+    static const char *const entry[] = {"sbn_program_run_*", "sbn_program_run_*", "sbn_program_counts_host",
+                                        "sbn_program_sample_host", "sbn_program_mpe_host"};
     if (!P) return fail(SBN_E_INVALID, "null program");
+    if ((P->kind == kMarginals ? kPosterior : P->kind) != kind)
+        return fail(SBN_E_INVALID, "a %s program runs through %s", name[P->kind], entry[P->kind]);
     if (n_rows <= 0) return fail(SBN_E_INVALID, "n_rows must be positive");
-    if (!out) return fail(SBN_E_INVALID, "null output");
     if (P->n_ev > 0 && !ev) return fail(SBN_E_INVALID, "null evidence");
     if (P->n_ev > 1 && ld_ev < n_rows) return fail(SBN_E_INVALID, "ld_ev < n_rows");
-    if (P->Q > 1 && ld_out < n_rows) return fail(SBN_E_INVALID, "ld_out < n_rows");
     if (P->mode == 0 && n_rows != 1) return fail(SBN_E_INVALID, "a flat program answers exactly one row");
-    if (P->counts) return fail(SBN_E_INVALID, "a counts program runs through sbn_program_counts_host");
-    if (P->sample) return fail(SBN_E_INVALID, "a sample program runs through sbn_program_sample_host");
-    if (P->mpe) return fail(SBN_E_INVALID, "an MPE program runs through sbn_program_mpe_host");
+    return SBN_OK;
+}
+
+// check_rows for the calls that write a posterior [Q][ld_out]
+int check_run_args(const sbn_program *P, const void *ev, int64_t ld_ev, int64_t n_rows, const void *out, int64_t ld_out) {
+    const int rc = check_rows(P, kPosterior, ev, ld_ev, n_rows);
+    if (rc != SBN_OK) return rc;
+    if (!out) return fail(SBN_E_INVALID, "null output");
+    if (P->Q > 1 && ld_out < n_rows) return fail(SBN_E_INVALID, "ld_out < n_rows");
+    return SBN_OK;
+}
+
+// Make the program's device current and grow its scratch to n_rows (it never shrinks).  The reservation is capped
+// by the free device memory, so it may stay below n_rows: the host paths then run in chunks.
+int reserve_rows(sbn_program *P, int64_t n_rows) {
+    SBN_CUDA(cudaSetDevice(P->device));
+    return n_rows > P->reserved_rows ? sbn_program_reserve(P, n_rows) : SBN_OK;
+}
+
+// Replay `g` on `stream`.  When `key` differs from the key it was captured for, capture it first: `issue()` issues
+// one run on the capture stream `cap`, and the launches it counts are what every replay adds to P->launches.
+template <typename Issue>
+int replay(sbn_program *P, CachedGraph &g, const GraphKey &key, cudaStream_t cap, cudaStream_t stream, Issue &&issue) {
+    if (!g.exec || !(g.key == key)) {
+        drop_graph(g);
+        SBN_CUDA(cudaStreamBeginCapture(cap, cudaStreamCaptureModeRelaxed));
+        const int64_t before = P->launches;
+        const int rc = issue();
+        cudaGraph_t graph = nullptr;
+        cudaError_t e = cudaStreamEndCapture(cap, &graph);
+        g.launches = P->launches - before;
+        P->launches = before;
+        if (rc == SBN_OK && e == cudaSuccess) e = cudaGraphInstantiate(&g.exec, graph, 0);
+        if (graph) cudaGraphDestroy(graph);
+        if (rc != SBN_OK) return rc;
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            g.exec = nullptr;
+            return fail(SBN_E_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
+        }
+        g.key = key;
+    }
+    SBN_CUDA(cudaGraphLaunch(g.exec, stream));
+    P->launches += g.launches;
+    return SBN_OK;
+}
+
+constexpr int64_t kSampleGraphMinRows = 4096;
+
+// One run of rows already on the device: a replay of the program's graph (captured on the program's stream) when
+// graphs are on, else plain launches on `stream`
+int run_rows(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out, int64_t ld_out,
+             cudaStream_t stream, const DrawnCodes &dc = {}) {
+    // a short sample / MPE chunk runs as plain launches: capturing and instantiating a graph costs more than it
+    // saves, and the short runs of a pattern whose rows are scattered through a frame come in many lengths
+    const bool short_chunk = (P->kind == kSample || P->kind == kMpe) && n_rows < kSampleGraphMinRows;
+    if (!P->use_graph || short_chunk) return issue_all(P, d_ev, ld_ev, n_rows, d_out, ld_out, stream, nullptr, dc);
+    const GraphKey key = {d_ev, ld_ev, n_rows, d_out, ld_out, P->d_partial, P->d_drawn, dc.n_draws, dc.ld_drawn};
+    const bool branched = P->use_branches && P->kind <= kMarginals;
+    return replay(P, P->graph, key, P->stream, stream, [&] {
+        return branched ? issue_branched(P, d_ev, ld_ev, n_rows, d_out, ld_out, P->stream)
+                        : issue_all(P, d_ev, ld_ev, n_rows, d_out, ld_out, P->stream, nullptr, dc);
+    });
+}
+
+// Walk a host batch in chunks of at most `cap` rows on the program's stream: upload each chunk's codes to
+// P->d_ev, then `body(r0, rows)` runs the chunk and downloads its outputs
+template <typename Body>
+int for_each_chunk(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t cap, Body &&body) {
+    for (int64_t r0 = 0; r0 < n_rows; r0 += cap) {
+        const int64_t rows = std::min(cap, n_rows - r0);
+        if (P->n_ev > 0)
+            SBN_CUDA(cudaMemcpy2DAsync(P->d_ev, static_cast<size_t>(P->ld), ev + r0, static_cast<size_t>(ld_ev),
+                                       static_cast<size_t>(rows), static_cast<size_t>(P->n_ev), cudaMemcpyHostToDevice,
+                                       P->stream));
+        const int rc = body(r0, rows);
+        if (rc != SBN_OK) return rc;
+    }
     return SBN_OK;
 }
 
@@ -1388,7 +1408,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
         delete P;
         return rc;
     }
-    if (P->mpe && f64) {
+    if (P->kind == kMpe && f64) {
         delete P;
         return fail(SBN_E_INVALID, "an MPE program runs in float32 only (its tables are logs: nothing underflows)");
     }
@@ -1461,9 +1481,9 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
                                        cudaMemcpyHostToDevice, P->stream));
         }
         SBN_CUDA_P(cudaStreamSynchronize(P->stream));
-        // The on-chip segments and paired steps assume every intermediate has ONE consumer; the factors of a
-        // marginals program feed several launches, so it runs on the classic per-step launches.
-        if (!P->marginals && !P->counts && !P->sample && !P->mpe) sbn_chain_plan(P);
+        // The on-chip segments and paired steps assume every intermediate has ONE consumer; the factors of the
+        // other kinds' programs feed several launches, so they run on the classic per-step launches.
+        if (P->kind == kPosterior) sbn_chain_plan(P);
     }
     {
         // opt every step-kernel instantiation into SBN_SMEM_BUDGET of dynamic shared memory
@@ -1484,7 +1504,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
             done[device] = true;
         }
     }
-    if (P->counts) {
+    if (P->kind == kCounts) {
         // the count table; the largest step's per-warp partial tables (count_grid caps them) are sized here and
         // allocated by each counts call only for its duration, so idle programs hold no partial tables
         for (const StepDesc &st : P->steps)
@@ -1497,7 +1517,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
     if (rc != SBN_OK) return bail(rc);
     {
         // pairs multiply the tables of two steps on the host: needs the outputs of the table steps above
-        cudaError_t e = P->marginals || P->counts || P->sample || P->mpe ? cudaSuccess : sbn_pair_plan(P);
+        cudaError_t e = P->kind == kPosterior ? sbn_pair_plan(P) : cudaSuccess;
         if (e != cudaSuccess) return bail(fail(SBN_E_CUDA, "planning the paired steps failed: %s", cudaGetErrorString(e)));
     }
     *out = P;
@@ -1584,58 +1604,17 @@ int sbn_program_reserve(sbn_program *P, int64_t max_rows) {
     return SBN_OK;
 }
 
-static int run_device_impl(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out,
-                           int64_t ld_out, void *stream_);
-
 int sbn_program_run_device(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out,
-                           int64_t ld_out, void *stream_) {
-    if (P && P->f64) return fail(SBN_E_INVALID, "float64 programs only run through sbn_program_run_host_f64");
-    return run_device_impl(P, d_ev, ld_ev, n_rows, d_out, ld_out, stream_);
-}
-
-static int run_device_impl(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out,
                            int64_t ld_out, void *stream_) {
     int rc = check_run_args(P, d_ev, ld_ev, n_rows, d_out, ld_out);
     if (rc != SBN_OK) return rc;
-    SBN_CUDA(cudaSetDevice(P->device));
-    if (n_rows > P->reserved_rows) {  // grows (never shrinks); capped by the free device memory
-        rc = sbn_program_reserve(P, n_rows);
-        if (rc != SBN_OK) return rc;
-    }
+    if (P->f64) return fail(SBN_E_INVALID, "float64 programs only run through sbn_program_run_host_f64");
+    rc = reserve_rows(P, n_rows);
+    if (rc != SBN_OK) return rc;
     if (n_rows > P->reserved_rows)
         return fail(SBN_E_NOMEM, "n_rows %lld exceeds the %lld rows of scratch that fit the device; use the host path "
                     "(it runs in chunks) or smaller batches", (long long)n_rows, (long long)P->reserved_rows);
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    if (!P->use_graph) return issue_all(P, d_ev, ld_ev, n_rows, d_out, ld_out, stream, nullptr);
-
-    auto &k = P->graph_key;
-    if (!P->exec || k.ev != d_ev || k.ld_ev != ld_ev || k.n_rows != n_rows || k.out != d_out || k.ld_out != ld_out) {
-        if (P->exec) {
-            cudaGraphExecDestroy(P->exec);
-            P->exec = nullptr;
-        }
-        cudaStream_t cap = P->stream;  // capture on the program's own stream, replay on the caller's
-        SBN_CUDA(cudaStreamBeginCapture(cap, cudaStreamCaptureModeRelaxed));
-        const int64_t before = P->launches;
-        rc = P->use_branches ? issue_branched(P, d_ev, ld_ev, n_rows, d_out, ld_out, cap)
-                             : issue_all(P, d_ev, ld_ev, n_rows, d_out, ld_out, cap, nullptr);
-        cudaGraph_t graph = nullptr;
-        cudaError_t e = cudaStreamEndCapture(cap, &graph);
-        P->graph_launches = P->launches - before;
-        P->launches = before;
-        if (rc != SBN_OK) {
-            if (graph) cudaGraphDestroy(graph);
-            return rc;
-        }
-        if (e != cudaSuccess) return fail(SBN_E_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
-        e = cudaGraphInstantiate(&P->exec, graph, 0);
-        cudaGraphDestroy(graph);
-        if (e != cudaSuccess) return fail(SBN_E_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
-        k = {d_ev, ld_ev, n_rows, d_out, ld_out};
-    }
-    SBN_CUDA(cudaGraphLaunch(P->exec, stream));
-    P->launches += P->graph_launches;
-    return SBN_OK;
+    return run_rows(P, d_ev, ld_ev, n_rows, d_out, ld_out, static_cast<cudaStream_t>(stream_));
 }
 
 static int run_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, void *out_, int64_t ld_out,
@@ -1643,18 +1622,14 @@ static int run_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int
     int rc = check_run_args(P, ev, ld_ev, n_rows, out_, want_totals ? n_rows : ld_out);
     if (rc != SBN_OK) return rc;
     if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the run call");
-    if (want_totals && P->marginals)
+    if (want_totals && P->kind == kMarginals)
         return fail(SBN_E_INVALID, "a marginals program has no single normaliser; P(event) comes from a program without targets");
     const size_t elem = f64 ? 8 : 4;
     char *out = static_cast<char *>(out_);
-    SBN_CUDA(cudaSetDevice(P->device));
-    if (n_rows > P->reserved_rows) {
-        // the chunk capacity follows the largest batch seen so far (a program first used for one
-        // row must not answer a later million-row batch one row at a time); the reservation is
-        // capped by the free device memory, larger batches run in chunks
-        rc = sbn_program_reserve(P, n_rows);
-        if (rc != SBN_OK) return rc;
-    }
+    // the chunk capacity follows the largest batch seen so far (a program first used for one row must not answer a
+    // later million-row batch one row at a time)
+    rc = reserve_rows(P, n_rows);
+    if (rc != SBN_OK) return rc;
     const int64_t cap = P->reserved_rows;
     // Transfer-bound programs (a handful of launches for megabytes of codes in and posteriors
     // out: Asia is ONE batched launch for 4 MB + 8 MB per million rows) are pipelined: the batch is
@@ -1684,9 +1659,39 @@ static int run_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int
         }
         cudaStream_t s_in = P->branch[0], s_run = P->stream, s_out = P->branch[1];
         const int64_t range = round_up((n_rows + kRanges - 1) / kRanges, 32);
-        // the whole fan-out is issued into a stream capture and replayed as ONE graph launch when the
-        // host buffers are pinned (a dozen copies, launches and event edges cost CPU time of the order
-        // of what they overlap); the graph is kept for the (buffers, rows) it was built for
+        // the side streams fork from s_run and join back into it; a few plain launches per range, nothing to
+        // amortise inside
+        auto issue_ranges = [&]() -> int {
+            cudaEvent_t fork = P->pipe_events[0], j_in = P->pipe_events[1 + 2 * kMaxRanges], j_out = P->pipe_events[2 + 2 * kMaxRanges];
+            SBN_CUDA(cudaEventRecord(fork, s_run));
+            SBN_CUDA(cudaStreamWaitEvent(s_in, fork, 0));
+            SBN_CUDA(cudaStreamWaitEvent(s_out, fork, 0));
+            for (int64_t r0 = 0, k = 0; r0 < n_rows; r0 += range, ++k) {
+                const int64_t rows = std::min(range, n_rows - r0);
+                cudaEvent_t up = P->pipe_events[1 + 2 * k], done = P->pipe_events[2 + 2 * k];
+                if (P->n_ev > 0) {
+                    SBN_CUDA(cudaMemcpy2DAsync(P->d_ev + r0, static_cast<size_t>(P->ld), ev + r0, static_cast<size_t>(ld_ev),
+                                               static_cast<size_t>(rows), static_cast<size_t>(P->n_ev), cudaMemcpyHostToDevice, s_in));
+                    SBN_CUDA(cudaEventRecord(up, s_in));
+                    SBN_CUDA(cudaStreamWaitEvent(s_run, up, 0));
+                }
+                char *d_out = reinterpret_cast<char *>(P->d_out) + r0 * elem;
+                const int rc = issue_all(P, P->d_ev + r0, P->ld, rows, reinterpret_cast<float *>(d_out), P->ld, s_run, nullptr);
+                if (rc != SBN_OK) return rc;
+                SBN_CUDA(cudaEventRecord(done, s_run));
+                SBN_CUDA(cudaStreamWaitEvent(s_out, done, 0));
+                SBN_CUDA(cudaMemcpy2DAsync(out + r0 * elem, static_cast<size_t>(ld_out) * elem, d_out, static_cast<size_t>(P->ld) * elem,
+                                           static_cast<size_t>(rows) * elem, static_cast<size_t>(P->Q), cudaMemcpyDeviceToHost, s_out));
+            }
+            SBN_CUDA(cudaEventRecord(j_in, s_in));
+            SBN_CUDA(cudaStreamWaitEvent(s_run, j_in, 0));
+            SBN_CUDA(cudaEventRecord(j_out, s_out));
+            SBN_CUDA(cudaStreamWaitEvent(s_run, j_out, 0));
+            return SBN_OK;
+        };
+        // the whole fan-out is replayed as ONE graph launch when the host buffers are pinned (a dozen copies,
+        // launches and event edges cost CPU time of the order of what they overlap); the graph is kept for the
+        // (buffers, rows) it was built for
         auto pinned = [](const void *ptr) {
             cudaPointerAttributes a;
             if (cudaPointerGetAttributes(&a, ptr) != cudaSuccess) {
@@ -1695,89 +1700,21 @@ static int run_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int
             }
             return a.type == cudaMemoryTypeHost;
         };
-        const bool as_graph = graph_allowed(P) && pinned(out) && (P->n_ev == 0 || pinned(ev));
-        auto &key = P->pipe_key;
-        const bool hit = as_graph && P->pipe_exec && key.ev == ev && key.ld_ev == ld_ev && key.n_rows == n_rows && key.out == out &&
-                         key.ld_out == ld_out;
-        if (!hit) {
-            if (P->pipe_exec) {
-                cudaGraphExecDestroy(P->pipe_exec);
-                P->pipe_exec = nullptr;
-            }
-            const bool graph_was = P->use_graph;
-            P->use_graph = false;  // a few plain launches per range: nothing to amortise inside
-            cudaError_t e = cudaSuccess;
-            if (as_graph) {
-                e = cudaStreamBeginCapture(s_run, cudaStreamCaptureModeRelaxed);
-                if (e == cudaSuccess) e = cudaEventRecord(P->pipe_events[0], s_run);
-                if (e == cudaSuccess) e = cudaStreamWaitEvent(s_in, P->pipe_events[0], 0);
-                if (e == cudaSuccess) e = cudaStreamWaitEvent(s_out, P->pipe_events[0], 0);
-            }
-            const int64_t before = P->launches;
-            int k = 0;
-            for (int64_t r0 = 0; r0 < n_rows && rc == SBN_OK && e == cudaSuccess; r0 += range, ++k) {
-                const int64_t rows = std::min(range, n_rows - r0);
-                cudaEvent_t up = P->pipe_events[1 + 2 * k], done = P->pipe_events[2 + 2 * k];
-                if (P->n_ev > 0) {
-                    e = cudaMemcpy2DAsync(P->d_ev + r0, static_cast<size_t>(P->ld), ev + r0, static_cast<size_t>(ld_ev),
-                                          static_cast<size_t>(rows), static_cast<size_t>(P->n_ev), cudaMemcpyHostToDevice, s_in);
-                    if (e == cudaSuccess) e = cudaEventRecord(up, s_in);
-                    if (e == cudaSuccess) e = cudaStreamWaitEvent(s_run, up, 0);
-                    if (e != cudaSuccess) break;
-                }
-                rc = run_device_impl(P, P->d_ev + r0, P->ld, rows, reinterpret_cast<float *>(reinterpret_cast<char *>(P->d_out) + r0 * elem),
-                                     P->ld, s_run);
-                if (rc != SBN_OK) break;
-                e = cudaEventRecord(done, s_run);
-                if (e == cudaSuccess) e = cudaStreamWaitEvent(s_out, done, 0);
-                // (P(event) runs are not pipelined: d_total is indexed by the row inside the launch)
-                if (e == cudaSuccess)
-                    e = cudaMemcpy2DAsync(out + r0 * elem, static_cast<size_t>(ld_out) * elem, reinterpret_cast<char *>(P->d_out) + r0 * elem,
-                                          static_cast<size_t>(P->ld) * elem, static_cast<size_t>(rows) * elem, static_cast<size_t>(P->Q),
-                                          cudaMemcpyDeviceToHost, s_out);
-            }
-            P->use_graph = graph_was;
-            if (as_graph) {
-                // join the side streams back into the origin, end the capture
-                cudaEvent_t j_in = P->pipe_events[1 + 2 * kMaxRanges], j_out = P->pipe_events[2 + 2 * kMaxRanges];
-                if (e == cudaSuccess) e = cudaEventRecord(j_in, s_in);
-                if (e == cudaSuccess) e = cudaStreamWaitEvent(s_run, j_in, 0);
-                if (e == cudaSuccess) e = cudaEventRecord(j_out, s_out);
-                if (e == cudaSuccess) e = cudaStreamWaitEvent(s_run, j_out, 0);
-                cudaGraph_t graph = nullptr;
-                const cudaError_t e_end = cudaStreamEndCapture(s_run, &graph);
-                P->pipe_launches = P->launches - before;
-                P->launches = before;
-                if (e == cudaSuccess) e = e_end;
-                if (e == cudaSuccess && rc == SBN_OK) e = cudaGraphInstantiate(&P->pipe_exec, graph, 0);
-                if (graph) cudaGraphDestroy(graph);
-                if (rc != SBN_OK) return rc;
-                if (e != cudaSuccess) {
-                    cudaGetLastError();
-                    return fail(SBN_E_CUDA, "pipelined graph capture failed: %s", cudaGetErrorString(e));
-                }
-                key = {ev, ld_ev, n_rows, out, ld_out};
-            } else {
-                cudaError_t e1 = cudaStreamSynchronize(s_in), e2 = cudaStreamSynchronize(s_run), e3 = cudaStreamSynchronize(s_out);
-                if (rc != SBN_OK) return rc;
-                if (e != cudaSuccess || e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess)
-                    return fail(SBN_E_CUDA, "pipelined run failed: %s",
-                                cudaGetErrorString(e != cudaSuccess ? e : e1 != cudaSuccess ? e1 : e2 != cudaSuccess ? e2 : e3));
-                return SBN_OK;
-            }
+        if (P->use_graph && pinned(out) && (P->n_ev == 0 || pinned(ev)))
+            rc = replay(P, P->pipe_graph, {ev, ld_ev, n_rows, out, ld_out}, s_run, s_run, issue_ranges);
+        else
+            rc = issue_ranges();
+        if (rc != SBN_OK) {  // the side streams may not have joined s_run
+            cudaStreamSynchronize(s_in);
+            cudaStreamSynchronize(s_out);
         }
-        SBN_CUDA(cudaGraphLaunch(P->pipe_exec, s_run));
-        P->launches += P->pipe_launches;
-        SBN_CUDA(cudaStreamSynchronize(s_run));
+        const cudaError_t e = cudaStreamSynchronize(s_run);
+        if (rc != SBN_OK) return rc;
+        SBN_CUDA(e);
         return SBN_OK;
     }
-    for (int64_t r0 = 0; r0 < n_rows; r0 += cap) {
-        const int64_t rows = std::min(cap, n_rows - r0);
-        if (P->n_ev > 0)
-            SBN_CUDA(cudaMemcpy2DAsync(P->d_ev, static_cast<size_t>(P->ld), ev + r0, static_cast<size_t>(ld_ev),
-                                       static_cast<size_t>(rows), static_cast<size_t>(P->n_ev), cudaMemcpyHostToDevice,
-                                       P->stream));
-        rc = run_device_impl(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
+    rc = for_each_chunk(P, ev, ld_ev, n_rows, cap, [&](int64_t r0, int64_t rows) -> int {
+        const int rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
         if (rc != SBN_OK) return rc;
         if (want_totals)
             SBN_CUDA(cudaMemcpyAsync(out + r0 * elem, P->d_total, static_cast<size_t>(rows) * elem,
@@ -1786,7 +1723,9 @@ static int run_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int
             SBN_CUDA(cudaMemcpy2DAsync(out + r0 * elem, static_cast<size_t>(ld_out) * elem, P->d_out,
                                        static_cast<size_t>(P->ld) * elem, static_cast<size_t>(rows) * elem,
                                        static_cast<size_t>(P->Q), cudaMemcpyDeviceToHost, P->stream));
-    }
+        return SBN_OK;
+    });
+    if (rc != SBN_OK) return rc;
     SBN_CUDA(cudaStreamSynchronize(P->stream));
     return SBN_OK;
 }
@@ -1808,25 +1747,35 @@ int sbn_program_evidence_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_
     return run_host_common(P, ev, ld_ev, n_rows, prob, n_rows, true, true);
 }
 
-static int counts_chunks(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, void *prob,
-                         size_t elem);
+// The chunks of a counts call: P(observed) per chunk, then the batch's counts added into `counts`
+static int add_expected_counts(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, void *prob,
+                               size_t elem) {
+    SBN_CUDA(cudaMemsetAsync(P->d_counts, 0, static_cast<size_t>(P->n_counts) * 8, P->stream));
+    const int rc = for_each_chunk(P, ev, ld_ev, n_rows, P->reserved_rows, [&](int64_t r0, int64_t rows) -> int {
+        // the graph reads the tables and the count table by address, so it replays the values sbn_program_set_tables uploads
+        const int rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
+        if (rc != SBN_OK) return rc;
+        SBN_CUDA(cudaMemcpyAsync(static_cast<char *>(prob) + r0 * elem, P->d_out, static_cast<size_t>(rows) * elem,
+                                 cudaMemcpyDeviceToHost, P->stream));
+        return SBN_OK;
+    });
+    if (rc != SBN_OK) return rc;
+    std::vector<double> h(static_cast<size_t>(P->n_counts));
+    SBN_CUDA(cudaMemcpyAsync(h.data(), P->d_counts, h.size() * 8, cudaMemcpyDeviceToHost, P->stream));
+    SBN_CUDA(cudaStreamSynchronize(P->stream));
+    for (int64_t i = 0; i < P->n_counts; ++i) counts[i] += h[static_cast<size_t>(i)];
+    return SBN_OK;
+}
 
 static int counts_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, int64_t n_counts,
                               void *prob, bool f64) {
-    if (!P) return fail(SBN_E_INVALID, "null program");
-    if (!P->counts) return fail(SBN_E_INVALID, "not a counts program (planner.build_counts_plan)");
+    int rc = check_rows(P, kCounts, ev, ld_ev, n_rows);
+    if (rc != SBN_OK) return rc;
     if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the counts call");
-    if (n_rows <= 0) return fail(SBN_E_INVALID, "n_rows must be positive");
     if (!counts || !prob) return fail(SBN_E_INVALID, "null output");
     if (n_counts != P->n_counts) return fail(SBN_E_INVALID, "the count table has %lld entries, not %lld", (long long)P->n_counts, (long long)n_counts);
-    if (P->n_ev > 0 && !ev) return fail(SBN_E_INVALID, "null evidence");
-    if (P->n_ev > 1 && ld_ev < n_rows) return fail(SBN_E_INVALID, "ld_ev < n_rows");
-    if (P->mode == 0 && n_rows != 1) return fail(SBN_E_INVALID, "a flat program answers exactly one row");
-    SBN_CUDA(cudaSetDevice(P->device));
-    if (n_rows > P->reserved_rows) {
-        const int rc = sbn_program_reserve(P, n_rows);
-        if (rc != SBN_OK) return rc;
-    }
+    rc = reserve_rows(P, n_rows);
+    if (rc != SBN_OK) return rc;
     // the per-warp partial tables live for this call only: a program that is not running holds none of them
     {
         const cudaError_t e = cudaMalloc(&P->d_partial, static_cast<size_t>(std::max<int64_t>(1, P->partial_doubles)) * 8);
@@ -1837,64 +1786,11 @@ static int counts_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, 
                         (long long)(P->partial_doubles * 8), cudaGetErrorString(e));
         }
     }
-    const int rc = counts_chunks(P, ev, ld_ev, n_rows, counts, prob, f64 ? 8 : 4);
+    rc = add_expected_counts(P, ev, ld_ev, n_rows, counts, prob, f64 ? 8 : 4);
     cudaStreamSynchronize(P->stream);  // nothing may still read the partial tables
     cudaFree(P->d_partial);
     P->d_partial = nullptr;
     return rc;
-}
-
-static int counts_chunks(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, void *prob,
-                         size_t elem) {
-    const int64_t cap = P->reserved_rows;
-    SBN_CUDA(cudaMemsetAsync(P->d_counts, 0, static_cast<size_t>(P->n_counts) * 8, P->stream));
-    for (int64_t r0 = 0; r0 < n_rows; r0 += cap) {
-        const int64_t rows = std::min(cap, n_rows - r0);
-        if (P->n_ev > 0)
-            SBN_CUDA(cudaMemcpy2DAsync(P->d_ev, static_cast<size_t>(P->ld), ev + r0, static_cast<size_t>(ld_ev),
-                                       static_cast<size_t>(rows), static_cast<size_t>(P->n_ev), cudaMemcpyHostToDevice, P->stream));
-        if (!P->use_graph) {
-            const int rc = issue_counts(P, P->d_ev, P->ld, rows, P->d_out, P->stream);
-            if (rc != SBN_OK) return rc;
-        } else {
-            // one graph per chunk size; it reads the tables and the count table by address, so it replays the
-            // values sbn_program_set_tables uploads
-            auto &k = P->graph_key;
-            if (!P->exec || k.ev != P->d_ev || k.n_rows != rows || k.out != reinterpret_cast<float *>(P->d_counts) ||
-                P->graph_partial != P->d_partial) {
-                if (P->exec) {
-                    cudaGraphExecDestroy(P->exec);
-                    P->exec = nullptr;
-                }
-                SBN_CUDA(cudaStreamBeginCapture(P->stream, cudaStreamCaptureModeRelaxed));
-                const int64_t before = P->launches;
-                const int rc = issue_counts(P, P->d_ev, P->ld, rows, P->d_out, P->stream);
-                cudaGraph_t graph = nullptr;
-                cudaError_t e = cudaStreamEndCapture(P->stream, &graph);
-                P->graph_launches = P->launches - before;
-                P->launches = before;
-                if (rc != SBN_OK) {
-                    if (graph) cudaGraphDestroy(graph);
-                    return rc;
-                }
-                if (e != cudaSuccess) return fail(SBN_E_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
-                e = cudaGraphInstantiate(&P->exec, graph, 0);
-                cudaGraphDestroy(graph);
-                if (e != cudaSuccess) return fail(SBN_E_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
-                k = {P->d_ev, P->ld, rows, reinterpret_cast<float *>(P->d_counts), P->ld};
-                P->graph_partial = P->d_partial;
-            }
-            SBN_CUDA(cudaGraphLaunch(P->exec, P->stream));
-            P->launches += P->graph_launches;
-        }
-        SBN_CUDA(cudaMemcpyAsync(static_cast<char *>(prob) + r0 * elem, P->d_out, static_cast<size_t>(rows) * elem,
-                                 cudaMemcpyDeviceToHost, P->stream));
-    }
-    std::vector<double> h(static_cast<size_t>(P->n_counts));
-    SBN_CUDA(cudaMemcpyAsync(h.data(), P->d_counts, h.size() * 8, cudaMemcpyDeviceToHost, P->stream));
-    SBN_CUDA(cudaStreamSynchronize(P->stream));
-    for (int64_t i = 0; i < P->n_counts; ++i) counts[i] += h[static_cast<size_t>(i)];
-    return SBN_OK;
 }
 
 int sbn_program_counts_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, int64_t n_counts,
@@ -1909,7 +1805,7 @@ int sbn_program_counts_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev
 
 static int set_tables_common(sbn_program *P, const void *tables, int64_t n, bool f64) {
     if (!P) return fail(SBN_E_INVALID, "null program");
-    if (!P->counts)
+    if (P->kind != kCounts)
         return fail(SBN_E_INVALID, "only counts programs take new tables (other programs fold table products into their launches)");
     if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the table call");
     if (n != P->n_table_floats || (n > 0 && !tables))
@@ -1935,27 +1831,18 @@ int sbn_program_set_tables_f64(sbn_program *P, const double *tables, int64_t n_t
     return set_tables_common(P, tables, n_table_doubles, true);
 }
 
-constexpr int64_t kSampleGraphMinRows = 4096;
-
-// The host path of sample programs and (mpe = true, one draw, no seed) of MPE programs: the decoded codes of a
+// The host path of sample programs and (kind = kMpe, one draw, no seed) of MPE programs: the decoded codes of a
 // chunk are the drawn-code buffer, the per-row output is P(observed) (sample) or max log P(x, e) (MPE).
 static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws, uint64_t seed,
-                              int64_t row_base, uint8_t *out, void *prob, bool f64, bool mpe = false) {
-    if (!P) return fail(SBN_E_INVALID, "null program");
-    if (mpe && !P->mpe) return fail(SBN_E_INVALID, "not an MPE program (planner.build_mpe_plan)");
-    if (!mpe && !P->sample) return fail(SBN_E_INVALID, "not a sample program (planner.build_sample_plan)");
+                              int64_t row_base, uint8_t *out, void *prob, bool f64, ProgramKind kind = kSample) {
+    int rc = check_rows(P, kind, ev, ld_ev, n_rows);
+    if (rc != SBN_OK) return rc;
     if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the sample call");
-    if (n_rows <= 0) return fail(SBN_E_INVALID, "n_rows must be positive");
     if (n_draws <= 0 || n_draws > INT32_MAX) return fail(SBN_E_INVALID, "n_draws must be in 1 .. 2^31 - 1");
     if (row_base < 0) return fail(SBN_E_INVALID, "row_base must not be negative");
     if ((P->n_sampled > 0 && !out) || !prob) return fail(SBN_E_INVALID, "null output");
-    if (P->n_ev > 0 && !ev) return fail(SBN_E_INVALID, "null evidence");
-    if (P->n_ev > 1 && ld_ev < n_rows) return fail(SBN_E_INVALID, "ld_ev < n_rows");
-    SBN_CUDA(cudaSetDevice(P->device));
-    if (n_rows > P->reserved_rows) {
-        const int rc = sbn_program_reserve(P, n_rows);
-        if (rc != SBN_OK) return rc;
-    }
+    rc = reserve_rows(P, n_rows);
+    if (rc != SBN_OK) return rc;
     // the drawn codes of a chunk ([n_sampled][n_draws] bytes + one flag byte per row) take at most half of the
     // free device memory: larger batches run in more chunks
     const int64_t per_row = static_cast<int64_t>(P->n_sampled) * n_draws + 1;
@@ -1966,8 +1853,8 @@ static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, 
         const int64_t budget = static_cast<int64_t>(free_b / 2) + P->drawn_bytes;
         if (round_up(cap, 32) * per_row > budget) cap = std::max<int64_t>(32, budget / per_row / 32 * 32);
     }
-    const int64_t ld_drawn = round_up(std::min(cap, n_rows), 32);
-    const int64_t bytes = ld_drawn * per_row;
+    const DrawnCodes dc = {n_draws, round_up(std::min(cap, n_rows), 32)};
+    const int64_t bytes = dc.ld_drawn * per_row;
     if (bytes > P->drawn_bytes) {
         SBN_CUDA(cudaStreamSynchronize(P->stream));
         cudaFree(P->d_drawn);
@@ -1981,60 +1868,20 @@ static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, 
         }
         P->drawn_bytes = bytes;
     }
+    const bool mpe = kind == kMpe;
     if (!mpe && !P->d_sample_args) SBN_CUDA(cudaMalloc(&P->d_sample_args, 4 * sizeof(uint32_t)));
     const size_t elem = f64 ? 8 : 4;
     const Slot &ps = P->slots[P->post_slot];  // MPE program: max log P(x, e), [1][ld] or one value for every row
-    auto issue = [&](int64_t rows) {
-        return mpe ? issue_mpe(P, P->d_ev, P->ld, rows, ld_drawn, P->stream)
-                   : issue_sample(P, P->d_ev, P->ld, rows, n_draws, ld_drawn, P->d_out, P->stream);
-    };
-    for (int64_t r0 = 0; r0 < n_rows; r0 += cap) {
-        const int64_t rows = std::min(cap, n_rows - r0);
-        if (P->n_ev > 0)
-            SBN_CUDA(cudaMemcpy2DAsync(P->d_ev, static_cast<size_t>(P->ld), ev + r0, static_cast<size_t>(ld_ev),
-                                       static_cast<size_t>(rows), static_cast<size_t>(P->n_ev), cudaMemcpyHostToDevice, P->stream));
+    rc = for_each_chunk(P, ev, ld_ev, n_rows, cap, [&](int64_t r0, int64_t rows) -> int {
         // read by the sample steps at run time, so that one captured graph serves every seed and chunk
         const uint64_t first = static_cast<uint64_t>(row_base + r0);
         const uint32_t args[4] = {static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32), static_cast<uint32_t>(first),
                                   static_cast<uint32_t>(first >> 32)};
         if (!mpe) SBN_CUDA(cudaMemcpyAsync(P->d_sample_args, args, sizeof args, cudaMemcpyHostToDevice, P->stream));
-        // a short chunk runs as plain launches: capturing and instantiating a graph costs more than it saves, and
-        // the short runs of a pattern whose rows are scattered through a frame come in many lengths
-        if (!P->use_graph || rows < kSampleGraphMinRows) {
-            const int rc = issue(rows);
-            if (rc != SBN_OK) return rc;
-        } else {
-            // one graph per (chunk size, n_draws, drawn-code buffer)
-            auto &k = P->graph_key;
-            if (!P->exec || k.ev != P->d_ev || k.n_rows != rows || k.out != reinterpret_cast<float *>(P->d_drawn) ||
-                k.ld_out != ld_drawn || P->graph_draws != n_draws) {
-                if (P->exec) {
-                    cudaGraphExecDestroy(P->exec);
-                    P->exec = nullptr;
-                }
-                SBN_CUDA(cudaStreamBeginCapture(P->stream, cudaStreamCaptureModeRelaxed));
-                const int64_t before = P->launches;
-                const int rc = issue(rows);
-                cudaGraph_t graph = nullptr;
-                cudaError_t e = cudaStreamEndCapture(P->stream, &graph);
-                P->graph_launches = P->launches - before;
-                P->launches = before;
-                if (rc != SBN_OK) {
-                    if (graph) cudaGraphDestroy(graph);
-                    return rc;
-                }
-                if (e != cudaSuccess) return fail(SBN_E_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
-                e = cudaGraphInstantiate(&P->exec, graph, 0);
-                cudaGraphDestroy(graph);
-                if (e != cudaSuccess) return fail(SBN_E_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
-                k = {P->d_ev, P->ld, rows, reinterpret_cast<float *>(P->d_drawn), ld_drawn};
-                P->graph_draws = n_draws;
-            }
-            SBN_CUDA(cudaGraphLaunch(P->exec, P->stream));
-            P->launches += P->graph_launches;
-        }
+        const int rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream, dc);
+        if (rc != SBN_OK) return rc;
         if (P->n_sampled > 0)
-            SBN_CUDA(cudaMemcpy2DAsync(out + r0, static_cast<size_t>(n_rows), P->d_drawn, static_cast<size_t>(ld_drawn),
+            SBN_CUDA(cudaMemcpy2DAsync(out + r0, static_cast<size_t>(n_rows), P->d_drawn, static_cast<size_t>(dc.ld_drawn),
                                        static_cast<size_t>(rows), static_cast<size_t>(P->n_sampled * n_draws),
                                        cudaMemcpyDeviceToHost, P->stream));
         if (!mpe || ps.batched)
@@ -2042,7 +1889,9 @@ static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, 
                                      static_cast<size_t>(rows) * elem, cudaMemcpyDeviceToHost, P->stream));
         else if (r0 == 0)
             SBN_CUDA(cudaMemcpyAsync(prob, ps.ptr, elem, cudaMemcpyDeviceToHost, P->stream));
-    }
+        return SBN_OK;
+    });
+    if (rc != SBN_OK) return rc;
     SBN_CUDA(cudaStreamSynchronize(P->stream));
     if (mpe && !ps.batched) std::fill(static_cast<float *>(prob) + 1, static_cast<float *>(prob) + n_rows, *static_cast<float *>(prob));
     return SBN_OK;
@@ -2059,7 +1908,7 @@ int sbn_program_sample_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev
 }
 
 int sbn_program_mpe_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, uint8_t *codes, float *log_prob) {
-    return sample_host_common(P, ev, ld_ev, n_rows, 1, 0, 0, codes, log_prob, false, true);
+    return sample_host_common(P, ev, ld_ev, n_rows, 1, 0, 0, codes, log_prob, false, kMpe);
 }
 
 int sbn_program_profile(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out,
@@ -2069,11 +1918,8 @@ int sbn_program_profile(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int6
     if (P->f64) return fail(SBN_E_INVALID, "profiling is for float32 programs");
     const int64_t n = static_cast<int64_t>(P->steps.size()) + 1;
     if (!step_ms || n_step_ms < n) return fail(SBN_E_INVALID, "step_ms needs %lld entries", (long long)n);
-    SBN_CUDA(cudaSetDevice(P->device));
-    if (n_rows > P->reserved_rows) {
-        rc = sbn_program_reserve(P, n_rows);
-        if (rc != SBN_OK) return rc;
-    }
+    rc = reserve_rows(P, n_rows);
+    if (rc != SBN_OK) return rc;
     if (n_rows > P->reserved_rows) return fail(SBN_E_NOMEM, "n_rows exceeds the scratch that fits the device");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     std::vector<cudaEvent_t> ev(n + 1);
@@ -2149,18 +1995,6 @@ int sbn_program_step_roles(const sbn_program *P, int32_t *roles, int64_t n_roles
         }
     }
     return SBN_OK;
-}
-
-static void drop_graphs(sbn_program *P) {
-    // captured launches embed the kernel variants and pointers of the moment they were captured
-    if (P->exec) {
-        cudaGraphExecDestroy(P->exec);
-        P->exec = nullptr;
-    }
-    if (P->pipe_exec) {
-        cudaGraphExecDestroy(P->pipe_exec);
-        P->pipe_exec = nullptr;
-    }
 }
 
 int sbn_program_set_graph(sbn_program *P, int enabled) {

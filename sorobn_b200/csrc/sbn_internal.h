@@ -76,27 +76,51 @@ inline int64_t round_up(int64_t v, int64_t m) { return (v + m - 1) / m * m; }
 struct SbnSegment;  // sbn_chain.h
 struct SbnPair;     // sbn_pair.h
 
+// What a program computes, fixed by its header version (4 .. 8 in this order)
+enum ProgramKind {
+    kPosterior,  // kind-0 / 1 steps, then the normalised posterior slot
+    kMarginals,  // kind-2 readouts write the posterior, already normalised; no posterior slot
+    kCounts,     // kind-3 steps add expected counts, post_slot holds P(observed)
+    kSample,     // kind-4 steps draw codes, post_slot holds P(observed)
+    kMpe,        // log tables, max-sum upward pass, kind-5 argmax steps decode into the drawn-code buffer with
+                 // one draw, post_slot holds max log P(x, e)
+};
+
+// Every address and size a captured graph bakes in: it is replayed only for an equal key
+struct GraphKey {
+    const void *ev = nullptr;
+    int64_t ld_ev = 0, n_rows = 0;
+    const void *out = nullptr;
+    int64_t ld_out = 0;
+    const void *partial = nullptr;  // counts program: the per-warp partial tables
+    const void *drawn = nullptr;    // sample / MPE program: the drawn-code buffer, its draws and pitch
+    int64_t n_draws = 0, ld_drawn = 0;
+    bool operator==(const GraphKey &o) const {
+        return ev == o.ev && out == o.out && ld_ev == o.ld_ev && n_rows == o.n_rows && ld_out == o.ld_out &&
+               partial == o.partial && drawn == o.drawn && n_draws == o.n_draws && ld_drawn == o.ld_drawn;
+    }
+};
+struct CachedGraph {
+    cudaGraphExec_t exec = nullptr;
+    GraphKey key;
+    int64_t launches = 0;  // kernel launches one replay stands for (sbn_program::launches)
+};
+
 struct sbn_program {
     int device = 0;
     int n_sms = 1;     // multiprocessors of `device`: the grid-size heuristics count waves in them
     bool f64 = false;  // single-event programs computed and returned in double
+    ProgramKind kind = kPosterior;
     int mode = 0, n_ev = 0, Q = 0, post_slot = 0, post_batched = 0;
-    bool marginals = false;  // version-5 program: kind-2 readouts write the posterior, already normalised
-    bool counts = false;     // version-6 program: kind-3 steps add expected counts, post_slot holds P(observed)
     int64_t n_counts = 0;    // counts program: entries of the count table
     int64_t n_table_floats = 0;  // size of the table blob (sbn_program_set_tables replaces it in place)
     double *d_counts = nullptr;   // counts program: the run's count table [n_counts]
     double *d_partial = nullptr;  // counts program: per-warp partial tables of one count step (during a counts call only)
-    const double *graph_partial = nullptr;  // the partial tables the captured counts graph writes
     int64_t partial_doubles = 0;
-    bool sample = false;          // version-7 program: kind-4 steps draw codes, post_slot holds P(observed)
-    bool mpe = false;             // version-8 program: log tables, max-sum upward pass, kind-5 argmax steps,
-                                  // post_slot holds max log P(x, e); also uses n_sampled / d_drawn with one draw
     int n_sampled = 0;            // sample / MPE program: drawn-code rows (one per unobserved variable)
     uint8_t *d_drawn = nullptr;   // sample program: drawn codes [n_sampled][n_draws][ld_drawn], then flags [ld_drawn]
     int64_t drawn_bytes = 0;
     uint32_t *d_sample_args = nullptr;  // seed lo, seed hi, row_base lo, row_base hi of the current chunk
-    int64_t graph_draws = 0;      // n_draws of the captured sample graph
     std::vector<std::pair<int64_t, int64_t>> tables;  // (offset, size) in floats
     std::vector<int64_t> table_padded;
     float *d_tables = nullptr;
@@ -119,28 +143,14 @@ struct sbn_program {
     cudaStream_t branch[kBranches] = {nullptr, nullptr, nullptr, nullptr};
     std::vector<cudaEvent_t> step_done;  // one event per step (+ normalise), capture-only
     std::vector<cudaEvent_t> pipe_events;  // run_host pipelining: fork, (upload done, kernels done) per column range, joins
-    cudaGraphExec_t pipe_exec = nullptr;   // the pipelined host run as one graph (pinned host buffers)
-    struct {
-        const void *ev;
-        int64_t ld_ev, n_rows;
-        const void *out;
-        int64_t ld_out;
-    } pipe_key = {nullptr, 0, 0, nullptr, 0};
-    int64_t pipe_launches = 0;
     bool use_branches = false;  // measured: no gain on the grid plan (one long chain); opt-in
 
     bool use_graph = true;
     bool use_tiled = true;
     bool use_slab = true;
     bool use_preload = true;  // tiled kernel: operand preload schedule where instantiated (else the x-loop)
-    cudaGraphExec_t exec = nullptr;
-    struct {
-        const uint8_t *ev;
-        int64_t ld_ev, n_rows;
-        float *out;
-        int64_t ld_out;
-    } graph_key = {nullptr, 0, 0, nullptr, 0};
-    int64_t graph_launches = 0;
+    CachedGraph graph;       // one run of rows on the device
+    CachedGraph pipe_graph;  // the pipelined host run (pinned host buffers)
 
     int64_t launches = 0;
     int64_t setup_launches = 0;  // evidence-independent launches issued once at creation

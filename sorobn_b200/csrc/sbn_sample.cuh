@@ -34,12 +34,13 @@
 struct SbnSampleIn {
     const void *ptr;                 // table / slot base (device), float or double
     int32_t batched;                 // 1: entry e of row b is at e * ld + b
-    int32_t n_terms;
+    int32_t n_ev;                    // gathered (col stride card) terms
     int32_t smem_off;                // float offset of the staged copy, -1 = read global
     int32_t stage_floats;
-    int32_t t_col[SBN_SAMPLE_MAX_TERMS];     // < n_ev: evidence column; otherwise drawn-code row t_col - n_ev
-    int32_t t_stride[SBN_SAMPLE_MAX_TERMS];
-    int32_t t_card[SBN_SAMPLE_MAX_TERMS];
+    int32_t ev_col[SBN_SAMPLE_MAX_TERMS];    // < SbnSample::n_ev: evidence column; otherwise drawn-code row
+                                             // ev_col - SbnSample::n_ev
+    int32_t ev_stride[SBN_SAMPLE_MAX_TERMS];
+    int32_t ev_card[SBN_SAMPLE_MAX_TERMS];
 };
 
 struct SbnSample {
@@ -77,11 +78,11 @@ __device__ __forceinline__ void sbn_decode_operands(const SbnSample &p, const fl
         if (i < p.n_in) {
             const SbnSampleIn &in = p.in[i];
             int64_t off = 0;
-            for (int t = 0; t < in.n_terms; ++t) {
-                const int col = in.t_col[t];
+            for (int t = 0; t < in.n_ev; ++t) {
+                const int col = in.ev_col[t];
                 const int code = col < p.n_ev ? p.ev[static_cast<int64_t>(col) * p.ld_ev + b]
                                                : p.drawn[(static_cast<int64_t>(col - p.n_ev) * p.n_draws + d) * p.ld_drawn + b];
-                off += static_cast<int64_t>(min(code, in.t_card[t] - 1)) * in.t_stride[t];
+                off += static_cast<int64_t>(min(code, in.ev_card[t] - 1)) * in.ev_stride[t];
             }
             if (in.batched) {
                 src[i] = static_cast<const T *>(in.ptr) + b + off * p.ld;
