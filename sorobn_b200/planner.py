@@ -354,8 +354,19 @@ def build_plan(net: CompiledNet, query, evidence, mode=MODE_BATCHED, order=None,
     query / evidence are sequences of var ids.  `evidence` fixes the evidence
     *columns*; their values arrive at run time.
     """
-    return _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evidence, allow_empty_query,
-                  fuse_elims, None)
+    query, evidence = tuple(query), tuple(evidence)
+    if not query and not allow_empty_query:
+        # bayes_net.py:840-841
+        raise ValueError("At least one query variable has to be specified")
+    if not query and not evidence:
+        raise ValueError("nothing to compute: no query variable and no evidence")
+    if set(query) & set(evidence):
+        # bayes_net.py:843-845
+        raise ValueError("A query variable cannot be part of the event")
+    if len(set(query)) != len(query):
+        raise ValueError("duplicate variable in query or event")
+    return _build(net, VERSION, evidence, query=query, mode=mode, order=order, max_in=max_in,
+                  lift_evidence=lift_evidence, fuse_elims=fuse_elims, merge_sum_outs=merge_sum_outs)
 
 
 def build_marginals_plan(net: CompiledNet, evidence, targets=None, mode=MODE_BATCHED, order=None, max_in=MAX_IN,
@@ -374,7 +385,8 @@ def build_marginals_plan(net: CompiledNet, evidence, targets=None, mode=MODE_BAT
         raise ValueError("A query variable cannot be part of the event")
     if len(set(targets)) != len(targets):
         raise ValueError("duplicate target variable")
-    return _build(net, (), evidence, mode, order, max_in, False, lift_evidence, True, fuse_elims, targets)
+    return _build(net, VERSION_MARGINALS, evidence, targets=targets, mode=mode, order=order, max_in=max_in,
+                  lift_evidence=lift_evidence, fuse_elims=fuse_elims)
 
 
 def build_counts_plan(net: CompiledNet, evidence, mode=MODE_BATCHED, order=None, max_in=MAX_IN, lift_evidence=True,
@@ -384,7 +396,8 @@ def build_counts_plan(net: CompiledNet, evidence, mode=MODE_BATCHED, order=None,
     Its count table is laid out by `count_layout`."""
     evidence = tuple(evidence)
     hidden = tuple(v for v in range(len(net.names)) if v not in set(evidence))
-    return _build(net, (), evidence, mode, order, max_in, False, lift_evidence, True, fuse_elims, hidden, counts=True)
+    return _build(net, VERSION_COUNTS, evidence, targets=hidden, mode=mode, order=order, max_in=max_in,
+                  lift_evidence=lift_evidence, fuse_elims=fuse_elims)
 
 
 def build_sample_plan(net: CompiledNet, evidence, order=None, max_in=MAX_IN, lift_evidence=True, fuse_elims=None) -> Plan:
@@ -393,8 +406,8 @@ def build_sample_plan(net: CompiledNet, evidence, order=None, max_in=MAX_IN, lif
     top-down.  `Plan.sampled` names the variable of every drawn-code row."""
     evidence = tuple(evidence)
     hidden = tuple(v for v in range(len(net.names)) if v not in set(evidence))
-    return _build(net, (), evidence, MODE_BATCHED, order, max_in, False, lift_evidence, True, fuse_elims, hidden,
-                  sample=KIND_SAMPLE)
+    return _build(net, VERSION_SAMPLE, evidence, targets=hidden, order=order, max_in=max_in,
+                  lift_evidence=lift_evidence, fuse_elims=fuse_elims)
 
 
 def build_mpe_plan(net: CompiledNet, evidence, order=None, max_in=MAX_IN, lift_evidence=True, fuse_elims=None) -> Plan:
@@ -404,8 +417,8 @@ def build_mpe_plan(net: CompiledNet, evidence, order=None, max_in=MAX_IN, lift_e
     do not max to 1 -- and `Plan.sampled` names the variable of every decoded-code row."""
     evidence = tuple(evidence)
     hidden = tuple(v for v in range(len(net.names)) if v not in set(evidence))
-    return _build(net, (), evidence, MODE_BATCHED, order, max_in, False, lift_evidence, True, fuse_elims, hidden,
-                  sample=KIND_ARGMAX)
+    return _build(net, VERSION_MPE, evidence, targets=hidden, order=order, max_in=max_in,
+                  lift_evidence=lift_evidence, fuse_elims=fuse_elims)
 
 
 def count_layout(net: CompiledNet):
@@ -433,72 +446,34 @@ def refresh_tables(plan: Plan, cpts):
     return blob64.astype(np.float32), blob64
 
 
-def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evidence, allow_empty_query, fuse_elims,
-           targets, counts=False, sample=None):
-    if merge_sum_outs is None:
-        merge_sum_outs = os.environ.get("SOROBN_B200_MERGE", "0") == "1"
-    if fuse_elims is None:
-        fuse_elims = os.environ.get("SOROBN_B200_FUSE", "1") == "1"
-    query = tuple(query)
-    evidence = tuple(evidence)
-    if not query and not allow_empty_query:
-        # bayes_net.py:840-841
-        raise ValueError("At least one query variable has to be specified")
-    if not query and not evidence and targets is None:
-        raise ValueError("nothing to compute: no query variable and no evidence")
-    if set(query) & set(evidence):
-        # bayes_net.py:843-845
-        raise ValueError("A query variable cannot be part of the event")
-    if len(set(query)) != len(query) or len(set(evidence)) != len(evidence):
-        raise ValueError("duplicate variable in query or event")
-    card = net.card
-    for v in evidence:
-        if card[v] > 255:
-            raise ValueError(f"evidence variable {net.names[v]!r} has {card[v]} states; state codes are uint8")
+class _Builder:
+    """The planning state every program kind shares: the shipped tables, the steps emitted so far and
+    the next logical id, with the launch-building rules over them (`emit` and the products built on
+    it).  `_build` makes one per plan and runs the upward pass through it; the kind's tail adds its
+    own steps and ends with `finish`."""
 
-    # bayes_net.py:763-766
-    relevant = {*query, *evidence, *(targets or ())}
-    for v in list(relevant):
-        relevant |= net.ancestors(v)
-    hidden = relevant - set(query) - set(evidence)
-    ev_col = {v: i for i, v in enumerate(evidence)}
+    def __init__(self, net, evidence, mode, max_in, lift_evidence, tables):
+        self.net, self.card = net, net.card
+        self.evidence = evidence
+        self.ev_col = {v: i for i, v in enumerate(evidence)}
+        self.mode, self.max_in, self.lift_evidence = mode, max_in, lift_evidence
+        self.order = None  # elimination order (var ids), set by `_build`
+        self.steps = []
+        self.tables = tables  # var ids whose CPTs are shipped, in table order
+        self.table_arrays = []
+        self.table_axes = []  # variable of every axis of table_arrays[t], outermost first
+        self.next_id = 0
 
-    # bayes_net.py:768-776 -- one factor per relevant CPT; evidence axes become
-    # per-row gathers instead of boolean filters
-    tables = sorted(relevant)
-    factors = []
-    table_arrays = []
-    table_axes = []  # variable of every axis of table_arrays[t], outermost first
-    for t, v in enumerate(tables):
-        scope = net.scope(v)
-        # Shipped layout: free axes first (reference order), evidence axes innermost.  Rows of
-        # a warp differ only in their evidence codes, so their gathers of one entry then fall
-        # into one 32-byte sector / distinct shared-memory banks instead of `stride` apart.
-        perm = [i for i, u in enumerate(scope) if u not in ev_col] + [i for i, u in enumerate(scope) if u in ev_col]
-        arr = np.ascontiguousarray(np.transpose(net.cpt[v], perm))
-        table_arrays.append(arr)
-        pscope = [scope[i] for i in perm]
-        table_axes.append(list(pscope))
-        shape = [int(card[u]) for u in pscope]
-        strides = [int(np.prod(shape[i + 1:], dtype=np.int64)) for i in range(len(shape))]
-        free = [(u, s) for u, s in zip(pscope, strides) if u not in ev_col]
-        ev = tuple((ev_col[u], s, int(card[u])) for u, s in zip(pscope, strides) if u in ev_col)
-        if len(ev) > MAX_EV:
-            raise ValueError(f"CPT of {net.names[v]!r} has {len(ev)} evidence axes; the kernel supports {MAX_EV}")
-        factors.append(_Factor(False, t, tuple(u for u, _ in free), tuple(s for _, s in free), ev, False))
+    def size(self, vs):
+        """Joint states of the variables `vs`."""
+        return int(np.prod([self.card[v] for v in vs], dtype=np.int64)) if vs else 1
 
-    if order is None:
-        order = _min_fill_order([f.vars for f in factors], hidden, card)
-    else:
-        order = list(order)
-        if set(order) != hidden or len(order) != len(hidden):
-            raise ValueError("elimination order must be a permutation of the hidden variables")
+    def largest(self, inputs):
+        """The largest batched operand (the largest table when none is batched)."""
+        return max(inputs, key=lambda f: (f.batched, self.size(f.vars)))
 
-    steps = []
-    next_id = [0]
-
-    def emit(inputs, elim, out_vars, may_lift=True):
-        """One fused launch: multiply `inputs`, sum out `elim` (None: product only).
+    def emit(self, inputs, elims, out_vars, may_lift=True):
+        """One fused launch: multiply `inputs`, sum out `elims` (empty: product only).
         out_vars is given fastest axis first.  The output gets a logical id; physical
         slots are assigned after the merge pass.
 
@@ -509,19 +484,20 @@ def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evide
         launch; consumers gather from it like from a CPT.  The reference filters every CPT by
         the event first (bayes_net.py:772-774); filtering after multiplying gives the same
         numbers and turns per-row work into per-call work."""
-        elims = () if elim is None else (tuple(elim) if isinstance(elim, (tuple, list)) else (elim,))
+        card, evidence = self.card, self.evidence
+        elims = tuple(elims)
         ecards = tuple(int(card[e]) for e in elims)
         dep = any(f.depends_on_evidence for f in inputs)
-        batched = dep and mode == MODE_BATCHED
+        batched = dep and self.mode == MODE_BATCHED
         if len(out_vars) > MAX_AXES:
             raise ValueError(f"a factor over {len(out_vars)} variables exceeds the kernel's {MAX_AXES} axes")
         cards = tuple(int(card[u]) for u in out_vars)
-        size = int(np.prod(cards, dtype=np.int64)) if cards else 1
+        size = self.size(out_vars)
         if size >= 2**31:
             raise ValueError("a factor with >= 2^31 entries per row does not fit the 32-bit scope index")
 
         lifted_cols = None
-        if batched and lift_evidence and may_lift and not any(f.batched for f in inputs):
+        if batched and self.lift_evidence and may_lift and not any(f.batched for f in inputs):
             cols = []
             for f in inputs:
                 for col, _, c in f.ev:
@@ -532,8 +508,8 @@ def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evide
                 lifted_cols = cols
 
         ins = []
-        out_id = next_id[0]
-        next_id[0] += 1
+        out_id = self.next_id
+        self.next_id += 1
         if lifted_cols is not None:
             ev_vars = [evidence[col] for col, _ in lifted_cols]
             axes = tuple(ev_vars) + tuple(out_vars)  # evidence axes innermost
@@ -544,31 +520,21 @@ def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evide
                 es = tuple(pos.get(e, 0) for e in elims)
                 plain = _Factor(f.is_slot, f.buf, f.vars, f.strides, (), False)  # evidence axes are output axes here
                 ins.append((plain, es, tuple(pos.get(u, 0) for u in axes)))
-            steps.append(Step(KIND_FLAT, ins, out_id, axes, axis_cards, elims, ecards))
-            strides, acc = [], 1
-            for c in axis_cards:
-                strides.append(acc)
-                acc *= c
+            self.steps.append(Step(KIND_FLAT, ins, out_id, axes, axis_cards, elims, ecards))
+            strides = _dense_strides(axis_cards)
             n_ev = len(lifted_cols)
             ev = tuple((col, strides[k], c) for k, (col, c) in enumerate(lifted_cols))
-            return _Factor(True, out_id, tuple(out_vars), tuple(strides[n_ev:]), ev, False)
+            return _Factor(True, out_id, tuple(out_vars), strides[n_ev:], ev, False)
 
         for f in inputs:
             pos = {u: s for u, s in zip(f.vars, f.strides)}
             es = tuple(pos.get(e, 0) for e in elims)
             ins.append((f, es, tuple(pos.get(u, 0) for u in out_vars)))
-        steps.append(Step(KIND_BATCHED if batched else KIND_FLAT, ins, out_id, tuple(out_vars), cards, elims, ecards))
-        out_strides = []
-        acc = 1
-        for c in cards:
-            out_strides.append(acc)
-            acc *= c
-        return _Factor(True, out_id, tuple(out_vars), tuple(out_strides), (), batched)
+        self.steps.append(Step(KIND_BATCHED if batched else KIND_FLAT, ins, out_id, tuple(out_vars), cards, elims,
+                               ecards))
+        return _Factor(True, out_id, tuple(out_vars), _dense_strides(cards), (), batched)
 
-    def fsize(f):
-        return int(np.prod([card[u] for u in f.vars], dtype=np.int64)) if f.vars else 1
-
-    def axis_order(inputs, out_set):
+    def axis_order(self, inputs, out_set):
         """Fastest-first order of the output axes (`_tile_axes` in the kernel docs).
 
         Axes 0 and 1 span the register tile of csrc/sbn_step_tiled: an input that lacks
@@ -577,8 +543,9 @@ def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evide
         (batched inputs weigh double: they come from L1/L2/HBM, tables from shared
         memory) and the cheapest pair wins; the remaining axes follow the largest
         batched input's own order so that its reads stay sequential."""
+        card = self.card
         out = sorted(out_set)
-        big = max(inputs, key=lambda f: (f.batched, fsize(f)))
+        big = self.largest(inputs)
         tail = [u for _, u in sorted(zip(big.strides, big.vars)) if u in out_set]
         tail += [u for u in out if u not in big.vars]
         if len(out) < 2:
@@ -599,53 +566,151 @@ def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evide
                     best_key, best = key, (a0, a1)
         return [best[0], best[1]] + [u for u in tail if u not in best]
 
-    def lifted_size(fs):
-        vs = set().union(*[f.vars for f in fs])
-        cols = {(col, c) for f in fs for col, _, c in f.ev}
-        return int(np.prod([card[u] for u in vs], dtype=np.int64)) * int(np.prod([c for _, c in cols], dtype=np.int64))
-
-    def combine_tables(inputs, limit=TILED_MAX_IN):
+    def combine_tables(self, inputs, limit=TILED_MAX_IN):
         """A launch with more than TILED_MAX_IN factors falls off the tiled kernel.  When the
         surplus is small tables, multiply those together first: a table-only product is an
         evidence-independent flat launch (see `emit`), and the big launch then gathers one
         value where it gathered several."""
         inputs = list(inputs)
-        if mode != MODE_BATCHED or not lift_evidence:
+        if self.mode != MODE_BATCHED or not self.lift_evidence:
             return inputs
         while len(inputs) > limit:
             tabs = [f for f in inputs if not f.batched]
             best = None
             for i in range(len(tabs)):
                 for j in range(i + 1, len(tabs)):
-                    sz = lifted_size([tabs[i], tabs[j]])
-                    n_cols = len({col for f in (tabs[i], tabs[j]) for col, _, _ in f.ev})
+                    fa, fb = tabs[i], tabs[j]
+                    cols = {(col, c) for f in (fa, fb) for col, _, c in f.ev}
+                    sz = self.size(set(fa.vars) | set(fb.vars)) * int(np.prod([c for _, c in cols], dtype=np.int64))
+                    n_cols = len({col for col, _ in cols})
                     if sz <= LIFT_MAX and n_cols <= MAX_EV and (best is None or sz < best[0]):
-                        best = (sz, tabs[i], tabs[j])
+                        best = (sz, fa, fb)
             if best is None:
                 break
             _, fa, fb = best
             inputs = [f for f in inputs if f is not fa and f is not fb]
-            inputs.append(emit([fa, fb], None, sorted(set(fa.vars) | set(fb.vars))))
+            inputs.append(self.emit([fa, fb], (), sorted(set(fa.vars) | set(fb.vars))))
         return inputs
 
-    def product_chain(inputs, elim, final_vars=None):
+    def fold(self, inputs):
+        """At most max_in factors per launch: bayes_net.py:256 reduces pairwise; multiply the
+        smallest max_in together first while there are more."""
+        inputs = list(inputs)
+        while len(inputs) > self.max_in:
+            inputs.sort(key=lambda f: self.size(f.vars))
+            head, inputs = inputs[:self.max_in], inputs[self.max_in:]
+            inputs.append(self.emit(head, (), self.axis_order(head, set().union(*[f.vars for f in head]))))
+        return inputs
+
+    def product_chain(self, inputs, elims, final_vars=None):
+        """Multiply `inputs` and sum out `elims` in one launch, after combining and folding the
+        surplus factors.  With `final_vars`, a product-only launch over exactly those axes."""
         # a launch that sums out several variables keeps to the preload schedule's 3 inputs
-        fused = isinstance(elim, (tuple, list)) and len(elim) > 1
-        inputs = combine_tables(inputs, PRELOAD_MAX_IN if fused else TILED_MAX_IN)
-        # bayes_net.py:256 reduces pairwise; fuse up to max_in factors per launch and
-        # fold the smallest ones first when there are more
-        while len(inputs) > max_in:
-            inputs.sort(key=fsize)
-            head, inputs = inputs[:max_in], inputs[max_in:]
-            union = set().union(*[f.vars for f in head])
-            inputs.append(emit(head, None, axis_order(head, union)))
-        union = set().union(*[f.vars for f in inputs]) if inputs else set()
+        inputs = self.fold(self.combine_tables(inputs, PRELOAD_MAX_IN if len(elims) > 1 else TILED_MAX_IN))
+        union = set().union(*[f.vars for f in inputs])
         if final_vars is not None:
             assert union == set(final_vars), (union, final_vars)
-            return emit(inputs, None, list(final_vars), may_lift=False)
-        elims = () if elim is None else (tuple(elim) if isinstance(elim, (tuple, list)) else (elim,))
-        out_set = union - set(elims)
-        return emit(inputs, elims if elims else None, axis_order(inputs, out_set))
+            return self.emit(inputs, (), list(final_vars), may_lift=False)
+        return self.emit(inputs, elims, self.axis_order(inputs, union - set(elims)))
+
+    def message(self, inputs, out_vars, elims):
+        """sum_{elims} prod(inputs) over out_vars, at most MAX_ELIM variables / MAX_Z joint states per launch:
+        the first launch multiplies and sums out the first group, each later one sums out the next group."""
+        card = self.card
+        groups, cur, z = [], [], 1
+        for v in sorted(elims, key=lambda v: (-int(card[v]), v)):
+            if cur and (len(cur) >= MAX_ELIM or z * int(card[v]) > MAX_Z):
+                groups.append(cur)
+                cur, z = [], 1
+            cur.append(v)
+            z *= int(card[v])
+        if cur:
+            groups.append(cur)
+        inputs = self.fold(self.combine_tables(inputs, PRELOAD_MAX_IN if groups and len(groups[0]) > 1
+                                               else TILED_MAX_IN))
+        if not groups:
+            return self.emit(inputs, (), self.axis_order(inputs, set(out_vars)))
+        rest = [v for g in groups for v in g]
+        f = None
+        for g in groups:
+            rest = [v for v in rest if v not in g]
+            keep = set(out_vars) | set(rest)
+            src = inputs if f is None else [f]
+            f = self.emit(src, tuple(g), self.axis_order(src, keep))
+        return f
+
+    def finish(self, version, post, Q, query=(), **fields):
+        """Assign the slots, build the Plan and serialise it.  `post` is the factor the header's slot
+        holds (None for a marginals plan: its readouts write the posterior)."""
+        slots, where = _assign_slots(self.steps, keep_unbatched=(self.mode == MODE_BATCHED),
+                                     park_batched=(version == VERSION))
+        plan = Plan(mode=self.mode, query=query, evidence=self.evidence, order=list(self.order), tables=self.tables,
+                    slots=slots, steps=self.steps, post_slot=-1 if post is None else where[post.buf], Q=Q,
+                    version=version, table_axes=[list(a) for a in self.table_axes],
+                    table_scopes=[self.net.scope(v) for v in self.tables], **fields)
+        plan._card = self.card
+        _serialise(plan, self.table_arrays)
+        return plan
+
+
+def _dense_strides(cards):
+    """Element strides of a dense array over `cards`, axis 0 fastest."""
+    strides, acc = [], 1
+    for c in cards:
+        strides.append(acc)
+        acc *= c
+    return tuple(strides)
+
+
+def _build(net, version, evidence, query=(), targets=(), mode=MODE_BATCHED, order=None, max_in=MAX_IN,
+           lift_evidence=True, fuse_elims=None, merge_sum_outs=None):
+    """A plan of program `version` (VERSION, VERSION_MARGINALS, ...): the upward pass of variable
+    elimination, then the kind's tail.  `targets` are kept relevant besides the query and the evidence:
+    a marginals plan reads them out, and counts, sample and MPE plans pass every unobserved variable."""
+    if fuse_elims is None:
+        fuse_elims = os.environ.get("SOROBN_B200_FUSE", "1") == "1"
+    if len(set(evidence)) != len(evidence):
+        raise ValueError("duplicate variable in query or event")
+    card = net.card
+    for v in evidence:
+        if card[v] > 255:
+            raise ValueError(f"evidence variable {net.names[v]!r} has {card[v]} states; state codes are uint8")
+
+    # bayes_net.py:763-766
+    relevant = {*query, *evidence, *targets}
+    for v in list(relevant):
+        relevant |= net.ancestors(v)
+    hidden = relevant - set(query) - set(evidence)
+    b = _Builder(net, evidence, mode, max_in, lift_evidence, sorted(relevant))
+    ev_col = b.ev_col
+
+    # bayes_net.py:768-776 -- one factor per relevant CPT; evidence axes become
+    # per-row gathers instead of boolean filters
+    factors = []
+    for t, v in enumerate(b.tables):
+        scope = net.scope(v)
+        # Shipped layout: free axes first (reference order), evidence axes innermost.  Rows of
+        # a warp differ only in their evidence codes, so their gathers of one entry then fall
+        # into one 32-byte sector / distinct shared-memory banks instead of `stride` apart.
+        perm = [i for i, u in enumerate(scope) if u not in ev_col] + [i for i, u in enumerate(scope) if u in ev_col]
+        b.table_arrays.append(np.ascontiguousarray(np.transpose(net.cpt[v], perm)))
+        pscope = [scope[i] for i in perm]
+        b.table_axes.append(list(pscope))
+        shape = [int(card[u]) for u in pscope]
+        strides = [int(np.prod(shape[i + 1:], dtype=np.int64)) for i in range(len(shape))]
+        free = [(u, s) for u, s in zip(pscope, strides) if u not in ev_col]
+        ev = tuple((ev_col[u], s, int(card[u])) for u, s in zip(pscope, strides) if u in ev_col)
+        if len(ev) > MAX_EV:
+            raise ValueError(f"CPT of {net.names[v]!r} has {len(ev)} evidence axes; the kernel supports {MAX_EV}")
+        factors.append(_Factor(False, t, tuple(u for u, _ in free), tuple(s for _, s in free), ev, False))
+
+    if order is None:
+        order = _min_fill_order([f.vars for f in factors], hidden, card)
+    else:
+        order = list(order)
+        if set(order) != hidden or len(order) != len(hidden):
+            raise ValueError("elimination order must be a permutation of the hidden variables")
+    b.order = order
 
     # bayes_net.py:778-786
     # Fused eliminations.  A later variable w of the order joins x's launch when every factor
@@ -654,7 +719,7 @@ def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evide
     # separate launches walk, but the intermediate over w is never written and read back, and
     # the tile axes are chosen for the launch's real output.
     gone = set()
-    buckets = []  # marginals plans: (F_k, eliminated variables, U_k, lambda_k) per launch of the loop below
+    buckets = []  # (F_k, eliminated variables, U_k, lambda_k) per launch of the loop below
     for k, x in enumerate(order):
         if x in gone:
             continue
@@ -679,44 +744,31 @@ def _build(net, query, evidence, mode, order, max_in, merge_sum_outs, lift_evide
                 elims.append(w)
                 z *= int(card[w])
         gone.update(elims)
-        bucket_factors = list(touching)
-        factors.append(product_chain(touching, tuple(elims)))
-        if targets is not None:
-            buckets.append((bucket_factors, tuple(elims), set().union(*[f.vars for f in bucket_factors]), factors[-1]))
+        factors.append(b.product_chain(touching, tuple(elims)))
+        buckets.append((touching, tuple(elims), set().union(*[f.vars for f in touching]), factors[-1]))
 
-    if sample is not None:
-        return _sample_passes(net, evidence, order, max_in, buckets, factors, steps, tables, table_arrays, table_axes,
-                              emit, combine_tables, axis_order, fsize, sample)
-    if counts:
-        return _counts_passes(net, evidence, mode, order, max_in, buckets, factors, steps, tables, table_arrays,
-                              table_axes, emit, combine_tables, axis_order, fsize)
-    if targets is not None:
-        return _marginals_passes(net, evidence, mode, order, max_in, targets, buckets, factors, steps, tables,
-                                 table_arrays, emit, combine_tables, axis_order, fsize)
+    if version == VERSION_MARGINALS:
+        return _marginals_passes(b, buckets, factors, targets)
+    if version == VERSION_COUNTS:
+        return _counts_passes(b, buckets, factors)
+    if version in (VERSION_SAMPLE, VERSION_MPE):
+        return _sample_passes(b, buckets, factors, version)
 
     # bayes_net.py:788-794: product of what is left; the answer's levels are sorted
     # by name (bayes_net.py:872-873) and rows by state (sort_index, :875)
     q_sorted = tuple(sorted(query, key=lambda v: net.names[v]))
-    post = product_chain(factors, None, final_vars=tuple(reversed(q_sorted)))
-    Q = fsize(post)
-
-    steps = _merge_sum_outs(steps, merge_sum_outs)
+    post = b.product_chain(factors, (), final_vars=tuple(reversed(q_sorted)))
+    if merge_sum_outs is None:
+        merge_sum_outs = os.environ.get("SOROBN_B200_MERGE", "0") == "1"
+    b.steps = _merge_sum_outs(b.steps, merge_sum_outs)
     if mode == MODE_BATCHED:
         if os.environ.get("SOROBN_B200_DFS", "1") == "1":
-            steps = _depth_first_order(steps)
-        _relayout_big_tables(steps, table_arrays, table_axes, evidence, card)
-    slots, post_slot = _assign_slots(steps, post.buf, keep_unbatched=(mode == MODE_BATCHED))
-
-    plan = Plan(mode=mode, query=q_sorted, evidence=evidence, order=list(order), tables=tables,
-                slots=slots, steps=steps, post_slot=post_slot, Q=Q,
-                table_axes=[list(a) for a in table_axes], table_scopes=[net.scope(v) for v in tables])
-    plan._card = card
-    _serialise(plan, table_arrays)
-    return plan
+            b.steps = _depth_first_order(b.steps)
+        _relayout_big_tables(b.steps, b.table_arrays, b.table_axes, evidence, card)
+    return b.finish(VERSION, post, b.size(post.vars), query=q_sorted)
 
 
-def _marginals_passes(net, evidence, mode, order, max_in, targets, buckets, leftovers, steps, tables, table_arrays,
-                      emit, combine_tables, axis_order, fsize):
+def _marginals_passes(b, buckets, leftovers, targets):
     """Downward pass and readouts of a marginals plan (DESIGN.md "Marginals of every variable").
 
     `buckets` are the launches of the upward pass: (F_k, eliminated variables, U_k, lambda_k).
@@ -727,118 +779,63 @@ def _marginals_passes(net, evidence, mode, order, max_in, targets, buckets, left
     What is left after the upward pass are per-row scalars (the root buckets' messages and the
     tables of evidence-only variables); a root bucket's pi is the product of the others, so that
     every bucket belief is P(U_k, e) and a row of probability zero stays NaN as in `build_plan`."""
-    card = net.card
-
-    def joint(vs):
-        return int(np.prod([card[v] for v in vs], dtype=np.int64)) if vs else 1
-
-    t_sorted = tuple(sorted(targets, key=lambda v: net.names[v]))
-    read = {t: min((joint(U), k) for k, (_, _, U, _) in enumerate(buckets) if t in U)[1] for t in t_sorted}
-    pi, fold = _downward(net, max_in, buckets, leftovers, read.values(), emit, combine_tables, axis_order, fsize)
-
-    offsets, q = {}, 0
+    card, names = b.card, b.net.names
+    t_sorted = tuple(sorted(targets, key=lambda v: names[v]))
+    read = {t: _smallest_bucket(b, buckets, {t}) for t in t_sorted}
+    pi = _downward(b, buckets, leftovers, read.values())
+    q = 0
     for t in t_sorted:
-        offsets[t] = q
-        q += int(card[t])
-    for t in t_sorted:
-        k = read[t]
-        F_k, _, U_k, _ = buckets[k]
-        inputs = fold(([pi[k]] if pi[k] is not None else []) + list(F_k))
-        # joint states of the summed-out variables are walked first-variable fastest: the variables the
-        # largest batched operand lacks go first, so each of its entries is read in one stretch
-        big = max(inputs, key=lambda f: (f.batched, fsize(f)))
-        pos_big = dict(zip(big.vars, big.strides))
-        elims = sorted(U_k - {t}, key=lambda v: (v in pos_big, pos_big.get(v, 0), v))
-        if joint(elims) > MARGINAL_MAX_Z or joint(elims) * int(card[t]) >= 2**31:
-            raise ValueError(f"the bucket read for {net.names[t]!r} is too large for a readout: {joint(elims)} joint "
+        ins, elims, ecards = _bucket_read(b, buckets[read[t]], pi[read[t]], (t,))
+        cz = b.size(elims)
+        if cz > MARGINAL_MAX_Z or cz * int(card[t]) >= 2**31:
+            raise ValueError(f"the bucket read for {names[t]!r} is too large for a readout: {cz} joint "
                              f"states summed out (at most {MARGINAL_MAX_Z}) x {int(card[t])} target states (below 2^31)")
-        ins = []
-        for f in inputs:
-            pos = dict(zip(f.vars, f.strides))
-            ins.append((f, tuple(pos.get(e, 0) for e in elims), (pos.get(t, 0),)))
-        steps.append(Step(KIND_MARGINAL, ins, -1, (t,), (int(card[t]),), tuple(elims),
-                          tuple(int(card[e]) for e in elims), q_offset=offsets[t]))
-
-    steps[:] = _prune_dead(steps)
-    slots = _assign_slots_shared(steps, keep_unbatched=(mode == MODE_BATCHED))[0]
-    plan = Plan(mode=mode, query=(), evidence=evidence, order=list(order), tables=tables, slots=slots, steps=steps,
-                post_slot=-1, Q=q, version=VERSION_MARGINALS, targets=t_sorted)
-    plan._card = card
-    _serialise(plan, table_arrays)
-    return plan
+        b.steps.append(Step(KIND_MARGINAL, ins, -1, (t,), (int(card[t]),), elims, ecards, q_offset=q))
+        q += int(card[t])
+    b.steps = _prune_dead(b.steps)
+    return b.finish(VERSION_MARGINALS, None, q, targets=t_sorted)
 
 
-def _counts_passes(net, evidence, mode, order, max_in, buckets, leftovers, steps, tables, table_arrays, table_axes,
-                   emit, combine_tables, axis_order, fsize):
+def _counts_passes(b, buckets, leftovers):
     """Downward pass and count steps of a counts plan (DESIGN.md "Expected counts and EM").
 
     The unobserved members M_v of v's family are read from the smallest bucket k with M_v in U_k (the
     bucket the CPT of v entered has them all):
         counts_v(M_v; key(row)) += sum_{U_k - M_v} pi_k * prod_{f in F_k} f / P(observed),
     where P(observed) is the product of every leftover scalar of the upward pass, computed once."""
-    card = net.card
-    ev_col = {v: i for i, v in enumerate(evidence)}
+    card, names, ev_col = b.card, b.net.names, b.ev_col
+    members = {v: [u for u in b.net.scope(v) if u not in ev_col] for v in range(len(names))}
+    read = {v: _smallest_bucket(b, buckets, set(M)) for v, M in members.items() if M}
+    pi = _downward(b, buckets, leftovers, read.values())
+    prob = b.emit(b.fold(leftovers), (), [], may_lift=False)
 
-    def joint(vs):
-        return int(np.prod([card[v] for v in vs], dtype=np.int64)) if vs else 1
-
-    n_vars = len(net.names)
-    members = {v: [u for u in net.scope(v) if u not in ev_col] for v in range(n_vars)}
-    read = {}
-    for v in range(n_vars):
-        if members[v]:
-            M = set(members[v])
-            read[v] = min((joint(U), k) for k, (_, _, U, _) in enumerate(buckets) if M <= U)[1]
-    pi, fold = _downward(net, max_in, buckets, leftovers, read.values(), emit, combine_tables, axis_order, fsize)
-    prob = emit(fold(list(leftovers)), None, [], may_lift=False)
-
-    c_offsets, n_counts = count_layout(net)
-    for v in range(n_vars):
-        scope = net.scope(v)
+    c_offsets, n_counts = count_layout(b.net)
+    for v, M in members.items():
+        scope = b.net.scope(v)
         shape = [int(card[u]) for u in scope]
         stride = {u: int(np.prod(shape[i + 1:], dtype=np.int64)) for i, u in enumerate(scope)}
         key = tuple((ev_col[u], stride[u], int(card[u])) for u in scope if u in ev_col)
         if len(key) > MAX_EV:
-            raise ValueError(f"the family of {net.names[v]!r} has {len(key)} observed members; the kernel gathers {MAX_EV}")
-        M = members[v]
+            raise ValueError(f"the family of {names[v]!r} has {len(key)} observed members; the kernel gathers {MAX_EV}")
         if not M:  # fully observed family: a histogram of the rows' keys
-            steps.append(Step(KIND_COUNT, [], -1, (), (), (), (), q_offset=c_offsets[v], key=key, norm=prob))
+            b.steps.append(Step(KIND_COUNT, [], -1, (), (), (), (), q_offset=c_offsets[v], key=key, norm=prob))
             continue
-        k = read[v]
-        F_k, _, U_k, _ = buckets[k]
-        inputs = fold(([pi[k]] if pi[k] is not None else []) + list(F_k))
-        big = max(inputs, key=lambda f: (f.batched, fsize(f)))
-        pos_big = dict(zip(big.vars, big.strides))
-        elims = sorted(U_k - set(M), key=lambda u: (u in pos_big, pos_big.get(u, 0), u))
         out_vars = tuple(reversed(M))  # v (count-table stride 1) is the fastest output axis
-        cs = joint(out_vars)
-        if joint(elims) > MARGINAL_MAX_Z or cs > MARGINAL_MAX_Z or joint(elims) * cs >= 2**31:
-            raise ValueError(f"the bucket read for the family of {net.names[v]!r} is too large for a count step: "
-                             f"{joint(elims)} joint states summed out and {cs} family states (each at most "
+        ins, elims, ecards = _bucket_read(b, buckets[read[v]], pi[read[v]], out_vars)
+        cz, cs = b.size(elims), b.size(out_vars)
+        if cz > MARGINAL_MAX_Z or cs > MARGINAL_MAX_Z or cz * cs >= 2**31:
+            raise ValueError(f"the bucket read for the family of {names[v]!r} is too large for a count step: "
+                             f"{cz} joint states summed out and {cs} family states (each at most "
                              f"{MARGINAL_MAX_Z}, their product below 2^31)")
-        ins = []
-        for f in inputs:
-            pos = dict(zip(f.vars, f.strides))
-            ins.append((f, tuple(pos.get(e, 0) for e in elims), tuple(pos.get(u, 0) for u in out_vars)))
-        steps.append(Step(KIND_COUNT, ins, -1, out_vars, tuple(int(card[u]) for u in out_vars), tuple(elims),
-                          tuple(int(card[e]) for e in elims), q_offset=c_offsets[v], key=key,
-                          cstrides=tuple(stride[u] for u in out_vars), norm=prob))
-
-    steps[:] = _prune_dead(steps)
-    slots, where = _assign_slots_shared(steps, keep_unbatched=(mode == MODE_BATCHED))
-    p_slot = where[prob.buf]
-    plan = Plan(mode=mode, query=(), evidence=evidence, order=list(order), tables=tables, slots=slots, steps=steps,
-                post_slot=p_slot, Q=1, version=VERSION_COUNTS, n_counts=n_counts, count_offsets=c_offsets,
-                table_axes=[list(a) for a in table_axes], table_scopes=[net.scope(v) for v in tables])
-    plan._card = card
-    _serialise(plan, table_arrays)
-    return plan
+        b.steps.append(Step(KIND_COUNT, ins, -1, out_vars, tuple(int(card[u]) for u in out_vars), elims, ecards,
+                            q_offset=c_offsets[v], key=key, cstrides=tuple(stride[u] for u in out_vars), norm=prob))
+    b.steps = _prune_dead(b.steps)
+    return b.finish(VERSION_COUNTS, prob, 1, n_counts=n_counts, count_offsets=c_offsets)
 
 
-def _sample_passes(net, evidence, order, max_in, buckets, leftovers, steps, tables, table_arrays, table_axes, emit,
-                   combine_tables, axis_order, fsize, kind=KIND_SAMPLE):
+def _sample_passes(b, buckets, leftovers, version):
     """Sample steps of a sample plan (DESIGN.md "Posterior samples"), or argmax steps of an MPE plan
-    (`kind` KIND_ARGMAX, DESIGN.md "Most probable explanation").
+    (`version` VERSION_MPE, DESIGN.md "Most probable explanation").
 
     Bucket k eliminated X_k and sent lambda_k(S_k) to a later bucket.  Walking the buckets in reverse
     elimination order, every variable of S_k has been drawn when bucket k is reached, and
@@ -847,54 +844,67 @@ def _sample_passes(net, evidence, order, max_in, buckets, leftovers, steps, tabl
     domain of an MPE plan the same steps mean max-sum: lambda_k(S_k) = max_{X_k} sum_{f in F_k} log f,
     the leftovers sum to max log P(x, e), and the argmax of sum_{f in F_k} log f(X_k, S_k = decoded, e)
     is X_k's state in the maximising assignment."""
-    card = net.card
-    n_ev = len(evidence)
-    _, fold = _downward(net, max_in, buckets, leftovers, (), emit, combine_tables, axis_order, fsize)
+    kind = KIND_SAMPLE if version == VERSION_SAMPLE else KIND_ARGMAX
+    card, names = b.card, b.net.names
+    n_ev = len(b.evidence)
     # the folds (products of the factors beyond max_in) do not depend on the draws: they all run before
     # the sample steps, which then form one contiguous run at the end of the program
-    inputs_of = [fold(list(buckets[k][0])) for k in range(len(buckets))]
-    prob = emit(fold(list(leftovers)), None, [], may_lift=False)
+    inputs_of = [b.fold(F) for F, _, _, _ in buckets]
+    prob = b.emit(b.fold(leftovers), (), [], may_lift=False)
 
     drawn = {}  # var id -> drawn-code row
     for k in reversed(range(len(buckets))):
         _, X, _, _ = buckets[k]
         for x in X:
             if int(card[x]) > SAMPLE_MAX_CARD:
-                raise ValueError(f"{net.names[x]!r} has {int(card[x])} states; drawn codes are uint8 (at most "
+                raise ValueError(f"{names[x]!r} has {int(card[x])} states; drawn codes are uint8 (at most "
                                  f"{SAMPLE_MAX_CARD} states)")
-        cz = int(np.prod([int(card[x]) for x in X], dtype=np.int64))
+        cz = b.size(X)
         if cz > MAX_Z:
-            raise ValueError(f"the bucket of {[net.names[x] for x in X]} has {cz} joint states; a sample step draws "
+            raise ValueError(f"the bucket of {[names[x] for x in X]} has {cz} joint states; a sample step draws "
                              f"from at most {MAX_Z}")
         ins = []
         for f in inputs_of[k]:
             pos = dict(zip(f.vars, f.strides))
             terms = tuple(f.ev) + tuple((n_ev + drawn[u], pos[u], int(card[u])) for u in f.vars if u not in X)
             if len(terms) > SAMPLE_MAX_TERMS:
-                raise ValueError(f"a factor of the bucket of {[net.names[x] for x in X]} gathers {len(terms)} observed "
+                raise ValueError(f"a factor of the bucket of {[names[x] for x in X]} gathers {len(terms)} observed "
                                  f"or drawn variables; a sample step gathers at most {SAMPLE_MAX_TERMS}")
             g = _Factor(f.is_slot, f.buf, f.vars, f.strides, terms, f.batched)
             ins.append((g, tuple(pos.get(x, 0) for x in X), ()))
-        steps.append(Step(kind, ins, -1, (), (), tuple(X), tuple(int(card[x]) for x in X),
-                          q_offset=len(drawn), norm=prob))
+        b.steps.append(Step(kind, ins, -1, (), (), tuple(X), tuple(int(card[x]) for x in X),
+                            q_offset=len(drawn), norm=prob))
         for x in X:
             drawn[x] = len(drawn)
-
-    slots, where = _assign_slots_shared(steps, keep_unbatched=True)
-    plan = Plan(mode=MODE_BATCHED, query=(), evidence=evidence, order=list(order), tables=tables, slots=slots,
-                steps=steps, post_slot=where[prob.buf], Q=1,
-                version=VERSION_SAMPLE if kind == KIND_SAMPLE else VERSION_MPE,
-                table_axes=[list(a) for a in table_axes], table_scopes=[net.scope(v) for v in tables],
-                sampled=tuple(sorted(drawn, key=drawn.get)))
-    plan._card = card
-    _serialise(plan, table_arrays)
-    return plan
+    return b.finish(version, prob, 1, sampled=tuple(sorted(drawn, key=drawn.get)))
 
 
-def _downward(net, max_in, buckets, leftovers, reads, emit, combine_tables, axis_order, fsize):
+def _smallest_bucket(b, buckets, M):
+    """The bucket a step reads the variables `M` from: the smallest whose scope U_k holds them all."""
+    return min((b.size(U), k) for k, (_, _, U, _) in enumerate(buckets) if M <= U)[1]
+
+
+def _bucket_read(b, bucket, pi_k, out_vars):
+    """The operands of a step that reads `out_vars` from `bucket` (F_k, X_k, U_k, lambda_k) with
+    downward message `pi_k`, summing out U_k - out_vars: (inputs with their (summed-out strides,
+    output strides), the summed-out variables, their cards).  The caller checks the sizes."""
+    F_k, _, U_k, _ = bucket
+    inputs = b.fold(([pi_k] if pi_k is not None else []) + list(F_k))
+    # joint states of the summed-out variables are walked first-variable fastest: the variables the
+    # largest batched operand lacks go first, so each of its entries is read in one stretch
+    big = b.largest(inputs)
+    pos_big = dict(zip(big.vars, big.strides))
+    elims = tuple(sorted(U_k - set(out_vars), key=lambda v: (v in pos_big, pos_big.get(v, 0), v)))
+    ins = []
+    for f in inputs:
+        pos = dict(zip(f.vars, f.strides))
+        ins.append((f, tuple(pos.get(e, 0) for e in elims), tuple(pos.get(u, 0) for u in out_vars)))
+    return ins, elims, tuple(int(b.card[e]) for e in elims)
+
+
+def _downward(b, buckets, leftovers, reads):
     """Downward messages pi_k of the buckets on the way from a root to every bucket in `reads`
-    (`_marginals_passes`).  Returns (pi, fold)."""
-    card = net.card
+    (`_marginals_passes`, `_counts_passes`)."""
     n = len(buckets)
     owner = {id(lam): k for k, (_, _, _, lam) in enumerate(buckets)}
     parent = [None] * n
@@ -910,41 +920,6 @@ def _downward(net, max_in, buckets, leftovers, reads, emit, combine_tables, axis
             need[k] = True
             k = parent[k]
 
-    def fold(inputs):
-        """At most max_in factors per launch: multiply the smallest ones first (as product_chain)."""
-        inputs = list(inputs)
-        while len(inputs) > max_in:
-            inputs.sort(key=fsize)
-            head, inputs = inputs[:max_in], inputs[max_in:]
-            union = set().union(*[f.vars for f in head])
-            inputs.append(emit(head, None, axis_order(head, union)))
-        return inputs
-
-    def message(inputs, out_vars, elims):
-        """sum_{elims} prod(inputs) over out_vars, at most MAX_ELIM variables / MAX_Z joint states per launch:
-        the first launch multiplies and sums out the first group, each later one sums out the next group."""
-        groups, cur, z = [], [], 1
-        for v in sorted(elims, key=lambda v: (-int(card[v]), v)):
-            if cur and (len(cur) >= MAX_ELIM or z * int(card[v]) > MAX_Z):
-                groups.append(cur)
-                cur, z = [], 1
-            cur.append(v)
-            z *= int(card[v])
-        if cur:
-            groups.append(cur)
-        inputs = combine_tables(inputs, PRELOAD_MAX_IN if groups and len(groups[0]) > 1 else TILED_MAX_IN)
-        inputs = fold(inputs)
-        rest = [v for g in groups for v in g]
-        if not groups:
-            return emit(inputs, None, axis_order(inputs, set(out_vars)))
-        f = None
-        for g in groups:
-            rest = [v for v in rest if v not in g]
-            keep = set(out_vars) | set(rest)
-            src = inputs if f is None else [f]
-            f = emit(src, tuple(g), axis_order(src, keep))
-        return f
-
     pi = {}
     for k in reversed(range(n)):  # a parent is eliminated after its children
         if not need[k]:
@@ -952,14 +927,14 @@ def _downward(net, max_in, buckets, leftovers, reads, emit, combine_tables, axis
         lam_k = buckets[k][3]
         if parent[k] is None:
             others = [f for f in leftovers if f is not lam_k]
-            pi[k] = emit(fold(others), None, [], may_lift=False) if others else None
+            pi[k] = b.emit(b.fold(others), (), [], may_lift=False) if others else None
             continue
         p = parent[k]
         F_p, _, U_p, _ = buckets[p]
         inputs = ([pi[p]] if pi[p] is not None else []) + [f for f in F_p if f is not lam_k]
         S_k = set(lam_k.vars)
-        pi[k] = message(inputs, S_k, U_p - S_k) if inputs else None
-    return pi, fold
+        pi[k] = b.message(inputs, S_k, U_p - S_k) if inputs else None
+    return pi
 
 
 def _prune_dead(steps):
@@ -972,60 +947,6 @@ def _prune_dead(steps):
             if st.norm is not None:
                 used.add(st.norm.buf)
     return keep[::-1]
-
-
-def _assign_slots_shared(steps, keep_unbatched):
-    """`_assign_slots` for plans whose intermediates have several consumers (the factors of a
-    bucket feed its upward message, its downward messages and its readouts): a slot is released
-    after its last consumer.  The output slot is taken before the inputs are released, so a launch
-    never writes a buffer it reads.  Readouts write the posterior, not a slot; count steps write the
-    count table and also read P(observed) (`Step.norm`).  Returns (slots, logical id -> slot)."""
-    remaining = {}
-    for st in steps:
-        for f, _, _ in st.inputs:
-            if f.is_slot:
-                remaining[f.buf] = remaining.get(f.buf, 0) + 1
-        if st.norm is not None:
-            remaining[st.norm.buf] = remaining.get(st.norm.buf, 0) + 1
-    slots, where = [], {}
-
-    def alloc(batched, size):
-        best = None
-        for i, (b, sz, free) in enumerate(slots):
-            if free and b == batched and sz >= size and (best is None or sz < slots[best][1]):
-                best = i
-        if best is None:
-            slots.append([batched, size, False])
-            return len(slots) - 1
-        slots[best][2] = False
-        return best
-
-    def release(buf):
-        remaining[buf] -= 1
-        if remaining[buf] == 0:
-            phys = where[buf]
-            slots[phys][2] = not (keep_unbatched and not slots[phys][0])
-
-    for st in steps:
-        writes_slot = st.kind not in (KIND_MARGINAL, KIND_COUNT, KIND_SAMPLE, KIND_ARGMAX)
-        if writes_slot:
-            size = int(np.prod(st.cards, dtype=np.int64)) if st.cards else 1
-            st.out_slot = alloc(st.kind == KIND_BATCHED, size)
-        new_inputs = []
-        for f, es, ss in st.inputs:
-            if f.is_slot:
-                phys = where[f.buf]
-                release(f.buf)
-                f = _Factor(True, phys, f.vars, f.strides, f.ev, f.batched)
-            new_inputs.append((f, es, ss))
-        st.inputs = new_inputs
-        if st.norm is not None:
-            release(st.norm.buf)
-        if writes_slot:
-            where[st.out_id] = st.out_slot
-    if not slots:  # every operand is a CPT: the engine still expects one scratch slot
-        slots.append([False, 1, True])
-    return [(bool(b), int(sz)) for b, sz, _ in slots], where
 
 
 def _relayout_big_tables(steps, table_arrays, table_axes, evidence, card):
@@ -1156,16 +1077,31 @@ def _depth_first_order(steps):
     return out
 
 
-def _assign_slots(steps, post_id, keep_unbatched=False):
+def _assign_slots(steps, keep_unbatched, park_batched):
     """Physical scratch slots by liveness: an output slot is taken before the step's inputs
     are released (a launch never writes a buffer it reads), best fit among the free slots
-    of the same kind, and every intermediate dies with its single consumer.
+    of the same kind, and an intermediate is released after its last consumer.  An
+    intermediate of a posterior plan has a single consumer; one of the other kinds may have
+    several (the factors of a bucket feed its upward message, its downward messages and its
+    readouts).  `Step.norm`, the P(observed) a count, sample or argmax step reads, counts as a
+    read.  Steps of kinds 2 to 5 write the posterior, the count table or drawn codes, not a
+    slot.  Returns (slots, logical id -> slot).
 
     keep_unbatched: the evidence-independent tables of a batched program are computed ONCE, when
     the program is created (csrc/sbn_api.cu `run_table_steps`), and then read by every run; their
-    slots are never recycled (they are a few KB each)."""
+    slots are never recycled (they are a few KB each).
+
+    park_batched (posterior plans): the batched inputs of a batched step are released one batched
+    step LATE.  The engine may run a step and its consumer as ONE launch that reads the first step's
+    operand and writes the second step's output (csrc/sbn_pair.h), so those two must never share a
+    buffer; it plans such launches for posterior programs only."""
+    remaining = {}  # logical id -> reads still to come
+    for st in steps:
+        for buf in [f.buf for f, _, _ in st.inputs if f.is_slot] + ([st.norm.buf] if st.norm is not None else []):
+            remaining[buf] = remaining.get(buf, 0) + 1
     slots = []  # [batched, size, free]
     where = {}  # logical id -> physical slot
+    parked = []
 
     def alloc(batched, size):
         best = None
@@ -1178,30 +1114,39 @@ def _assign_slots(steps, post_id, keep_unbatched=False):
         slots[best][2] = False
         return best
 
-    # The batched inputs of a batched step are released one batched step LATE: the engine may run a
-    # step and its consumer as ONE launch that reads the first step's operand and writes the second
-    # step's output (csrc/sbn_pair.h), so those two must never share a buffer.
-    parked = []
+    def release(buf, late):
+        remaining[buf] -= 1
+        if remaining[buf] == 0:
+            phys = where[buf]
+            if late and slots[phys][0]:
+                parked.append(phys)
+            else:
+                slots[phys][2] = not (keep_unbatched and not slots[phys][0])
+
     for st in steps:
-        size = int(np.prod(st.cards, dtype=np.int64)) if st.cards else 1
-        st.out_slot = alloc(st.kind == KIND_BATCHED, size)
-        if st.kind == KIND_BATCHED:
+        writes_slot = st.kind in (KIND_FLAT, KIND_BATCHED)
+        if writes_slot:
+            st.out_slot = alloc(st.kind == KIND_BATCHED, int(np.prod(st.cards, dtype=np.int64)) if st.cards else 1)
+        late = park_batched and st.kind == KIND_BATCHED
+        if late:
             for phys in parked:
                 slots[phys][2] = True
-            parked = []
+            parked.clear()
         new_inputs = []
         for f, es, ss in st.inputs:
             if f.is_slot:
-                phys = where.pop(f.buf)
-                if slots[phys][0] and st.kind == KIND_BATCHED:
-                    parked.append(phys)
-                else:
-                    slots[phys][2] = not (keep_unbatched and not slots[phys][0])
+                phys = where[f.buf]
+                release(f.buf, late)
                 f = _Factor(True, phys, f.vars, f.strides, f.ev, f.batched)
             new_inputs.append((f, es, ss))
         st.inputs = new_inputs
-        where[st.out_id] = st.out_slot
-    return [(bool(b), int(sz)) for b, sz, _ in slots], where[post_id]
+        if st.norm is not None:
+            release(st.norm.buf, late)
+        if writes_slot:
+            where[st.out_id] = st.out_slot
+    if not slots:  # every operand is a CPT: the engine still expects one scratch slot
+        slots.append([False, 1, True])
+    return [(bool(b), int(sz)) for b, sz, _ in slots], where
 
 
 def _blobs(table_arrays):

@@ -174,6 +174,16 @@ def test_refreshed_tables_equal_a_fresh_plan_bitwise(wl):
     assert blob32.tobytes() == fresh.table_blob.tobytes()
 
 
+@pytest.mark.parametrize("wl", ["grid10x10", "dag50"])
+def test_refreshed_tables_of_a_marginals_plan_are_its_own_blobs(wl):
+    w = workloads.WORKLOADS[wl]()
+    net = w.build()._compiled
+    plan = planner.build_marginals_plan(net, [net.index[e] for e in w.evidence[2:]])
+    blob32, blob64 = planner.refresh_tables(plan, net.cpt)
+    assert blob64.tobytes() == plan.table_blob64.tobytes()
+    assert blob32.tobytes() == plan.table_blob.tobytes()
+
+
 def test_version_4_and_5_words_are_unchanged_by_the_counts_planner():
     bn = examples.asia()
     net = bn._compiled
