@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SBN_ABI_VERSION 12
+#define SBN_ABI_VERSION 13
 
 #define SBN_OK 0
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
@@ -140,7 +140,10 @@ int sbn_program_sample_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld
  * argmax over every unobserved variable jointly of P(unobserved, the row's observed cells); ties go to the
  * first joint state of a bucket (first variable fastest).  log_prob[b] = that maximum, log P(x*, e), or
  * -inf for a row whose observed cells have probability zero (its codes are meaningless).  Large batches
- * run in chunks. */
+ * run in chunks.
+ * The same call runs a marginal MAP program (planner.build_map_plan, version 9; created in float32 only):
+ * the decoded variables are its MAP variables, every other unobserved variable is summed out, and
+ * log_prob[b] = max over the MAP variables of log P(x_MAP, the row's observed cells). */
 int sbn_program_mpe_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
                          uint8_t *codes /* [n_decoded][n_rows] */, float *log_prob /* [n_rows] */);
 

@@ -27,6 +27,9 @@ pattern (planner.build_counts_plan, csrc/sbn_count.cuh).  `sample_many` draws ex
 samples of the missing cells and latent nodes, one sample program per pattern
 (planner.build_sample_plan, csrc/sbn_sample.cuh).  `mpe_many` / `mpe` find their most probable
 explanation, one log-domain max-sum program per pattern (planner.build_mpe_plan, csrc/sbn_mpe.cuh).
+`map_many` / `map` find the marginal MAP state of chosen variables (by default the missing cells), the
+other unobserved variables summed out: one log-sum-exp, then max-sum program per pattern
+(planner.build_map_plan).
 """
 from __future__ import annotations
 
@@ -49,9 +52,9 @@ def _as_list(obj):
 
 
 class _PatternRunner:
-    """The device programs of one missingness pattern (a counts, sample or MPE plan): the float32 program,
-    and the float64 one for the rows it flags (created when first needed; never for an MPE plan, whose logs
-    do not underflow).  `set_cpts` gives both new tables in place (counts programs)."""
+    """The device programs of one missingness pattern (a counts, sample, MPE or MAP plan): the float32 program,
+    and the float64 one for the rows it flags (created when first needed; never for an MPE or MAP plan, whose
+    logs do not underflow).  `set_cpts` gives both new tables in place (counts programs)."""
 
     def __init__(self, plan, device):
         from . import engine  # raises if libsorobn_b200.so cannot be loaded
@@ -507,16 +510,23 @@ class BayesNet:
         """The cached MPE program of one missingness pattern."""
         return self._pattern_runner("mpe", ev)
 
-    def _pattern_runner(self, kind, ev):
-        """The cached programs of one missingness pattern, `kind` "counts", "sample" or "mpe" (dropped by
-        `prepare()`, as every program)."""
+    def _map_runner(self, ev, map_vars):
+        """The cached marginal MAP program of one missingness pattern and MAP set (sorted var ids)."""
+        return self._pattern_runner("map", ev, map_vars)
+
+    def _pattern_runner(self, kind, ev, map_vars=None):
+        """The cached programs of one missingness pattern, `kind` "counts", "sample", "mpe" or "map" (a "map"
+        program is keyed by its MAP variables too; dropped by `prepare()`, as every program)."""
         with self._cache_lock:
-            key = (kind, ev, self.device)
+            key = (kind, ev, self.device) if kind != "map" else (kind, ev, map_vars, self.device)
             hit = self._engine_cache.get(key)
             if hit is None:
-                build = {"counts": _planner.build_counts_plan, "sample": _planner.build_sample_plan,
-                         "mpe": _planner.build_mpe_plan}[kind]
-                hit = self._engine_cache[key] = _PatternRunner(build(self._compiled, ev), self.device)
+                if kind == "map":
+                    plan = _planner.build_map_plan(self._compiled, ev, map_vars)
+                else:
+                    plan = {"counts": _planner.build_counts_plan, "sample": _planner.build_sample_plan,
+                            "mpe": _planner.build_mpe_plan}[kind](self._compiled, ev)
+                hit = self._engine_cache[key] = _PatternRunner(plan, self.device)
                 self._evict()
             else:
                 self._engine_cache.move_to_end(key)
@@ -636,6 +646,76 @@ class BayesNet:
         """The most probable explanation of one event: `mpe_many(pd.DataFrame([event])).iloc[0]`, a Series
         indexed by node name."""
         return self.mpe_many(pd.DataFrame([event])).iloc[0]
+
+    def map_many(self, events: pd.DataFrame, variables=None, return_log_proba: bool = False):
+        """The marginal MAP state of every row of `events`, computed on the GPU: the joint state of the MAP
+        variables that maximises P(MAP variables, the row's observed cells), every other unobserved variable
+        summed out.
+
+        A missing cell is None or NaN; a node without a column is unobserved.  With `variables=None` the MAP
+        variables of a row are its missing cells and every node without a column is summed out: the answer
+        `impute_many` gives, for any number of missing cells.  With `variables=[...]` the listed nodes are
+        decoded, latent ones included; a listed node the row observes is copied through, and every other
+        unobserved node is summed out (its missing cells stay missing).  Returns one row per row of `events`
+        (same index) whose columns are those of `events` and `variables`, sorted, with dtypes inferred as in
+        `mpe_many`.  With `return_log_proba=True` returns (frame, Series of log P(MAP state, observed cells)
+        in float64, same index).  Ties go to the first joint state of a bucket of the elimination (first
+        variable fastest).  Raises ValueError for a value outside its variable's domain and for rows whose
+        observed cells have probability zero.
+
+        Unlike `impute_many`, which builds the dense posterior over the joint of the missing columns, the
+        cost grows with the number of variables, not with their joint.  Unlike `mpe_many`, the unobserved
+        variables outside the MAP set are summed out, not maximised.  Rows are grouped by missingness pattern;
+        each pattern is one marginal MAP program (planner.build_map_plan): the upward pass of variable
+        elimination in the log domain, log-sum-exp over the summed variables, then max over the MAP ones,
+        then one argmax per MAP bucket, top-down."""
+        groups = self._count_patterns(events)
+        net = self._compiled
+        listed = None
+        if variables is not None:
+            unknown = [v for v in variables if v not in net.index]
+            if unknown:
+                raise ValueError(f"{unknown[:5]} are not nodes of the network")
+            listed = sorted({net.index[v] for v in variables})
+        columns = [net.index[c] for c in events.columns]
+        out_vars = sorted(set(columns) | set(listed or ()), key=lambda v: net.names[v])
+        n_rows = len(events.index)
+        codes = np.zeros((len(net.names), n_rows), dtype=np.uint8)
+        known = np.zeros((len(net.names), n_rows), dtype=bool)  # observed or decoded
+        log_p = np.zeros(n_rows, dtype=np.float64)
+        for ev, rows, ev_codes in groups:
+            observed = set(ev)
+            if listed is None:
+                map_vars = tuple(v for v in sorted(columns) if v not in observed)
+            else:
+                map_vars = tuple(v for v in listed if v not in observed)
+            for i, v in enumerate(ev):
+                codes[v][rows] = ev_codes[i]
+                known[v][rows] = True
+            if not map_vars and not ev:
+                continue  # nothing observed, nothing to decode: log P = log 1
+            # fetched right before it runs, as in `sample_many`
+            runner = self._map_runner(ev, map_vars)
+            decoded, lp = runner.f32.map(ev_codes, len(rows))
+            impossible = ~(lp > -np.inf)
+            if impossible.any():
+                raise ValueError(f"{int(impossible.sum())} row(s) have observed cells of probability zero "
+                                 f"(first: {events.index[rows[impossible][0]]!r}); they have no MAP state")
+            for j, v in enumerate(runner.plan.sampled):
+                codes[v][rows] = decoded[j]
+                known[v][rows] = True
+            log_p[rows] = lp
+        frame = pd.DataFrame({net.names[v]: np.where(known[v], np.asarray(net.domains[v], dtype=object)[codes[v]], None)
+                              for v in out_vars}, index=events.index)
+        frame = frame.infer_objects().sort_index(axis="columns")
+        if return_log_proba:
+            return frame, pd.Series(log_p, index=events.index)
+        return frame
+
+    def map(self, event: dict, variables=None) -> pd.Series:
+        """The marginal MAP state of one event: `map_many(pd.DataFrame([event]), variables).iloc[0]`, a Series
+        indexed by node name."""
+        return self.map_many(pd.DataFrame([event]), variables).iloc[0]
 
     @staticmethod
     def _draw(program, ev_codes, rows, n, seed):

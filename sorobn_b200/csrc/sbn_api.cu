@@ -57,7 +57,10 @@ constexpr int kVersionCounts = 6;     // planner.build_counts_plan: kind-3 count
 constexpr int kVersionSample = 7;     // planner.build_sample_plan: kind-4 sample steps, P(observed) in the posterior slot
 constexpr int kVersionMpe = 8;        // planner.build_mpe_plan: log tables, max-sum steps, kind-5 argmax steps,
                                       // max log P(x, e) in the posterior slot
+constexpr int kVersionMap = 9;        // planner.build_map_plan: version 8 plus a reduction word on kind-0 / 1 steps
+                                      // (1 = log-sum-exp, 0 = max), max log P(x_MAP, e) in the posterior slot
 static_assert(kVersionMpe - kVersion == kMpe, "one program kind per header version, in order");
+static_assert(kVersionMap - kVersion == kMap, "one program kind per header version, in order");
 constexpr int64_t kMarginalZoffMax = 1 << 24;  // int32 words of one readout's joint-state offset table
 constexpr int kMaxElim = 3;
 constexpr int kMaxZ = 256;
@@ -70,12 +73,14 @@ namespace {
 int parse(sbn_program *P, const int32_t *w, int64_t n) {
     if (n < kHeaderWords) return fail(SBN_E_INVALID, "program shorter than its header");
     if (w[0] != kMagic) return fail(SBN_E_INVALID, "bad program magic 0x%x", w[0]);
-    if (w[1] < kVersion || w[1] > kVersionMpe)
-        return fail(SBN_E_INVALID, "program version %d, engine expects %d, %d, %d, %d or %d", w[1], kVersion,
-                    kVersionMarginals, kVersionCounts, kVersionSample, kVersionMpe);
+    if (w[1] < kVersion || w[1] > kVersionMap)
+        return fail(SBN_E_INVALID, "program version %d, engine expects %d, %d, %d, %d, %d or %d", w[1], kVersion,
+                    kVersionMarginals, kVersionCounts, kVersionSample, kVersionMpe, kVersionMap);
     P->kind = static_cast<ProgramKind>(w[1] - kVersion);
-    const bool marginals = P->kind == kMarginals, counts = P->kind == kCounts, mpe = P->kind == kMpe;
-    const bool decodes = P->kind == kSample || mpe;  // sample and MPE programs share the words of their last steps
+    const bool marginals = P->kind == kMarginals, counts = P->kind == kCounts, mpe = sbn_log_domain(P->kind);
+    const bool map = P->kind == kMap;
+    // sample, MPE and marginal MAP programs share the words of their last steps
+    const bool decodes = P->kind == kSample || mpe;
     P->mode = w[2];
     P->n_ev = w[3];
     const int n_tables = w[4], n_slots = w[5], n_steps = w[6];
@@ -92,9 +97,9 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
     if (decodes) {
         P->n_sampled = w[10];
         if (P->Q != 1 || P->mode != 1 || P->n_sampled < 0)
-            return fail(SBN_E_INVALID, mpe ? "bad MPE header" : "bad sample header");
+            return fail(SBN_E_INVALID, map ? "bad MAP header" : mpe ? "bad MPE header" : "bad sample header");
     }
-    // sample program: kind-4 steps draw codes; MPE program: kind-5 steps decode them (same words)
+    // sample program: kind-4 steps draw codes; MPE / MAP program: kind-5 steps decode them (same words)
     const int decode_kind = mpe ? 5 : 4;
     int n_drawn = 0;  // sample / MPE program: drawn-code rows written by the sample / argmax steps so far
     if (marginals ? (P->post_slot != -1 || P->post_batched != 0) : (P->post_slot < 0 || P->post_slot >= n_slots))
@@ -142,6 +147,13 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             if (st.out_slot != -1 || n_axes != 0 || n_elim < 1 || n_elim > SBN_SAMPLE_MAX_X || st.q_offset != n_drawn ||
                 n_drawn + n_elim > P->n_sampled)
                 return fail(SBN_E_INVALID, mpe ? "step %d: bad argmax step" : "step %d: bad sample step", s);
+        }
+        if (map && (st.kind == 0 || st.kind == 1)) {
+            // the reduction of the eliminated variables: 1 = log-sum-exp, 0 = max (and every product-only step)
+            if (!need(1)) return fail(SBN_E_INVALID, "truncated step %d", s);
+            const int reduce = w[p++];
+            if (reduce != 0 && reduce != 1) return fail(SBN_E_INVALID, "step %d: bad reduction %d", s, reduce);
+            st.logsumexp = reduce == 1;
         }
         if (count) {
             // c_offset, the observed members' gathers and the count-table strides of the output axes
@@ -558,8 +570,8 @@ void plan_tiles(sbn_program *P, std::vector<int32_t> *words) {
     }
     for (StepDesc &st : P->steps) {
         st.tile = 0;
-        // an MPE program's steps run on the max-sum kernels only (launch_step), which have no tiled variant
-        if (st.kind != 1 || P->kind == kMpe || st.in.size() > static_cast<size_t>(kTiledMaxIn)) continue;
+        // an MPE / MAP program's steps run on the log-domain kernels only (launch_step), which have no tiled variant
+        if (st.kind != 1 || sbn_log_domain(P->kind) || st.in.size() > static_cast<size_t>(kTiledMaxIn)) continue;
 
         int64_t smem = 0;
         for (const InDesc &in : st.in)
@@ -836,25 +848,29 @@ cudaError_t set_tiled_attrs() {
     return e;
 }
 
-// A step of an MPE program (log tables): the max-sum instantiations of the flat and the plain batched kernel,
-// whatever the program's switches say -- the tiled, paired, TMA, join and on-chip kernels are sum-product only.
-cudaError_t launch_maxsum(const StepDesc &st, const SbnStep &q, cudaStream_t stream) {
+// A step of an MPE or marginal MAP program (log tables): the max-sum or, for a step that sums out (marginal MAP),
+// the log-sum-exp instantiations of the flat and the plain batched kernel, whatever the program's switches say --
+// the tiled, paired, TMA, join and on-chip kernels are sum-product only.
+cudaError_t launch_log_domain(const StepDesc &st, const SbnStep &q, cudaStream_t stream) {
     if (st.kind == 0) {
         const int threads = 256;
         const int64_t grid = (st.n_out + threads - 1) / threads;
-        sbn_launch(sbn_step_flat<float, SbnMaxSum>, dim3(static_cast<unsigned>(grid)), dim3(threads), 0, stream, q);
+        if (st.logsumexp)
+            sbn_launch(sbn_step_flat<float, SbnLogSumExp>, dim3(static_cast<unsigned>(grid)), dim3(threads), 0, stream, q);
+        else
+            sbn_launch(sbn_step_flat<float, SbnMaxSum>, dim3(static_cast<unsigned>(grid)), dim3(threads), 0, stream, q);
         return cudaGetLastError();
     }
     if (st.kind != 1 || q.tile_off != nullptr) return cudaErrorInvalidValue;
     const int64_t rest = st.n_out / (static_cast<int64_t>(q.n_axes > 0 ? q.card[0] : 1) * (q.n_axes > 1 ? q.card[1] : 1));
     const int64_t grid = static_cast<int64_t>(q.n_bblocks) * q.n_tile1 * rest;
     if (grid >= (1LL << 31)) return cudaErrorInvalidConfiguration;
-    return sbn_batched_maxsum_launch(q, grid, stream);
+    return st.logsumexp ? sbn_batched_logsumexp_launch(q, grid, stream) : sbn_batched_maxsum_launch(q, grid, stream);
 }
 
 cudaError_t launch_step(sbn_program *P, const StepDesc &st, const SbnStep &q, cudaStream_t stream) {
     P->launches++;
-    if (P->kind == kMpe) return launch_maxsum(st, q, stream);
+    if (sbn_log_domain(P->kind)) return launch_log_domain(st, q, stream);
     if (st.kind == 1 && q.tile_off != nullptr && P->kind != kMarginals && sbn_tma_eligible(P, st))
         return sbn_tma_launch(P, st, q.ev, q.ld_ev, q.n_rows, stream);
     if (st.kind == 1 && q.tile_off != nullptr && sbn_join_rows(P, st, q) > 0) return sbn_join_launch(P, st, q, stream);
@@ -1032,7 +1048,7 @@ cudaError_t launch_sample(sbn_program *P, const StepDesc &st, int k, const uint8
     for (size_t j = 0; j < st.ecards.size(); ++j) m.x_card[j] = st.ecards[j];
     const int64_t smem = bind_operands(P, st, m.in);
     m.smem_floats = static_cast<int32_t>(smem);
-    if (P->kind == kMpe) return sbn_argmax_launch(m, static_cast<size_t>(smem) * 4, stream);
+    if (sbn_log_domain(P->kind)) return sbn_argmax_launch(m, static_cast<size_t>(smem) * 4, stream);
     if (P->f64) return sbn_sample_launch<double>(m, 0, stream);
     return sbn_sample_launch<float>(m, static_cast<size_t>(smem) * 4, stream);
 }
@@ -1191,7 +1207,8 @@ int issue_all(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows
         case kCounts: SBN_CUDA(launch_prob(P, n_rows, d_out, nullptr, stream)); break;
         case kSample: SBN_CUDA(launch_prob(P, n_rows, d_out, dc.flags(P), stream)); break;
         case kMarginals:  // the readouts normalise
-        case kMpe: break;
+        case kMpe:
+        case kMap: break;
     }
     if (events) SBN_CUDA(cudaEventRecord(events[k + 1], stream));
     return SBN_OK;
@@ -1274,11 +1291,11 @@ int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n
 // The checks every run shares: the program is of the kind the entry point runs (kPosterior: the run, evidence
 // and profile calls, which take posterior and marginals programs), and the rows and their evidence are well formed
 int check_rows(const sbn_program *P, ProgramKind kind, const void *ev, int64_t ld_ev, int64_t n_rows) {
-    static const char *const name[] = {"posterior", "marginals", "counts", "sample", "MPE"};
+    static const char *const name[] = {"posterior", "marginals", "counts", "sample", "MPE", "MAP"};
     static const char *const entry[] = {"sbn_program_run_*", "sbn_program_run_*", "sbn_program_counts_host",
-                                        "sbn_program_sample_host", "sbn_program_mpe_host"};
+                                        "sbn_program_sample_host", "sbn_program_mpe_host", "sbn_program_mpe_host"};
     if (!P) return fail(SBN_E_INVALID, "null program");
-    if ((P->kind == kMarginals ? kPosterior : P->kind) != kind)
+    if ((P->kind == kMarginals ? kPosterior : P->kind == kMap ? kMpe : P->kind) != kind)
         return fail(SBN_E_INVALID, "a %s program runs through %s", name[P->kind], entry[P->kind]);
     if (n_rows <= 0) return fail(SBN_E_INVALID, "n_rows must be positive");
     if (P->n_ev > 0 && !ev) return fail(SBN_E_INVALID, "null evidence");
@@ -1339,7 +1356,7 @@ int run_rows(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows,
              cudaStream_t stream, const DrawnCodes &dc = {}) {
     // a short sample / MPE chunk runs as plain launches: capturing and instantiating a graph costs more than it
     // saves, and the short runs of a pattern whose rows are scattered through a frame come in many lengths
-    const bool short_chunk = (P->kind == kSample || P->kind == kMpe) && n_rows < kSampleGraphMinRows;
+    const bool short_chunk = (P->kind == kSample || sbn_log_domain(P->kind)) && n_rows < kSampleGraphMinRows;
     if (!P->use_graph || short_chunk) return issue_all(P, d_ev, ld_ev, n_rows, d_out, ld_out, stream, nullptr, dc);
     const GraphKey key = {d_ev, ld_ev, n_rows, d_out, ld_out, P->d_partial, P->d_drawn, dc.n_draws, dc.ld_drawn};
     const bool branched = P->use_branches && P->kind <= kMarginals;
@@ -1408,9 +1425,10 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
         delete P;
         return rc;
     }
-    if (P->kind == kMpe && f64) {
+    if (sbn_log_domain(P->kind) && f64) {
+        const char *what = P->kind == kMap ? "MAP" : "MPE";
         delete P;
-        return fail(SBN_E_INVALID, "an MPE program runs in float32 only (its tables are logs: nothing underflows)");
+        return fail(SBN_E_INVALID, "an %s program runs in float32 only (its tables are logs: nothing underflows)", what);
     }
     for (size_t t = 0; t < P->tables.size(); ++t) {
         if (P->tables[t].first + P->table_padded[t] > n_table_floats) {
@@ -1500,7 +1518,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
             SBN_CUDA_P(sbn_count_set_attrs());
             SBN_CUDA_P(sbn_sample_set_attrs());
             SBN_CUDA_P(sbn_argmax_set_attrs());
-            SBN_CUDA_P(sbn_batched_maxsum_set_attrs());
+            SBN_CUDA_P(sbn_batched_logdomain_set_attrs());
             done[device] = true;
         }
     }
@@ -1831,8 +1849,9 @@ int sbn_program_set_tables_f64(sbn_program *P, const double *tables, int64_t n_t
     return set_tables_common(P, tables, n_table_doubles, true);
 }
 
-// The host path of sample programs and (kind = kMpe, one draw, no seed) of MPE programs: the decoded codes of a
-// chunk are the drawn-code buffer, the per-row output is P(observed) (sample) or max log P(x, e) (MPE).
+// The host path of sample programs and (kind = kMpe, one draw, no seed) of MPE and marginal MAP programs: the
+// decoded codes of a chunk are the drawn-code buffer, the per-row output is P(observed) (sample) or max log P(x, e)
+// (MPE; max log P(x_MAP, e) for MAP).
 static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws, uint64_t seed,
                               int64_t row_base, uint8_t *out, void *prob, bool f64, ProgramKind kind = kSample) {
     int rc = check_rows(P, kind, ev, ld_ev, n_rows);

@@ -63,6 +63,8 @@ struct StepDesc {
     // sample step of a sample program (kind 4, sbn_sample.cuh): the `ecards` variables are drawn (not summed
     // out) into drawn-code rows q_offset ..; an input's `ev` terms may name drawn rows (col >= n_ev).
     // An argmax step of an MPE program (kind 5, sbn_mpe.cuh) has the same layout and decodes instead.
+    // kind-0 / 1 step of a marginal MAP program: its eliminated variables are summed out by log-sum-exp (else maximised)
+    bool logsumexp = false;
 };
 struct Slot {
     bool batched;
@@ -76,7 +78,7 @@ inline int64_t round_up(int64_t v, int64_t m) { return (v + m - 1) / m * m; }
 struct SbnSegment;  // sbn_chain.h
 struct SbnPair;     // sbn_pair.h
 
-// What a program computes, fixed by its header version (4 .. 8 in this order)
+// What a program computes, fixed by its header version (4 .. 9 in this order)
 enum ProgramKind {
     kPosterior,  // kind-0 / 1 steps, then the normalised posterior slot
     kMarginals,  // kind-2 readouts write the posterior, already normalised; no posterior slot
@@ -84,7 +86,12 @@ enum ProgramKind {
     kSample,     // kind-4 steps draw codes, post_slot holds P(observed)
     kMpe,        // log tables, max-sum upward pass, kind-5 argmax steps decode into the drawn-code buffer with
                  // one draw, post_slot holds max log P(x, e)
+    kMap,        // marginal MAP: an MPE program whose kind-0 / 1 steps each sum out (log-sum-exp) or maximise,
+                 // post_slot holds max log P(x_MAP, e); it runs through the MPE entry point
 };
+
+// Programs on log tables (MPE and marginal MAP): float32 only, the log-domain step kernels only
+inline bool sbn_log_domain(ProgramKind k) { return k == kMpe || k == kMap; }
 
 // Every address and size a captured graph bakes in: it is replayed only for an equal key
 struct GraphKey {

@@ -152,14 +152,39 @@ __device__ __forceinline__ float4 sbn_mul4(float4 a, float4 b) {
 // profiles and tests/kernel_census.py read them -- and their code.  Max-sum (`out = max_x sum_i in_i`) runs the
 // log-domain programs of the most probable explanation (planner.build_mpe_plan): additions and maxima
 // only, so there is no FMA to contract and a CPU replay in float32 is bitwise equal.
-struct SbnSumProduct {
+//
+// The kernels reduce through an accumulator: `Acc<T>` starts at `start<T>()`, takes every term with
+// `add` and gives the output with `finish` (`Acc4`, `start4`, `add4`, `finish4`: the same for the four rows
+// of a float4).  For a semiring (SbnSemiring below) the accumulator is the value itself, `add` is `plus` and
+// `finish` returns it, so the sum-product and max-sum kernels compile to the code they had.  Log-sum-exp
+// (SbnLogSumExp) needs a running maximum and a rescaled sum.
+template <typename R>
+struct SbnSemiring {
+    template <typename T> using Acc = T;
+    template <typename T> static __device__ __forceinline__ T start() { return R::template zero<T>(); }
+    template <typename T> static __device__ __forceinline__ void add(T &a, T t) { a = R::plus(a, t); }
+    template <typename T> static __device__ __forceinline__ T finish(T a) { return a; }
+    using Acc4 = float4;
+    static __device__ __forceinline__ float4 start4() {
+        const float z = R::template zero<float>();
+        return make_float4(z, z, z, z);
+    }
+    static __device__ __forceinline__ void add4(float4 &a, float4 t) {
+        a.x = R::plus(a.x, t.x);
+        a.y = R::plus(a.y, t.y);
+        a.z = R::plus(a.z, t.z);
+        a.w = R::plus(a.w, t.w);
+    }
+    static __device__ __forceinline__ float4 finish4(float4 a) { return a; }
+};
+struct SbnSumProduct : SbnSemiring<SbnSumProduct> {
     template <typename T> static __device__ __forceinline__ T one() { return T(1); }
     template <typename T> static __device__ __forceinline__ T zero() { return T(0); }
     template <typename T> static __device__ __forceinline__ T times(T a, T b) { return a * b; }
     template <typename T> static __device__ __forceinline__ T plus(T a, T b) { return a + b; }
     static __device__ __forceinline__ float4 times4(float4 a, float4 b) { return sbn_mul4(a, b); }
 };
-struct SbnMaxSum {
+struct SbnMaxSum : SbnSemiring<SbnMaxSum> {
     template <typename T> static __device__ __forceinline__ T one() { return T(0); }
     template <typename T> static __device__ __forceinline__ T zero() { return static_cast<T>(__int_as_float(0xff800000)); }
     template <typename T> static __device__ __forceinline__ T times(T a, T b) { return a + b; }
@@ -169,6 +194,61 @@ struct SbnMaxSum {
     }
     static __device__ __forceinline__ float4 times4(float4 a, float4 b) {
         return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+    }
+};
+// Log-sum-exp (`out = log sum_x exp(sum_i in_i)`): the buckets of summed-out variables of the marginal MAP
+// programs (planner.build_map_plan).  The terms combine as in max-sum; the reduction is online: m is the
+// largest term so far and s = sum exp(t - m), rescaled by exp(m_old - m_new) when m grows, and the output is
+// m + log(s).  Every exp argument is <= 0, so nothing overflows, and s >= 1 once a term is finite.  A term of
+// -inf adds nothing, so a bucket of impossible states gives -inf, never NaN.  expf / logf are the accurate
+// library functions (the library is built without fast math).
+struct SbnLogSumExp {
+    template <typename T> static __device__ __forceinline__ T one() { return T(0); }
+    template <typename T> static __device__ __forceinline__ T times(T a, T b) { return a + b; }
+    static __device__ __forceinline__ float4 times4(float4 a, float4 b) {
+        return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+    }
+    template <typename T> struct Acc {
+        T m, s;
+    };
+    template <typename T> static __device__ __forceinline__ T neg_inf() {
+        return static_cast<T>(__int_as_float(0xff800000));
+    }
+    template <typename T> static __device__ __forceinline__ T exp_(T x) {
+        if constexpr (std::is_same<T, float>::value) return expf(x);
+        else return exp(x);
+    }
+    template <typename T> static __device__ __forceinline__ T log_(T x) {
+        if constexpr (std::is_same<T, float>::value) return logf(x);
+        else return log(x);
+    }
+    template <typename T> static __device__ __forceinline__ Acc<T> start() { return {neg_inf<T>(), T(0)}; }
+    template <typename T> static __device__ __forceinline__ void add(Acc<T> &a, T t) {
+        if (t > a.m) {
+            a.s = a.s * exp_(a.m - t) + T(1);
+            a.m = t;
+        } else if (t > neg_inf<T>()) {
+            a.s += exp_(t - a.m);
+        }
+    }
+    template <typename T> static __device__ __forceinline__ T finish(Acc<T> a) {
+        return a.m == neg_inf<T>() ? a.m : a.m + log_(a.s);
+    }
+    struct Acc4 {
+        Acc<float> x, y, z, w;
+    };
+    static __device__ __forceinline__ Acc4 start4() {
+        const Acc<float> a = start<float>();
+        return {a, a, a, a};
+    }
+    static __device__ __forceinline__ void add4(Acc4 &a, float4 t) {
+        add(a.x, t.x);
+        add(a.y, t.y);
+        add(a.z, t.z);
+        add(a.w, t.w);
+    }
+    static __device__ __forceinline__ float4 finish4(const Acc4 &a) {
+        return make_float4(finish(a.x), finish(a.y), finish(a.z), finish(a.w));
     }
 };
 template <typename... R>
@@ -191,7 +271,8 @@ struct SbnPolicy<R> {
 // Thread = 4 consecutive rows (one float4) looping over the tile, one output per
 // iteration; the eliminated axis is reduced in-thread (strided float4 loads, each fully
 // coalesced across the warp); operands shared by consecutive outputs are L1 hits.
-// Policy: none (sum-product), or SbnMaxSum for the log-domain MPE programs.
+// Policy: none (sum-product), SbnMaxSum for the log-domain MPE programs, or SbnLogSumExp for the summed
+// buckets of the marginal MAP programs.
 template <int N_IN, int CX, typename... Policy>
 __global__ void __launch_bounds__(SBN_THREADS) sbn_step_batched(const __grid_constant__ SbnStep p) {
     using R = typename SbnPolicy<Policy...>::type;
@@ -273,8 +354,8 @@ __global__ void __launch_bounds__(SBN_THREADS) sbn_step_batched(const __grid_con
 #pragma unroll
         for (int i = 0; i < N_IN; ++i) e0[i] = off[i] + d1 * (p.n_axes > 1 ? p.in[i].stride[1] : 0);
         for (int d0 = 0; d0 < c0; ++d0) {
-            const float z0 = R::template zero<float>(), o1 = R::template one<float>();
-            float4 acc = make_float4(z0, z0, z0, z0);
+            const float o1 = R::template one<float>();
+            typename R::Acc4 acc = R::start4();
             auto term = [&](int x) {
                 float4 prod = make_float4(o1, o1, o1, o1);
 #pragma unroll
@@ -293,10 +374,7 @@ __global__ void __launch_bounds__(SBN_THREADS) sbn_step_batched(const __grid_con
                     }
                     prod = R::times4(prod, v);
                 }
-                acc.x = R::plus(acc.x, prod.x);
-                acc.y = R::plus(acc.y, prod.y);
-                acc.z = R::plus(acc.z, prod.z);
-                acc.w = R::plus(acc.w, prod.w);
+                R::add4(acc, prod);
             };
             if constexpr (CX > 0) {
 #pragma unroll
@@ -305,7 +383,7 @@ __global__ void __launch_bounds__(SBN_THREADS) sbn_step_batched(const __grid_con
 #pragma unroll 4
                 for (int x = 0; x < cx; ++x) term(x);
             }
-            *reinterpret_cast<float4 *>(p.out + static_cast<int64_t>(o_rest + d1 * c0 + d0) * ld + b) = acc;
+            *reinterpret_cast<float4 *>(p.out + static_cast<int64_t>(o_rest + d1 * c0 + d0) * ld + b) = R::finish4(acc);
 #pragma unroll
             for (int i = 0; i < N_IN; ++i) e0[i] += p.n_axes > 0 ? p.in[i].stride[0] : 0;
         }
@@ -883,7 +961,7 @@ __global__ void __launch_bounds__(256) sbn_step_flat(const __grid_constant__ Sbn
         for (int i = 0; i < SBN_MAX_IN; ++i)
             if (i < p.n_in) off[i] += d * p.in[i].stride[j];
     }
-    T acc = R::template zero<T>();
+    typename R::template Acc<T> acc = R::template start<T>();
     for (int x = 0; x < p.cx; ++x) {
         T prod = R::template one<T>();
 #pragma unroll
@@ -891,9 +969,9 @@ __global__ void __launch_bounds__(256) sbn_step_flat(const __grid_constant__ Sbn
             if (i < p.n_in)
                 prod = R::times(prod, __ldg(reinterpret_cast<const T *>(p.in[i].ptr) + off[i] +
                                             (p.zoff ? __ldg(p.zoff + i * p.cx + x) : x * p.in[i].sx)));
-        acc = R::plus(acc, prod);
+        R::add(acc, prod);
     }
-    reinterpret_cast<T *>(p.out)[o] = acc;
+    reinterpret_cast<T *>(p.out)[o] = R::finish(acc);
 }
 
 // ---------------------------------------------------------------------- normalise

@@ -61,10 +61,11 @@ cudaError_t sbn_tiled_u2_launch(int key, const SbnStep &q, int tile, bool preloa
 cudaError_t sbn_tiled_c_launch(int key, const SbnStep &q, int tile, bool preload, int64_t grid, cudaStream_t stream);
 cudaError_t sbn_slab_launch(int nu, const SbnStep &q, int tile, int64_t grid, cudaStream_t stream);
 cudaError_t sbn_batched_launch(const SbnStep &q, int64_t grid, cudaStream_t stream);
-cudaError_t sbn_batched_maxsum_launch(const SbnStep &q, int64_t grid, cudaStream_t stream);  // MPE programs
+cudaError_t sbn_batched_maxsum_launch(const SbnStep &q, int64_t grid, cudaStream_t stream);  // MPE and MAP programs
+cudaError_t sbn_batched_logsumexp_launch(const SbnStep &q, int64_t grid, cudaStream_t stream);  // MAP programs
 cudaError_t sbn_tiled_u0_set_attrs();
 cudaError_t sbn_tiled_u1_set_attrs();
 cudaError_t sbn_tiled_u2_set_attrs();   // + the slab variants
 cudaError_t sbn_tiled_c_set_attrs();
 cudaError_t sbn_batched_set_attrs();
-cudaError_t sbn_batched_maxsum_set_attrs();
+cudaError_t sbn_batched_logdomain_set_attrs();  // the max-sum and log-sum-exp instantiations

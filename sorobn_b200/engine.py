@@ -16,7 +16,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libsorobn_
 _lib = None
 
 SBN_OK = 0
-ABI_VERSION = 12
+ABI_VERSION = 13
 
 
 class EngineError(RuntimeError):
@@ -303,6 +303,14 @@ class Program:
         _check(load().sbn_program_mpe_host(self._h, codes.ctypes.data if self.n_ev else None, n_rows, n_rows,
                                            out.ctypes.data, log_prob.ctypes.data))
         return out, log_prob
+
+    def map(self, codes: np.ndarray, n_rows: int):
+        """Marginal MAP programs (planner.build_map_plan): (decoded codes uint8 [n_map, n_rows] of the MAP
+        variables in the order of `plan.sampled`, max log P(x_MAP, e) float32 [n_rows], -inf for a row of
+        probability zero), host path.  The engine runs them through the MPE entry point."""
+        if self.plan.version != 9:
+            raise ValueError(f"a version-{self.plan.version} program is not a marginal MAP program")
+        return self.mpe(codes, n_rows)
 
     def run_device(self, d_ev: int, ld_ev: int, n_rows: int, d_out: int, ld_out: int, stream: int = 0):
         """Device path: raw device pointers, asynchronous on `stream`."""

@@ -118,6 +118,19 @@ the decoded separator: the first joint state z (first variable fastest) with the
 
 Logs, because the maximum is a product of one entry of every CPT: it shrinks with the network and with
 every observed cell, past the float32 range of the sum-product programs, where its log cannot underflow.
+
+Marginal MAP programs (`build_map_plan`, VERSION 9) find, for every row, the joint state of chosen MAP
+variables that maximises P(x_MAP, e), every other unobserved variable summed out.  They are MPE programs
+whose elimination order puts every summed variable before any MAP variable, and whose kind-0 / kind-1
+steps carry one more word, the reduction of their eliminated variables:
+
+    kind 0/1 : kind n_in out_slot n_axes n_elim reduce | cards | ecards | inputs as above
+
+`reduce` 1 = log-sum-exp, `out = log sum_x exp(sum_i in_i[...])` (a bucket of summed variables); 0 = max,
+as in version 8 (a bucket of MAP variables, and every product-only step).  No launch mixes the two.
+Argmax steps (kind 5, the words of version 8) decode the MAP buckets only: their separators hold MAP and
+observed variables alone, because every summed variable is gone by then.  `p_slot` holds
+max_{x_MAP} log P(x_MAP, e).
 """
 from __future__ import annotations
 
@@ -155,6 +168,8 @@ SAMPLE_MAX_CARD = 255  # a sampled variable's states (its codes are uint8)
 SAMPLE_MAX_TERMS = 16  # gathered (col stride card) terms per input of a sample step (csrc: SBN_SAMPLE_MAX_TERMS)
 KIND_ARGMAX = 5  # decode one bucket's eliminated variables given the decoded separator (MPE programs only)
 VERSION_MPE = 8
+VERSION_MAP = 9  # marginal MAP: the MPE words plus a reduction word on kind-0 / kind-1 steps
+REDUCE_MAX, REDUCE_LOGSUMEXP = 0, 1
 HEADER_WORDS = 12
 
 
@@ -218,6 +233,7 @@ class Step:
     key: tuple = ()  # KIND_COUNT: ((ev_col, stride, card), ...) of the observed family members
     cstrides: tuple = ()  # KIND_COUNT: count-table stride of every output axis
     norm: object = None  # KIND_COUNT / KIND_SAMPLE / KIND_ARGMAX: the factor in the header's p_slot
+    reduce: int = REDUCE_MAX  # kind 0 / 1 of a marginal MAP plan: REDUCE_LOGSUMEXP sums its elims out
 
     @property
     def cx(self):
@@ -276,7 +292,7 @@ class Plan:
             # normalise: read unnormalised posterior, write posterior (a marginals program's
             # readouts write their segments normalised, counted above)
             total += 8 * self.Q
-        elif self.version in (VERSION_COUNTS, VERSION_SAMPLE, VERSION_MPE):
+        elif self.version in (VERSION_COUNTS, VERSION_SAMPLE, VERSION_MPE, VERSION_MAP):
             total += 4  # P(observed) (max log P(x, e)) out
         total += len(self.evidence)  # uint8 codes
         return total
@@ -309,10 +325,11 @@ class Plan:
         return max([size for batched, size in self.slots if batched] or [0])
 
 
-def _min_fill_order(scopes, hidden, card):
+def _min_fill_order(scopes, hidden, card, first=None):
     """Greedy min-fill (ties: smaller clique, then lower var id).  The reference
     eliminates in set-iteration order (bayes_net.py:779), which is arbitrary and
-    does not change the answer; BASELINE.json asks for min-fill."""
+    does not change the answer; BASELINE.json asks for min-fill.  With `first`, every
+    variable of `first` is eliminated before any other (min-fill within each group)."""
     adj = {}
     for sc in scopes:
         for a in sc:
@@ -323,7 +340,8 @@ def _min_fill_order(scopes, hidden, card):
     order = []
     while remaining:
         best_key, best_v = None, None
-        for v in remaining:
+        pool = remaining if first is None else ([v for v in remaining if v in first] or remaining)
+        for v in pool:
             nb = list(adj[v])
             fill = 0
             for i in range(len(nb)):
@@ -421,6 +439,26 @@ def build_mpe_plan(net: CompiledNet, evidence, order=None, max_in=MAX_IN, lift_e
                   lift_evidence=lift_evidence, fuse_elims=fuse_elims)
 
 
+def build_map_plan(net: CompiledNet, evidence, map_vars, order=None, max_in=MAX_IN, lift_evidence=True,
+                   fuse_elims=None) -> Plan:
+    """Plan the marginal MAP state of `map_vars` for every row (a version-9 program, see the module
+    docstring): the joint state of the MAP variables that maximises P(x_MAP, e), every other unobserved
+    variable summed out.  Only the MAP variables, the evidence and their ancestors are relevant: a barren
+    summed variable sums to one and drops out.  The upward pass eliminates the summed variables first
+    (log-sum-exp), then the MAP variables (max-sum); one argmax step per MAP bucket follows, top-down.
+    `order`, if given, must list every summed variable before any MAP variable.  `Plan.sampled` names the
+    variable of every decoded-code row."""
+    evidence, map_vars = tuple(evidence), tuple(map_vars)
+    if len(set(map_vars)) != len(map_vars):
+        raise ValueError("duplicate MAP variable")
+    if set(map_vars) & set(evidence):
+        raise ValueError("A MAP variable cannot be part of the event")
+    if not map_vars and not evidence:
+        raise ValueError("nothing to compute: no MAP variable and no evidence")
+    return _build(net, VERSION_MAP, evidence, targets=map_vars, order=order, max_in=max_in,
+                  lift_evidence=lift_evidence, fuse_elims=fuse_elims)
+
+
 def count_layout(net: CompiledNet):
     """(first count-table entry of every var id's family, total entries): the dense `[*parents, v]`
     arrays of the CPTs in CompiledNet order, concatenated."""
@@ -463,6 +501,7 @@ class _Builder:
         self.table_arrays = []
         self.table_axes = []  # variable of every axis of table_arrays[t], outermost first
         self.next_id = 0
+        self.summed = frozenset()  # marginal MAP plans: the variables a launch sums out by log-sum-exp
 
     def size(self, vs):
         """Joint states of the variables `vs`."""
@@ -487,6 +526,9 @@ class _Builder:
         card, evidence = self.card, self.evidence
         elims = tuple(elims)
         ecards = tuple(int(card[e]) for e in elims)
+        n_summed = sum(e in self.summed for e in elims)
+        assert n_summed in (0, len(elims)), "a launch may not both sum out and maximise"
+        reduce = REDUCE_LOGSUMEXP if n_summed else REDUCE_MAX
         dep = any(f.depends_on_evidence for f in inputs)
         batched = dep and self.mode == MODE_BATCHED
         if len(out_vars) > MAX_AXES:
@@ -520,7 +562,7 @@ class _Builder:
                 es = tuple(pos.get(e, 0) for e in elims)
                 plain = _Factor(f.is_slot, f.buf, f.vars, f.strides, (), False)  # evidence axes are output axes here
                 ins.append((plain, es, tuple(pos.get(u, 0) for u in axes)))
-            self.steps.append(Step(KIND_FLAT, ins, out_id, axes, axis_cards, elims, ecards))
+            self.steps.append(Step(KIND_FLAT, ins, out_id, axes, axis_cards, elims, ecards, reduce=reduce))
             strides = _dense_strides(axis_cards)
             n_ev = len(lifted_cols)
             ev = tuple((col, strides[k], c) for k, (col, c) in enumerate(lifted_cols))
@@ -531,7 +573,7 @@ class _Builder:
             es = tuple(pos.get(e, 0) for e in elims)
             ins.append((f, es, tuple(pos.get(u, 0) for u in out_vars)))
         self.steps.append(Step(KIND_BATCHED if batched else KIND_FLAT, ins, out_id, tuple(out_vars), cards, elims,
-                               ecards))
+                               ecards, reduce=reduce))
         return _Factor(True, out_id, tuple(out_vars), _dense_strides(cards), (), batched)
 
     def axis_order(self, inputs, out_set):
@@ -683,6 +725,8 @@ def _build(net, version, evidence, query=(), targets=(), mode=MODE_BATCHED, orde
     hidden = relevant - set(query) - set(evidence)
     b = _Builder(net, evidence, mode, max_in, lift_evidence, sorted(relevant))
     ev_col = b.ev_col
+    if version == VERSION_MAP:
+        b.summed = frozenset(hidden - set(targets))  # every relevant unobserved variable that is not MAP
 
     # bayes_net.py:768-776 -- one factor per relevant CPT; evidence axes become
     # per-row gathers instead of boolean filters
@@ -705,11 +749,13 @@ def _build(net, version, evidence, query=(), targets=(), mode=MODE_BATCHED, orde
         factors.append(_Factor(False, t, tuple(u for u, _ in free), tuple(s for _, s in free), ev, False))
 
     if order is None:
-        order = _min_fill_order([f.vars for f in factors], hidden, card)
+        order = _min_fill_order([f.vars for f in factors], hidden, card, first=b.summed if b.summed else None)
     else:
         order = list(order)
         if set(order) != hidden or len(order) != len(hidden):
             raise ValueError("elimination order must be a permutation of the hidden variables")
+        if any(v in b.summed for v in order[len(b.summed):]):
+            raise ValueError("a marginal MAP order must eliminate every summed variable before any MAP variable")
     b.order = order
 
     # bayes_net.py:778-786
@@ -732,7 +778,7 @@ def _build(net, version, evidence, query=(), targets=(), mode=MODE_BATCHED, orde
             for w in order[k + 1:]:
                 if len(elims) >= MAX_ELIM:
                     break
-                if w in gone or w not in union or z * int(card[w]) > MAX_Z:
+                if w in gone or w not in union or z * int(card[w]) > MAX_Z or (w in b.summed) != (x in b.summed):
                     continue
                 extra = [f for f in factors if w in f.vars]
                 if any(f.batched or not set(f.vars) <= union for f in extra):
@@ -744,14 +790,20 @@ def _build(net, version, evidence, query=(), targets=(), mode=MODE_BATCHED, orde
                 elims.append(w)
                 z *= int(card[w])
         gone.update(elims)
-        factors.append(b.product_chain(touching, tuple(elims)))
+        try:
+            factors.append(b.product_chain(touching, tuple(elims)))
+        except ValueError as e:
+            if version != VERSION_MAP:
+                raise
+            # the constrained order can build factors min-fill alone would not: say where
+            raise ValueError(f"the bucket of {[net.names[v] for v in elims]}: {e}") from e
         buckets.append((touching, tuple(elims), set().union(*[f.vars for f in touching]), factors[-1]))
 
     if version == VERSION_MARGINALS:
         return _marginals_passes(b, buckets, factors, targets)
     if version == VERSION_COUNTS:
         return _counts_passes(b, buckets, factors)
-    if version in (VERSION_SAMPLE, VERSION_MPE):
+    if version in (VERSION_SAMPLE, VERSION_MPE, VERSION_MAP):
         return _sample_passes(b, buckets, factors, version)
 
     # bayes_net.py:788-794: product of what is left; the answer's levels are sorted
@@ -843,17 +895,23 @@ def _sample_passes(b, buckets, leftovers, version):
     P(observed) is the product of the upward pass's leftover scalars, as in a counts plan.  In the log
     domain of an MPE plan the same steps mean max-sum: lambda_k(S_k) = max_{X_k} sum_{f in F_k} log f,
     the leftovers sum to max log P(x, e), and the argmax of sum_{f in F_k} log f(X_k, S_k = decoded, e)
-    is X_k's state in the maximising assignment."""
+    is X_k's state in the maximising assignment.
+
+    A marginal MAP plan (`version` VERSION_MAP, DESIGN.md "Marginal MAP") decodes its MAP buckets only.  Its
+    summed buckets come first in the order, so a MAP bucket's factors, and its separator, hold MAP and
+    observed variables alone: the same decode over lambda_k(S_k) = max_{X_k} sum_{f in F_k} log f, where
+    the f are CPTs and the log-sum-exp messages of the summed buckets."""
     kind = KIND_SAMPLE if version == VERSION_SAMPLE else KIND_ARGMAX
     card, names = b.card, b.net.names
     n_ev = len(b.evidence)
+    decodes = [k for k, (_, X, _, _) in enumerate(buckets) if not (set(X) & b.summed)]
     # the folds (products of the factors beyond max_in) do not depend on the draws: they all run before
     # the sample steps, which then form one contiguous run at the end of the program
-    inputs_of = [b.fold(F) for F, _, _, _ in buckets]
+    inputs_of = {k: b.fold(buckets[k][0]) for k in decodes}
     prob = b.emit(b.fold(leftovers), (), [], may_lift=False)
 
     drawn = {}  # var id -> drawn-code row
-    for k in reversed(range(len(buckets))):
+    for k in reversed(decodes):
         _, X, _, _ = buckets[k]
         for x in X:
             if int(card[x]) > SAMPLE_MAX_CARD:
@@ -1171,19 +1229,19 @@ def _serialise(plan: Plan, table_arrays):
     # float64 copy: only the CPU checker (oracle/program_interp.py) reads it, to
     # separate planner errors from fp32 rounding; the device gets the fp32 blob
     plan.table_blob64, offsets = _blobs(table_arrays)
-    if plan.version == VERSION_MPE:
-        # max-sum programs work on logs; a zero entry (and the padding) is -inf
+    if plan.version in (VERSION_MPE, VERSION_MAP):
+        # max-sum and log-sum-exp programs work on logs; a zero entry (and the padding) is -inf
         with np.errstate(divide="ignore"):
             plan.table_blob64 = np.log(plan.table_blob64)
     plan.table_blob = plan.table_blob64.astype(np.float32)
     plan.table_offsets = offsets
 
     extra = [0, 0]
-    if plan.version in (VERSION, VERSION_COUNTS, VERSION_SAMPLE, VERSION_MPE):
+    if plan.version in (VERSION, VERSION_COUNTS, VERSION_SAMPLE, VERSION_MPE, VERSION_MAP):
         post = [plan.post_slot, int(plan.slots[plan.post_slot][0])]
         if plan.version == VERSION_COUNTS:
             extra = [plan.n_counts, 0]
-        elif plan.version in (VERSION_SAMPLE, VERSION_MPE):
+        elif plan.version in (VERSION_SAMPLE, VERSION_MPE, VERSION_MAP):
             extra = [len(plan.sampled), 0]
     else:
         post = [-1, 0]  # the readouts write the posterior themselves
@@ -1205,6 +1263,8 @@ def _serialise(plan: Plan, table_arrays):
             w += list(st.cstrides)
         elif st.kind in (KIND_SAMPLE, KIND_ARGMAX):
             w.append(st.q_offset)
+        elif plan.version == VERSION_MAP:
+            w.append(st.reduce)
         w += list(st.cards)
         w += list(st.ecards)
         for f, estrides, strides in st.inputs:
