@@ -12,7 +12,7 @@
 //
 //   * one thread = one row, the grid and the bulk-TMA table staging of sbn_sample_step;
 //   * w(z) = ((0 + in_0) + in_1) + ... in input order, in float: additions only, so a CPU replay
-//     (tests/mpe_interp.py) is bitwise equal.  An impossible row (every w = -inf) decodes to state 0; its
+//     (oracle/program_interp.py) is bitwise equal.  An impossible row (every w = -inf) decodes to state 0; its
 //     max log P(x, e), in the program's p_slot, is -inf.
 #pragma once
 #include "sbn_kernels.cuh"

@@ -12,7 +12,7 @@
 //     65535 draws): a warp reads 32 consecutive rows of one operand entry when their drawn separators agree;
 //   * `zoff` ([n_in][cz]) is the row-invariant part of every operand's offset, built on the host; a
 //     batched operand's gathered offset is multiplied by the row pitch;
-//   * the arithmetic is fixed, so that a CPU replay (tests/sample_interp.py) follows it exactly: w(z) is
+//   * the arithmetic is fixed, so that a CPU replay (oracle/program_interp.py) follows it exactly: w(z) is
 //     the product of the entries in input order in T (multiplies only); the total and the cumulative sums
 //     are double sums in z order.  The pick is the first z with cum(z) > u * total, else the last z with
 //     w(z) > 0.  The weights are walked twice (the total, then the cumulative sums) instead of being held:

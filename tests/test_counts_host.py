@@ -1,40 +1,14 @@
 """The host side of expected_counts / fit_em, on the CPU: the device programs are replaced by the
-version-6 interpreter (tests/counts_interp.py), which refuses to run after close() as a real program
+version-6 interpreter (oracle/program_interp.py), which refuses to run after close() as a real program
 handle does."""
 import numpy as np
 import pandas as pd
 import pytest
 
-import counts_interp
 import em_oracle
+from interpreted_program import InterpretedProgram
 from oracle import ve_oracle
 from sorobn_b200 import engine, examples, workloads
-
-
-class InterpretedProgram:
-    """engine.Program for counts plans, executed by the interpreter in float64."""
-
-    live = []
-
-    def __init__(self, plan, device=None, f64=False):
-        self.plan, self.f64 = plan, f64
-        self.blob = plan.table_blob64 if f64 else plan.table_blob
-        self.closed = False
-        InterpretedProgram.live.append(self)
-
-    def counts(self, codes, n_rows):
-        if self.closed:
-            raise engine.EngineError("libsorobn_b200 error -1: null program", code=-1)
-        dtype = np.float64 if self.f64 else np.float32
-        return counts_interp.run(self.plan.words, self.blob, codes, n_rows=n_rows, dtype=dtype)
-
-    def set_tables(self, blob):
-        if self.closed:
-            raise engine.EngineError("libsorobn_b200 error -1: null program", code=-1)
-        self.blob = np.asarray(blob)
-
-    def close(self):
-        self.closed = True
 
 
 @pytest.fixture

@@ -1,6 +1,6 @@
 """Counts plans (planner.build_counts_plan, version-6 programs) and the EM oracle, checked on the CPU.
 
-tests/counts_interp.py executes the serialised words with numpy, so a pass here means the bucket
+oracle/program_interp.py executes the serialised words with numpy, so a pass here means the bucket
 choice, the keys, the strides, the count-table offsets and the slot reuse the device will see are
 right: the counts must equal tests/em_oracle.py (per row, `ve_oracle.query` of the unobserved family
 members given the observed cells)."""
@@ -8,9 +8,8 @@ members given the observed cells)."""
 import numpy as np
 import pytest
 
-import counts_interp
 import em_oracle
-from oracle import ve_oracle
+from oracle import program_interp, ve_oracle
 from sorobn_b200 import examples, planner, workloads
 
 EXAMPLES = ["alarm", "asia", "sprinkler", "grades"]
@@ -41,7 +40,7 @@ def check(bn, missing, n=40, seed=0, rtol=1e-12):
     plan = planner.build_counts_plan(net, observed)
     assert plan.version == 6 and plan.words[1] == 6 and plan.n_counts == planner.count_layout(net)[1]
     codes = sample(net, n, seed, observed)
-    got, prob = counts_interp.run(plan.words, plan.table_blob64, codes, n_rows=n)
+    got, prob = program_interp.run_counts(plan.words, plan.table_blob64, codes, n_rows=n)
     rows = rows_of(net, codes, observed)
     want = oracle_vector(net, dn, rows)
     assert np.allclose(got, want, rtol=rtol, atol=1e-12 * n), (missing, np.max(np.abs(got - want)))
@@ -79,7 +78,7 @@ def test_a_fully_observed_pattern_is_the_histogram(name):
     codes = sample(net, n, 5, range(len(net.names)))
     plan = planner.build_counts_plan(net, range(len(net.names)))
     assert all(st.kind == planner.KIND_COUNT and not st.inputs for st in plan.steps if st.kind == planner.KIND_COUNT)
-    got, _ = counts_interp.run(plan.words, plan.table_blob64, codes)
+    got, _ = program_interp.run_counts(plan.words, plan.table_blob64, codes)
     offsets, _ = planner.count_layout(net)
     for v in range(len(net.names)):
         scope = net.scope(v)
@@ -100,7 +99,7 @@ def test_rows_without_any_observed_cell_give_the_prior():
     bn = examples.grades()
     net = bn._compiled
     plan = planner.build_counts_plan(net, ())
-    got, prob = counts_interp.run(plan.words, plan.table_blob64, np.zeros((0, 3), np.uint8), n_rows=3)
+    got, prob = program_interp.run_counts(plan.words, plan.table_blob64, np.zeros((0, 3), np.uint8), n_rows=3)
     want = oracle_vector(net, oracle_net(bn), [{}] * 3)
     assert np.allclose(got, want, rtol=1e-12) and np.allclose(prob, 1.0)
 
@@ -125,8 +124,8 @@ def test_float32_interpretation_stays_within_2e_6():
     observed = [net.index[e] for e in w.evidence[3:]]
     plan = planner.build_counts_plan(net, observed)
     codes = sample(net, 64, 4, observed)
-    got64, _ = counts_interp.run(plan.words, plan.table_blob64, codes)
-    got32, prob = counts_interp.run(plan.words, plan.table_blob, codes, dtype=np.float32)
+    got64, _ = program_interp.run_counts(plan.words, plan.table_blob64, codes)
+    got32, prob = program_interp.run_counts(plan.words, plan.table_blob, codes, dtype=np.float32)
     assert np.isfinite(prob).all()
     big = got64 > 1e-3
     assert np.max(np.abs(got32 - got64)[big] / got64[big]) < 2e-6
@@ -139,7 +138,7 @@ def test_rows_out_of_range_and_impossible_rows_add_nothing():
     plan = planner.build_counts_plan(net, ev)
     # Rain = F, Sprinkler = F, Wet grass = T has probability zero
     codes = np.array([[0, 1], [0, 1], [1, 1]], dtype=np.uint8)  # domains sorted: False = 0
-    got, prob = counts_interp.run(plan.words, plan.table_blob64, codes)
+    got, prob = program_interp.run_counts(plan.words, plan.table_blob64, codes)
     assert np.isnan(prob[0]) and prob[1] > 0
     want = oracle_vector(net, oracle_net(bn), rows_of(net, codes[:, 1:], ev))
     assert np.allclose(got, want, rtol=1e-12)

@@ -1,5 +1,5 @@
 """Marginal MAP on the device (BayesNet.map_many, the log-sum-exp and max-sum step kernels and sbn_argmax_step),
-against the float32 replay of the words (tests/map_interp.py) and the float64 oracle (tests/map_oracle.py)."""
+against the float32 replay of the words (oracle/program_interp.py) and the float64 oracle (tests/map_oracle.py)."""
 import os
 import subprocess
 import sys
@@ -8,10 +8,9 @@ import numpy as np
 import pandas as pd
 import pytest
 
-import map_interp
 import map_oracle
 from conftest import ROOT
-from oracle import ve_oracle
+from oracle import program_interp, ve_oracle
 from sorobn_b200 import engine, examples, planner, workloads
 from test_gpu_sample import networks
 
@@ -56,7 +55,7 @@ def test_log_values_match_the_replay_and_decisions_the_oracle():
             for n_rows in ROWS:
                 c = np.ascontiguousarray(codes[:, :n_rows])
                 got, lp = program.map(c, n_rows)
-                want, wlp = map_interp.run(plan.words, plan.table_blob, c, n_rows=n_rows, dtype=np.float32)
+                want, wlp = program_interp.run_mpe(plan.words, plan.table_blob, c, n_rows=n_rows, dtype=np.float32)
                 assert lp.dtype == np.float32 and got.shape == want.shape
                 fin = np.isfinite(wlp)
                 assert np.array_equal(np.isfinite(lp), fin), (name, m, n_rows)
@@ -158,7 +157,7 @@ def test_twelve_or_more_missing_cells_per_row():
     for ev, rows, codes in groups:
         m = tuple(sorted(net.index[c] for c in X.columns if net.index[c] not in ev))
         plan = planner.build_map_plan(net, ev, m)
-        d64, l64 = map_interp.run(plan.words, plan.table_blob64, codes, n_rows=len(rows), dtype=np.float64)
+        d64, l64 = program_interp.run_mpe(plan.words, plan.table_blob64, codes, n_rows=len(rows), dtype=np.float64)
         assert np.all(np.abs(log_p.to_numpy()[rows] - l64) <= TOL * np.maximum(1.0, np.abs(l64)))
 
 
@@ -184,7 +183,7 @@ def test_row_counts_around_the_graph_threshold_and_large_batches(n):
     program = engine.Program(plan, device=0)
     got, lp = program.map(codes, n)
     if n < 10_000:
-        want, wlp = map_interp.run(plan.words, plan.table_blob, codes, dtype=np.float32)
+        want, wlp = program_interp.run_mpe(plan.words, plan.table_blob, codes, dtype=np.float32)
         assert np.array_equal(got, want)
         assert np.all(np.abs(lp - wlp) <= RTOL * np.maximum(1.0, np.abs(wlp)))
     pieces = [program.map(np.ascontiguousarray(codes[:, a:a + 4096]), min(4096, n - a)) for a in range(0, n, 4096)]

@@ -2,7 +2,7 @@
 network of the variant corpus (tests/kernel_corpus.py: build_marginals), against the float64 oracle.
 
 Per network, the plan targets every variable that is not evidence.  The reference is the float64 CPU
-interpreter of the same plan (tests/marginals_interp.py), itself held to ve_oracle.query on a sample
+interpreter of the same plan (oracle/program_interp.py), itself held to ve_oracle.query on a sample
 of rows.  Every entry of every row is checked, at row counts around the readout's 128-thread CTA and
 the step kernels' edges: 1e-6 relative, exact zeros exactly 0, impossible rows NaN, and a NaN segment
 on a possible row only where the float32 range rule explains it.  The float64 batch and the float64
@@ -24,8 +24,7 @@ import pytest
 
 import kernel_census
 import kernel_corpus
-import marginals_interp
-from oracle import ve_oracle
+from oracle import program_interp, ve_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -48,9 +47,9 @@ class MCase:
         self.spec, self.net, self.dn, self.plan, self.evidence = kernel_corpus.build_marginals(name)
         self.n = n_rows
         self.codes = kernel_corpus.evidence_rows(self.spec, self.evidence, n_rows, seed=1)
-        self.starts = marginals_interp.segment_starts(self.plan)
+        self.starts = program_interp.segment_starts(self.plan)
         if reference:  # the census needs the programs only
-            self.want = marginals_interp.run(self.plan.words, self.plan.table_blob64, self.codes, n_rows=n_rows)
+            self.want = program_interp.run_marginals(self.plan.words, self.plan.table_blob64, self.codes, n_rows=n_rows)
             self.p_e = np.array([self.evidence_probability(b) for b in range(n_rows)])
         self.default = engine.Program(self.plan)
         self.plain = engine.Program(self.plan)
@@ -104,7 +103,7 @@ def test_marginals_case_matches_oracle(name):
     full = None
     for n in ROW_COUNTS:
         out = c.default.run(np.ascontiguousarray(codes[:, :n]), n)
-        worst, _ = marginals_interp.check_posterior(out, c.want[:, :n], c.starts, p_event=c.p_e[:n])
+        worst, _ = program_interp.check_posterior(out, c.want[:, :n], c.starts, p_event=c.p_e[:n])
         assert worst < RTOL, (n, worst)
         full = out
     flagged = np.flatnonzero(np.isnan(full).any(axis=0) & ~np.isnan(c.want).all(axis=0))
@@ -117,11 +116,11 @@ def test_marginals_case_matches_oracle(name):
     for other in (c.plain, c.branched):
         assert np.allclose(other.run(codes, N_MAX), full, rtol=3e-6, atol=1e-30, equal_nan=True)
     # float64: the batch on every row, the single-event program on the edge rows and the flagged ones
-    worst, _ = marginals_interp.check_posterior(c.batched64.run(codes, N_MAX), c.want, c.starts)
+    worst, _ = program_interp.check_posterior(c.batched64.run(codes, N_MAX), c.want, c.starts)
     assert worst < 1e-12, worst
     for b in sorted({0, N_MAX - 1, *flagged[:4].tolist()}):
         one = np.ascontiguousarray(codes[:, b:b + 1])
-        worst, _ = marginals_interp.check_posterior(c.flat64.run(one, 1), c.want[:, b:b + 1], c.starts)
+        worst, _ = program_interp.check_posterior(c.flat64.run(one, 1), c.want[:, b:b + 1], c.starts)
         assert worst < 1e-12, (b, worst)
     c.close()
 
@@ -131,7 +130,7 @@ def test_large_batch_on_the_benchmark_grid():
     test): every entry against the float64 interpreter, a sample of rows against the oracle."""
     c = MCase(BIG_NAME, BIG_ROWS)
     out = c.default.run(c.codes, BIG_ROWS)
-    worst, _ = marginals_interp.check_posterior(out, c.want, c.starts, p_event=c.p_e)
+    worst, _ = program_interp.check_posterior(out, c.want, c.starts, p_event=c.p_e)
     assert worst < RTOL, worst
     c.check_oracle(oracle_rows(c, BIG_ROWS))
     c.close()

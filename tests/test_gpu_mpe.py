@@ -1,5 +1,5 @@
 """The most probable explanation on the device (BayesNet.mpe_many, the max-sum step kernels and
-sbn_argmax_step), against the float32 interpreter bit for bit (tests/mpe_interp.py) and the float64 oracle
+sbn_argmax_step), against the float32 interpreter bit for bit (oracle/program_interp.py) and the float64 oracle
 (tests/mpe_oracle.py)."""
 import os
 import subprocess
@@ -9,10 +9,9 @@ import numpy as np
 import pandas as pd
 import pytest
 
-import mpe_interp
 import mpe_oracle
 from conftest import ROOT
-from oracle import ve_oracle
+from oracle import program_interp, ve_oracle
 from sorobn_b200 import engine, examples, planner, workloads
 from test_gpu_sample import networks
 
@@ -40,7 +39,7 @@ def test_codes_and_log_probabilities_equal_the_float32_interpreter_bitwise():
         for n_rows in ROWS:
             c = np.ascontiguousarray(codes[:, :n_rows])
             got, lp = program.mpe(c, n_rows)
-            want, wlp = mpe_interp.run(plan.words, plan.table_blob, c, n_rows=n_rows, dtype=np.float32)
+            want, wlp = program_interp.run_mpe(plan.words, plan.table_blob, c, n_rows=n_rows, dtype=np.float32)
             assert np.array_equal(got, want), (name, n_rows)
             assert lp.dtype == np.float32 and np.array_equal(lp.view(np.uint32), wlp.view(np.uint32)), (name, n_rows)
         program.close()
@@ -56,7 +55,7 @@ def test_graph_path_and_chunks_equal_the_interpreter():
     codes = np.ascontiguousarray(workloads.forward_sample_codes(net, n, 4)[list(observed)])
     program = engine.Program(plan, device=0)
     got, lp = program.mpe(codes, n)
-    want, wlp = mpe_interp.run(plan.words, plan.table_blob, codes, dtype=np.float32)
+    want, wlp = program_interp.run_mpe(plan.words, plan.table_blob, codes, dtype=np.float32)
     assert np.array_equal(got, want) and np.array_equal(lp, wlp)
     again = program.mpe(codes, n)
     assert np.array_equal(again[0], got) and np.array_equal(again[1].view(np.uint32), lp.view(np.uint32))
@@ -69,7 +68,7 @@ def test_graph_path_and_chunks_equal_the_interpreter():
     # no evidence at all: one max log P for every row, broadcast from an evidence-independent slot
     free = engine.Program(planner.build_mpe_plan(net, ()), device=0)
     d, l = free.mpe(np.zeros((0, 5000), dtype=np.uint8), 5000)
-    wd, wl = mpe_interp.run(free.plan.words, free.plan.table_blob, np.zeros((0, 1), dtype=np.uint8), n_rows=1)
+    wd, wl = program_interp.run_mpe(free.plan.words, free.plan.table_blob, np.zeros((0, 1), dtype=np.uint8), n_rows=1)
     assert (d == wd).all() and (l == wl[0]).all()
 
 
@@ -81,7 +80,7 @@ def test_explanations_against_the_float64_oracle():
         c = np.ascontiguousarray(codes[:, :n_rows])
         got, lp = engine.Program(plan, device=0).mpe(c, n_rows)
         if name == "grid10x10":  # too wide for the dense oracle: the float64 interpreter is the reference
-            d64, l64 = mpe_interp.run(plan.words, plan.table_blob64, c, dtype=np.float64)
+            d64, l64 = program_interp.run_mpe(plan.words, plan.table_blob64, c, dtype=np.float64)
             assert np.all(np.abs(lp - l64) <= TOL * np.maximum(1.0, np.abs(l64)))
             near_ties += int((got != d64).any(axis=0).sum())
             checked += n_rows

@@ -1,5 +1,5 @@
 """Exact posterior draws on the device (BayesNet.sample_many, the sample kernel sbn_sample_step), against
-the CPU replay of the same random stream (tests/sample_interp.py), marginals_many and the programs'
+the CPU replay of the same random stream (oracle/program_interp.py), marginals_many and the programs'
 float64 twins."""
 import os
 import subprocess
@@ -10,8 +10,8 @@ import pandas as pd
 import pytest
 
 import kernel_corpus
-import sample_interp
 from conftest import ROOT
+from oracle import program_interp
 from sorobn_b200 import engine, examples, planner, workloads
 
 pytestmark = pytest.mark.gpu
@@ -54,10 +54,10 @@ def replay(plan, program, codes, n_rows, n_draws, seed, f64, rtol):
     drawn, prob = program.sample(codes, n_rows, n_draws, seed)
     dtype = np.float64 if f64 else np.float32
     blob = plan.table_blob64 if f64 else plan.table_blob
-    mine, p_mine, info = sample_interp.run(plan.words, blob, codes, n_rows=n_rows, n_draws=n_draws, seed=seed, dtype=dtype,
-                                           given=drawn)
+    mine, p_mine, info = program_interp.run_sample(plan.words, blob, codes, n_rows=n_rows, n_draws=n_draws, seed=seed,
+                                                   dtype=dtype, given=drawn)
     ok = ~np.isnan(prob)
-    p_ref = sample_interp.run(plan.words, plan.table_blob64, codes, n_rows=n_rows, seed=seed)[1]
+    p_ref = program_interp.run_sample(plan.words, plan.table_blob64, codes, n_rows=n_rows, seed=seed)[1]
     if f64:
         assert np.array_equal(np.isnan(prob), np.isnan(p_ref))
     assert np.all(np.abs(prob[ok] - p_ref[ok]) <= (1e-9 if f64 else 1e-4) * p_ref[ok]), (n_rows, n_draws)
@@ -151,7 +151,7 @@ def test_rows_below_the_float32_range_are_drawn_in_float64():
     observed = tuple(net.index[c] for c in rows.columns)
     codes = np.ascontiguousarray(rows.to_numpy().T.astype(np.uint8))
     plan = planner.build_sample_plan(net, observed)
-    _, p64, _ = sample_interp.run(plan.words, plan.table_blob64, codes)
+    _, p64, _ = program_interp.run_sample(plan.words, plan.table_blob64, codes)
     # random codes on 57 of 60 nodes: with these seeds every row has a positive probability below 1e-30; the
     # filter keeps the test's premise should the generator change
     keep = np.flatnonzero((p64 > 0) & (p64 < 1e-30))

@@ -1,7 +1,7 @@
 """Marginal MAP plans (planner.build_map_plan, version-9 programs) and BayesNet.map_many, checked on the CPU.
 
 tests/map_oracle.py finds the marginal MAP state in float64 without the planner (brute force, and the
-argmax of the dense posterior); tests/map_interp.py executes the serialised words.  The host side of
+argmax of the dense posterior); oracle/program_interp.py executes the serialised words.  The host side of
 `map_many` runs with the device programs replaced by the float32 interpreter."""
 import json
 import os
@@ -11,10 +11,10 @@ import pandas as pd
 import pytest
 
 import kernel_corpus
-import map_interp
 import map_oracle
 from conftest import build_network, load_golden
-from oracle import ve_oracle
+from interpreted_program import InterpretedProgram
+from oracle import program_interp, ve_oracle
 from sorobn_b200 import engine, examples, planner, workloads
 
 EXAMPLES = ["alarm", "asia", "sprinkler", "grades"]
@@ -115,8 +115,8 @@ def test_interpreter_finds_the_oracles_state(name):
         plan = planner.build_map_plan(net, observed, m)
         assert sorted(plan.sampled) == list(m)
         codes = np.ascontiguousarray(codes_all[list(observed)])
-        d64, l64 = map_interp.run(plan.words, plan.table_blob64, codes, n_rows=n_rows, dtype=np.float64)
-        d32, l32 = map_interp.run(plan.words, plan.table_blob, codes, n_rows=n_rows, dtype=np.float32)
+        d64, l64 = program_interp.run_mpe(plan.words, plan.table_blob64, codes, n_rows=n_rows, dtype=np.float64)
+        d32, l32 = program_interp.run_mpe(plan.words, plan.table_blob, codes, n_rows=n_rows, dtype=np.float32)
         assert l64.dtype == np.float64 and l32.dtype == np.float32
         if not observed:
             codes = np.zeros((0, n_rows), dtype=np.uint8)
@@ -143,7 +143,7 @@ def test_impute_goldens_are_reproduced(name):
         plan = planner.build_map_plan(net, observed, m)
         codes = np.array([[net.domains[v].index(sample[net.names[v]])] for v in observed], dtype=np.uint8).reshape(len(observed), 1)
         for blob, dtype, tol in ((plan.table_blob64, np.float64, 1e-9), (plan.table_blob, np.float32, TOL)):
-            d, lp = map_interp.run(plan.words, blob, codes, n_rows=1, dtype=dtype)
+            d, lp = program_interp.run_mpe(plan.words, blob, codes, n_rows=1, dtype=dtype)
             ev = {k: v for k, v in sample.items() if v is not None}
             mine = {net.names[v]: net.domains[v][d[j, 0]] for j, v in enumerate(plan.sampled)}
             want = {k: filled[k] for k in mine}
@@ -166,7 +166,7 @@ def test_an_impossible_row_has_log_probability_minus_infinity():
     event = {"Rain": False, "Sprinkler": False, "Wet grass": True}
     codes = np.array([[net.domains[v].index(event[net.names[v]])] for v in observed], dtype=np.uint8)
     for blob, dtype in ((plan.table_blob, np.float32), (plan.table_blob64, np.float64)):
-        _, lp = map_interp.run(plan.words, blob, codes, dtype=dtype)
+        _, lp = program_interp.run_mpe(plan.words, blob, codes, dtype=dtype)
         assert lp[0] == -np.inf and not np.isnan(lp[0])
 
 
@@ -227,7 +227,7 @@ def test_a_map_set_of_every_unobserved_variable_is_the_mpe_plan():
         mp = planner.build_map_plan(net, observed, hidden)
         assert mp.order == mpe.order and mp.sampled == mpe.sampled
         assert all(st.reduce == planner.REDUCE_MAX for st in mp.steps)
-        hdr, _, _, steps = map_interp.parse(mp.words)
+        hdr, _, _, steps = program_interp.parse(mp.words)
         stripped = list(mp.words[:planner.HEADER_WORDS + 2 * hdr["n_tables"] + 2 * hdr["n_slots"]])
         p = len(stripped)
         w = [int(x) for x in mp.words]
@@ -314,24 +314,6 @@ def test_benchmark_grid_plan_counts():
 
 
 # --------------------------------------------------------------------- map_many on the interpreter
-class InterpretedProgram:
-    """engine.Program for marginal MAP plans, executed by the float32 interpreter."""
-
-    live = []
-
-    def __init__(self, plan, device=None, f64=False):
-        assert not f64, "MAP programs run in float32 only"
-        self.plan = plan
-        InterpretedProgram.live.append(self)
-
-    def map(self, codes, n_rows):
-        assert self.plan.version == planner.VERSION_MAP
-        return map_interp.run(self.plan.words, self.plan.table_blob, codes, n_rows=n_rows, dtype=np.float32)
-
-    def close(self):
-        pass
-
-
 @pytest.fixture
 def interpreted(monkeypatch):
     InterpretedProgram.live = []

@@ -1,6 +1,6 @@
 """Marginals plans of every network of the variant corpus (tests/kernel_corpus.py), on the CPU.
 
-tests/marginals_interp.py runs each plan: in float64 against the float64 oracle at 1e-12, and in
+oracle/program_interp.py runs each plan: in float64 against the float64 oracle at 1e-12, and in
 float32 with the readout kernel's arithmetic (float32 products summed in runs of 32, the runs' sums
 added in float64) against the float64 run at the project's 1e-6.  A readout sums every joint state
 of its bucket but the target per entry -- 625 on the benchmark grid, 2,187 and 2,560 on two corpus
@@ -13,8 +13,7 @@ import numpy as np
 import pytest
 
 import kernel_corpus
-import marginals_interp
-from oracle import ve_oracle
+from oracle import program_interp, ve_oracle
 from sorobn_b200 import planner
 
 N_ROWS = 64
@@ -24,7 +23,7 @@ def runs(name):
     """The corpus network's marginals plan, 64 evidence rows, the float64 run of the plan, and P(e)."""
     spec, net, dn, plan, evidence = kernel_corpus.build_marginals(name)
     codes = kernel_corpus.evidence_rows(spec, evidence, N_ROWS, seed=1)
-    want = marginals_interp.run(plan.words, plan.table_blob64, codes, n_rows=N_ROWS)
+    want = program_interp.run_marginals(plan.words, plan.table_blob64, codes, n_rows=N_ROWS)
     p_e = np.array([ve_oracle.evidence_probability(dn, dict(zip(evidence, map(int, codes[:, b])))) if evidence else 1.0
                     for b in range(N_ROWS)])
     return spec, net, dn, plan, evidence, codes, want, p_e
@@ -33,7 +32,7 @@ def runs(name):
 @pytest.mark.parametrize("name", kernel_corpus.MARGINALS_CASES)
 def test_corpus_marginals_plan(name):
     spec, net, dn, plan, evidence, codes, want, p_e = runs(name)
-    starts = marginals_interp.segment_starts(plan)
+    starts = program_interp.segment_starts(plan)
     assert plan.Q == sum(int(net.card[t]) for t in plan.targets)
     assert sorted(plan.targets) == sorted(set(range(len(net.names))) - {net.index[e] for e in evidence})
     # float64 against the oracle, every target, on rows 0, n - 1 and others between
@@ -49,8 +48,8 @@ def test_corpus_marginals_plan(name):
             assert np.allclose(got, ref, rtol=1e-12, atol=1e-300), (b, net.names[t], got, ref)
             assert (got[ref == 0] == 0).all(), (b, net.names[t], got, ref)
     # float32 tables and steps, the readout kernel's double partial sums, at 1e-6 on every entry
-    got32 = marginals_interp.run(plan.words, plan.table_blob, codes, n_rows=N_ROWS, dtype=np.float32)
-    worst, flagged = marginals_interp.check_posterior(got32, want, starts, p_event=p_e)
+    got32 = program_interp.run_marginals(plan.words, plan.table_blob, codes, n_rows=N_ROWS, dtype=np.float32)
+    worst, flagged = program_interp.check_posterior(got32, want, starts, p_event=p_e)
     assert worst < 1e-6, worst
 
 
@@ -69,10 +68,10 @@ def test_float32_readout_accumulator_breaks_1e6(name, cz):
     """The readout as it was first written, a float32 accumulator, on the networks where it misses 1e-6."""
     spec, net, dn, plan, evidence, codes, want, p_e = runs(name)
     assert max(st.cx for st in plan.steps if st.kind == planner.KIND_MARGINAL) == cz
-    starts = marginals_interp.segment_starts(plan)
-    old = marginals_interp.run(plan.words, plan.table_blob, codes, n_rows=N_ROWS, dtype=np.float32,
-                               readout_acc=np.float32)
-    worst, _ = marginals_interp.check_posterior(old, want, starts, p_event=p_e)
+    starts = program_interp.segment_starts(plan)
+    old = program_interp.run_marginals(plan.words, plan.table_blob, codes, n_rows=N_ROWS, dtype=np.float32,
+                                       readout_acc=np.float32)
+    worst, _ = program_interp.check_posterior(old, want, starts, p_event=p_e)
     assert worst > 1e-6, worst
 
 

@@ -1,6 +1,6 @@
 """Marginals plans (planner.build_marginals_plan, version-5 programs), checked on the CPU.
 
-tests/marginals_interp.py executes the serialised words with numpy, so a pass here means the
+oracle/program_interp.py executes the serialised words with numpy, so a pass here means the
 bucket tree (upward messages, downward messages, readouts), the strides, the evidence gathers and
 the slot reuse the device will see are right: every target's segment must equal the reference's
 single-variable answers (tests/golden) and oracle.ve_oracle.query."""
@@ -9,9 +9,8 @@ import hashlib
 import numpy as np
 import pytest
 
-import marginals_interp
 from conftest import build_network, case_event, dense_answer, golden_names, load_golden
-from oracle import ve_oracle
+from oracle import program_interp, ve_oracle
 from sorobn_b200 import BayesNet, planner, synthetic, workloads
 
 
@@ -63,7 +62,7 @@ def test_marginals_plan_matches_reference_goldens(name):
                 if mode == planner.MODE_FLAT and b >= 2:
                     break
                 sub = codes[:, b:b + 1] if mode == planner.MODE_FLAT else codes
-                got = marginals_interp.run(plan.words, plan.table_blob64, sub, n_rows=1 if mode == planner.MODE_FLAT else len(rows))
+                got = program_interp.run_marginals(plan.words, plan.table_blob64, sub, n_rows=1 if mode == planner.MODE_FLAT else len(rows))
                 col = 0 if mode == planner.MODE_FLAT else b
                 seg = segments(plan, net, got)
                 for case in cases:
@@ -96,8 +95,8 @@ def test_float32_interpretation_on_the_benchmark_grid():
     n = 256  # a float32 readout accumulator is off by 1.8e-6 on one of these rows: the check must see that
     codes = wl.codes(bn, n, seed=3)
     plan = planner.build_marginals_plan(net, [net.index[e] for e in wl.evidence])
-    got64 = marginals_interp.run(plan.words, plan.table_blob64, codes)
-    got32 = marginals_interp.run(plan.words, plan.table_blob, codes, dtype=np.float32)
+    got64 = program_interp.run_marginals(plan.words, plan.table_blob64, codes)
+    got32 = program_interp.run_marginals(plan.words, plan.table_blob, codes, dtype=np.float32)
     assert np.isfinite(got32).all()
     assert np.max(np.abs(got32 - got64) / np.maximum(got64, 1e-300) * (got64 > 1e-12)) < 1e-6
     assert np.allclose(got32.sum(axis=0), 70, rtol=1e-5)
@@ -109,8 +108,6 @@ def test_float32_interpretation_on_the_benchmark_grid():
 
 
 def marginals_interp_v4(plan, codes):
-    from oracle import program_interp
-
     return program_interp.run(plan.words, plan.table_blob64, codes)
 
 
@@ -122,7 +119,7 @@ def _check_against_oracle(bn, ev_vars, targets, B, seed):
         else np.zeros((0, B), np.uint8)
     plan = planner.build_marginals_plan(net, [net.index[e] for e in ev_vars],
                                         targets=None if targets is None else [net.index[t] for t in targets])
-    got = marginals_interp.run(plan.words, plan.table_blob64, codes, n_rows=B)
+    got = program_interp.run_marginals(plan.words, plan.table_blob64, codes, n_rows=B)
     seg = segments(plan, net, got)
     if targets is not None:
         assert sorted(seg) == sorted(targets)
@@ -186,7 +183,7 @@ def test_impossible_rows_are_nan():
     dom = {v: net.domains[net.index[v]] for v in ev}
     rows = [(False, False, True), (True, False, True)]
     codes = np.array([[dom[v].index(r[i]) for r in rows] for i, v in enumerate(ev)], dtype=np.uint8)
-    got = marginals_interp.run(plan.words, plan.table_blob64, codes)
+    got = program_interp.run_marginals(plan.words, plan.table_blob64, codes)
     assert np.isnan(got[:, 0]).all()
     assert np.isfinite(got[:, 1]).all()
 

@@ -1,17 +1,17 @@
 """MPE plans (planner.build_mpe_plan, version-8 programs) and BayesNet.mpe_many, checked on the CPU.
 
 tests/mpe_oracle.py finds the most probable explanation in float64 without the planner (brute force,
-and dense max-sum elimination with a traceback); tests/mpe_interp.py executes the serialised words.
+and dense max-sum elimination with a traceback); oracle/program_interp.py executes the serialised words.
 The host side of `mpe_many` runs with the device programs replaced by the float32 interpreter, which
 follows the kernels' arithmetic exactly."""
 import numpy as np
 import pandas as pd
 import pytest
 
-import mpe_interp
 import mpe_oracle
 from conftest import build_network, load_golden
-from oracle import ve_oracle
+from interpreted_program import InterpretedProgram
+from oracle import program_interp, ve_oracle
 from sorobn_b200 import engine, examples, planner, workloads
 
 EXAMPLES = ["alarm", "asia", "sprinkler", "grades"]
@@ -81,8 +81,8 @@ def test_interpreter_finds_the_oracles_explanation(name):
     for observed in patterns(len(net.names), 3):
         plan = planner.build_mpe_plan(net, observed)
         codes = np.ascontiguousarray(codes_all[list(observed)])
-        d64, l64 = mpe_interp.run(plan.words, plan.table_blob64, codes, n_rows=n_rows, dtype=np.float64)
-        d32, l32 = mpe_interp.run(plan.words, plan.table_blob, codes, n_rows=n_rows, dtype=np.float32)
+        d64, l64 = program_interp.run_mpe(plan.words, plan.table_blob64, codes, n_rows=n_rows, dtype=np.float64)
+        d32, l32 = program_interp.run_mpe(plan.words, plan.table_blob, codes, n_rows=n_rows, dtype=np.float32)
         assert l64.dtype == np.float64 and l32.dtype == np.float32
         for b in range(n_rows):
             ev = {net.names[v]: net.domains[v][codes[i, b]] for i, v in enumerate(observed)}
@@ -106,7 +106,7 @@ def test_an_impossible_row_has_log_probability_minus_infinity():
     codes = np.array([[net.domains[v].index(event[net.names[v]])] for v in observed], dtype=np.uint8)
     assert mpe_oracle.max_sum(oracle_net(bn), event)[1] == -np.inf
     for blob, dtype in ((plan.table_blob, np.float32), (plan.table_blob64, np.float64)):
-        _, lp = mpe_interp.run(plan.words, blob, codes, dtype=dtype)
+        _, lp = program_interp.run_mpe(plan.words, blob, codes, dtype=dtype)
         assert lp[0] == -np.inf
 
 
@@ -196,26 +196,6 @@ def test_benchmark_grid_plan_counts():
 
 
 # --------------------------------------------------------------------- mpe_many on the interpreter
-class InterpretedProgram:
-    """engine.Program for MPE plans, executed by the float32 interpreter."""
-
-    live = []
-
-    def __init__(self, plan, device=None, f64=False):
-        assert not f64, "MPE programs run in float32 only"
-        self.plan = plan
-        self.closed = False
-        InterpretedProgram.live.append(self)
-
-    def mpe(self, codes, n_rows):
-        if self.closed:
-            raise engine.EngineError("libsorobn_b200 error -1: null program", code=-1)
-        return mpe_interp.run(self.plan.words, self.plan.table_blob, codes, n_rows=n_rows, dtype=np.float32)
-
-    def close(self):
-        self.closed = True
-
-
 @pytest.fixture
 def interpreted(monkeypatch):
     InterpretedProgram.live = []

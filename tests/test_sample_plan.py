@@ -1,6 +1,6 @@
 """Sample plans (planner.build_sample_plan, version-7 programs) and BayesNet.sample_many, checked on the CPU.
 
-tests/sample_interp.py executes the serialised words with numpy.  Every sample step's normalised
+oracle/program_interp.py executes the serialised words with numpy.  Every sample step's normalised
 conditional must equal the oracle's posterior of the step's variables given the row's observed cells
 and the variables drawn before them (`ve_oracle.query`), and seeded draws must follow the oracle's
 joint posterior.  The host side of `sample_many` runs with the device programs replaced by the
@@ -10,9 +10,9 @@ import pandas as pd
 import pytest
 from scipy import stats
 
-import sample_interp
 from conftest import build_network, load_golden
-from oracle import ve_oracle
+from interpreted_program import InterpretedProgram
+from oracle import program_interp, ve_oracle
 from sorobn_b200 import engine, examples, planner, workloads
 
 EXAMPLES = ["alarm", "asia", "sprinkler", "grades"]
@@ -33,7 +33,7 @@ def check_against_oracle(bn, observed, n_rows=3, n_draws=2, seed=1):
     dn = oracle_net(bn)
     plan = planner.build_sample_plan(net, observed)
     codes = np.ascontiguousarray(workloads.forward_sample_codes(net, n_rows, seed)[list(observed)])
-    drawn, prob, info = sample_interp.run(plan.words, plan.table_blob64, codes, n_rows=n_rows, n_draws=n_draws, seed=seed)
+    drawn, prob, info = program_interp.run_sample(plan.words, plan.table_blob64, codes, n_rows=n_rows, n_draws=n_draws, seed=seed)
     assert not np.isnan(prob).any()
     worst = 0.0
     for st in info:
@@ -97,7 +97,7 @@ def test_seeded_joint_frequencies_follow_the_posterior(name, observed):
     plan = planner.build_sample_plan(net, obs)
     codes = np.ascontiguousarray(workloads.forward_sample_codes(net, 3, 9)[list(obs)])
     n = 20000
-    drawn, prob, _ = sample_interp.run(plan.words, plan.table_blob64, codes, n_draws=n, seed=12345)
+    drawn, prob, _ = program_interp.run_sample(plan.words, plan.table_blob64, codes, n_draws=n, seed=12345)
     names = [net.names[v] for v in plan.sampled]
     for b in range(codes.shape[1]):
         ev = {net.names[v]: net.domains[v][codes[i, b]] for i, v in enumerate(obs)}
@@ -141,32 +141,6 @@ def test_version_4_to_6_words_are_unchanged_by_the_sample_planner():
 
 
 # ---------------------------------------------------------------- sample_many on the interpreter
-class InterpretedProgram:
-    """engine.Program for sample plans, executed by the interpreter.  The float32 program flags the rows
-    whose P(observed) is below `flag_below` (the range rule, raised so that the float64 path runs)."""
-
-    live = []
-    flag_below = None
-    calls = []
-
-    def __init__(self, plan, device=None, f64=False):
-        self.plan, self.f64 = plan, f64
-        self.closed = False
-        InterpretedProgram.live.append(self)
-
-    def sample(self, codes, n_rows, n_draws, seed, row_base=0):
-        if self.closed:
-            raise engine.EngineError("libsorobn_b200 error -1: null program", code=-1)
-        InterpretedProgram.calls.append((self.f64, int(n_rows)))
-        min_total = None if self.f64 or self.flag_below is None else self.flag_below
-        drawn, prob, _ = sample_interp.run(self.plan.words, self.plan.table_blob64, codes, n_rows=n_rows, n_draws=n_draws,
-                                           seed=seed, row_base=row_base, min_total=min_total)
-        return drawn, prob.astype(np.float64 if self.f64 else np.float32)
-
-    def close(self):
-        self.closed = True
-
-
 @pytest.fixture
 def interpreted(monkeypatch):
     InterpretedProgram.live = []
@@ -215,7 +189,7 @@ def alone(bn, X, b, n, seed):
     ev = tuple(sorted(net.index[c] for c in X.columns if pd.notna(X[c].iloc[b])))
     plan = planner.build_sample_plan(net, ev)
     codes = np.array([[net.domains[v].index(X[net.names[v]].iloc[b])] for v in ev], dtype=np.uint8).reshape(len(ev), 1)
-    drawn, _, _ = sample_interp.run(plan.words, plan.table_blob64, codes, n_rows=1, n_draws=n, seed=seed, row_base=b)
+    drawn, _, _ = program_interp.run_sample(plan.words, plan.table_blob64, codes, n_rows=1, n_draws=n, seed=seed, row_base=b)
     return {net.names[v]: list(np.asarray(net.domains[v], dtype=object)[drawn[j, :, 0]]) for j, v in enumerate(plan.sampled)}
 
 
@@ -264,7 +238,7 @@ def test_rows_the_float32_program_flags_are_drawn_by_the_float64_program(interpr
     ev = tuple(sorted(net.index[c] for c in X.columns))
     plan = planner.build_sample_plan(net, ev)
     codes = np.array([[net.domains[v].index(x) for x in X[net.names[v]]] for v in ev], dtype=np.uint8)
-    want, p, _ = sample_interp.run(plan.words, plan.table_blob64, codes, n_draws=2, seed=3)
+    want, p, _ = program_interp.run_sample(plan.words, plan.table_blob64, codes, n_draws=2, seed=3)
     interpreted.flag_below = float(np.median(p))
     got = bn.sample_many(X, n=2, seed=3)
     assert any(f64 for f64, _ in interpreted.calls) and any(not f64 for f64, _ in interpreted.calls)
