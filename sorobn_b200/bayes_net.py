@@ -51,38 +51,58 @@ def _as_list(obj):
     return obj if isinstance(obj, list) else [obj]
 
 
-class _PatternRunner:
-    """The device programs of one missingness pattern (a counts, sample, MPE or MAP plan): the float32 program,
-    and the float64 one for the rows it flags (created when first needed; never for an MPE or MAP plan, whose
-    logs do not underflow).  `set_cpts` gives both new tables in place (counts programs)."""
+class _Programs:
+    """The float32 and float64 device programs of one plan on one device, each created when first needed; every
+    exact-inference entry of the program cache is one.  `set_cpts` gives both new tables in place."""
 
     def __init__(self, plan, device):
-        from . import engine  # raises if libsorobn_b200.so cannot be loaded
-
         self.plan, self.device = plan, device
-        self.f32 = engine.Program(plan, device=device)
-        self._f64 = None
-        self._blob64 = None
+        self._programs = {}  # f64 -> engine.Program
+        self._blobs = None  # (float32, float64) tables of the last set_cpts
 
-    def set_cpts(self, cpts):
-        blob32, self._blob64 = _planner.refresh_tables(self.plan, cpts)
-        self.f32.set_tables(blob32)
-        if self._f64 is not None:
-            self._f64.set_tables(self._blob64)
+    def program(self, f64):
+        prog = self._programs.get(f64)
+        if prog is None:
+            from . import engine  # raises if libsorobn_b200.so cannot be loaded
+
+            prog = self._programs[f64] = engine.Program(self.plan, device=self.device, f64=f64)
+            if self._blobs is not None:
+                prog.set_tables(self._blobs[f64])
+        return prog
+
+    def f32(self):
+        return self.program(False)
 
     def f64(self):
-        if self._f64 is None:
-            from . import engine
+        return self.program(True)
 
-            self._f64 = engine.Program(self.plan, device=self.device, f64=True)
-            if self._blob64 is not None:
-                self._f64.set_tables(self._blob64)
-        return self._f64
+    def set_cpts(self, cpts):
+        self._blobs = _planner.refresh_tables(self.plan, cpts)
+        for f64, prog in self._programs.items():
+            prog.set_tables(self._blobs[f64])
 
     def close(self):
-        self.f32.close()
-        if self._f64 is not None:
-            self._f64.close()
+        for prog in self._programs.values():
+            prog.close()
+
+
+def _posterior_series(post, index, name):
+    """One event's posterior (float64, or None for a value outside its variable's domain) as the reference gives
+    it: states of probability zero left out, empty for evidence of probability zero (NaN)."""
+    if post is None or np.isnan(post).any():
+        return pd.Series([], index=index[:0], name=name, dtype=np.float64)
+    keep = post > 0
+    if keep.all():
+        return pd.Series(post, index=index, name=name)
+    return pd.Series(post[keep], index=index[keep], name=name)
+
+
+def _check_possible(index, rows, impossible, consequence):
+    """ValueError for the rows at positions `rows[impossible]` of a frame with `index`, whose observed cells have
+    probability zero; `consequence` ends the message."""
+    if impossible.any():
+        raise ValueError(f"{int(impossible.sum())} row(s) have observed cells of probability zero "
+                         f"(first: {index[rows[impossible][0]]!r}); {consequence}")
 
 
 class BayesNet:
@@ -125,8 +145,8 @@ class BayesNet:
         self.P = {}
         self._P_sizes = {}
         self._compiled = None
-        # compiled device programs, one per (query vars, evidence vars, mode); least recently
-        # used ones are dropped (their streams, graph and scratch are freed with them)
+        # device objects: the `_Programs` of one plan on one device, keyed (*plan key, device), and Gibbs
+        # samplers; least recently used ones are closed (their streams, graph and scratch are freed with them)
         self._engine_cache = OrderedDict()
         self._cache_lock = threading.RLock()  # query_many(devices=...) looks programs up from worker threads
         self.max_cached_programs = 128
@@ -375,7 +395,7 @@ class BayesNet:
         offsets, n_counts = _planner.count_layout(net)
         # each pattern's programs are fetched right before they run: with more patterns than the cache holds,
         # fetching one may close the least recently used ones, which have run by then
-        counts, _ = self._e_step(X, groups, lambda k, ev: self._counts_runner(ev), n_counts)
+        counts, _ = self._e_step(X, groups, lambda k, ev: self._pattern_runner("counts", ev), n_counts)
         out = {}
         for v, name in enumerate(net.names):
             size = int(np.prod(net.cpt[v].shape))
@@ -411,7 +431,7 @@ class BayesNet:
         net = self._compiled
         offsets, n_counts = _planner.count_layout(net)
         n_rows = len(X.index)
-        runners = [_PatternRunner(_planner.build_counts_plan(net, ev), self.device) for ev, _, _ in groups]
+        runners = [_Programs(_planner.build_counts_plan(net, ev), self.device) for ev, _, _ in groups]
         cpts = [np.array(c, dtype=np.float64) for c in net.cpt]
         lls = []
         try:
@@ -448,21 +468,21 @@ class BayesNet:
 
     def _family_index(self, v, parents_only=False):
         """Index of every combination of the compiled domains of [*parents, v] (or of the parents alone)."""
+        scope = list(self._compiled.scope(v))
+        return self._states_index(scope[:-1] if parents_only else scope)
+
+    def _states_index(self, var_ids):
+        """Index of every joint state of the compiled domains of `var_ids`, one level per variable."""
         net = self._compiled
-        scope = list(net.scope(v))[:-1] if parents_only else list(net.scope(v))
-        names = [net.names[u] for u in scope]
-        if len(scope) == 1:
-            return pd.Index(net.domains[scope[0]], name=names[0])
-        return pd.MultiIndex.from_product([net.domains[u] for u in scope], names=names)
+        names = [net.names[v] for v in var_ids]
+        if len(var_ids) == 1:
+            return pd.Index(net.domains[var_ids[0]], name=names[0])
+        return pd.MultiIndex.from_product([net.domains[v] for v in var_ids], names=names)
 
     def _count_patterns(self, X):
         """[(observed var ids, sorted; positions of the rows; uint8 codes [n_observed, n_rows])] per
         missingness pattern of `X`."""
-        if self._compiled is None:
-            self._compile()
-            if self._compiled is None:
-                raise ValueError("every node needs a CPT in P before computing expected counts; call prepare()")
-        net = self._compiled
+        net = self._net("computing expected counts")
         cols = list(X.columns)
         for c in cols:
             if c not in net.index:
@@ -471,13 +491,11 @@ class BayesNet:
         missing = X.isna().to_numpy().reshape(n, len(cols))
         codes = np.zeros((len(cols), n), dtype=np.uint8)
         for i, c in enumerate(cols):
-            v = net.index[c]
-            idx = pd.Index(net.domains[v]).get_indexer(pd.Index(X[c].to_numpy()))
-            bad = (idx < 0) & ~missing[:, i]
+            codes[i], unknown = self._encode_column(net.index[c], X[c].to_numpy())
+            bad = unknown & ~missing[:, i]
             if bad.any():
                 b = int(np.flatnonzero(bad)[0])
                 raise ValueError(f"column {c!r}: {X[c].iloc[b]!r} (row {X.index[b]!r}) is not a state of the variable")
-            codes[i] = np.where(idx < 0, 0, idx).astype(np.uint8)
         if n == 0:
             return []
         # group the rows by their observed-column bitmask, packed into 64-bit words (np.unique(axis=0) on the
@@ -498,39 +516,25 @@ class BayesNet:
             groups.append((ev, rows, np.ascontiguousarray(codes[[col_of[v] for v in ev]][:, rows])))
         return groups
 
-    def _counts_runner(self, ev):
-        """The cached counts programs of one missingness pattern."""
-        return self._pattern_runner("counts", ev)
-
-    def _sample_runner(self, ev):
-        """The cached sample programs of one missingness pattern."""
-        return self._pattern_runner("sample", ev)
-
-    def _mpe_runner(self, ev):
-        """The cached MPE program of one missingness pattern."""
-        return self._pattern_runner("mpe", ev)
-
-    def _map_runner(self, ev, map_vars):
-        """The cached marginal MAP program of one missingness pattern and MAP set (sorted var ids)."""
-        return self._pattern_runner("map", ev, map_vars)
-
     def _pattern_runner(self, kind, ev, map_vars=None):
         """The cached programs of one missingness pattern, `kind` "counts", "sample", "mpe" or "map" (a "map"
-        program is keyed by its MAP variables too; dropped by `prepare()`, as every program)."""
-        with self._cache_lock:
-            key = (kind, ev, self.device) if kind != "map" else (kind, ev, map_vars, self.device)
-            hit = self._engine_cache.get(key)
-            if hit is None:
-                if kind == "map":
-                    plan = _planner.build_map_plan(self._compiled, ev, map_vars)
-                else:
-                    plan = {"counts": _planner.build_counts_plan, "sample": _planner.build_sample_plan,
-                            "mpe": _planner.build_mpe_plan}[kind](self._compiled, ev)
-                hit = self._engine_cache[key] = _PatternRunner(plan, self.device)
-                self._evict()
-            else:
-                self._engine_cache.move_to_end(key)
-            return hit
+        plan is keyed by its MAP variables, sorted var ids, too)."""
+        extra = (map_vars,) if kind == "map" else ()
+        build = getattr(_planner, f"build_{kind}_plan")
+        return self._programs((kind, ev, *extra), lambda: build(self._compiled, ev, *extra))
+
+    @staticmethod
+    def _run_pattern(runner, run, codes, rows):
+        """run(program, codes, rows) -> (result, P(observed)) on a pattern's float32 program, then on its float64
+        program for the rows the float32 one flags (P(observed) NaN).  Returns (float32 result, P(observed)
+        float64, positions of the flagged rows, their float64 result or None); a row still NaN is impossible."""
+        out, prob = run(runner.f32(), codes, rows)
+        prob = prob.astype(np.float64)
+        flagged = np.flatnonzero(np.isnan(prob))
+        again = None
+        if len(flagged):
+            again, prob[flagged] = run(runner.f64(), np.ascontiguousarray(codes[:, flagged]), rows[flagged])
+        return out, prob, flagged, again
 
     def _e_step(self, X, groups, runner_of, n_counts):
         """(expected counts [n_counts], observed-data log-likelihood) of every pattern's rows;
@@ -539,18 +543,11 @@ class BayesNet:
         counts = np.zeros(n_counts, dtype=np.float64)
         ll = 0.0
         for k, (ev, rows, codes) in enumerate(groups):
-            runner = runner_of(k, ev)
-            c, prob = runner.f32.counts(codes, len(rows))
+            c, prob, _, again = self._run_pattern(runner_of(k, ev), lambda p, c, r: p.counts(c, len(r)), codes, rows)
             counts += c
-            prob = prob.astype(np.float64)
-            flagged = np.flatnonzero(np.isnan(prob))
-            if len(flagged):
-                c, prob[flagged] = runner.f64().counts(np.ascontiguousarray(codes[:, flagged]), len(flagged))
-                counts += c
-            impossible = np.isnan(prob)
-            if impossible.any():
-                raise ValueError(f"{int(impossible.sum())} row(s) have observed cells of probability zero "
-                                 f"(first: {X.index[rows[impossible][0]]!r}); their expected counts are undefined")
+            if again is not None:
+                counts += again
+            _check_possible(X.index, rows, np.isnan(prob), "their expected counts are undefined")
             ll += float(np.log(prob).sum())
         return counts, ll
 
@@ -580,25 +577,19 @@ class BayesNet:
         for ev, rows, ev_codes in groups:
             # fetched right before it runs: with more patterns than the cache holds, fetching one may close
             # the least recently used programs, which have run by then
-            runner = self._sample_runner(ev)
-            drawn, prob = self._draw(runner.f32, ev_codes, rows, n, seed)
-            flagged = np.flatnonzero(np.isnan(prob))
-            if len(flagged):
-                drawn[:, :, flagged], prob[flagged] = self._draw(runner.f64(), np.ascontiguousarray(ev_codes[:, flagged]),
-                                                                 rows[flagged], n, seed)
-            impossible = np.isnan(prob)
-            if impossible.any():
-                raise ValueError(f"{int(impossible.sum())} row(s) have observed cells of probability zero "
-                                 f"(first: {events.index[rows[impossible][0]]!r}); they have no posterior to sample from")
+            runner = self._pattern_runner("sample", ev)
+            drawn, prob, flagged, again = self._run_pattern(runner, lambda p, c, r: self._draw(p, c, r, n, seed),
+                                                            ev_codes, rows)
+            if again is not None:
+                drawn[:, :, flagged] = again
+            _check_possible(events.index, rows, np.isnan(prob), "they have no posterior to sample from")
             for i, v in enumerate(ev):
                 codes[v][rows] = ev_codes[i][:, None]
             for j, v in enumerate(runner.plan.sampled):
                 codes[v][rows] = drawn[j].T
         index = pd.MultiIndex.from_arrays([np.repeat(events.index.to_numpy(), n), np.tile(np.arange(n), n_rows)],
                                           names=[events.index.name, "draw"])
-        frame = pd.DataFrame({name: np.asarray(net.domains[v], dtype=object)[codes[v].reshape(-1)]
-                              for v, name in enumerate(net.names)}, index=index)
-        return frame.infer_objects().sort_index(axis="columns")
+        return self._codes_frame(codes.reshape(len(net.names), -1), index)
 
     def mpe_many(self, events: pd.DataFrame, return_log_proba: bool = False):
         """The most probable explanation of every row of `events`, computed on the GPU: the joint state of
@@ -617,30 +608,9 @@ class BayesNet:
         missingness pattern; each pattern is one MPE program (planner.build_mpe_plan): the upward pass of
         variable elimination in the log domain with max in place of sum, then one argmax per bucket,
         top-down (csrc/sbn_mpe.cuh)."""
-        groups = self._count_patterns(events)
-        net = self._compiled
-        n_rows = len(events.index)
-        codes = np.zeros((len(net.names), n_rows), dtype=np.uint8)
-        log_p = np.zeros(n_rows, dtype=np.float64)
-        for ev, rows, ev_codes in groups:
-            # fetched right before it runs, as in `sample_many`
-            runner = self._mpe_runner(ev)
-            decoded, lp = runner.f32.mpe(ev_codes, len(rows))
-            impossible = ~(lp > -np.inf)
-            if impossible.any():
-                raise ValueError(f"{int(impossible.sum())} row(s) have observed cells of probability zero "
-                                 f"(first: {events.index[rows[impossible][0]]!r}); they have nothing to explain")
-            for i, v in enumerate(ev):
-                codes[v][rows] = ev_codes[i]
-            for j, v in enumerate(runner.plan.sampled):
-                codes[v][rows] = decoded[j]
-            log_p[rows] = lp
-        frame = pd.DataFrame({name: np.asarray(net.domains[v], dtype=object)[codes[v]]
-                              for v, name in enumerate(net.names)}, index=events.index)
-        frame = frame.infer_objects().sort_index(axis="columns")
-        if return_log_proba:
-            return frame, pd.Series(log_p, index=events.index)
-        return frame
+        codes, _, log_p = self._decode(events, self._count_patterns(events), "mpe", "they have nothing to explain")
+        frame = self._codes_frame(codes, events.index)
+        return (frame, pd.Series(log_p, index=events.index)) if return_log_proba else frame
 
     def mpe(self, event: dict) -> pd.Series:
         """The most probable explanation of one event: `mpe_many(pd.DataFrame([event])).iloc[0]`, a Series
@@ -678,44 +648,54 @@ class BayesNet:
                 raise ValueError(f"{unknown[:5]} are not nodes of the network")
             listed = sorted({net.index[v] for v in variables})
         columns = [net.index[c] for c in events.columns]
+        chosen = sorted(columns) if listed is None else listed
+        codes, known, log_p = self._decode(events, groups, "map", "they have no MAP state",
+                                           lambda ev: tuple(v for v in chosen if v not in ev))
         out_vars = sorted(set(columns) | set(listed or ()), key=lambda v: net.names[v])
-        n_rows = len(events.index)
-        codes = np.zeros((len(net.names), n_rows), dtype=np.uint8)
-        known = np.zeros((len(net.names), n_rows), dtype=bool)  # observed or decoded
-        log_p = np.zeros(n_rows, dtype=np.float64)
-        for ev, rows, ev_codes in groups:
-            observed = set(ev)
-            if listed is None:
-                map_vars = tuple(v for v in sorted(columns) if v not in observed)
-            else:
-                map_vars = tuple(v for v in listed if v not in observed)
-            for i, v in enumerate(ev):
-                codes[v][rows] = ev_codes[i]
-                known[v][rows] = True
-            if not map_vars and not ev:
-                continue  # nothing observed, nothing to decode: log P = log 1
-            # fetched right before it runs, as in `sample_many`
-            runner = self._map_runner(ev, map_vars)
-            decoded, lp = runner.f32.map(ev_codes, len(rows))
-            impossible = ~(lp > -np.inf)
-            if impossible.any():
-                raise ValueError(f"{int(impossible.sum())} row(s) have observed cells of probability zero "
-                                 f"(first: {events.index[rows[impossible][0]]!r}); they have no MAP state")
-            for j, v in enumerate(runner.plan.sampled):
-                codes[v][rows] = decoded[j]
-                known[v][rows] = True
-            log_p[rows] = lp
-        frame = pd.DataFrame({net.names[v]: np.where(known[v], np.asarray(net.domains[v], dtype=object)[codes[v]], None)
-                              for v in out_vars}, index=events.index)
-        frame = frame.infer_objects().sort_index(axis="columns")
-        if return_log_proba:
-            return frame, pd.Series(log_p, index=events.index)
-        return frame
+        frame = self._codes_frame(codes, events.index, out_vars, known)
+        return (frame, pd.Series(log_p, index=events.index)) if return_log_proba else frame
 
     def map(self, event: dict, variables=None) -> pd.Series:
         """The marginal MAP state of one event: `map_many(pd.DataFrame([event]), variables).iloc[0]`, a Series
         indexed by node name."""
         return self.map_many(pd.DataFrame([event]), variables).iloc[0]
+
+    def _decode(self, events, groups, kind, consequence, map_vars_of=None):
+        """(codes [n_nodes, n], known [n_nodes, n] (observed or decoded), log P [n]) of the MPE (`kind` "mpe")
+        or marginal MAP ("map") programs of the pattern groups of `events`: the observed codes copied through,
+        the decoded ones in `plan.sampled` order.  MAP takes the MAP variables of a pattern from
+        `map_vars_of(observed var ids)` and skips a pattern that observes and decodes nothing (log P = log 1)."""
+        net = self._compiled
+        n_rows = len(events.index)
+        codes = np.zeros((len(net.names), n_rows), dtype=np.uint8)
+        known = np.zeros((len(net.names), n_rows), dtype=bool)
+        log_p = np.zeros(n_rows, dtype=np.float64)
+        for ev, rows, ev_codes in groups:
+            map_vars = None if map_vars_of is None else map_vars_of(ev)
+            for i, v in enumerate(ev):
+                codes[v][rows] = ev_codes[i]
+                known[v][rows] = True
+            if map_vars == () and not ev:
+                continue
+            # fetched right before it runs, as in `sample_many`
+            runner = self._pattern_runner(kind, ev, map_vars)
+            decoded, lp = getattr(runner.f32(), kind)(ev_codes, len(rows))
+            _check_possible(events.index, rows, ~(lp > -np.inf), consequence)
+            for j, v in enumerate(runner.plan.sampled):
+                codes[v][rows] = decoded[j]
+                known[v][rows] = True
+            log_p[rows] = lp
+        return codes, known, log_p
+
+    def _codes_frame(self, codes, index, variables=None, known=None):
+        """The frame of state codes [n_nodes, n]: one column per var id in `variables` (default: every node) of
+        its domain values, None where `known` is False, the columns sorted and their dtypes inferred."""
+        net = self._compiled
+        columns = {}
+        for v in range(len(net.names)) if variables is None else variables:
+            values = np.asarray(net.domains[v], dtype=object)[codes[v]]
+            columns[net.names[v]] = values if known is None else np.where(known[v], values, None)
+        return pd.DataFrame(columns, index=index).infer_objects().sort_index(axis="columns")
 
     @staticmethod
     def _draw(program, ev_codes, rows, n, seed):
@@ -733,11 +713,7 @@ class BayesNet:
         Vectorised over the n samples on the host; the stream comes from `seed`."""
         if method != "forward":
             raise ValueError("Unknown method, must be one of: forward")
-        if self._compiled is None:
-            self._compile()
-            if self._compiled is None:
-                raise ValueError("every node needs a CPT in P before sampling; call prepare()")
-        net = self._compiled
+        net = self._net("sampling")
         init = init or {}
         rng = np.random.default_rng(self._rng.getrandbits(63))
         n = int(n)
@@ -751,81 +727,110 @@ class BayesNet:
             cdf = np.cumsum(probs, axis=-1)
             u = rng.random((n, 1)) * cdf[:, -1:]
             codes[v] = np.minimum((u > cdf).sum(axis=-1), table.shape[-1] - 1)
-        frame = pd.DataFrame({name: np.asarray(net.domains[v], dtype=object)[codes[v]] for v, name in enumerate(net.names)})
-        frame = frame.infer_objects().sort_index(axis="columns")
+        frame = self._codes_frame(codes, None)
         return frame if n > 1 else frame.iloc[0]
 
     # ---------------------------------------------------------------------- query
-    def _plan(self, query, evidence_vars, mode, robust=False, device=None, marginals=False, replica=0):
-        """(plan, program) of P(query | evidence vars), cached.  marginals=True: `query` are the targets of
-        a marginals program (planner.build_marginals_plan), cached under its own mode key.  replica=k > 0:
-        a separate program on the same device, for the k-th other thread that runs this query there at the
-        same time (a program's scratch, staging buffers and graph capture serve one caller at a time)."""
-        with self._cache_lock:
-            return self._plan_locked(query, evidence_vars, mode, robust, device, marginals, replica)
-
-    def _plan_locked(self, query, evidence_vars, mode, robust, device, marginals=False, replica=0):
+    def _net(self, purpose):
+        """The compiled network, compiled now if `P` has been completed since; ValueError while a node has no CPT."""
         if self._compiled is None:
             self._compile()
             if self._compiled is None:
-                raise ValueError("every node needs a CPT in P before querying; call prepare()")
-        net = self._compiled
+                raise ValueError(f"every node needs a CPT in P before {purpose}; call prepare()")
+        return self._compiled
+
+    def _cached(self, key, build):
+        """The cache entry under `key`, built by `build()` on a miss.  A hit becomes the most recently used entry;
+        a miss closes the least recently used entries beyond `max_cached_programs`."""
+        with self._cache_lock:
+            hit = self._engine_cache.get(key)
+            if hit is None:
+                hit = self._engine_cache[key] = build()
+                self._evict()
+            else:
+                self._engine_cache.move_to_end(key)
+            return hit
+
+    def _programs(self, plan_key, build_plan, device=None, replica=0):
+        """The cached `_Programs` of the plan `plan_key` names, on `device` (default: the network's).  replica=k > 0:
+        separate programs on the same device, for the k-th other thread that runs this plan there at the same
+        time (a program's scratch, staging buffers and graph capture serve one caller at a time).  The plan is
+        shared by every device and replica: a miss takes it from another entry of the same plan before calling
+        `build_plan()`."""
         device = self.device if device is None else device
-        key = (tuple(query), tuple(evidence_vars), ("marginals", mode) if marginals else mode, robust,
-               (device, replica) if replica else device)
-        hit = self._engine_cache.get(key)
-        if hit is None:
+
+        def build():
+            twin = next((v for k, v in self._engine_cache.items() if k[:-1] == plan_key), None)
+            return _Programs(twin.plan if twin is not None else build_plan(), device)
+
+        return self._cached((*plan_key, (device, replica) if replica else device), build)
+
+    def _query_programs(self, query, evidence_vars, mode, device=None, marginals=False, replica=0):
+        """The cached `_Programs` of P(query | evidence vars), plan key (query, evidence vars, mode, marginals);
+        marginals=True: `query` are the targets of a marginals program (planner.build_marginals_plan)."""
+        net = self._net("querying")
+
+        def build_plan():
             for name in (*query, *evidence_vars):
                 if name not in net.index:
                     raise KeyError(name)
-            twin = next((v for k, v in self._engine_cache.items() if isinstance(v, tuple) and k[:4] == key[:4]), None)
-            if twin:
-                plan = twin[0]  # the same plan serves every device
-            elif marginals:
-                plan = _planner.build_marginals_plan(net, [net.index[e] for e in evidence_vars],
-                                                     targets=[net.index[q] for q in query], mode=mode)
-            else:
-                plan = _planner.build_plan(net, [net.index[q] for q in query], [net.index[e] for e in evidence_vars],
-                                           mode=mode, allow_empty_query=True)
-            from . import engine  # raises if libsorobn_b200.so cannot be loaded
+            ev = [net.index[e] for e in evidence_vars]
+            if marginals:
+                return _planner.build_marginals_plan(net, ev, targets=[net.index[q] for q in query], mode=mode)
+            return _planner.build_plan(net, [net.index[q] for q in query], ev, mode=mode, allow_empty_query=True)
 
-            # single-event programs run in float64 (latency-bound anyway); batches in float32,
-            # except the robust re-run of flagged rows (mode key "batched64")
-            hit = (plan, engine.Program(plan, device=device, f64=(mode == _planner.MODE_FLAT or robust)))
-            self._engine_cache[key] = hit
-            self._evict()
-        else:
-            self._engine_cache.move_to_end(key)
-        return hit
+        return self._programs((tuple(query), tuple(evidence_vars), mode, marginals), build_plan, device, replica)
+
+    def _plan(self, query, evidence_vars, mode, robust=False, device=None, marginals=False, replica=0):
+        """(plan, program) of P(query | evidence vars), cached: the float64 program of a single-event
+        (MODE_FLAT) plan, which is latency-bound anyway; of a batched plan the float32 program, or with `robust`
+        the float64 one that settles the rows the float32 program flags.  The other arguments are
+        `_query_programs`'."""
+        with self._cache_lock:
+            entry = self._query_programs(query, evidence_vars, mode, device, marginals, replica)
+            return entry.plan, entry.program(mode == _planner.MODE_FLAT or robust)
 
     def _evict(self):
         """Drop the least recently used device objects (programs and samplers) beyond the cap."""
         while len(self._engine_cache) > self.max_cached_programs:
             _, old = self._engine_cache.popitem(last=False)
-            (old[1] if isinstance(old, tuple) else old).close()
+            old.close()
 
-    def _encode_events(self, evidence_vars, columns):
-        """State values -> uint8 codes [n_ev, B].  Unknown values get code 255 and the
-        row is reported as impossible evidence (the reference's boolean filter at
-        bayes_net.py:772-774 leaves an empty factor, hence an empty answer)."""
-        net = self._compiled
-        n = len(columns[0]) if columns else 0
+    def _encode_column(self, v, values):
+        """(uint8 codes of `values` in the sorted domain of var id `v`, 0 where a value is not a state of it; the
+        mask of those values, missing ones included)."""
+        idx = pd.Index(self._compiled.domains[v]).get_indexer(pd.Index(values))
+        unknown = idx < 0
+        return np.where(unknown, 0, idx).astype(np.uint8), unknown
+
+    def _encode_events(self, events, evidence_vars):
+        """The columns `evidence_vars` of the frame `events` -> (uint8 codes [n_ev, n], bad [n]).  A row with a
+        value outside its variable's domain is bad: the reference's boolean filter at bayes_net.py:772-774 leaves
+        an empty factor, hence an empty answer."""
+        n = len(events.index)
         codes = np.empty((len(evidence_vars), n), dtype=np.uint8)
         bad = np.zeros(n, dtype=bool)
-        for i, (name, col) in enumerate(zip(evidence_vars, columns)):
-            dom = pd.Index(net.domains[net.index[name]])
-            c = dom.get_indexer(pd.Index(col))
-            bad |= c < 0
-            codes[i] = np.where(c < 0, 0, c).astype(np.uint8)
+        for i, name in enumerate(evidence_vars):
+            codes[i], unknown = self._encode_column(self._compiled.index[name], events[name].to_numpy())
+            bad |= unknown
         return codes, bad
 
-    def _answer_index(self, plan):
+    def _event_posterior(self, program, evidence_vars, event):
+        """The float64 posterior of one event on a single-event program, or None when a value is outside its
+        variable's domain (the reference's filter leaves nothing).  One event is launch-latency bound on the
+        device (~20 us): the host side must not cost ten times that, so state codes come from per-variable
+        dicts."""
         net = self._compiled
-        names = [net.names[v] for v in plan.query]
-        doms = [net.domains[v] for v in plan.query]
-        if len(names) == 1:
-            return pd.Index(doms[0], name=names[0])
-        return pd.MultiIndex.from_product(doms, names=names)
+        codes = np.empty((len(evidence_vars), 1), dtype=np.uint8)
+        for i, v in enumerate(evidence_vars):
+            code = self._code_of(net.index[v]).get(event[v], -1)
+            if code < 0:
+                return None
+            codes[i, 0] = code
+        return program.run(codes, 1)[:, 0].astype(np.float64)
+
+    def _answer_index(self, plan):
+        return self._states_index(plan.query)
 
     def query(self, *query, event: dict, algorithm="exact", n_iterations=100) -> pd.Series:
         """Answer P(query | event) (bayes_net.py:796-875), exact inference on the GPU.
@@ -840,41 +845,24 @@ class BayesNet:
         for q in query:
             if q in event:
                 raise ValueError("A query variable cannot be part of the event")
+        name = f"P({', '.join(map(str, query))})"
         if algorithm in ("gibbs", "likelihood", "rejection"):
-            freq = self._sample_query(algorithm, query, tuple(event), [[event[v]] for v in event], 1, n_iterations)
-            values = freq[0][:, 0].astype(np.float64)
-            name = f"P({', '.join(map(str, query))})"
+            events = pd.DataFrame({v: [event[v]] for v in event}, index=[0])
+            freq, index = self._sample_query(algorithm, query, events, n_iterations)
+            values = freq[:, 0].astype(np.float64)
             if np.isnan(values).any():  # rejection sampling kept no sample: the reference's answer is empty
-                return pd.Series([], index=freq[1][:0], name=name, dtype=np.float64)
-            answer = pd.Series(values, index=freq[1], name=name)
+                return pd.Series([], index=index[:0], name=name, dtype=np.float64)
+            answer = pd.Series(values, index=index, name=name)
             return answer[answer > 0]  # the reference only lists the states that were sampled
         if algorithm != "exact":
             raise ValueError("Unknown algorithm, must be one of: exact, gibbs, likelihood, rejection")
 
         ev_vars = tuple(event)
         plan, program = self._plan(query, ev_vars, _planner.MODE_FLAT)
-        # One event is launch-latency bound on the device (~20 us): the host side must not cost ten
-        # times that.  State codes come from per-variable dicts, the answer's index is cached on the plan.
-        net = self._compiled
-        codes = np.empty((len(ev_vars), 1), dtype=np.uint8)
-        bad = False
-        for i, v in enumerate(ev_vars):
-            code = self._code_of(net.index[v]).get(event[v], -1)
-            bad |= code < 0
-            codes[i, 0] = max(code, 0)
-        index = getattr(plan, "_answer_index_cache", None)
+        index = getattr(plan, "_answer_index_cache", None)  # cached on the plan: the warm path stays lean
         if index is None:
             index = plan._answer_index_cache = self._answer_index(plan)
-        name = f"P({', '.join(map(str, query))})"
-        if bad:  # a value outside the variable's domain: the reference's filter leaves nothing
-            return pd.Series([], index=index[:0], name=name, dtype=np.float64)
-        post = program.run(codes, 1)[:, 0].astype(np.float64)
-        if np.isnan(post).any():  # impossible evidence: P(event) == 0
-            return pd.Series([], index=index[:0], name=name, dtype=np.float64)
-        keep = post > 0
-        if keep.all():
-            return pd.Series(post, index=index, name=name)
-        return pd.Series(post[keep], index=index[keep], name=name)
+        return _posterior_series(self._event_posterior(program, ev_vars, event), index, name)
 
     def _code_of(self, v):
         """state value -> uint8 code of variable id `v` (position in its sorted domain)."""
@@ -887,36 +875,30 @@ class BayesNet:
             table = cache[v] = {value: k for k, value in enumerate(self._compiled.domains[v])}
         return table
 
-    def _sample_query(self, algorithm, query, ev_vars, columns, n_rows, n_iterations):
-        """The approximate algorithms on the device, per evidence row: one Gibbs chain
-        (bayes_net.py:665-737), or n_iterations forward samples for likelihood weighting
+    def _sample_query(self, algorithm, query, events, n_iterations):
+        """The approximate algorithms on the device, per row of `events` (columns = evidence variables): one
+        Gibbs chain (bayes_net.py:665-737), or n_iterations forward samples for likelihood weighting
         (:621-663) / rejection sampling (:577-619).  Returns (estimates [Q, n_rows], index)."""
-        if self._compiled is None:
-            self._compile()
-            if self._compiled is None:
-                raise ValueError("every node needs a CPT in P before querying; call prepare()")
-        net = self._compiled
+        net = self._net("querying")
+        ev_vars = tuple(events.columns)
         for name in (*query, *ev_vars):
             if name not in net.index:
                 raise KeyError(name)
-        key = ("sampler", tuple(query), tuple(ev_vars))
-        sampler = self._engine_cache.get(key)
         q_sorted = sorted(query)  # same key as the exact path (planner: sorted by name) and bayes_net.py:873
-        if sampler is None:
+
+        def build():
             from . import engine
 
             nonevents = sorted(set(self.nodes) - set(ev_vars))  # bayes_net.py:697, the Gibbs cycle order
-            sampler = engine.GibbsSampler(net, [net.index[q] for q in q_sorted], [net.index[e] for e in ev_vars],
-                                          [net.index[v] for v in nonevents], device=self.device)
-            self._engine_cache[key] = sampler
-            self._evict()
-        codes, bad = self._encode_events(ev_vars, columns)
+            return engine.GibbsSampler(net, [net.index[q] for q in q_sorted], [net.index[e] for e in ev_vars],
+                                       [net.index[v] for v in nonevents], device=self.device)
+
+        sampler = self._cached(("sampler", tuple(query), ev_vars), build)
+        codes, bad = self._encode_events(events, ev_vars)
         if bad.any():
             raise ValueError("an event value is not a state of its variable")
-        freq = sampler.run(codes, n_rows, n_iterations, self._rng.getrandbits(63), algorithm=algorithm)
-        doms = [net.domains[net.index[q]] for q in q_sorted]
-        index = pd.Index(doms[0], name=q_sorted[0]) if len(q_sorted) == 1 else pd.MultiIndex.from_product(doms, names=q_sorted)
-        return freq, index
+        freq = sampler.run(codes, len(events.index), n_iterations, self._rng.getrandbits(63), algorithm=algorithm)
+        return freq, self._states_index([net.index[q] for q in q_sorted])
 
     def query_many(self, *query, events: pd.DataFrame, algorithm="exact", n_iterations=100,
                    devices: typing.Sequence[int] | None = None) -> pd.DataFrame:
@@ -936,61 +918,71 @@ class BayesNet:
             if q in ev_vars:
                 raise ValueError("A query variable cannot be part of the event")
         if algorithm in ("gibbs", "likelihood", "rejection"):
-            freq, index = self._sample_query(algorithm, query, ev_vars, [events[v].to_numpy() for v in ev_vars],
-                                             len(events.index), n_iterations)
+            freq, index = self._sample_query(algorithm, query, events, n_iterations)
             return pd.DataFrame(freq.T.astype(np.float64), index=events.index, columns=index)
         if algorithm != "exact":
             raise ValueError("Unknown algorithm, must be one of: exact, gibbs, likelihood, rejection")
         plan, _ = self._plan(query, ev_vars, _planner.MODE_BATCHED, device=None if devices is None else devices[0])
-        n = len(events.index)
-        if n == 0:
-            return pd.DataFrame(np.zeros((0, plan.Q)), index=events.index, columns=self._answer_index(plan))
-        codes, bad = self._encode_events(ev_vars, [events[v].to_numpy() for v in ev_vars])
-        if not ev_vars:
-            bad = np.zeros(n, dtype=bool)
+        return self._posterior_frame(query, events, self._answer_index(plan), devices=devices)
+
+    def _posterior_frame(self, query, events, columns, marginals=False, devices=None):
+        """The posterior of every row of `events` as a frame with `columns`: encoded, run on the device(s) with
+        the float64 rescue, and NaN for the rows with a value outside its variable's domain."""
+        if len(events.index) == 0:
+            return pd.DataFrame(np.zeros((0, len(columns))), index=events.index, columns=columns)
+        ev_vars = tuple(events.columns)
+        codes, bad = self._encode_events(events, ev_vars)
         if devices is None or len(devices) <= 1:
-            post = self._posterior_codes(query, ev_vars, codes, bad, device=None if devices is None else devices[0])
+            post = self._posterior_codes(query, ev_vars, codes, bad, device=None if devices is None else devices[0],
+                                         marginals=marginals)
         else:
             post = self._posterior_codes_multi(query, ev_vars, codes, bad, list(devices))
-        out = pd.DataFrame(post.T, index=events.index, columns=self._answer_index(plan))
+        return self._answer_frame(post, events.index, columns, bad)
+
+    @staticmethod
+    def _answer_frame(post, index, columns, bad):
+        """The posteriors [Q, n] as a frame, the bad rows NaN."""
+        out = pd.DataFrame(post.T, index=index, columns=columns)
         if bad.any():
-            out.loc[events.index[bad]] = np.nan
+            out.loc[index[bad]] = np.nan
         return out
 
     def _posterior_codes(self, query, ev_vars, codes, bad, device=None, marginals=False, replica=0):
-        """Posterior float64 [Q, n] for uint8 evidence codes [n_ev, n] on one device.  Rows the
-        float32 program flags (NaN: impossible evidence, or an entry below the float32 range)
-        are settled in float64 -- a few one by one with the single-event program, many as one
-        batch with the batched float64 program; a row that is still NaN there is impossible.
-        marginals=True: `query` are the targets of a marginals program (every segment normalised)."""
-        n = codes.shape[1] if len(ev_vars) else len(bad)
-        _, program = self._plan(query, ev_vars, _planner.MODE_BATCHED, device=device, marginals=marginals, replica=replica)
-        post = self._run_evicting(program, codes, n).astype(np.float64)  # [Q, n]
-        suspect = np.isnan(post).any(axis=0) & ~bad
-        rows = np.nonzero(suspect)[0]
+        """Posterior float64 [Q, n] for uint8 evidence codes [n_ev, n] on one device, the rows the float32
+        program flags settled by `_rescue`.  marginals=True: `query` are the targets of a marginals program
+        (every segment normalised)."""
+        entry = self._query_programs(query, ev_vars, _planner.MODE_BATCHED, device, marginals, replica)
+        post = self._run_evicting(entry, codes, len(bad)).astype(np.float64)  # [Q, n]
+        return self._rescue(post, np.isnan(post).any(axis=0) & ~bad, codes, "run", query, ev_vars, device, marginals,
+                            replica)
+
+    def _rescue(self, out, flagged, codes, method, query, ev_vars, device=None, marginals=False, replica=0):
+        """Settle in float64 the `flagged` rows (last axis of `out`) of a batched float32 program's `method`
+        ("run": posteriors, or "evidence": P(event)): flagged rows are NaN, for impossible evidence or an entry
+        below the float32 range.  More than 8 run as one batch on the batched plan's float64 program, fewer one
+        by one on the single-event program; a row still NaN there is impossible."""
+        rows = np.flatnonzero(flagged)
         if len(rows) > 8:
-            _, robust = self._plan(query, ev_vars, _planner.MODE_BATCHED, robust=True, device=device, marginals=marginals,
-                                   replica=replica)
-            post[:, rows] = robust.run(np.ascontiguousarray(codes[:, rows]), len(rows))
+            _, robust = self._plan(query, ev_vars, _planner.MODE_BATCHED, robust=True, device=device,
+                                   marginals=marginals, replica=replica)
+            out[..., rows] = getattr(robust, method)(np.ascontiguousarray(codes[:, rows]), len(rows))
         elif len(rows):
-            _, flat = self._plan(query, ev_vars, _planner.MODE_FLAT, device=device, marginals=marginals, replica=replica)
+            _, flat = self._plan(query, ev_vars, _planner.MODE_FLAT, device=device, marginals=marginals,
+                                 replica=replica)
             for b in rows:
-                post[:, b] = flat.run(np.ascontiguousarray(codes[:, b:b + 1]), 1)[:, 0]
-        return post
+                out[..., b] = getattr(flat, method)(np.ascontiguousarray(codes[:, b:b + 1]), 1)[..., 0]
+        return out
 
     def _targets(self, variables, ev_vars):
         """Target names of a marginals query, sorted: `variables`, or every variable that is not evidence."""
-        if self._compiled is None:
-            self._compile()
-            if self._compiled is None:
-                raise ValueError("every node needs a CPT in P before querying; call prepare()")
+        net = self._net("querying")
         if variables is None:
             variables = [n for n in self.nodes if n not in set(ev_vars)]
         variables = list(variables)
         for v in variables:
             if v in ev_vars:
                 raise ValueError("A query variable cannot be part of the event")
-            if v not in self._compiled.index:
+            if v not in net.index:
                 raise KeyError(v)
         if not variables:
             raise ValueError("At least one query variable has to be specified")
@@ -1005,22 +997,11 @@ class BayesNet:
         Returns one row per evidence row; the columns are a MultiIndex of (variable, state), variables
         sorted by name, states sorted.  Zero-probability states stay (as 0.0); impossible rows and rows
         with a value outside its variable's domain are NaN."""
-        ev_vars = tuple(events.columns)
-        targets = self._targets(variables, ev_vars)
+        targets = self._targets(variables, tuple(events.columns))
         net = self._compiled
         columns = pd.MultiIndex.from_tuples([(t, s) for t in targets for s in net.domains[net.index[t]]],
                                             names=["variable", "state"])
-        n = len(events.index)
-        if n == 0:
-            return pd.DataFrame(np.zeros((0, len(columns))), index=events.index, columns=columns)
-        codes, bad = self._encode_events(ev_vars, [events[v].to_numpy() for v in ev_vars])
-        if not ev_vars:
-            bad = np.zeros(n, dtype=bool)
-        post = self._posterior_codes(targets, ev_vars, codes, bad, marginals=True)
-        out = pd.DataFrame(post.T, index=events.index, columns=columns)
-        if bad.any():
-            out.loc[events.index[bad]] = np.nan
-        return out
+        return self._posterior_frame(targets, events, columns, marginals=True)
 
     def marginals(self, event: dict, variables=None) -> dict:
         """`marginals_many` for one event, in float64 (as `query`): {variable: Series}, each Series equal to
@@ -1029,28 +1010,17 @@ class BayesNet:
         ev_vars = tuple(event)
         targets = self._targets(variables, ev_vars)
         net = self._compiled
-        plan, program = self._plan(targets, ev_vars, _planner.MODE_FLAT, marginals=True)
-        codes = np.empty((len(ev_vars), 1), dtype=np.uint8)
-        bad = False
-        for i, v in enumerate(ev_vars):
-            code = self._code_of(net.index[v]).get(event[v], -1)
-            bad |= code < 0
-            codes[i, 0] = max(code, 0)
-        post = None if bad else program.run(codes, 1)[:, 0].astype(np.float64)
+        _, program = self._plan(targets, ev_vars, _planner.MODE_FLAT, marginals=True)
+        post = self._event_posterior(program, ev_vars, event)
         out, q = {}, 0
         for t in targets:
-            index = pd.Index(net.domains[net.index[t]], name=t)
-            seg = None if post is None else post[q:q + len(index)]
+            index = self._states_index([net.index[t]])
+            out[t] = _posterior_series(None if post is None else post[q:q + len(index)], index, f"P({t})")
             q += len(index)
-            if seg is None or np.isnan(seg).any():
-                out[t] = pd.Series([], index=index[:0], name=f"P({t})", dtype=np.float64)
-            else:
-                keep = seg > 0
-                out[t] = pd.Series(seg[keep], index=index[keep], name=f"P({t})")
         return out
 
-    def _run_evicting(self, program, codes, n):
-        """`program.run`, retried once after closing every OTHER cached device object when the device
+    def _run_evicting(self, entry, codes, n):
+        """`entry.f32().run`, retried once after closing every OTHER cached device object when the device
         is out of memory: each program owns a scratch arena sized for its largest batch (3.9 GB for
         100k rows of the benchmark grid), and a BayesNet caches up to `max_cached_programs` of them --
         many evidence patterns at large batches would otherwise exhaust the GPU long before the LRU
@@ -1058,15 +1028,14 @@ class BayesNet:
         from . import engine
 
         try:
-            return program.run(codes, n)
+            return entry.f32().run(codes, n)
         except engine.EngineError as exc:
             if exc.code != engine.SBN_E_NOMEM:
                 raise
         with self._cache_lock:
-            for key in [k for k, v in self._engine_cache.items() if (v[1] if isinstance(v, tuple) else v) is not program]:
-                old = self._engine_cache.pop(key)
-                (old[1] if isinstance(old, tuple) else old).close()
-        return program.run(codes, n)
+            for key in [k for k, v in self._engine_cache.items() if v is not entry]:
+                self._engine_cache.pop(key).close()
+        return entry.f32().run(codes, n)
 
     def _posterior_codes_multi(self, query, ev_vars, codes, bad, devices):
         """Row-shard `_posterior_codes` over several GPUs of this process: contiguous balanced
@@ -1137,17 +1106,10 @@ class BayesNet:
             index = pd.MultiIndex.from_frame(X[list(ev_vars)])
         if n == 0:
             return pd.Series([], index=index, name=name, dtype=np.float64)
-        plan, program = self._plan((), ev_vars, _planner.MODE_BATCHED)
-        codes, bad = self._encode_events(ev_vars, [X[v].to_numpy() for v in ev_vars])
+        _, program = self._plan((), ev_vars, _planner.MODE_BATCHED)
+        codes, bad = self._encode_events(X, ev_vars)
         prob = program.evidence(codes, n).astype(np.float64)
-        rows = np.nonzero(np.isnan(prob) & ~bad)[0]
-        if len(rows) > 8:  # below the float32 range (or exactly zero): settle in float64
-            _, robust = self._plan((), ev_vars, _planner.MODE_BATCHED, robust=True)
-            prob[rows] = robust.evidence(np.ascontiguousarray(codes[:, rows]), len(rows))
-        elif len(rows):
-            _, flat = self._plan((), ev_vars, _planner.MODE_FLAT)
-            for b in rows:
-                prob[b] = flat.evidence(np.ascontiguousarray(codes[:, b:b + 1]), 1)[0]
+        prob = self._rescue(prob, np.isnan(prob) & ~bad, codes, "evidence", (), ev_vars)
         prob[np.isnan(prob) | bad] = 0.0
         return pd.Series(prob, index=index, name=name)
 

@@ -175,6 +175,7 @@ class Program:
         self.Q = int(plan.Q)
         self.n_ev = len(plan.evidence)
         self.f64 = bool(f64)
+        self.dtype = np.float64 if self.f64 else np.float32
         self._h = ctypes.c_void_p()
         words = np.ascontiguousarray(plan.words, dtype=np.int32)
         if self.f64:
@@ -227,81 +228,74 @@ class Program:
         return dict(zip(keys, [int(x) for x in buf]))
 
     # --------------------------------------------------------------------- runs
+    def _evidence(self, codes, n_rows):
+        """(uint8 evidence codes [n_ev, n_rows], C-contiguous, and their pointer: None for a program without
+        evidence columns); ValueError for another shape.  Keep the array alive until the call returns."""
+        codes = np.ascontiguousarray(codes, dtype=np.uint8)
+        if self.n_ev and codes.shape != (self.n_ev, n_rows):
+            raise ValueError(f"evidence codes have shape {codes.shape}, expected {(self.n_ev, n_rows)}")
+        return codes, codes.ctypes.data if self.n_ev else None
+
+    def _fn(self, name):
+        """The C entry point `name`, or its `_f64` twin for a float64 program."""
+        return getattr(load(), name + "_f64" if self.f64 else name)
+
     def run(self, codes: np.ndarray, n_rows: int, out: np.ndarray | None = None) -> np.ndarray:
         """Host path: evidence codes uint8 [n_ev, n_rows] in, posterior float32
         [Q, n_rows] out (copies H2D, every step, D2H, synchronises)."""
         n_rows = int(n_rows)
-        codes = np.ascontiguousarray(codes, dtype=np.uint8)
-        if self.n_ev:
-            if codes.shape != (self.n_ev, n_rows):
-                raise ValueError(f"evidence codes have shape {codes.shape}, expected {(self.n_ev, n_rows)}")
-        dtype = np.float64 if self.f64 else np.float32
+        codes, ev_ptr = self._evidence(codes, n_rows)
         if out is None:
-            out = np.empty((self.Q, n_rows), dtype=dtype)
-        elif out.shape != (self.Q, n_rows) or out.dtype != dtype or not out.flags.c_contiguous:
-            raise ValueError(f"out must be a C-contiguous {dtype.__name__} [Q, n_rows] array")
-        ev_ptr = codes.ctypes.data if self.n_ev else None
-        fn = load().sbn_program_run_host_f64 if self.f64 else load().sbn_program_run_host
-        _check(fn(self._h, ev_ptr, n_rows, n_rows, out.ctypes.data, n_rows))
+            out = np.empty((self.Q, n_rows), dtype=self.dtype)
+        elif out.shape != (self.Q, n_rows) or out.dtype != self.dtype or not out.flags.c_contiguous:
+            raise ValueError(f"out must be a C-contiguous {self.dtype.__name__} [Q, n_rows] array")
+        _check(self._fn("sbn_program_run_host")(self._h, ev_ptr, n_rows, n_rows, out.ctypes.data, n_rows))
         return out
 
     def evidence(self, codes: np.ndarray, n_rows: int) -> np.ndarray:
         """P(event) per evidence row (the normaliser of the posterior), host path."""
         n_rows = int(n_rows)
-        codes = np.ascontiguousarray(codes, dtype=np.uint8)
-        if self.n_ev and codes.shape != (self.n_ev, n_rows):
-            raise ValueError(f"evidence codes have shape {codes.shape}, expected {(self.n_ev, n_rows)}")
-        out = np.empty(n_rows, dtype=np.float64 if self.f64 else np.float32)
-        fn = load().sbn_program_evidence_host_f64 if self.f64 else load().sbn_program_evidence_host
-        _check(fn(self._h, codes.ctypes.data if self.n_ev else None, n_rows, n_rows, out.ctypes.data))
+        codes, ev_ptr = self._evidence(codes, n_rows)
+        out = np.empty(n_rows, dtype=self.dtype)
+        _check(self._fn("sbn_program_evidence_host")(self._h, ev_ptr, n_rows, n_rows, out.ctypes.data))
         return out
 
     def counts(self, codes: np.ndarray, n_rows: int):
         """Counts programs (planner.build_counts_plan): (expected counts float64 [n_counts] summed over the
         rows, P(observed) [n_rows], NaN for a row the float32 range rule flags), host path."""
         n_rows = int(n_rows)
-        codes = np.ascontiguousarray(codes, dtype=np.uint8)
-        if self.n_ev and codes.shape != (self.n_ev, n_rows):
-            raise ValueError(f"evidence codes have shape {codes.shape}, expected {(self.n_ev, n_rows)}")
+        codes, ev_ptr = self._evidence(codes, n_rows)
         counts = np.zeros(int(self.plan.n_counts), dtype=np.float64)
-        prob = np.empty(n_rows, dtype=np.float64 if self.f64 else np.float32)
-        fn = load().sbn_program_counts_host_f64 if self.f64 else load().sbn_program_counts_host
-        _check(fn(self._h, codes.ctypes.data if self.n_ev else None, n_rows, n_rows, counts.ctypes.data, counts.size,
-                  prob.ctypes.data))
+        prob = np.empty(n_rows, dtype=self.dtype)
+        _check(self._fn("sbn_program_counts_host")(self._h, ev_ptr, n_rows, n_rows, counts.ctypes.data, counts.size,
+                                                   prob.ctypes.data))
         return counts, prob
 
     def set_tables(self, blob: np.ndarray):
         """Replace a counts program's tables (planner.refresh_tables gives the blob of new CPTs)."""
-        blob = np.ascontiguousarray(blob, dtype=np.float64 if self.f64 else np.float32)
-        fn = load().sbn_program_set_tables_f64 if self.f64 else load().sbn_program_set_tables
-        _check(fn(self._h, blob.ctypes.data, blob.size))
+        blob = np.ascontiguousarray(blob, dtype=self.dtype)
+        _check(self._fn("sbn_program_set_tables")(self._h, blob.ctypes.data, blob.size))
 
     def sample(self, codes: np.ndarray, n_rows: int, n_draws: int, seed: int, row_base: int = 0):
         """Sample programs (planner.build_sample_plan): (drawn codes uint8 [n_sampled, n_draws, n_rows] in
         the order of `plan.sampled`, P(observed) [n_rows], NaN for a row the float32 range rule flags), host
         path.  Row b's draws depend only on (seed, row_base + b, draw index)."""
         n_rows, n_draws = int(n_rows), int(n_draws)
-        codes = np.ascontiguousarray(codes, dtype=np.uint8)
-        if self.n_ev and codes.shape != (self.n_ev, n_rows):
-            raise ValueError(f"evidence codes have shape {codes.shape}, expected {(self.n_ev, n_rows)}")
+        codes, ev_ptr = self._evidence(codes, n_rows)
         out = np.empty((len(self.plan.sampled), n_draws, n_rows), dtype=np.uint8)
-        prob = np.empty(n_rows, dtype=np.float64 if self.f64 else np.float32)
-        fn = load().sbn_program_sample_host_f64 if self.f64 else load().sbn_program_sample_host
-        _check(fn(self._h, codes.ctypes.data if self.n_ev else None, n_rows, n_rows, n_draws,
-                  int(seed) & (2**64 - 1), int(row_base), out.ctypes.data, prob.ctypes.data))
+        prob = np.empty(n_rows, dtype=self.dtype)
+        _check(self._fn("sbn_program_sample_host")(self._h, ev_ptr, n_rows, n_rows, n_draws, int(seed) & (2**64 - 1),
+                                                   int(row_base), out.ctypes.data, prob.ctypes.data))
         return out, prob
 
     def mpe(self, codes: np.ndarray, n_rows: int):
         """MPE programs (planner.build_mpe_plan): (decoded codes uint8 [n_decoded, n_rows] in the order of
         `plan.sampled`, max log P(x, e) float32 [n_rows], -inf for a row of probability zero), host path."""
         n_rows = int(n_rows)
-        codes = np.ascontiguousarray(codes, dtype=np.uint8)
-        if self.n_ev and codes.shape != (self.n_ev, n_rows):
-            raise ValueError(f"evidence codes have shape {codes.shape}, expected {(self.n_ev, n_rows)}")
+        codes, ev_ptr = self._evidence(codes, n_rows)
         out = np.empty((len(self.plan.sampled), n_rows), dtype=np.uint8)
         log_prob = np.empty(n_rows, dtype=np.float32)
-        _check(load().sbn_program_mpe_host(self._h, codes.ctypes.data if self.n_ev else None, n_rows, n_rows,
-                                           out.ctypes.data, log_prob.ctypes.data))
+        _check(load().sbn_program_mpe_host(self._h, ev_ptr, n_rows, n_rows, out.ctypes.data, log_prob.ctypes.data))
         return out, log_prob
 
     def map(self, codes: np.ndarray, n_rows: int):

@@ -170,7 +170,6 @@ def query_many_sharded(bn, *query, events, group=None, dst: int = 0):
     `events`; rank r answers `row_shard(len(events), r, world)`.  Returns the DataFrame on the
     global rank `dst`, None elsewhere.  Rows flagged by the float32 program are settled in
     float64 on the rank that owns them, before the gather."""
-    import pandas as pd
     import torch
     import torch.distributed as dist
 
@@ -178,9 +177,7 @@ def query_many_sharded(bn, *query, events, group=None, dst: int = 0):
     plan, _ = bn._plan(query, ev_vars, 1)
     n = len(events.index)
     world, rank = dist.get_world_size(group), dist.get_rank(group)
-    codes, bad = bn._encode_events(ev_vars, [events[v].to_numpy() for v in ev_vars])
-    if not ev_vars:
-        bad = np.zeros(n, dtype=bool)
+    codes, bad = bn._encode_events(events, ev_vars)
     backend = dist.get_backend(group)
     device = f"cuda:{torch.cuda.current_device()}" if backend == "nccl" else None
 
@@ -191,7 +188,4 @@ def query_many_sharded(bn, *query, events, group=None, dst: int = 0):
     post = run_sharded(codes, n, run_fn, group=group, dst=dst, device=device)
     if post is None:
         return None
-    out = pd.DataFrame(post.cpu().numpy().astype(np.float64).T, index=events.index, columns=bn._answer_index(plan))
-    if bad.any():
-        out.loc[events.index[bad]] = np.nan
-    return out
+    return bn._answer_frame(post.cpu().numpy().astype(np.float64), events.index, bn._answer_index(plan), bad)

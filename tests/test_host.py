@@ -276,7 +276,7 @@ def test_chow_liu_matches_reference_edges():
     assert learned.is_tree and learned._compiled is not None
 
 
-def test_out_of_memory_evicts_other_cached_programs_and_retries():
+def test_out_of_memory_evicts_other_cache_entries_and_retries():
     """A program whose scratch does not fit is retried once after every OTHER cached device object
     has been closed (each owns an arena sized for its largest batch)."""
     from sorobn_b200 import BayesNet, engine
@@ -294,10 +294,13 @@ def test_out_of_memory_evicts_other_cached_programs_and_retries():
         def close(self):
             self.closed = True
 
+        def f32(self):  # a cache entry that is its own float32 program
+            return self
+
     bn = BayesNet(("A", "B"))
     mine, other, sampler = FakeProgram(True), FakeProgram(False), FakeProgram(False)
-    bn._engine_cache[("q1",)] = ("plan", mine)
-    bn._engine_cache[("q2",)] = ("plan", other)
+    bn._engine_cache[("q1",)] = mine
+    bn._engine_cache[("q2",)] = other
     bn._engine_cache[("sampler", "q3")] = sampler
     out = bn._run_evicting(mine, np.zeros((1, 4), dtype=np.uint8), 4)
     assert out.shape == (2, 4) and mine.calls == 2 and not mine.closed

@@ -411,7 +411,7 @@ def test_map_of_one_event_and_errors(interpreted):
     assert empty.shape == (0, 4) and list(empty.columns) == sorted(X.columns)
 
 
-def test_the_map_programs_are_keyed_by_their_variables(monkeypatch):
+def test_the_map_pattern_programs_are_keyed_by_their_variables(monkeypatch):
     class FakeProgram:
         def __init__(self, plan, device=None, f64=False):
             self.plan = plan
@@ -421,7 +421,7 @@ def test_the_map_programs_are_keyed_by_their_variables(monkeypatch):
 
     monkeypatch.setattr(engine, "Program", FakeProgram)
     bn = examples.asia()
-    a = bn._map_runner((0,), (1,))
-    assert a.plan.version == planner.VERSION_MAP and bn._map_runner((0,), (1,)) is a
-    assert bn._map_runner((0,), (1, 2)) is not a
+    a = bn._pattern_runner("map", (0,), (1,))
+    assert a.plan.version == planner.VERSION_MAP and bn._pattern_runner("map", (0,), (1,)) is a
+    assert bn._pattern_runner("map", (0,), (1, 2)) is not a
     assert bn._pattern_runner("mpe", (0,)).plan.version == planner.VERSION_MPE

@@ -283,7 +283,7 @@ def test_errors_and_an_empty_frame(interpreted):
     assert got.shape == (0, len(bn.nodes)) and len(log_p) == 0
 
 
-def test_the_mpe_programs_share_the_pattern_cache(monkeypatch):
+def test_the_mpe_pattern_programs_share_the_pattern_cache(monkeypatch):
     class FakeProgram:
         def __init__(self, plan, device=None, f64=False):
             self.plan = plan
@@ -295,4 +295,4 @@ def test_the_mpe_programs_share_the_pattern_cache(monkeypatch):
     bn = examples.asia()
     mpe = bn._pattern_runner("mpe", (0,))
     assert mpe.plan.version == planner.VERSION_MPE and bn._pattern_runner("mpe", (0,)) is mpe
-    assert bn._sample_runner((0,)) is not mpe and bn._sample_runner((0,)).plan.version == planner.VERSION_SAMPLE
+    assert bn._pattern_runner("sample", (0,)) is not mpe and bn._pattern_runner("sample", (0,)).plan.version == planner.VERSION_SAMPLE

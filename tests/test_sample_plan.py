@@ -241,15 +241,15 @@ def test_rows_the_float32_program_flags_are_drawn_by_the_float64_program(interpr
     want, p, _ = program_interp.run_sample(plan.words, plan.table_blob64, codes, n_draws=2, seed=3)
     interpreted.flag_below = float(np.median(p))
     got = bn.sample_many(X, n=2, seed=3)
-    assert any(f64 for f64, _ in interpreted.calls) and any(not f64 for f64, _ in interpreted.calls)
-    assert sum(n for f64, n in interpreted.calls if f64) == int((p < np.median(p)).sum())
+    assert any(f64 for _, _, f64, _ in interpreted.calls) and any(not f64 for _, _, f64, _ in interpreted.calls)
+    assert sum(n for _, _, f64, n in interpreted.calls if f64) == int((p < np.median(p)).sum())
     for j, v in enumerate(plan.sampled):
         assert list(got[net.names[v]]) == list(np.asarray(net.domains[v], dtype=object)[want[j].T.reshape(-1)])
 
 
-def test_the_counts_programs_keep_their_cache_entry_point(monkeypatch):
-    """`_counts_runner` (used by tools/em_bench.py) and `_sample_runner` share the program cache under their
-    own keys."""
+def test_the_counts_and_sample_pattern_programs_share_the_cache(monkeypatch):
+    """`_pattern_runner("counts", ...)` (used by tools/em_bench.py) and `_pattern_runner("sample", ...)` share the
+    program cache under their own keys."""
     class FakeProgram:
         def __init__(self, plan, device=None, f64=False):
             self.plan = plan
@@ -259,7 +259,7 @@ def test_the_counts_programs_keep_their_cache_entry_point(monkeypatch):
 
     monkeypatch.setattr(engine, "Program", FakeProgram)
     bn = examples.asia()
-    counts = bn._counts_runner((0,))
-    samples = bn._sample_runner((0,))
+    counts = bn._pattern_runner("counts", (0,))
+    samples = bn._pattern_runner("sample", (0,))
     assert counts.plan.version == planner.VERSION_COUNTS and samples.plan.version == planner.VERSION_SAMPLE
-    assert bn._counts_runner((0,)) is counts and bn._sample_runner((0,)) is samples
+    assert bn._pattern_runner("counts", (0,)) is counts and bn._pattern_runner("sample", (0,)) is samples

@@ -83,7 +83,7 @@ def main():
             t0 = time.perf_counter()
             groups = bn._count_patterns(X)
             t1 = time.perf_counter()
-            bn._e_step(X, groups, lambda k, ev: bn._counts_runner(ev), n_counts)
+            bn._e_step(X, groups, lambda k, ev: bn._pattern_runner("counts", ev), n_counts)
             t2 = time.perf_counter()
             host.append(t1 - t0)
             estep.append(t2 - t1)
