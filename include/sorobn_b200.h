@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SBN_ABI_VERSION 13
+#define SBN_ABI_VERSION 14
 
 #define SBN_OK 0
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
@@ -99,6 +99,23 @@ int sbn_program_run_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev
  * a row below the float32 range (re-run it with a float64 program). */
 int sbn_program_evidence_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, float *prob);
 int sbn_program_evidence_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *prob);
+
+/* Soft (likelihood, virtual) evidence: a posterior or marginals program planned with soft variables
+ * (planner.build_plan / build_marginals_plan `soft=`) runs through these calls only, and they refuse
+ * every other program.  `lik` is [n_rows][ld_lik] row-major: one column per state of every soft
+ * variable (variables sorted by name, states in domain order, ld_lik >= that count), non-negative; a
+ * row's posterior is P(query | e) with every P(x) weighted by prod_v lik_v(x_v), which is unchanged
+ * when a variable's row is scaled.  `lik` is host memory, or device memory of the program's device
+ * when `lik_on_device` is non-zero (read on the program's stream: the caller's writes must be
+ * complete).  Codes and `out` are host memory, as for run_host.  `log_evidence` (double [n_rows], or
+ * null; posterior programs only) receives log P(e, lik) = log sum_x P(x, e) prod_v lik_v(x_v); NaN
+ * where the float32 range rule flags the row, or for a row of probability zero (an all-zero lik_v
+ * makes one). */
+int sbn_program_run_soft_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
+                              int64_t ld_lik, int lik_on_device, float *out, int64_t ld_out, double *log_evidence);
+int sbn_program_run_soft_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
+                                  const double *lik, int64_t ld_lik, int lik_on_device, double *out, int64_t ld_out,
+                                  double *log_evidence);
 
 /* Expected counts (the E-step of expectation-maximisation) of a counts program
  * (planner.build_counts_plan, version 6; the run and evidence calls refuse it, and these calls refuse

@@ -832,13 +832,16 @@ class BayesNet:
     def _answer_index(self, plan):
         return self._states_index(plan.query)
 
-    def query(self, *query, event: dict, algorithm="exact", n_iterations=100) -> pd.Series:
+    def query(self, *query, event: dict, algorithm="exact", n_iterations=100, likelihoods: dict | None = None) -> pd.Series:
         """Answer P(query | event) (bayes_net.py:796-875), exact inference on the GPU.
 
         The answer is a Series named "P(q1, q2)" indexed by the query variables
         (levels sorted by name, rows sorted by state); states with zero posterior
         are left out, as the reference's zero-filtering join does
         (bayes_net.py:253-256).
+
+        likelihoods: soft evidence, {node: a vector over the node's sorted domain, or a {state: weight}
+        dict}, as in `query_many`; computed in float64.
         """
         if not query:
             raise ValueError("At least one query variable has to be specified")
@@ -846,6 +849,15 @@ class BayesNet:
             if q in event:
                 raise ValueError("A query variable cannot be part of the event")
         name = f"P({', '.join(map(str, query))})"
+        if likelihoods is not None:
+            self._check_soft_call(algorithm, None)
+            ev_vars = tuple(event)
+            soft, lik = self._soft_matrix(likelihoods, 1, ev_vars, single=True)
+            entry = self._soft_programs(query, ev_vars, soft, marginals=False)
+            index = self._answer_index(entry.plan)
+            codes, bad = self._encode_events(pd.DataFrame({v: [event[v]] for v in ev_vars}, index=[0]), ev_vars)
+            post = None if bad[0] else entry.f64().run_soft(codes, lik, 1)[:, 0]
+            return _posterior_series(post, index, name)
         if algorithm in ("gibbs", "likelihood", "rejection"):
             events = pd.DataFrame({v: [event[v]] for v in event}, index=[0])
             freq, index = self._sample_query(algorithm, query, events, n_iterations)
@@ -901,7 +913,7 @@ class BayesNet:
         return freq, self._states_index([net.index[q] for q in q_sorted])
 
     def query_many(self, *query, events: pd.DataFrame, algorithm="exact", n_iterations=100,
-                   devices: typing.Sequence[int] | None = None) -> pd.DataFrame:
+                   devices: typing.Sequence[int] | None = None, likelihoods: dict | None = None) -> pd.DataFrame:
         """Batched `query`: one posterior per row of `events` (columns = evidence
         variables).  Returns a DataFrame with one row per evidence row and one column
         per joint state of the query variables (same order as `query`'s index);
@@ -910,13 +922,26 @@ class BayesNet:
         devices: CUDA device ids to shard the rows over (exact algorithm).  Rows are independent,
         so each device answers a contiguous slice with its own program (one host thread per
         device; the C ABI call releases the GIL) and the slices land in one host array: there is
-        no collective.  One process per GPU under torchrun is `sorobn_b200.sharding.query_many_sharded`."""
+        no collective.  One process per GPU under torchrun is `sorobn_b200.sharding.query_many_sharded`.
+
+        likelihoods: soft (virtual) evidence, {node: values}, one likelihood over the node's states
+        per row: P(query | row) is then proportional to sum P(x, row) * prod_node values[node](x_node).
+        `values` is a [len(events), card] numpy array or torch tensor (columns in the node's sorted
+        domain order; a CUDA tensor is read on the device) or a DataFrame whose columns are the node's
+        states.  Entries must be finite and non-negative; a row of zeros makes the row impossible (NaN),
+        and scaling a row changes nothing.  A soft node may be queried, but may not be a column of
+        `events`.  Exact algorithm only, on one device."""
         if not query:
             raise ValueError("At least one query variable has to be specified")
         ev_vars = tuple(events.columns)
         for q in query:
             if q in ev_vars:
                 raise ValueError("A query variable cannot be part of the event")
+        if likelihoods is not None:
+            self._check_soft_call(algorithm, devices)
+            soft, lik = self._soft_matrix(likelihoods, len(events.index), ev_vars)
+            plan = self._soft_programs(query, ev_vars, soft, marginals=False).plan
+            return self._soft_frame(query, events, soft, lik, self._answer_index(plan), marginals=False)
         if algorithm in ("gibbs", "likelihood", "rejection"):
             freq, index = self._sample_query(algorithm, query, events, n_iterations)
             return pd.DataFrame(freq.T.astype(np.float64), index=events.index, columns=index)
@@ -973,6 +998,116 @@ class BayesNet:
                 out[..., b] = getattr(flat, method)(np.ascontiguousarray(codes[:, b:b + 1]), 1)[..., 0]
         return out
 
+    # ---------------------------------------------------------------- soft evidence
+    @staticmethod
+    def _check_soft_call(algorithm, devices):
+        if algorithm != "exact":
+            raise ValueError("soft evidence (likelihoods) needs algorithm='exact'")
+        if devices is not None:
+            raise ValueError("soft evidence (likelihoods) runs on one device: devices=[...] is not supported")
+
+    def _soft_matrix(self, likelihoods, n, ev_vars, single=False):
+        """(soft node names sorted, likelihoods [n, sum of cards]: a numpy float64 array, or a torch tensor on the
+        device when any value is a CUDA tensor) of `likelihoods` {node: values}; ValueError for a node that is not
+        in the network or is a hard-evidence column, for a wrong shape, a state outside the node's domain, or an
+        entry that is NaN, infinite or negative.  `single` (one event): a value may also be a 1-D vector or a
+        {state: weight} dict."""
+        net = self._net("querying")
+        if not isinstance(likelihoods, dict) or not likelihoods:
+            raise ValueError("likelihoods must be a non-empty {node: values} dict")
+        names = sorted(likelihoods)
+        blocks = []
+        for name in names:
+            if name not in net.index:
+                raise ValueError(f"likelihoods for {name!r}, which is not a node of the network")
+            if name in ev_vars:
+                raise ValueError(f"{name!r} has both hard evidence and likelihoods")
+            domain = net.domains[net.index[name]]
+            values = likelihoods[name]
+            if single and isinstance(values, dict):
+                values = pd.DataFrame([values])
+            if isinstance(values, (pd.DataFrame, pd.Series)):
+                frame = values.to_frame().T if isinstance(values, pd.Series) else values
+                unknown = [c for c in frame.columns if c not in set(domain)]
+                if unknown:
+                    raise ValueError(f"likelihoods for {name!r}: {unknown[:5]} are not states of the node")
+                values = frame.reindex(columns=domain).to_numpy(dtype=np.float64)
+            elif not type(values).__module__.startswith("torch"):
+                values = np.asarray(values, dtype=np.float64)
+            if single and values.ndim == 1:
+                values = values.reshape(1, -1)
+            if tuple(values.shape) != (n, len(domain)):
+                raise ValueError(f"likelihoods for {name!r} have shape {tuple(values.shape)}, expected {(n, len(domain))}")
+            blocks.append(values)
+        torch_blocks = [b for b in blocks if not isinstance(b, np.ndarray)]
+        cuda = next((b.device for b in torch_blocks if b.is_cuda), None)
+        if cuda is None:
+            lik = np.concatenate([b if isinstance(b, np.ndarray) else b.detach().cpu().numpy().astype(np.float64)
+                                  for b in blocks], axis=1)
+            finite, negative = np.isfinite(lik).all(), (lik < 0).any()
+        else:
+            import torch
+
+            lik = torch.cat([torch.as_tensor(b).to(device=cuda, dtype=torch.float64) for b in blocks], dim=1)
+            finite, negative = bool(torch.isfinite(lik).all()), bool((lik < 0).any())
+        if not finite:
+            raise ValueError("likelihoods must be finite (no NaN or inf)")
+        if negative:
+            raise ValueError("likelihoods must be non-negative")
+        return tuple(names), lik
+
+    def _soft_programs(self, query, ev_vars, soft, marginals):
+        """The cached `_Programs` of P(query | hard columns `ev_vars`, likelihoods of `soft`), plan key (query,
+        evidence vars, mode, marginals, soft nodes): batched only, the float64 twin settles flagged rows."""
+        net = self._net("querying")
+
+        def build_plan():
+            for name in (*query, *ev_vars):
+                if name not in net.index:
+                    raise KeyError(name)
+            ev, sv = [net.index[e] for e in ev_vars], [net.index[s] for s in soft]
+            if marginals:
+                return _planner.build_marginals_plan(net, ev, targets=[net.index[q] for q in query], soft=sv)
+            return _planner.build_plan(net, [net.index[q] for q in query], ev, allow_empty_query=True, soft=sv)
+
+        return self._programs((tuple(query), tuple(ev_vars), _planner.MODE_BATCHED, marginals, tuple(soft)), build_plan)
+
+    def _soft_codes(self, query, ev_vars, soft, codes, bad, lik, marginals, log_evidence=False):
+        """(posterior float64 [Q, n], log P(e, lik) [n] or None) of a soft-evidence program; the rows the float32
+        program flags (NaN) re-run on the float64 program with their likelihoods; rows with a value outside its
+        variable's domain (`bad`) are left to the caller."""
+        entry = self._soft_programs(query, ev_vars, soft, marginals)
+        n = len(bad)
+        res = entry.f32().run_soft(codes, lik, n, log_evidence=log_evidence)
+        post, log_ev = res if log_evidence else (res, None)
+        post = post.astype(np.float64)
+        flagged = np.isnan(post).any(axis=0) & ~bad
+        if log_evidence:
+            flagged |= np.isnan(log_ev) & ~bad
+        rows = np.flatnonzero(flagged)
+        if len(rows):
+            if isinstance(lik, np.ndarray):
+                sub = lik[rows]
+            else:
+                import torch
+
+                sub = lik[torch.as_tensor(rows, device=lik.device)]
+            again = entry.f64().run_soft(np.ascontiguousarray(codes[:, rows]), sub, len(rows), log_evidence=log_evidence)
+            if log_evidence:
+                post[:, rows], log_ev[rows] = again
+            else:
+                post[:, rows] = again
+        return post, log_ev
+
+    def _soft_frame(self, query, events, soft, lik, columns, marginals):
+        """`_posterior_frame` with likelihoods: the posterior of every row of `events`."""
+        ev_vars = tuple(events.columns)
+        if len(events.index) == 0:
+            return pd.DataFrame(np.zeros((0, len(columns))), index=events.index, columns=columns)
+        codes, bad = self._encode_events(events, ev_vars)
+        post, _ = self._soft_codes(query, ev_vars, soft, codes, bad, lik, marginals)
+        return self._answer_frame(post, events.index, columns, bad)
+
     def _targets(self, variables, ev_vars):
         """Target names of a marginals query, sorted: `variables`, or every variable that is not evidence."""
         net = self._net("querying")
@@ -988,7 +1123,7 @@ class BayesNet:
             raise ValueError("At least one query variable has to be specified")
         return tuple(sorted(set(variables)))
 
-    def marginals_many(self, events: pd.DataFrame, variables=None) -> pd.DataFrame:
+    def marginals_many(self, events: pd.DataFrame, variables=None, likelihoods: dict | None = None) -> pd.DataFrame:
         """The posterior marginal of every variable in `variables` (default: every variable that is not
         a column of `events`), for every row of `events`, from ONE device program: an upward and a
         downward pass over the bucket tree of the elimination, then one readout per variable
@@ -996,11 +1131,16 @@ class BayesNet:
 
         Returns one row per evidence row; the columns are a MultiIndex of (variable, state), variables
         sorted by name, states sorted.  Zero-probability states stay (as 0.0); impossible rows and rows
-        with a value outside its variable's domain are NaN."""
-        targets = self._targets(variables, tuple(events.columns))
+        with a value outside its variable's domain are NaN.  `likelihoods`: soft evidence, as in
+        `query_many`; a soft node may be a target."""
+        ev_vars = tuple(events.columns)
+        targets = self._targets(variables, ev_vars)
         net = self._compiled
         columns = pd.MultiIndex.from_tuples([(t, s) for t in targets for s in net.domains[net.index[t]]],
                                             names=["variable", "state"])
+        if likelihoods is not None:
+            soft, lik = self._soft_matrix(likelihoods, len(events.index), ev_vars)
+            return self._soft_frame(targets, events, soft, lik, columns, marginals=True)
         return self._posterior_frame(targets, events, columns, marginals=True)
 
     def marginals(self, event: dict, variables=None) -> dict:
@@ -1086,7 +1226,7 @@ class BayesNet:
         fjd = pd.Series(post, index=self._answer_index(plan), name=f"P({', '.join(map(str, names))})")
         return fjd if keep_zeros else fjd[post > 0]
 
-    def predict_proba(self, X: typing.Union[dict, pd.DataFrame]):
+    def predict_proba(self, X: typing.Union[dict, pd.DataFrame], likelihoods: dict | None = None):
         """Probability of each row of `X` (bayes_net.py:934-962).
 
         The reference builds the full joint, sums out the columns `X` lacks and looks the
@@ -1094,16 +1234,17 @@ class BayesNet:
         evidence and no query variable: same number, no joint, any network size.  Rows of
         probability zero give 0.0 (the reference's joint has no such row and raises
         KeyError).  With a single column the reference returns the whole marginal instead
-        of per-row values; this returns per-row values in every case."""
+        of per-row values; this returns per-row values in every case.
+
+        likelihoods: soft evidence, as in `query_many`: each row then gives
+        P(row, likelihoods) = sum_x P(x, row) * prod_node values[node](x_node)."""
+        if likelihoods is not None:
+            with np.errstate(under="ignore"):
+                return np.exp(self.predict_log_proba(X, likelihoods=likelihoods))
         if isinstance(X, dict):
             return self.predict_proba(pd.DataFrame([X])).iloc[0]
-        ev_vars = tuple(sorted(X.columns))
+        ev_vars, name, index = self._proba_index(X)
         n = len(X.index)
-        name = f"P({', '.join(map(str, ev_vars))})"
-        if len(ev_vars) == 1:
-            index = pd.Index(X[ev_vars[0]], name=ev_vars[0])
-        else:
-            index = pd.MultiIndex.from_frame(X[list(ev_vars)])
         if n == 0:
             return pd.Series([], index=index, name=name, dtype=np.float64)
         _, program = self._plan((), ev_vars, _planner.MODE_BATCHED)
@@ -1113,10 +1254,33 @@ class BayesNet:
         prob[np.isnan(prob) | bad] = 0.0
         return pd.Series(prob, index=index, name=name)
 
-    def predict_log_proba(self, X: typing.Union[dict, pd.DataFrame]):
-        """Log-likelihood of each row (bayes_net.py:964-973)."""
-        with np.errstate(divide="ignore"):
-            return np.log(self.predict_proba(X))
+    def _proba_index(self, X):
+        """(evidence columns sorted, Series name, index) of `predict_proba`'s answer for the frame `X`."""
+        ev_vars = tuple(sorted(X.columns))
+        name = f"P({', '.join(map(str, ev_vars))})"
+        if len(ev_vars) == 1:
+            return ev_vars, name, pd.Index(X[ev_vars[0]], name=ev_vars[0])
+        return ev_vars, name, pd.MultiIndex.from_frame(X[list(ev_vars)])
+
+    def predict_log_proba(self, X: typing.Union[dict, pd.DataFrame], likelihoods: dict | None = None):
+        """Log-likelihood of each row (bayes_net.py:964-973).  With `likelihoods` (soft evidence, as in
+        `query_many`), log P(row, likelihoods) straight from the device's log-normaliser, -inf for a row of
+        probability zero."""
+        if likelihoods is None:
+            with np.errstate(divide="ignore"):
+                return np.log(self.predict_proba(X))
+        single = isinstance(X, dict)  # one event: a likelihood may be a vector or a {state: weight} dict
+        frame = pd.DataFrame([X]) if single else X
+        ev_vars, name, index = self._proba_index(frame)
+        n = len(frame.index)
+        soft, lik = self._soft_matrix(likelihoods, n, ev_vars, single=single)
+        if n == 0:
+            return pd.Series([], index=index, name=name, dtype=np.float64)
+        codes, bad = self._encode_events(frame, ev_vars)
+        _, log_ev = self._soft_codes((), ev_vars, soft, codes, bad, lik, marginals=False, log_evidence=True)
+        log_ev[np.isnan(log_ev) | bad] = -np.inf
+        out = pd.Series(log_ev, index=index, name=name)
+        return out.iloc[0] if single else out
 
     def impute(self, sample: dict, **query_params) -> pd.Series:
         """Fill the `None` entries of `sample` with their most probable joint value

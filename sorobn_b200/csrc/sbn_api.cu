@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -26,6 +27,7 @@
 #include "sbn_mpe.cuh"
 #include "sbn_pair.h"
 #include "sbn_sample.cuh"
+#include "sbn_soft.cuh"
 #include "sbn_tma.h"
 
 namespace {
@@ -124,6 +126,22 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
     }
     if (!marginals && ((P->slots[P->post_slot].batched ? 1 : 0) != P->post_batched || P->slots[P->post_slot].size < P->Q))
         return fail(SBN_E_INVALID, "posterior slot mismatch");
+    if (P->kind == kPosterior || marginals) {
+        // soft evidence: (slot, card) of every likelihood, filled before step 0 (sbn_soft.cuh)
+        const int n_soft = w[10];
+        if (n_soft < 0 || (n_soft > 0 && P->mode != 1) || !need(2LL * n_soft))
+            return fail(SBN_E_INVALID, "bad soft-evidence section");
+        for (int v = 0; v < n_soft; ++v) {
+            const int slot = w[p], card = w[p + 1];
+            p += 2;
+            if (slot < 0 || slot >= n_slots || !P->slots[slot].batched || card < 1 || P->slots[slot].size < card)
+                return fail(SBN_E_INVALID, "bad likelihood %d", v);
+            for (const auto &o : P->soft)
+                if (o.first == slot) return fail(SBN_E_INVALID, "two likelihoods share slot %d", slot);
+            P->soft.push_back({slot, card});
+            P->n_lik += card;
+        }
+    }
     std::vector<int> written(marginals ? P->Q : 0, 0);  // posterior entries written by the readouts
     for (int s = 0; s < n_steps; ++s) {
         if (!need(5)) return fail(SBN_E_INVALID, "truncated step %d", s);
@@ -345,6 +363,17 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             if (P->steps[i].kind != 3) return fail(SBN_E_INVALID, "step %d comes between the count steps", i);
     } else if (P->steps.back().out_slot != P->post_slot) {
         return fail(SBN_E_INVALID, "last step does not write the posterior");
+    }
+    for (const auto &sv : P->soft) {
+        // a likelihood slot holds the pack's values from before step 0: its first access is a read (a later step
+        // may reuse the slot once the likelihood's readers are done)
+        for (const StepDesc &st : P->steps) {
+            bool read = false;
+            for (const InDesc &in : st.in) read |= in.is_slot && in.id == sv.first;
+            if (read) break;
+            if (st.kind <= 1 && st.out_slot == sv.first)
+                return fail(SBN_E_INVALID, "likelihood slot %d is written before it is read", sv.first);
+        }
     }
     return SBN_OK;
 }
@@ -692,6 +721,10 @@ void free_scratch(sbn_program *P) {
     cudaFree(P->d_ev);
     cudaFree(P->d_out);
     cudaFree(P->d_total);
+    cudaFree(P->d_lik);
+    cudaFree(P->d_log_max);
+    P->d_lik = nullptr;
+    P->d_log_max = nullptr;
     P->d_total = nullptr;
     P->d_arena = nullptr;
     P->d_ev = nullptr;
@@ -1100,6 +1133,22 @@ cudaError_t launch_normalise(sbn_program *P, float *d_out, int64_t ld_out, int64
     return cudaGetLastError();
 }
 
+// Soft-evidence program: fill the likelihood slots from P->lik (pitch P->ld_lik) and sum log(max) per row
+cudaError_t launch_soft_pack(sbn_program *P, int64_t n_rows, cudaStream_t stream) {
+    P->launches++;
+    const int threads = 256;
+    const unsigned grid = static_cast<unsigned>((n_rows + threads - 1) / threads);
+    const int32_t rows = static_cast<int32_t>(n_rows), n_soft = static_cast<int32_t>(P->soft.size());
+    if (P->f64)
+        sbn_soft_pack<double><<<grid, threads, 0, stream>>>(static_cast<const double *>(P->lik), P->ld_lik, rows, n_soft,
+                                                            P->d_soft, reinterpret_cast<double *>(P->d_arena), P->ld,
+                                                            P->d_log_max);
+    else
+        sbn_soft_pack<float><<<grid, threads, 0, stream>>>(static_cast<const float *>(P->lik), P->ld_lik, rows, n_soft,
+                                                           P->d_soft, P->d_arena, P->ld, P->d_log_max);
+    return cudaGetLastError();
+}
+
 // Evidence-independent steps of a batched program (products of CPTs, possibly keeping evidence
 // variables as ordinary axes) depend on the tables only: they run once, in create_common, and
 // every later run reads their outputs (19 of the 67 launches of the benchmark grid's step).
@@ -1155,6 +1204,7 @@ int issue_all(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows
               cudaStream_t stream, cudaEvent_t *events, const DrawnCodes &dc = {}) {
     // the flags of the sample steps start clear in every run, captured graph or not
     if (P->kind == kSample) SBN_CUDA(cudaMemsetAsync(dc.flags(P), 0, static_cast<size_t>(n_rows), stream));
+    if (!P->soft.empty()) SBN_CUDA(launch_soft_pack(P, n_rows, stream));
     SbnStep q;
     int k = 0;
     int n_decoded = 0;  // sample / argmax steps issued so far
@@ -1229,6 +1279,7 @@ int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n
     std::vector<std::vector<int>> readers(n_slots);
     std::vector<int> stream_of(n_steps, 0);
     cudaEvent_t fork = P->step_done[n_steps];  // reused as the fork event before any step
+    if (!P->soft.empty()) SBN_CUDA(launch_soft_pack(P, n_rows, origin));  // every branch forks after it
     SBN_CUDA(cudaEventRecord(fork, origin));
     bool joined[sbn_program::kBranches] = {false, false, false, false};
     int rr = 0;
@@ -1290,13 +1341,17 @@ int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n
 
 // The checks every run shares: the program is of the kind the entry point runs (kPosterior: the run, evidence
 // and profile calls, which take posterior and marginals programs), and the rows and their evidence are well formed
-int check_rows(const sbn_program *P, ProgramKind kind, const void *ev, int64_t ld_ev, int64_t n_rows) {
+int check_rows(const sbn_program *P, ProgramKind kind, const void *ev, int64_t ld_ev, int64_t n_rows, bool soft = false) {
     static const char *const name[] = {"posterior", "marginals", "counts", "sample", "MPE", "MAP"};
     static const char *const entry[] = {"sbn_program_run_*", "sbn_program_run_*", "sbn_program_counts_host",
                                         "sbn_program_sample_host", "sbn_program_mpe_host", "sbn_program_mpe_host"};
     if (!P) return fail(SBN_E_INVALID, "null program");
     if ((P->kind == kMarginals ? kPosterior : P->kind == kMap ? kMpe : P->kind) != kind)
         return fail(SBN_E_INVALID, "a %s program runs through %s", name[P->kind], entry[P->kind]);
+    if (!P->soft.empty() && !soft)
+        return fail(SBN_E_INVALID, "a %s program with soft evidence runs through sbn_program_run_soft_host", name[P->kind]);
+    if (P->soft.empty() && soft)
+        return fail(SBN_E_INVALID, "a %s program without soft evidence runs through sbn_program_run_host", name[P->kind]);
     if (n_rows <= 0) return fail(SBN_E_INVALID, "n_rows must be positive");
     if (P->n_ev > 0 && !ev) return fail(SBN_E_INVALID, "null evidence");
     if (P->n_ev > 1 && ld_ev < n_rows) return fail(SBN_E_INVALID, "ld_ev < n_rows");
@@ -1305,8 +1360,9 @@ int check_rows(const sbn_program *P, ProgramKind kind, const void *ev, int64_t l
 }
 
 // check_rows for the calls that write a posterior [Q][ld_out]
-int check_run_args(const sbn_program *P, const void *ev, int64_t ld_ev, int64_t n_rows, const void *out, int64_t ld_out) {
-    const int rc = check_rows(P, kPosterior, ev, ld_ev, n_rows);
+int check_run_args(const sbn_program *P, const void *ev, int64_t ld_ev, int64_t n_rows, const void *out, int64_t ld_out,
+                   bool soft = false) {
+    const int rc = check_rows(P, kPosterior, ev, ld_ev, n_rows, soft);
     if (rc != SBN_OK) return rc;
     if (!out) return fail(SBN_E_INVALID, "null output");
     if (P->Q > 1 && ld_out < n_rows) return fail(SBN_E_INVALID, "ld_out < n_rows");
@@ -1358,7 +1414,8 @@ int run_rows(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows,
     // saves, and the short runs of a pattern whose rows are scattered through a frame come in many lengths
     const bool short_chunk = (P->kind == kSample || sbn_log_domain(P->kind)) && n_rows < kSampleGraphMinRows;
     if (!P->use_graph || short_chunk) return issue_all(P, d_ev, ld_ev, n_rows, d_out, ld_out, stream, nullptr, dc);
-    const GraphKey key = {d_ev, ld_ev, n_rows, d_out, ld_out, P->d_partial, P->d_drawn, dc.n_draws, dc.ld_drawn};
+    const GraphKey key = {d_ev, ld_ev, n_rows, d_out, ld_out, P->d_partial, P->d_drawn, dc.n_draws, dc.ld_drawn, P->lik,
+                          P->ld_lik};
     const bool branched = P->use_branches && P->kind <= kMarginals;
     return replay(P, P->graph, key, P->stream, stream, [&] {
         return branched ? issue_branched(P, d_ev, ld_ev, n_rows, d_out, ld_out, P->stream)
@@ -1501,7 +1558,23 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
         SBN_CUDA_P(cudaStreamSynchronize(P->stream));
         // The on-chip segments and paired steps assume every intermediate has ONE consumer; the factors of the
         // other kinds' programs feed several launches, so they run on the classic per-step launches.
-        if (P->kind == kPosterior) sbn_chain_plan(P);
+        // (nor do the likelihood slots of soft evidence fit them: no step writes those)
+        if (P->kind == kPosterior && P->soft.empty()) sbn_chain_plan(P);
+    }
+    if (!P->soft.empty()) {
+        // the pack's descriptors: (row offset of the slot in the batched arena, card) per likelihood
+        P->use_tma = false;  // the TMA pipeline kernel is not planned for soft programs either
+        std::vector<int32_t> desc;
+        for (const auto &sv : P->soft) {
+            int64_t off = 0;
+            for (int s = 0; s < sv.first; ++s)
+                if (P->slots[s].batched) off += P->slots[s].size;
+            desc.push_back(static_cast<int32_t>(off));
+            desc.push_back(sv.second);
+        }
+        SBN_CUDA_P(cudaMalloc(&P->d_soft, desc.size() * 4));
+        SBN_CUDA_P(cudaMemcpyAsync(P->d_soft, desc.data(), desc.size() * 4, cudaMemcpyHostToDevice, P->stream));
+        SBN_CUDA_P(cudaStreamSynchronize(P->stream));
     }
     {
         // opt every step-kernel instantiation into SBN_SMEM_BUDGET of dynamic shared memory
@@ -1563,6 +1636,7 @@ void sbn_program_destroy(sbn_program *P) {
     cudaFree(P->d_partial);
     cudaFree(P->d_drawn);
     cudaFree(P->d_sample_args);
+    cudaFree(P->d_soft);
     cudaFree(P->d_tile_off);
     cudaFree(P->d_tables);
     if (P->stream) cudaStreamDestroy(P->stream);
@@ -1584,7 +1658,9 @@ int sbn_program_reserve(sbn_program *P, int64_t max_rows) {
     SBN_CUDA(cudaStreamSynchronize(P->stream));
     free_scratch(P);
     const int64_t elem = P->f64 ? 8 : 4;
-    const int64_t per_row = batched_floats_per_row(P) * elem + P->n_ev + static_cast<int64_t>(P->Q) * elem + elem;
+    // (+ a soft program's staged likelihoods and sum log(max))
+    const int64_t per_row = batched_floats_per_row(P) * elem + P->n_ev + static_cast<int64_t>(P->Q) * elem + elem +
+                            (P->soft.empty() ? 0 : P->n_lik * elem + 8);
     size_t free_b = 0, total_b = 0;
     SBN_CUDA(cudaMemGetInfo(&free_b, &total_b));
     const int64_t budget = static_cast<int64_t>(free_b * 0.85);
@@ -1615,6 +1691,10 @@ int sbn_program_reserve(sbn_program *P, int64_t max_rows) {
     }
     SBN_CUDA(cudaMalloc(&P->d_out, static_cast<size_t>(P->Q) * ld * (P->f64 ? 8 : 4)));
     SBN_CUDA(cudaMalloc(&P->d_total, static_cast<size_t>(ld) * (P->f64 ? 8 : 4)));
+    if (!P->soft.empty()) {
+        SBN_CUDA(cudaMalloc(&P->d_lik, static_cast<size_t>(ld) * P->n_lik * elem));
+        SBN_CUDA(cudaMalloc(&P->d_log_max, static_cast<size_t>(ld) * 8));
+    }
     SBN_CUDA(cudaStreamSynchronize(P->stream));  // the memset must not race a caller's stream
     P->reserved_rows = rows;
     P->ld = ld;
@@ -1763,6 +1843,68 @@ int sbn_program_evidence_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, 
 
 int sbn_program_evidence_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *prob) {
     return run_host_common(P, ev, ld_ev, n_rows, prob, n_rows, true, true);
+}
+
+// A posterior or marginals program with soft evidence: per chunk, the codes and (host) likelihoods are staged,
+// the pack fills the likelihood slots inside the run (captured graph or not), the posterior comes back, and
+// with `log_evidence` log P(e, lik) = log(normaliser) + sum log(max).  Never pipelined.
+static int run_soft_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const void *lik,
+                           int64_t ld_lik, int lik_on_device, void *out_, int64_t ld_out, double *log_evidence, bool f64) {
+    int rc = check_run_args(P, ev, ld_ev, n_rows, out_, ld_out, true);
+    if (rc != SBN_OK) return rc;
+    if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the run call");
+    if (!lik) return fail(SBN_E_INVALID, "null likelihoods");
+    if (ld_lik < P->n_lik) return fail(SBN_E_INVALID, "ld_lik %lld < the %d likelihood columns", (long long)ld_lik, P->n_lik);
+    if (log_evidence && P->kind == kMarginals)
+        return fail(SBN_E_INVALID, "a marginals program has no single normaliser; log P(e, lik) comes from a posterior program");
+    const size_t elem = f64 ? 8 : 4;
+    char *out = static_cast<char *>(out_);
+    const char *src = static_cast<const char *>(lik);
+    rc = reserve_rows(P, n_rows);
+    if (rc != SBN_OK) return rc;
+    const int64_t cap = P->reserved_rows;
+    std::vector<char> total(log_evidence ? static_cast<size_t>(cap) * elem : 0);
+    std::vector<double> log_max(log_evidence ? static_cast<size_t>(cap) : 0);
+    rc = for_each_chunk(P, ev, ld_ev, n_rows, cap, [&](int64_t r0, int64_t rows) -> int {
+        const char *chunk = src + r0 * ld_lik * static_cast<int64_t>(elem);
+        if (lik_on_device) {
+            P->lik = chunk;
+            P->ld_lik = ld_lik;
+        } else {
+            SBN_CUDA(cudaMemcpy2DAsync(P->d_lik, static_cast<size_t>(P->n_lik) * elem, chunk, static_cast<size_t>(ld_lik) * elem,
+                                       static_cast<size_t>(P->n_lik) * elem, static_cast<size_t>(rows), cudaMemcpyHostToDevice,
+                                       P->stream));
+            P->lik = P->d_lik;
+            P->ld_lik = P->n_lik;
+        }
+        const int rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
+        if (rc != SBN_OK) return rc;
+        SBN_CUDA(cudaMemcpy2DAsync(out + r0 * elem, static_cast<size_t>(ld_out) * elem, P->d_out, static_cast<size_t>(P->ld) * elem,
+                                   static_cast<size_t>(rows) * elem, static_cast<size_t>(P->Q), cudaMemcpyDeviceToHost, P->stream));
+        if (!log_evidence) return SBN_OK;
+        SBN_CUDA(cudaMemcpyAsync(total.data(), P->d_total, static_cast<size_t>(rows) * elem, cudaMemcpyDeviceToHost, P->stream));
+        SBN_CUDA(cudaMemcpyAsync(log_max.data(), P->d_log_max, static_cast<size_t>(rows) * 8, cudaMemcpyDeviceToHost, P->stream));
+        SBN_CUDA(cudaStreamSynchronize(P->stream));
+        for (int64_t i = 0; i < rows; ++i) {
+            const double t = f64 ? reinterpret_cast<const double *>(total.data())[i] : reinterpret_cast<const float *>(total.data())[i];
+            log_evidence[r0 + i] = std::log(t) + log_max[i];  // NaN where the normaliser is flagged
+        }
+        return SBN_OK;
+    });
+    P->lik = nullptr;  // a device pointer is the caller's: forget it
+    if (rc != SBN_OK) return rc;
+    SBN_CUDA(cudaStreamSynchronize(P->stream));
+    return SBN_OK;
+}
+
+int sbn_program_run_soft_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
+                              int64_t ld_lik, int lik_on_device, float *out, int64_t ld_out, double *log_evidence) {
+    return run_soft_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, out, ld_out, log_evidence, false);
+}
+
+int sbn_program_run_soft_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
+                                  int64_t ld_lik, int lik_on_device, double *out, int64_t ld_out, double *log_evidence) {
+    return run_soft_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, out, ld_out, log_evidence, true);
 }
 
 // The chunks of a counts call: P(observed) per chunk, then the batch's counts added into `counts`
@@ -2031,7 +2173,7 @@ int sbn_program_set_tiled(sbn_program *P, int enabled) {
     P->use_preload = enabled != 4;
     P->use_slab = enabled != 5;
     if (enabled == 8) P->use_tma = false;
-    if (enabled == 9) P->use_tma = true;
+    if (enabled == 9) P->use_tma = P->soft.empty();  // not planned for soft-evidence programs
     if (enabled == 6) P->use_chain = false;
     if (enabled == 7) P->use_chain = true;
     if (enabled == 10) P->use_pair = false;

@@ -102,9 +102,12 @@ struct GraphKey {
     const void *partial = nullptr;  // counts program: the per-warp partial tables
     const void *drawn = nullptr;    // sample / MPE program: the drawn-code buffer, its draws and pitch
     int64_t n_draws = 0, ld_drawn = 0;
+    const void *lik = nullptr;      // soft-evidence program: the likelihoods the pack reads, and their pitch
+    int64_t ld_lik = 0;
     bool operator==(const GraphKey &o) const {
         return ev == o.ev && out == o.out && ld_ev == o.ld_ev && n_rows == o.n_rows && ld_out == o.ld_out &&
-               partial == o.partial && drawn == o.drawn && n_draws == o.n_draws && ld_drawn == o.ld_drawn;
+               partial == o.partial && drawn == o.drawn && n_draws == o.n_draws && ld_drawn == o.ld_drawn &&
+               lik == o.lik && ld_lik == o.ld_lik;
     }
 };
 struct CachedGraph {
@@ -128,6 +131,16 @@ struct sbn_program {
     uint8_t *d_drawn = nullptr;   // sample program: drawn codes [n_sampled][n_draws][ld_drawn], then flags [ld_drawn]
     int64_t drawn_bytes = 0;
     uint32_t *d_sample_args = nullptr;  // seed lo, seed hi, row_base lo, row_base hi of the current chunk
+    // soft evidence (posterior and marginals programs, sbn_soft.cuh): (slot, card) of every likelihood, in
+    // likelihood-column order; their pack descriptors; the staging buffer of host likelihoods [reserved][n_lik]
+    // (double when f64) and sum log(max) [ld] of the last run; the likelihoods the next issue reads
+    std::vector<std::pair<int, int>> soft;
+    int n_lik = 0;
+    int32_t *d_soft = nullptr;
+    void *d_lik = nullptr;
+    double *d_log_max = nullptr;
+    const void *lik = nullptr;
+    int64_t ld_lik = 0;
     std::vector<std::pair<int64_t, int64_t>> tables;  // (offset, size) in floats
     std::vector<int64_t> table_padded;
     float *d_tables = nullptr;

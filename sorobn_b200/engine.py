@@ -16,7 +16,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libsorobn_
 _lib = None
 
 SBN_OK = 0
-ABI_VERSION = 13
+ABI_VERSION = 14
 
 
 class EngineError(RuntimeError):
@@ -74,6 +74,9 @@ def load():
         getattr(lib, name).restype = i32
         getattr(lib, name).argtypes = [vp, vp, i64, i64, i64, c.c_uint64, i64, vp, vp]
     lib.sbn_program_mpe_host.restype = i32
+    for name in ("sbn_program_run_soft_host", "sbn_program_run_soft_host_f64"):
+        getattr(lib, name).restype = i32
+        getattr(lib, name).argtypes = [vp, vp, i64, i64, vp, i64, i32, vp, i64, vp]
     lib.sbn_program_mpe_host.argtypes = [vp, vp, i64, i64, vp, vp]
     lib.sbn_program_destroy.restype = None
     lib.sbn_program_destroy.argtypes = [vp]
@@ -119,6 +122,7 @@ EXPORTS = (
     "sbn_program_reserve", "sbn_program_run_host", "sbn_program_run_device", "sbn_program_profile",
     "sbn_program_step_roles", "sbn_program_counts_host", "sbn_program_counts_host_f64", "sbn_program_set_tables",
     "sbn_program_set_tables_f64", "sbn_program_sample_host", "sbn_program_sample_host_f64", "sbn_program_mpe_host",
+    "sbn_program_run_soft_host", "sbn_program_run_soft_host_f64",
     "sbn_program_info", "sbn_program_set_graph", "sbn_program_set_tiled", "sbn_gibbs_create", "sbn_gibbs_run_host",
     "sbn_sampler_run_host", "sbn_gibbs_conditional", "sbn_gibbs_destroy", "sbn_host_alloc", "sbn_host_free",
 )
@@ -251,6 +255,39 @@ class Program:
             raise ValueError(f"out must be a C-contiguous {self.dtype.__name__} [Q, n_rows] array")
         _check(self._fn("sbn_program_run_host")(self._h, ev_ptr, n_rows, n_rows, out.ctypes.data, n_rows))
         return out
+
+    def run_soft(self, codes: np.ndarray, lik, n_rows: int, log_evidence: bool = False):
+        """Host path of a program with soft evidence (planner `soft=`): evidence codes uint8 [n_ev, n_rows] and
+        likelihoods [n_rows, n_lik] (one column per state of every soft variable, `plan.soft` order) in,
+        posterior [Q, n_rows] out, and with `log_evidence` also log P(e, lik) float64 [n_rows] (posterior
+        programs).  `lik` is a numpy array or a torch tensor; a CUDA tensor on the program's device is read
+        in place, with no host round trip."""
+        n_rows = int(n_rows)
+        codes, ev_ptr = self._evidence(codes, n_rows)
+        n_lik = sum(int(self.plan._card[v]) for v in self.plan.soft)
+        on_device = False
+        if type(lik).__module__.startswith("torch"):
+            if lik.is_cuda:
+                import torch
+
+                if lik.device.index != self.device:
+                    raise ValueError(f"likelihoods on cuda:{lik.device.index}; the program runs on cuda:{self.device}")
+                lik = lik.to(torch.float64 if self.f64 else torch.float32).contiguous()
+                torch.cuda.current_stream(lik.device).synchronize()  # the program's stream reads it next
+                on_device = True
+            else:
+                lik = lik.numpy()
+        if not on_device:
+            lik = np.ascontiguousarray(lik, dtype=self.dtype)
+        if tuple(lik.shape) != (n_rows, n_lik):
+            raise ValueError(f"likelihoods have shape {tuple(lik.shape)}, expected {(n_rows, n_lik)}")
+        out = np.empty((self.Q, n_rows), dtype=self.dtype)
+        log_ev = np.empty(n_rows, dtype=np.float64) if log_evidence else None
+        ptr = lik.data_ptr() if on_device else lik.ctypes.data
+        _check(self._fn("sbn_program_run_soft_host")(self._h, ev_ptr, n_rows, n_rows, ptr, n_lik, int(on_device),
+                                                      out.ctypes.data, n_rows,
+                                                      None if log_ev is None else log_ev.ctypes.data))
+        return (out, log_ev) if log_evidence else out
 
     def evidence(self, codes: np.ndarray, n_rows: int) -> np.ndarray:
         """P(event) per evidence row (the normaliser of the posterior), host path."""

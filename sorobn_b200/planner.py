@@ -26,9 +26,10 @@ number of evidence rows.  Each program step is one fused
 Program layout (int32 words) -- parsed by csrc/sbn_api.cu and by
 oracle/program_interp.py (the CPU checker used in tests):
 
-    header : MAGIC VERSION mode n_ev n_tables n_slots n_steps Q post_slot post_batched 0 0
+    header : MAGIC VERSION mode n_ev n_tables n_slots n_steps Q post_slot post_batched n_soft 0
     tables : (offset_floats, size) * n_tables         -- into the float table blob
     slots  : (batched, size_per_row) * n_slots        -- scratch buffers
+    soft   : (slot, card) * n_soft                    -- likelihood slots (versions 4 and 5 only)
     steps  : kind n_in out_slot n_axes n_elim | cards[n_axes] | ecards[n_elim] |
              per input: is_slot id batched n_ev (col stride card)*n_ev estrides[n_elim] strides[n_axes]
 
@@ -44,6 +45,14 @@ input that spans both tile axes.
 `mode` 0 = flat (one evidence row, nothing batched: evidence offsets are uniform),
 1 = batched.  The posterior is produced by the last step into `post_slot`
 (`[Q]` or `[Q, B]`, unnormalised) and normalised per row by the engine.
+
+Soft evidence (`soft=` of `build_plan` and `build_marginals_plan`, batched versions 4 and 5 only): every
+soft variable v carries a per-row likelihood lambda_v over its states, one batched leaf factor over (v)
+in a slot no step writes.  The engine fills those slots before step 0 of every run (csrc/sbn_soft.cuh),
+each row divided by its maximum, from the caller's `[n_rows][ld_lik]` likelihood matrix whose columns are
+the soft variables sorted by name, states in domain order.  Header word 10 is `n_soft`, and the soft
+section lists `(slot, card)` per soft variable in that column order.  With `n_soft = 0` the words are
+those of a plan without soft evidence.
 
 Marginals programs (`build_marginals_plan`, VERSION 5) answer P(t | e) for many targets t at
 once.  They use the same words, with two differences:
@@ -262,6 +271,8 @@ class Plan:
     table_axes: list = None  # var ids of every shipped table's axes, outermost first (refresh_tables)
     table_scopes: list = None  # the CPT scope [*parents, v] every table was transposed from
     sampled: tuple = ()  # sample / MPE plans: the var id of every drawn (decoded) code row, in drawing order
+    soft: tuple = ()  # soft-evidence var ids, sorted by name (== likelihood column order)
+    soft_slots: tuple = ()  # the slot of every soft variable's likelihood, in `soft` order
 
     # ---- cost model (DESIGN.md "algorithmic bytes") -------------------------------
     def bytes_per_row(self, n_draws=1):
@@ -295,6 +306,9 @@ class Plan:
         elif self.version in (VERSION_COUNTS, VERSION_SAMPLE, VERSION_MPE, VERSION_MAP):
             total += 4  # P(observed) (max log P(x, e)) out
         total += len(self.evidence)  # uint8 codes
+        if self.soft:
+            # the pack reads the caller's likelihoods, writes them to their slots and writes sum log(max)
+            total += 8 * sum(int(self._card[v]) for v in self.soft) + 8
         return total
 
     def step_bytes_per_row(self):
@@ -365,18 +379,35 @@ def _min_fill_order(scopes, hidden, card, first=None):
     return order
 
 
+def _check_soft(net, evidence, soft, mode):
+    """`soft` as var ids sorted by name (the likelihood column order); ValueError for a bad set."""
+    soft = tuple(soft)
+    if not soft:
+        return ()
+    if len(set(soft)) != len(soft):
+        raise ValueError("duplicate soft-evidence variable")
+    if set(soft) & set(evidence):
+        raise ValueError("a soft-evidence variable cannot also be a hard-evidence column")
+    if mode != MODE_BATCHED:
+        raise ValueError("soft evidence needs a batched plan")
+    return tuple(sorted(soft, key=lambda v: net.names[v]))
+
+
 def build_plan(net: CompiledNet, query, evidence, mode=MODE_BATCHED, order=None, max_in=MAX_IN,
-               merge_sum_outs=None, lift_evidence=True, allow_empty_query=False, fuse_elims=None) -> Plan:
+               merge_sum_outs=None, lift_evidence=True, allow_empty_query=False, fuse_elims=None, soft=()) -> Plan:
     """Plan P(query | evidence) for `net`.
 
     query / evidence are sequences of var ids.  `evidence` fixes the evidence
-    *columns*; their values arrive at run time.
+    *columns*; their values arrive at run time.  `soft` are the var ids whose per-row
+    likelihoods arrive at run time (soft evidence, see the module docstring); a soft
+    variable may be queried.
     """
     query, evidence = tuple(query), tuple(evidence)
+    soft = _check_soft(net, evidence, soft, mode)
     if not query and not allow_empty_query:
         # bayes_net.py:840-841
         raise ValueError("At least one query variable has to be specified")
-    if not query and not evidence:
+    if not query and not evidence and not soft:
         raise ValueError("nothing to compute: no query variable and no evidence")
     if set(query) & set(evidence):
         # bayes_net.py:843-845
@@ -384,16 +415,18 @@ def build_plan(net: CompiledNet, query, evidence, mode=MODE_BATCHED, order=None,
     if len(set(query)) != len(query):
         raise ValueError("duplicate variable in query or event")
     return _build(net, VERSION, evidence, query=query, mode=mode, order=order, max_in=max_in,
-                  lift_evidence=lift_evidence, fuse_elims=fuse_elims, merge_sum_outs=merge_sum_outs)
+                  lift_evidence=lift_evidence, fuse_elims=fuse_elims, merge_sum_outs=merge_sum_outs, soft=soft)
 
 
 def build_marginals_plan(net: CompiledNet, evidence, targets=None, mode=MODE_BATCHED, order=None, max_in=MAX_IN,
-                         lift_evidence=True, fuse_elims=None) -> Plan:
+                         lift_evidence=True, fuse_elims=None, soft=()) -> Plan:
     """Plan P(t | evidence) for every target t at once (a version-5 program, see the module docstring).
 
     `targets` defaults to every variable that is not evidence.  The posterior is the
-    concatenation of the targets' marginals, targets sorted by name, states in domain order."""
+    concatenation of the targets' marginals, targets sorted by name, states in domain order.
+    `soft` are the var ids with per-row likelihoods, as for `build_plan`; they may be targets."""
     evidence = tuple(evidence)
+    soft = _check_soft(net, evidence, soft, mode)
     if targets is None:
         targets = [v for v in range(len(net.names)) if v not in set(evidence)]
     targets = tuple(targets)
@@ -404,7 +437,7 @@ def build_marginals_plan(net: CompiledNet, evidence, targets=None, mode=MODE_BAT
     if len(set(targets)) != len(targets):
         raise ValueError("duplicate target variable")
     return _build(net, VERSION_MARGINALS, evidence, targets=targets, mode=mode, order=order, max_in=max_in,
-                  lift_evidence=lift_evidence, fuse_elims=fuse_elims)
+                  lift_evidence=lift_evidence, fuse_elims=fuse_elims, soft=soft)
 
 
 def build_counts_plan(net: CompiledNet, evidence, mode=MODE_BATCHED, order=None, max_in=MAX_IN, lift_evidence=True,
@@ -502,6 +535,7 @@ class _Builder:
         self.table_axes = []  # variable of every axis of table_arrays[t], outermost first
         self.next_id = 0
         self.summed = frozenset()  # marginal MAP plans: the variables a launch sums out by log-sum-exp
+        self.soft = ()  # (var id, logical id of its likelihood) per soft-evidence variable, sorted by name
 
     def size(self, vs):
         """Joint states of the variables `vs`."""
@@ -685,11 +719,13 @@ class _Builder:
         """Assign the slots, build the Plan and serialise it.  `post` is the factor the header's slot
         holds (None for a marginals plan: its readouts write the posterior)."""
         slots, where = _assign_slots(self.steps, keep_unbatched=(self.mode == MODE_BATCHED),
-                                     park_batched=(version == VERSION))
+                                     park_batched=(version == VERSION),
+                                     preset=[(lid, int(self.card[v])) for v, lid in self.soft])
         plan = Plan(mode=self.mode, query=query, evidence=self.evidence, order=list(self.order), tables=self.tables,
                     slots=slots, steps=self.steps, post_slot=-1 if post is None else where[post.buf], Q=Q,
                     version=version, table_axes=[list(a) for a in self.table_axes],
-                    table_scopes=[self.net.scope(v) for v in self.tables], **fields)
+                    table_scopes=[self.net.scope(v) for v in self.tables], soft=tuple(v for v, _ in self.soft),
+                    soft_slots=tuple(where[lid] for _, lid in self.soft), **fields)
         plan._card = self.card
         _serialise(plan, self.table_arrays)
         return plan
@@ -705,10 +741,12 @@ def _dense_strides(cards):
 
 
 def _build(net, version, evidence, query=(), targets=(), mode=MODE_BATCHED, order=None, max_in=MAX_IN,
-           lift_evidence=True, fuse_elims=None, merge_sum_outs=None):
+           lift_evidence=True, fuse_elims=None, merge_sum_outs=None, soft=()):
     """A plan of program `version` (VERSION, VERSION_MARGINALS, ...): the upward pass of variable
     elimination, then the kind's tail.  `targets` are kept relevant besides the query and the evidence:
-    a marginals plan reads them out, and counts, sample and MPE plans pass every unobserved variable."""
+    a marginals plan reads them out, and counts, sample and MPE plans pass every unobserved variable.
+    `soft` (sorted by name) adds one batched likelihood factor per variable, read from a slot no step
+    writes; it enters the variable's bucket, or the final product of a queried variable."""
     if fuse_elims is None:
         fuse_elims = os.environ.get("SOROBN_B200_FUSE", "1") == "1"
     if len(set(evidence)) != len(evidence):
@@ -719,7 +757,7 @@ def _build(net, version, evidence, query=(), targets=(), mode=MODE_BATCHED, orde
             raise ValueError(f"evidence variable {net.names[v]!r} has {card[v]} states; state codes are uint8")
 
     # bayes_net.py:763-766
-    relevant = {*query, *evidence, *targets}
+    relevant = {*query, *evidence, *targets, *soft}
     for v in list(relevant):
         relevant |= net.ancestors(v)
     hidden = relevant - set(query) - set(evidence)
@@ -747,6 +785,10 @@ def _build(net, version, evidence, query=(), targets=(), mode=MODE_BATCHED, orde
         if len(ev) > MAX_EV:
             raise ValueError(f"CPT of {net.names[v]!r} has {len(ev)} evidence axes; the kernel supports {MAX_EV}")
         factors.append(_Factor(False, t, tuple(u for u, _ in free), tuple(s for _, s in free), ev, False))
+    # the likelihoods: batched leaf factors over one variable each, under logical ids no step produces
+    b.soft = tuple((v, b.next_id + k) for k, v in enumerate(soft))
+    b.next_id += len(soft)
+    factors += [_Factor(True, lid, (v,), (1,), (), True) for v, lid in b.soft]
 
     if order is None:
         order = _min_fill_order([f.vars for f in factors], hidden, card, first=b.summed if b.summed else None)
@@ -1101,7 +1143,8 @@ def _depth_first_order(steps):
     by_id = {st.out_id: i for i, st in enumerate(steps)}
     children = []
     for st in steps:
-        children.append([by_id[f.buf] for f, _, _ in st.inputs if f.is_slot])
+        # a likelihood slot (soft evidence) is filled before the steps: no step produces it
+        children.append([by_id[f.buf] for f, _, _ in st.inputs if f.is_slot and f.buf in by_id])
     size = [int(np.prod(st.cards, dtype=np.int64)) if st.kind == KIND_BATCHED else 0 for st in steps]
     peak = [0] * len(steps)
     order_of = [None] * len(steps)
@@ -1135,7 +1178,7 @@ def _depth_first_order(steps):
     return out
 
 
-def _assign_slots(steps, keep_unbatched, park_batched):
+def _assign_slots(steps, keep_unbatched, park_batched, preset=()):
     """Physical scratch slots by liveness: an output slot is taken before the step's inputs
     are released (a launch never writes a buffer it reads), best fit among the free slots
     of the same kind, and an intermediate is released after its last consumer.  An
@@ -1152,7 +1195,10 @@ def _assign_slots(steps, keep_unbatched, park_batched):
     park_batched (posterior plans): the batched inputs of a batched step are released one batched
     step LATE.  The engine may run a step and its consumer as ONE launch that reads the first step's
     operand and writes the second step's output (csrc/sbn_pair.h), so those two must never share a
-    buffer; it plans such launches for posterior programs only."""
+    buffer; it plans such launches for posterior programs only.
+
+    preset: (logical id, size per row) of the batched operands written before step 0 (the likelihoods of soft
+    evidence): each takes its own slot first, live until its last reader."""
     remaining = {}  # logical id -> reads still to come
     for st in steps:
         for buf in [f.buf for f, _, _ in st.inputs if f.is_slot] + ([st.norm.buf] if st.norm is not None else []):
@@ -1181,6 +1227,8 @@ def _assign_slots(steps, keep_unbatched, park_batched):
             else:
                 slots[phys][2] = not (keep_unbatched and not slots[phys][0])
 
+    for lid, size in preset:
+        where[lid] = alloc(True, size)
     for st in steps:
         writes_slot = st.kind in (KIND_FLAT, KIND_BATCHED)
         if writes_slot:
@@ -1245,6 +1293,8 @@ def _serialise(plan: Plan, table_arrays):
             extra = [len(plan.sampled), 0]
     else:
         post = [-1, 0]  # the readouts write the posterior themselves
+    if plan.version in (VERSION, VERSION_MARGINALS):
+        extra = [len(plan.soft), 0]
     w = [MAGIC, plan.version, plan.mode, len(plan.evidence), len(plan.tables), len(plan.slots), len(plan.steps),
          plan.Q, *post, *extra]
     assert len(w) == HEADER_WORDS
@@ -1252,6 +1302,8 @@ def _serialise(plan: Plan, table_arrays):
         w += [o, s]
     for b, s in plan.slots:
         w += [int(b), s]
+    for v, s in zip(plan.soft, plan.soft_slots):
+        w += [s, int(plan._card[v])]
     for st in plan.steps:
         w += [st.kind, len(st.inputs), st.out_slot, len(st.cards), len(st.ecards)]
         if st.kind == KIND_MARGINAL:
