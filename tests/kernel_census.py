@@ -74,12 +74,23 @@ def variants(launches):
     width, slab and several-eliminated-variables flags; batched: inputs and preload width; pairs:
     the two coefficient modes; triples: the group axis (the CTA's second block dimension); the join
     kernel: its input combination; the readout of marginals programs: element type and accumulator
-    count, `marginal<float,2>` ... `marginal<double,8>`."""
+    count, `marginal<float,2>` ... `marginal<double,8>`.
+
+    The log-domain instantiations (MPE and marginal MAP programs) carry their policy as a trailing
+    template argument and get items of their own, never a sum-product one: `batched N_IN=k SbnMaxSum`,
+    `batched N_IN=k SbnLogSumExp`, `flat<float> SbnMaxSum`, `flat<float> SbnLogSumExp`, and `argmax`
+    for the decode step."""
     out = set()
     for name, block_y in launches:
         m = re.match(r"(\w+)(?:<(.*)>)?$", name)
         kernel, targs = m.group(1), _targs(m.group(2)) if m.group(2) else ()
-        if kernel == "sbn_step_tiled":
+        if kernel == "sbn_step_batched" and len(targs) == 3:
+            out.add(f"batched N_IN={targs[0]} {targs[2]}")
+        elif kernel == "sbn_step_flat" and len(targs) == 2:
+            out.add(f"flat<{targs[0]}> {targs[1]}")
+        elif kernel == "sbn_argmax_step":
+            out.add("argmax")
+        elif kernel == "sbn_step_tiled":
             nu, na, nb, nc, t, _v, cx, slab, mx = targs
             combo = f"({nu},{na},{nb},{nc})"
             if slab == "true":

@@ -300,3 +300,140 @@ def required_items():
 # The networks the marginals tests run (build_marginals): every case, plus a naive Bayes network whose
 # 17-state targets take the readout's multi-pass path next to a 5-state one.
 MARGINALS_CASES = [c["name"] for c in CASES] + [NAIVE_BAYES_12]
+
+
+# ---- log-domain programs: most probable explanation and marginal MAP ----------------------------------------
+
+# A naive Bayes network with 60 children: the first four (f00 ... f03) are the MAP variables, the other 56 are
+# observed, and the class is summed out.  log P(x_MAP, e) then lies far below float32's range (log FLT_MIN = -87.3), the
+# reason the log domain exists: -200.7 ... -125.1 over the rows of `evidence_rows` (float64 replay).
+NAIVE_BAYES_60 = "naive60s5x17_map4"
+NAIVE_BAYES_60_LOG_P = (-205.0, -120.0)
+
+# The MAP sets of every log-domain case (variable ids): one, two and four unobserved variables whose joint has
+# at most 4,096 states, drawn once by tests/test_gpu_map.map_sets(net, observed, seed=1).
+MAP_SETS = {
+    "dag9p2s4x1x4x4_seed54_q1-8_e2": [(5,), (5, 7), (1, 6, 7, 8)],
+    "dag16p4s5x8_seed63_single8-0_q14_e3": [(6,), (6, 10), (0, 1, 10, 14)],
+    "dag14p4s5x8_seed1_zeros_q10-13_e1": [(7,), (7, 10), (1, 2, 10, 13)],
+    "dag8p2s37x3x2_seed3_q0-3_e2": [(4,), (4, 6)],
+    "dag7p2s13x9x4_seed5_q6_e2": [(4,), (4, 5)],
+    "dag6p2s37x2_seed1_q2_e2": [(2,), (2, 5)],
+    "grid10x10s5_seed0_q99_e30": [(48,), (51, 74), (3, 13, 81, 95)],
+    "grid10x10s4_seed0_q99_e30": [(48,), (51, 74), (3, 13, 81, 95)],
+    "grid10x10s3_seed0_q99_e30": [(48,), (51, 74), (3, 13, 81, 95)],
+    "grid10x10s2_seed0_q99_e30": [(48,), (51, 74), (3, 13, 81, 95)],
+    "dag300p1s17_seed2_q0_e5": [(142,), (153, 226)],
+    "dag300p1s17_seed5_q0_e6": [(143,), (154, 227)],
+    "dag300p1s17_seed16_q0_e7": [(144,), (155, 228)],
+    "dag300p1s17_seed34_q0_e8": [(143,), (153, 227)],
+    "dag16p4s8_seed0_q15_e2": [(7,), (7, 12), (0, 1, 12, 15)],
+    "grid7x7s5_seed39_q48_e18": [(23,), (26, 37), (1, 8, 38, 44)],
+    "grid8x8s4x5_seed10_q63_e9": [(29,), (30, 46), (1, 9, 51, 60)],
+    "dag15p4s6_seed79_q7_e2": [(7,), (7, 11), (0, 1, 11, 14)],
+    "grid10x10s5_seed60_q99_e26": [(50,), (52, 74), (3, 14, 80, 95)],
+    "grid10x10s4x5_seed76_q99_e29": [(44,), (46, 78), (4, 13, 82, 96)],
+    "grid8x8s5_seed74_q63_e11": [(31,), (32, 48), (1, 8, 50, 59)],
+    "dag19p7s3_seed93_q12_e3": [(10,), (10, 15), (0, 3, 15, 18)],
+    NAIVE_BAYES_60: [(1, 2, 3, 4)],
+}
+LOG_DOMAIN_CASES = list(MAP_SETS)
+
+# Coverage items each log-domain case reaches on the GPU: the census of its MPE program and of its MAP programs,
+# and their log_domain_items.
+LOG_DOMAIN_CLAIMS = {
+    'dag9p2s4x1x4x4_seed54_q1-8_e2': ['argmax', 'argmax cz=1', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=4 SbnMaxSum', 'batched N_IN=5 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'dag16p4s5x8_seed63_single8-0_q14_e3': ['argmax', 'argmax cz=1', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=4 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'dag14p4s5x8_seed1_zeros_q10-13_e1': ['argmax', 'argmax unstaged tables', 'batched N_IN=1 SbnLogSumExp', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnLogSumExp', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=4 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'dag8p2s37x3x2_seed3_q0-3_e2': ['argmax', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=4 SbnMaxSum', 'batched N_IN=6 SbnMaxSum', 'flat<float> SbnMaxSum'],
+    'dag7p2s13x9x4_seed5_q6_e2': ['argmax', 'batched N_IN=3 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'dag6p2s37x2_seed1_q2_e2': ['argmax', 'batched N_IN=2 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'grid10x10s5_seed0_q99_e30': ['argmax', 'batched N_IN=1 SbnLogSumExp', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnLogSumExp', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=4 SbnLogSumExp', 'batched N_IN=4 SbnMaxSum', 'batched N_IN=5 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'grid10x10s4_seed0_q99_e30': ['argmax', 'batched N_IN=1 SbnLogSumExp', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnLogSumExp', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=5 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'grid10x10s3_seed0_q99_e30': ['argmax', 'batched N_IN=1 SbnLogSumExp', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnLogSumExp', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=5 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'grid10x10s2_seed0_q99_e30': ['argmax', 'batched N_IN=1 SbnLogSumExp', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnLogSumExp', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=5 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'dag300p1s17_seed2_q0_e5': ['argmax', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=5 SbnLogSumExp', 'batched N_IN=5 SbnMaxSum', 'batched N_IN=8 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'dag300p1s17_seed5_q0_e6': ['argmax', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=6 SbnLogSumExp', 'batched N_IN=6 SbnMaxSum', 'batched N_IN=7 SbnMaxSum', 'batched N_IN=8 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'dag300p1s17_seed16_q0_e7': ['argmax', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=7 SbnLogSumExp', 'batched N_IN=7 SbnMaxSum', 'batched N_IN=8 SbnMaxSum', 'flat<float> SbnMaxSum'],
+    'dag300p1s17_seed34_q0_e8': ['argmax', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=4 SbnMaxSum', 'batched N_IN=8 SbnLogSumExp', 'batched N_IN=8 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'dag16p4s8_seed0_q15_e2': ['argmax', 'argmax unstaged tables', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnLogSumExp', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=4 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum', 'log-domain unstaged tables'],
+    'grid7x7s5_seed39_q48_e18': ['argmax', 'batched N_IN=1 SbnLogSumExp', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnLogSumExp', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=5 SbnMaxSum', 'batched N_IN=6 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'grid8x8s4x5_seed10_q63_e9': ['argmax', 'batched N_IN=1 SbnLogSumExp', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnLogSumExp', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=4 SbnLogSumExp', 'batched N_IN=4 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'dag15p4s6_seed79_q7_e2': ['argmax', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnLogSumExp', 'batched N_IN=3 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'grid10x10s5_seed60_q99_e26': ['argmax', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnLogSumExp', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=5 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'grid10x10s4x5_seed76_q99_e29': ['argmax', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnLogSumExp', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=4 SbnMaxSum', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'grid8x8s5_seed74_q63_e11': ['argmax', 'batched N_IN=1 SbnLogSumExp', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnLogSumExp', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=4 SbnLogSumExp', 'flat<float> SbnLogSumExp', 'flat<float> SbnMaxSum'],
+    'dag19p7s3_seed93_q12_e3': ['argmax', 'batched N_IN=1 SbnLogSumExp', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=2 SbnMaxSum', 'batched N_IN=3 SbnLogSumExp', 'batched N_IN=3 SbnMaxSum', 'batched N_IN=4 SbnLogSumExp', 'batched N_IN=4 SbnMaxSum', 'flat<float> SbnMaxSum'],
+    NAIVE_BAYES_60: ['argmax', 'batched N_IN=1 SbnMaxSum', 'batched N_IN=2 SbnLogSumExp', 'batched N_IN=7 SbnMaxSum', 'batched N_IN=8 SbnMaxSum', 'flat<float> SbnMaxSum'],
+}
+
+
+# Rows of every log-domain program held to the float64 oracles (the first ones of `evidence_rows`: every edge
+# code, then forward samples).  The oracles take up to 0.1 s a row on the dag300 and grid cases.
+LOG_DOMAIN_ORACLE_ROWS = 160
+
+
+def build_log_domain(name, n_rows):
+    """(spec, CompiledNet, DenseNet, observed var ids (sorted: the evidence columns), evidence codes
+    [n_observed, n_rows] from `evidence_rows`) of a log-domain case: a corpus case's network with its evidence
+    variables observed, or NAIVE_BAYES_60.  Its MAP sets are MAP_SETS[name]."""
+    if name == NAIVE_BAYES_60:
+        spec, seed = naive_bayes(n_children=60), 0
+        observed = tuple(range(5, 61))
+    else:
+        case = next(c for c in CASES if c["name"] == name)
+        spec, seed = make_spec(case), case["seed"]
+        observed = tuple(sorted(case["evidence"]))
+    codes = evidence_rows(spec, [spec.nodes[v] for v in observed], n_rows, seed=seed)
+    return spec, compiled_net(spec), dense_net(spec), observed, codes
+
+
+SMEM_BUDGET = 64 * 1024  # bytes of tables one step or argmax launch stages (csrc: SBN_SMEM_BUDGET)
+
+
+def _leaves_a_table_in_global(plan, st):
+    """Whether the engine reads one of a step's unbatched operands from global memory (__ldg): it stages them in
+    input order while their sizes, padded to 4 floats, still fit SMEM_BUDGET, and skips one that does not, so one
+    launch can mix staged and unstaged tables (build_params and bind_operands, csrc/sbn_api.cu)."""
+    size = [n for _, n in plan.table_offsets]
+    staged, left = 0, False
+    for f, _, _ in st.inputs:
+        if f.batched:
+            continue
+        padded = -(-(plan.slots[f.buf][1] if f.is_slot else size[f.buf]) // 4) * 4
+        if (staged + padded) * 4 <= SMEM_BUDGET:
+            staged += padded
+        else:
+            left = True
+    return left
+
+
+def log_domain_items(plan):
+    """Coverage items of an MPE or marginal MAP plan, read from the plan: a batched step or an argmax step with a
+    table left in global memory, and an argmax step over a single-state bucket."""
+    out = set()
+    for st in plan.steps:
+        if st.kind == planner.KIND_BATCHED and _leaves_a_table_in_global(plan, st):
+            out.add("log-domain unstaged tables")
+        elif st.kind == planner.KIND_ARGMAX:
+            if _leaves_a_table_in_global(plan, st):
+                out.add("argmax unstaged tables")
+            if st.cx == 1:
+                out.add("argmax cz=1")
+    return out
+
+
+LOG_DOMAIN_PLAN_ITEMS = ("log-domain unstaged tables", "argmax unstaged tables", "argmax cz=1")
+
+
+def log_domain_required_items():
+    """Every coverage item the log-domain programs of LOG_DOMAIN_CASES must reach: each instantiation
+    launch_log_domain (csrc/sbn_api.cu) dispatches, the argmax step, and the plan items."""
+    req = {f"batched N_IN={n} {r}" for n in range(1, 9) for r in ("SbnMaxSum", "SbnLogSumExp")}
+    req |= {"flat<float> SbnMaxSum", "flat<float> SbnLogSumExp", "argmax"}
+    return req | set(LOG_DOMAIN_PLAN_ITEMS)
+
+
+# Required log-domain items no case reaches, with the reason.  Empty: every one is reached.  The GPU test fails
+# when a case reaches a listed item, so that it moves into that case's claims.
+LOG_DOMAIN_OPEN = {}
