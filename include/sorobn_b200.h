@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SBN_ABI_VERSION 14
+#define SBN_ABI_VERSION 15
 
 #define SBN_OK 0
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
@@ -163,6 +163,35 @@ int sbn_program_sample_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld
  * log_prob[b] = max over the MAP variables of log P(x_MAP, the row's observed cells). */
 int sbn_program_mpe_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
                          uint8_t *codes /* [n_decoded][n_rows] */, float *log_prob /* [n_rows] */);
+
+/* Soft evidence on counts, sample, MPE and marginal MAP programs planned with soft variables
+ * (planner.build_pattern_plan `soft=`): these calls run them, the calls above refuse them, and these
+ * refuse a program without soft variables.  `lik`, `ld_lik` and `lik_on_device` are those of
+ * sbn_program_run_soft_host; a soft variable is unobserved, with its probabilities weighted by lik.
+ * Counts and sample: the outputs of sbn_program_counts_host / sbn_program_sample_host given the observed
+ * cells and lik, with prob[b] = P(observed, lik / max) (every row of lik divided by its maximum, so the
+ * float32 range rule keeps its meaning) and `log_evidence` (double [n_rows], or null) = log P(observed,
+ * lik) = log prob[b] + sum_v log max lik_v, NaN where prob[b] is flagged.  The sample streams are those of
+ * sbn_program_sample_host: the draws depend only on (seed, row_base + b, d) and the program.
+ * MPE and MAP (float32 programs; the likelihood slots hold log(lik / max)): `lik` is double, so that any
+ * finite scale reaches the log intact; the codes of sbn_program_mpe_host, and log_prob[b] = the program's
+ * float32 maximum plus the double sum_v log max lik_v, log P(x*, e, lik) on the caller's scale; -inf for a row
+ * of probability zero (an all-zero lik_v makes one). */
+int sbn_program_counts_soft_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
+                                 int64_t ld_lik, int lik_on_device, double *counts, int64_t n_counts, float *prob,
+                                 double *log_evidence);
+int sbn_program_counts_soft_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
+                                     const double *lik, int64_t ld_lik, int lik_on_device, double *counts,
+                                     int64_t n_counts, double *prob, double *log_evidence);
+int sbn_program_sample_soft_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
+                                 int64_t ld_lik, int lik_on_device, int64_t n_draws, uint64_t seed, int64_t row_base,
+                                 uint8_t *out, float *prob, double *log_evidence);
+int sbn_program_sample_soft_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
+                                     const double *lik, int64_t ld_lik, int lik_on_device, int64_t n_draws,
+                                     uint64_t seed, int64_t row_base, uint8_t *out, double *prob, double *log_evidence);
+int sbn_program_mpe_soft_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
+                              int64_t ld_lik, int lik_on_device, uint8_t *codes /* [n_decoded][n_rows] */,
+                              double *log_prob /* [n_rows] */);
 
 /* Same with DEVICE buffers, asynchronous on `stream` (a cudaStream_t; NULL = default
  * stream).  n_rows must not exceed the reserved chunk size. */

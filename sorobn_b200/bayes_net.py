@@ -97,6 +97,16 @@ def _posterior_series(post, index, name):
     return pd.Series(post[keep], index=index[keep], name=name)
 
 
+def _lik_rows(lik, rows):
+    """The likelihood rows at positions `rows` of a `BayesNet._soft_matrix` matrix: a numpy fancy index, or a torch
+    index on the tensor's device."""
+    if isinstance(lik, np.ndarray):
+        return lik[rows]
+    import torch
+
+    return lik[torch.as_tensor(np.asarray(rows), device=lik.device)]
+
+
 def _check_possible(index, rows, impossible, consequence):
     """ValueError for the rows at positions `rows[impossible]` of a frame with `index`, whose observed cells have
     probability zero; `consequence` ends the message."""
@@ -378,7 +388,7 @@ class BayesNet:
         return self.partial_fit(X)
 
     # ------------------------------------------------------- expected counts / EM
-    def expected_counts(self, X: pd.DataFrame) -> dict:
+    def expected_counts(self, X: pd.DataFrame, likelihoods: dict | None = None) -> dict:
         """The E-step of expectation-maximisation: for every node v, the sum over the rows of `X` of
         P(v, parents(v) | the row's observed cells), computed on the GPU.
 
@@ -389,20 +399,28 @@ class BayesNet:
 
         Rows are grouped by missingness pattern (the set of observed columns); each pattern is one
         counts program (planner.build_counts_plan), so the cost grows with the number of distinct
-        patterns as well as with the rows."""
+        patterns as well as with the rows.
+
+        likelihoods: soft (virtual) evidence, {node: values} with one likelihood row per row of `X`, as in
+        `query_many`: the counts are then those of P(v, parents(v) | observed cells, likelihoods).  A soft
+        node may not be a column of `X`; a row whose cells and likelihoods have probability zero (an
+        all-zero likelihood row makes one) raises ValueError."""
         groups = self._count_patterns(X)
+        soft = self._pattern_soft(likelihoods, X)
         net = self._compiled
         offsets, n_counts = _planner.count_layout(net)
         # each pattern's programs are fetched right before they run: with more patterns than the cache holds,
         # fetching one may close the least recently used ones, which have run by then
-        counts, _ = self._e_step(X, groups, lambda k, ev: self._pattern_runner("counts", ev), n_counts)
+        counts, _ = self._e_step(X, groups, lambda k, ev: self._pattern_runner("counts", ev, soft=soft[0]), n_counts,
+                                 soft[1])
         out = {}
         for v, name in enumerate(net.names):
             size = int(np.prod(net.cpt[v].shape))
             out[name] = pd.Series(counts[offsets[v]:offsets[v] + size], index=self._family_index(v), name=name)
         return out
 
-    def fit_em(self, X: pd.DataFrame, max_iter: int = 100, tol: float = 1e-6) -> "BayesNet":
+    def fit_em(self, X: pd.DataFrame, max_iter: int = 100, tol: float = 1e-6,
+               likelihoods: dict | None = None) -> "BayesNet":
         """Fit the CPTs to `X` by expectation-maximisation, when cells are missing (None / NaN) or nodes
         are latent (no column in `X`).
 
@@ -415,7 +433,11 @@ class BayesNet:
         Iteration stops when the observed-data log-likelihood sum_b log P(observed cells of b) rises by
         less than `tol` per row, or after `max_iter` iterations.  The log-likelihood of every iteration
         is kept in `em_log_likelihood_`; `_P_sizes` holds the final expected counts, so a later
-        `partial_fit` continues from them."""
+        `partial_fit` continues from them.
+
+        likelihoods: soft evidence (e.g. probabilistic labels of a latent node), as in `expected_counts`.  They
+        stay fixed across the iterations, and `em_log_likelihood_` holds sum_b log P(observed cells of b,
+        likelihoods of b), on the scale of the given likelihoods."""
         if int(max_iter) < 1:
             raise ValueError(f"max_iter must be at least 1, not {max_iter}")
         if all(n in self.P for n in self.nodes):
@@ -428,10 +450,11 @@ class BayesNet:
             raise ValueError(f"fit_em needs initial CPTs in P when nodes have no column in X ({latent[:5]}): a latent "
                              "variable's states and a start that breaks its symmetry must come from the user")
         groups = self._count_patterns(X)
+        soft, lik = self._pattern_soft(likelihoods, X)
         net = self._compiled
         offsets, n_counts = _planner.count_layout(net)
         n_rows = len(X.index)
-        runners = [_Programs(_planner.build_counts_plan(net, ev), self.device) for ev, _, _ in groups]
+        runners = [_Programs(_planner.build_pattern_plan(net, "counts", ev, soft=soft), self.device) for ev, _, _ in groups]
         cpts = [np.array(c, dtype=np.float64) for c in net.cpt]
         lls = []
         try:
@@ -439,7 +462,7 @@ class BayesNet:
                 if it:
                     for r in runners:
                         r.set_cpts(cpts)
-                counts, ll = self._e_step(X, groups, lambda k, ev: runners[k], n_counts)
+                counts, ll = self._e_step(X, groups, lambda k, ev: runners[k], n_counts, lik)
                 lls.append(ll)
                 fam = [counts[offsets[v]:offsets[v] + c.size].reshape(c.shape) for v, c in enumerate(cpts)]
                 if self.prior_count:
@@ -516,12 +539,24 @@ class BayesNet:
             groups.append((ev, rows, np.ascontiguousarray(codes[[col_of[v] for v in ev]][:, rows])))
         return groups
 
-    def _pattern_runner(self, kind, ev, map_vars=None):
+    def _pattern_runner(self, kind, ev, map_vars=None, soft=()):
         """The cached programs of one missingness pattern, `kind` "counts", "sample", "mpe" or "map" (a "map"
-        plan is keyed by its MAP variables, sorted var ids, too)."""
+        plan is keyed by its MAP variables, sorted var ids, too), with the soft-evidence var ids `soft` (sorted
+        by name; part of the key only when there are any)."""
         extra = (map_vars,) if kind == "map" else ()
-        build = getattr(_planner, f"build_{kind}_plan")
-        return self._programs((kind, ev, *extra), lambda: build(self._compiled, ev, *extra))
+        if not soft:
+            build = getattr(_planner, f"build_{kind}_plan")
+            return self._programs((kind, ev, *extra), lambda: build(self._compiled, ev, *extra))
+        return self._programs((kind, ev, *extra, soft),
+                              lambda: _planner.build_pattern_plan(self._compiled, kind, ev, soft=soft, map_vars=map_vars))
+
+    def _pattern_soft(self, likelihoods, events, single=False):
+        """(soft-evidence var ids sorted by name, likelihoods [n, sum of cards]) of `likelihoods` for the rows of
+        the frame `events`, whose columns may not be soft nodes (`_soft_matrix`); ((), None) without them."""
+        if likelihoods is None:
+            return (), None
+        names, lik = self._soft_matrix(likelihoods, len(events.index), tuple(events.columns), single=single)
+        return tuple(self._compiled.index[n] for n in names), lik
 
     @staticmethod
     def _run_pattern(runner, run, codes, rows):
@@ -536,22 +571,35 @@ class BayesNet:
             again, prob[flagged] = run(runner.f64(), np.ascontiguousarray(codes[:, flagged]), rows[flagged])
         return out, prob, flagged, again
 
-    def _e_step(self, X, groups, runner_of, n_counts):
+    def _e_step(self, X, groups, runner_of, n_counts, lik=None):
         """(expected counts [n_counts], observed-data log-likelihood) of every pattern's rows;
-        `runner_of(k, observed var ids)` gives the programs of pattern k.  Rows the float32 program flags
-        are settled by the float64 one; rows still without a probability raise."""
+        `runner_of(k, observed var ids)` gives the programs of pattern k, and `lik` the likelihoods of every row
+        of `X` for programs with soft evidence (the log-likelihood is then sum log P(observed, lik)).  Rows the
+        float32 program flags are settled by the float64 one; rows still without a probability raise."""
         counts = np.zeros(n_counts, dtype=np.float64)
         ll = 0.0
+
+        def run(p, c, r):
+            if lik is None:
+                return p.counts(c, len(r))
+            cnt, prob, log_ev = p.counts(c, len(r), lik=_lik_rows(lik, r), log_evidence=True)
+            return (cnt, log_ev), prob
+
         for k, (ev, rows, codes) in enumerate(groups):
-            c, prob, _, again = self._run_pattern(runner_of(k, ev), lambda p, c, r: p.counts(c, len(r)), codes, rows)
+            c, prob, flagged, again = self._run_pattern(runner_of(k, ev), run, codes, rows)
+            if lik is not None:
+                c, log_ev = c
+                if again is not None:
+                    again, log_ev[flagged] = again
             counts += c
             if again is not None:
                 counts += again
             _check_possible(X.index, rows, np.isnan(prob), "their expected counts are undefined")
-            ll += float(np.log(prob).sum())
+            ll += float(np.log(prob).sum()) if lik is None else float(log_ev.sum())
         return counts, ll
 
-    def sample_many(self, events: pd.DataFrame, n: int = 1, seed: int | None = None) -> pd.DataFrame:
+    def sample_many(self, events: pd.DataFrame, n: int = 1, seed: int | None = None,
+                    likelihoods: dict | None = None) -> pd.DataFrame:
         """`n` exact draws of every unobserved variable from P(unobserved | the row's observed cells), for
         every row of `events`, computed on the GPU.
 
@@ -565,11 +613,15 @@ class BayesNet:
 
         Rows are grouped by missingness pattern; each pattern is one sample program
         (planner.build_sample_plan): the upward pass of variable elimination, then one draw per bucket
-        of the elimination, top-down (csrc/sbn_sample.cuh)."""
+        of the elimination, top-down (csrc/sbn_sample.cuh).
+
+        likelihoods: soft evidence, as in `expected_counts`: the draws come from P(unobserved | observed
+        cells, likelihoods), and the soft nodes are drawn too."""
         if int(n) < 1:
             raise ValueError(f"n must be at least 1, not {n}")
         n = int(n)
         groups = self._count_patterns(events)
+        soft, lik = self._pattern_soft(likelihoods, events)
         net = self._compiled
         seed = self._rng.getrandbits(64) if seed is None else int(seed) & (2**64 - 1)
         n_rows = len(events.index)
@@ -577,8 +629,8 @@ class BayesNet:
         for ev, rows, ev_codes in groups:
             # fetched right before it runs: with more patterns than the cache holds, fetching one may close
             # the least recently used programs, which have run by then
-            runner = self._pattern_runner("sample", ev)
-            drawn, prob, flagged, again = self._run_pattern(runner, lambda p, c, r: self._draw(p, c, r, n, seed),
+            runner = self._pattern_runner("sample", ev, soft=soft)
+            drawn, prob, flagged, again = self._run_pattern(runner, lambda p, c, r: self._draw(p, c, r, n, seed, lik),
                                                             ev_codes, rows)
             if again is not None:
                 drawn[:, :, flagged] = again
@@ -591,7 +643,7 @@ class BayesNet:
                                           names=[events.index.name, "draw"])
         return self._codes_frame(codes.reshape(len(net.names), -1), index)
 
-    def mpe_many(self, events: pd.DataFrame, return_log_proba: bool = False):
+    def mpe_many(self, events: pd.DataFrame, return_log_proba: bool = False, likelihoods: dict | None = None):
         """The most probable explanation of every row of `events`, computed on the GPU: the joint state of
         every unobserved variable that maximises P(unobserved, the row's observed cells).
 
@@ -607,17 +659,28 @@ class BayesNet:
         columns, the cost grows with the number of variables, not with their joint.  Rows are grouped by
         missingness pattern; each pattern is one MPE program (planner.build_mpe_plan): the upward pass of
         variable elimination in the log domain with max in place of sum, then one argmax per bucket,
-        top-down (csrc/sbn_mpe.cuh)."""
-        codes, _, log_p = self._decode(events, self._count_patterns(events), "mpe", "they have nothing to explain")
+        top-down (csrc/sbn_mpe.cuh).
+
+        likelihoods: soft evidence, as in `expected_counts` (noisy observations: Viterbi-style decoding).  The
+        soft nodes are decoded too, and the log probability is log P(explanation, observed cells, likelihoods)
+        on the scale of the given likelihoods."""
+        return self._mpe_frame(events, return_log_proba, likelihoods)
+
+    def mpe(self, event: dict, likelihoods: dict | None = None) -> pd.Series:
+        """The most probable explanation of one event: `mpe_many(pd.DataFrame([event])).iloc[0]`, a Series
+        indexed by node name.  likelihoods: soft evidence of the event, {node: a vector over the node's sorted
+        domain, or a {state: weight} dict}, as in `query`."""
+        return self._mpe_frame(pd.DataFrame([event]), False, likelihoods, single=True).iloc[0]
+
+    def _mpe_frame(self, events, return_log_proba, likelihoods, single=False):
+        groups = self._count_patterns(events)
+        soft = self._pattern_soft(likelihoods, events, single)
+        codes, _, log_p = self._decode(events, groups, "mpe", "they have nothing to explain", soft=soft)
         frame = self._codes_frame(codes, events.index)
         return (frame, pd.Series(log_p, index=events.index)) if return_log_proba else frame
 
-    def mpe(self, event: dict) -> pd.Series:
-        """The most probable explanation of one event: `mpe_many(pd.DataFrame([event])).iloc[0]`, a Series
-        indexed by node name."""
-        return self.mpe_many(pd.DataFrame([event])).iloc[0]
-
-    def map_many(self, events: pd.DataFrame, variables=None, return_log_proba: bool = False):
+    def map_many(self, events: pd.DataFrame, variables=None, return_log_proba: bool = False,
+                 likelihoods: dict | None = None):
         """The marginal MAP state of every row of `events`, computed on the GPU: the joint state of the MAP
         variables that maximises P(MAP variables, the row's observed cells), every other unobserved variable
         summed out.
@@ -638,8 +701,16 @@ class BayesNet:
         variables outside the MAP set are summed out, not maximised.  Rows are grouped by missingness pattern;
         each pattern is one marginal MAP program (planner.build_map_plan): the upward pass of variable
         elimination in the log domain, log-sum-exp over the summed variables, then max over the MAP ones,
-        then one argmax per MAP bucket, top-down."""
+        then one argmax per MAP bucket, top-down.
+
+        likelihoods: soft evidence, as in `expected_counts`.  With `variables=None` the soft nodes are summed
+        out; list one to decode it.  The log probability is then log P(MAP state, observed cells,
+        likelihoods) on the scale of the given likelihoods."""
+        return self._map_frame(events, variables, return_log_proba, likelihoods)
+
+    def _map_frame(self, events, variables, return_log_proba, likelihoods, single=False):
         groups = self._count_patterns(events)
+        soft = self._pattern_soft(likelihoods, events, single)
         net = self._compiled
         listed = None
         if variables is not None:
@@ -650,21 +721,23 @@ class BayesNet:
         columns = [net.index[c] for c in events.columns]
         chosen = sorted(columns) if listed is None else listed
         codes, known, log_p = self._decode(events, groups, "map", "they have no MAP state",
-                                           lambda ev: tuple(v for v in chosen if v not in ev))
+                                           lambda ev: tuple(v for v in chosen if v not in ev), soft)
         out_vars = sorted(set(columns) | set(listed or ()), key=lambda v: net.names[v])
         frame = self._codes_frame(codes, events.index, out_vars, known)
         return (frame, pd.Series(log_p, index=events.index)) if return_log_proba else frame
 
-    def map(self, event: dict, variables=None) -> pd.Series:
+    def map(self, event: dict, variables=None, likelihoods: dict | None = None) -> pd.Series:
         """The marginal MAP state of one event: `map_many(pd.DataFrame([event]), variables).iloc[0]`, a Series
-        indexed by node name."""
-        return self.map_many(pd.DataFrame([event]), variables).iloc[0]
+        indexed by node name.  likelihoods: soft evidence of the event, as in `mpe`."""
+        return self._map_frame(pd.DataFrame([event]), variables, False, likelihoods, single=True).iloc[0]
 
-    def _decode(self, events, groups, kind, consequence, map_vars_of=None):
+    def _decode(self, events, groups, kind, consequence, map_vars_of=None, soft=((), None)):
         """(codes [n_nodes, n], known [n_nodes, n] (observed or decoded), log P [n]) of the MPE (`kind` "mpe")
         or marginal MAP ("map") programs of the pattern groups of `events`: the observed codes copied through,
         the decoded ones in `plan.sampled` order.  MAP takes the MAP variables of a pattern from
-        `map_vars_of(observed var ids)` and skips a pattern that observes and decodes nothing (log P = log 1)."""
+        `map_vars_of(observed var ids)` and skips a pattern that observes and decodes nothing (log P = log 1)
+        unless there is soft evidence.  `soft` is `_pattern_soft`'s (var ids, likelihoods of every row)."""
+        soft, lik = soft
         net = self._compiled
         n_rows = len(events.index)
         codes = np.zeros((len(net.names), n_rows), dtype=np.uint8)
@@ -675,11 +748,14 @@ class BayesNet:
             for i, v in enumerate(ev):
                 codes[v][rows] = ev_codes[i]
                 known[v][rows] = True
-            if map_vars == () and not ev:
+            if map_vars == () and not ev and not soft:
                 continue
             # fetched right before it runs, as in `sample_many`
-            runner = self._pattern_runner(kind, ev, map_vars)
-            decoded, lp = getattr(runner.f32(), kind)(ev_codes, len(rows))
+            runner = self._pattern_runner(kind, ev, map_vars, soft)
+            if lik is None:
+                decoded, lp = getattr(runner.f32(), kind)(ev_codes, len(rows))
+            else:
+                decoded, lp = getattr(runner.f32(), kind)(ev_codes, len(rows), lik=_lik_rows(lik, rows))
             _check_possible(events.index, rows, ~(lp > -np.inf), consequence)
             for j, v in enumerate(runner.plan.sampled):
                 codes[v][rows] = decoded[j]
@@ -698,13 +774,17 @@ class BayesNet:
         return pd.DataFrame(columns, index=index).infer_objects().sort_index(axis="columns")
 
     @staticmethod
-    def _draw(program, ev_codes, rows, n, seed):
+    def _draw(program, ev_codes, rows, n, seed, lik=None):
         """(drawn codes [n_sampled, n, len(rows)], P(observed) float64) of the rows at positions `rows`
         (sorted): one call per run of consecutive positions, whose first position is the call's row_base,
-        so that a row's random stream is its position whatever the grouping."""
+        so that a row's random stream is its position whatever the grouping.  `lik` (the likelihoods of every
+        position, for a program with soft evidence) is sliced along with each run."""
         starts = np.flatnonzero(np.r_[True, np.diff(rows) != 1])
-        parts = [program.sample(np.ascontiguousarray(ev_codes[:, a:b]), b - a, n, seed, row_base=int(rows[a]))
-                 for a, b in zip(starts, np.r_[starts[1:], len(rows)])]
+        parts = []
+        for a, b in zip(starts, np.r_[starts[1:], len(rows)]):
+            soft = {} if lik is None else {"lik": lik[int(rows[a]):int(rows[a]) + b - a]}
+            parts.append(program.sample(np.ascontiguousarray(ev_codes[:, a:b]), b - a, n, seed, row_base=int(rows[a]),
+                                        **soft))
         return np.concatenate([d for d, _ in parts], axis=2), np.concatenate([p for _, p in parts]).astype(np.float64)
 
     def sample(self, n=1, init: dict | None = None, method="forward"):
@@ -1086,13 +1166,8 @@ class BayesNet:
             flagged |= np.isnan(log_ev) & ~bad
         rows = np.flatnonzero(flagged)
         if len(rows):
-            if isinstance(lik, np.ndarray):
-                sub = lik[rows]
-            else:
-                import torch
-
-                sub = lik[torch.as_tensor(rows, device=lik.device)]
-            again = entry.f64().run_soft(np.ascontiguousarray(codes[:, rows]), sub, len(rows), log_evidence=log_evidence)
+            again = entry.f64().run_soft(np.ascontiguousarray(codes[:, rows]), _lik_rows(lik, rows), len(rows),
+                                         log_evidence=log_evidence)
             if log_evidence:
                 post[:, rows], log_ev[rows] = again
             else:

@@ -126,9 +126,10 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
     }
     if (!marginals && ((P->slots[P->post_slot].batched ? 1 : 0) != P->post_batched || P->slots[P->post_slot].size < P->Q))
         return fail(SBN_E_INVALID, "posterior slot mismatch");
-    if (P->kind == kPosterior || marginals) {
-        // soft evidence: (slot, card) of every likelihood, filled before step 0 (sbn_soft.cuh)
-        const int n_soft = w[10];
+    {
+        // soft evidence: (slot, card) of every likelihood, filled before step 0 (sbn_soft.cuh); n_soft is word 10
+        // of versions 4 and 5, word 11 of the others (their word 10 holds n_counts / n_sampled)
+        const int n_soft = P->kind == kPosterior || marginals ? w[10] : w[11];
         if (n_soft < 0 || (n_soft > 0 && P->mode != 1) || !need(2LL * n_soft))
             return fail(SBN_E_INVALID, "bad soft-evidence section");
         for (int v = 0; v < n_soft; ++v) {
@@ -1133,13 +1134,22 @@ cudaError_t launch_normalise(sbn_program *P, float *d_out, int64_t ld_out, int64
     return cudaGetLastError();
 }
 
-// Soft-evidence program: fill the likelihood slots from P->lik (pitch P->ld_lik) and sum log(max) per row
+// Bytes per likelihood entry of a soft-evidence program: double for a float64 program and for the log-domain kinds,
+// whose pack takes the log of each double ratio (their programs are float only, so the caller's scale must not
+// pass through float32 first)
+inline size_t lik_elem(const sbn_program *P) { return P->f64 || sbn_log_domain(P->kind) ? 8 : 4; }
+
+// Soft-evidence program: fill the likelihood slots from P->lik (pitch P->ld_lik) and sum log(max) per row; the
+// log-domain kinds store log(lik / max)
 cudaError_t launch_soft_pack(sbn_program *P, int64_t n_rows, cudaStream_t stream) {
     P->launches++;
     const int threads = 256;
     const unsigned grid = static_cast<unsigned>((n_rows + threads - 1) / threads);
     const int32_t rows = static_cast<int32_t>(n_rows), n_soft = static_cast<int32_t>(P->soft.size());
-    if (P->f64)
+    if (sbn_log_domain(P->kind))  // MPE / MAP: log(lik / max) into the slots of a max-sum / log-sum-exp program
+        sbn_soft_pack_log<<<grid, threads, 0, stream>>>(static_cast<const double *>(P->lik), P->ld_lik, rows, n_soft,
+                                                        P->d_soft, P->d_arena, P->ld, P->d_log_max);
+    else if (P->f64)
         sbn_soft_pack<double><<<grid, threads, 0, stream>>>(static_cast<const double *>(P->lik), P->ld_lik, rows, n_soft,
                                                             P->d_soft, reinterpret_cast<double *>(P->d_arena), P->ld,
                                                             P->d_log_max);
@@ -1348,10 +1358,15 @@ int check_rows(const sbn_program *P, ProgramKind kind, const void *ev, int64_t l
     if (!P) return fail(SBN_E_INVALID, "null program");
     if ((P->kind == kMarginals ? kPosterior : P->kind == kMap ? kMpe : P->kind) != kind)
         return fail(SBN_E_INVALID, "a %s program runs through %s", name[P->kind], entry[P->kind]);
+    static const char *const soft_entry[] = {"sbn_program_run_soft_host", "sbn_program_run_soft_host",
+                                             "sbn_program_counts_soft_host", "sbn_program_sample_soft_host",
+                                             "sbn_program_mpe_soft_host", "sbn_program_mpe_soft_host"};
+    static const char *const plain_entry[] = {"sbn_program_run_host", "sbn_program_run_host", "sbn_program_counts_host",
+                                              "sbn_program_sample_host", "sbn_program_mpe_host", "sbn_program_mpe_host"};
     if (!P->soft.empty() && !soft)
-        return fail(SBN_E_INVALID, "a %s program with soft evidence runs through sbn_program_run_soft_host", name[P->kind]);
+        return fail(SBN_E_INVALID, "a %s program with soft evidence runs through %s", name[P->kind], soft_entry[P->kind]);
     if (P->soft.empty() && soft)
-        return fail(SBN_E_INVALID, "a %s program without soft evidence runs through sbn_program_run_host", name[P->kind]);
+        return fail(SBN_E_INVALID, "a %s program without soft evidence runs through %s", name[P->kind], plain_entry[P->kind]);
     if (n_rows <= 0) return fail(SBN_E_INVALID, "n_rows must be positive");
     if (P->n_ev > 0 && !ev) return fail(SBN_E_INVALID, "null evidence");
     if (P->n_ev > 1 && ld_ev < n_rows) return fail(SBN_E_INVALID, "ld_ev < n_rows");
@@ -1660,7 +1675,7 @@ int sbn_program_reserve(sbn_program *P, int64_t max_rows) {
     const int64_t elem = P->f64 ? 8 : 4;
     // (+ a soft program's staged likelihoods and sum log(max))
     const int64_t per_row = batched_floats_per_row(P) * elem + P->n_ev + static_cast<int64_t>(P->Q) * elem + elem +
-                            (P->soft.empty() ? 0 : P->n_lik * elem + 8);
+                            (P->soft.empty() ? 0 : P->n_lik * static_cast<int64_t>(lik_elem(P)) + 8);
     size_t free_b = 0, total_b = 0;
     SBN_CUDA(cudaMemGetInfo(&free_b, &total_b));
     const int64_t budget = static_cast<int64_t>(free_b * 0.85);
@@ -1692,7 +1707,7 @@ int sbn_program_reserve(sbn_program *P, int64_t max_rows) {
     SBN_CUDA(cudaMalloc(&P->d_out, static_cast<size_t>(P->Q) * ld * (P->f64 ? 8 : 4)));
     SBN_CUDA(cudaMalloc(&P->d_total, static_cast<size_t>(ld) * (P->f64 ? 8 : 4)));
     if (!P->soft.empty()) {
-        SBN_CUDA(cudaMalloc(&P->d_lik, static_cast<size_t>(ld) * P->n_lik * elem));
+        SBN_CUDA(cudaMalloc(&P->d_lik, static_cast<size_t>(ld) * P->n_lik * lik_elem(P)));
         SBN_CUDA(cudaMalloc(&P->d_log_max, static_cast<size_t>(ld) * 8));
     }
     SBN_CUDA(cudaStreamSynchronize(P->stream));  // the memset must not race a caller's stream
@@ -1845,6 +1860,49 @@ int sbn_program_evidence_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_
     return run_host_common(P, ev, ld_ev, n_rows, prob, n_rows, true, true);
 }
 
+// The caller's likelihoods of a soft-evidence call ([n_rows][ld_lik], host memory or, with `on_device`, device memory
+// of the program's device) and, when `log_max` is set, where sum log(max) of every row goes (host, [n_rows])
+struct SoftLik {
+    bool soft = false;  // false: a call without soft evidence
+    const void *lik = nullptr;
+    int64_t ld_lik = 0;
+    int on_device = 0;
+    double *log_max = nullptr;
+};
+
+static int check_lik(const sbn_program *P, const SoftLik &s) {
+    if (!s.soft) return SBN_OK;
+    if (!s.lik) return fail(SBN_E_INVALID, "null likelihoods");
+    if (s.ld_lik < P->n_lik) return fail(SBN_E_INVALID, "ld_lik %lld < the %d likelihood columns", (long long)s.ld_lik, P->n_lik);
+    return SBN_OK;
+}
+
+// Point the next issue at rows [r0, r0 + rows) of the likelihoods: a device pointer in place, host rows copied into
+// the staging buffer (on the program's stream, ahead of the run)
+static int stage_lik(sbn_program *P, const SoftLik &s, int64_t r0, int64_t rows) {
+    if (!s.soft) return SBN_OK;
+    const size_t elem = lik_elem(P);
+    const char *chunk = static_cast<const char *>(s.lik) + r0 * s.ld_lik * static_cast<int64_t>(elem);
+    if (s.on_device) {
+        P->lik = chunk;
+        P->ld_lik = s.ld_lik;
+    } else {
+        SBN_CUDA(cudaMemcpy2DAsync(P->d_lik, static_cast<size_t>(P->n_lik) * elem, chunk, static_cast<size_t>(s.ld_lik) * elem,
+                                   static_cast<size_t>(P->n_lik) * elem, static_cast<size_t>(rows), cudaMemcpyHostToDevice,
+                                   P->stream));
+        P->lik = P->d_lik;
+        P->ld_lik = P->n_lik;
+    }
+    return SBN_OK;
+}
+
+// After a chunk's run: its rows' sum log(max), when the caller asked for them
+static int fetch_log_max(sbn_program *P, const SoftLik &s, int64_t r0, int64_t rows) {
+    if (s.soft && s.log_max)
+        SBN_CUDA(cudaMemcpyAsync(s.log_max + r0, P->d_log_max, static_cast<size_t>(rows) * 8, cudaMemcpyDeviceToHost, P->stream));
+    return SBN_OK;
+}
+
 // A posterior or marginals program with soft evidence: per chunk, the codes and (host) likelihoods are staged,
 // the pack fills the likelihood slots inside the run (captured graph or not), the posterior comes back, and
 // with `log_evidence` log P(e, lik) = log(normaliser) + sum log(max).  Never pipelined.
@@ -1853,31 +1911,22 @@ static int run_soft_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int
     int rc = check_run_args(P, ev, ld_ev, n_rows, out_, ld_out, true);
     if (rc != SBN_OK) return rc;
     if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the run call");
-    if (!lik) return fail(SBN_E_INVALID, "null likelihoods");
-    if (ld_lik < P->n_lik) return fail(SBN_E_INVALID, "ld_lik %lld < the %d likelihood columns", (long long)ld_lik, P->n_lik);
+    const SoftLik soft = {true, lik, ld_lik, lik_on_device, nullptr};
+    rc = check_lik(P, soft);
+    if (rc != SBN_OK) return rc;
     if (log_evidence && P->kind == kMarginals)
         return fail(SBN_E_INVALID, "a marginals program has no single normaliser; log P(e, lik) comes from a posterior program");
     const size_t elem = f64 ? 8 : 4;
     char *out = static_cast<char *>(out_);
-    const char *src = static_cast<const char *>(lik);
     rc = reserve_rows(P, n_rows);
     if (rc != SBN_OK) return rc;
     const int64_t cap = P->reserved_rows;
     std::vector<char> total(log_evidence ? static_cast<size_t>(cap) * elem : 0);
     std::vector<double> log_max(log_evidence ? static_cast<size_t>(cap) : 0);
     rc = for_each_chunk(P, ev, ld_ev, n_rows, cap, [&](int64_t r0, int64_t rows) -> int {
-        const char *chunk = src + r0 * ld_lik * static_cast<int64_t>(elem);
-        if (lik_on_device) {
-            P->lik = chunk;
-            P->ld_lik = ld_lik;
-        } else {
-            SBN_CUDA(cudaMemcpy2DAsync(P->d_lik, static_cast<size_t>(P->n_lik) * elem, chunk, static_cast<size_t>(ld_lik) * elem,
-                                       static_cast<size_t>(P->n_lik) * elem, static_cast<size_t>(rows), cudaMemcpyHostToDevice,
-                                       P->stream));
-            P->lik = P->d_lik;
-            P->ld_lik = P->n_lik;
-        }
-        const int rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
+        int rc = stage_lik(P, soft, r0, rows);
+        if (rc != SBN_OK) return rc;
+        rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
         if (rc != SBN_OK) return rc;
         SBN_CUDA(cudaMemcpy2DAsync(out + r0 * elem, static_cast<size_t>(ld_out) * elem, P->d_out, static_cast<size_t>(P->ld) * elem,
                                    static_cast<size_t>(rows) * elem, static_cast<size_t>(P->Q), cudaMemcpyDeviceToHost, P->stream));
@@ -1909,15 +1958,17 @@ int sbn_program_run_soft_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_
 
 // The chunks of a counts call: P(observed) per chunk, then the batch's counts added into `counts`
 static int add_expected_counts(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, void *prob,
-                               size_t elem) {
+                               size_t elem, const SoftLik &soft) {
     SBN_CUDA(cudaMemsetAsync(P->d_counts, 0, static_cast<size_t>(P->n_counts) * 8, P->stream));
     const int rc = for_each_chunk(P, ev, ld_ev, n_rows, P->reserved_rows, [&](int64_t r0, int64_t rows) -> int {
+        int rc = stage_lik(P, soft, r0, rows);
+        if (rc != SBN_OK) return rc;
         // the graph reads the tables and the count table by address, so it replays the values sbn_program_set_tables uploads
-        const int rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
+        rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
         if (rc != SBN_OK) return rc;
         SBN_CUDA(cudaMemcpyAsync(static_cast<char *>(prob) + r0 * elem, P->d_out, static_cast<size_t>(rows) * elem,
                                  cudaMemcpyDeviceToHost, P->stream));
-        return SBN_OK;
+        return fetch_log_max(P, soft, r0, rows);
     });
     if (rc != SBN_OK) return rc;
     std::vector<double> h(static_cast<size_t>(P->n_counts));
@@ -1928,8 +1979,10 @@ static int add_expected_counts(sbn_program *P, const uint8_t *ev, int64_t ld_ev,
 }
 
 static int counts_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, int64_t n_counts,
-                              void *prob, bool f64) {
-    int rc = check_rows(P, kCounts, ev, ld_ev, n_rows);
+                              void *prob, bool f64, const SoftLik &soft = {}) {
+    int rc = check_rows(P, kCounts, ev, ld_ev, n_rows, soft.soft);
+    if (rc != SBN_OK) return rc;
+    rc = check_lik(P, soft);
     if (rc != SBN_OK) return rc;
     if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the counts call");
     if (!counts || !prob) return fail(SBN_E_INVALID, "null output");
@@ -1946,11 +1999,41 @@ static int counts_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, 
                         (long long)(P->partial_doubles * 8), cudaGetErrorString(e));
         }
     }
-    rc = add_expected_counts(P, ev, ld_ev, n_rows, counts, prob, f64 ? 8 : 4);
+    rc = add_expected_counts(P, ev, ld_ev, n_rows, counts, prob, f64 ? 8 : 4, soft);
     cudaStreamSynchronize(P->stream);  // nothing may still read the partial tables
     cudaFree(P->d_partial);
     P->d_partial = nullptr;
+    P->lik = nullptr;  // a device pointer is the caller's: forget it
     return rc;
+}
+
+// log P(observed, lik) = log P(observed, lik / max) + sum log(max) of every row: NaN where `prob` is flagged
+static void add_log_max(const void *prob, bool f64, const std::vector<double> &log_max, double *log_evidence) {
+    for (size_t i = 0; i < log_max.size(); ++i) {
+        const double p = f64 ? static_cast<const double *>(prob)[i] : static_cast<const float *>(prob)[i];
+        log_evidence[i] = std::log(p) + log_max[i];
+    }
+}
+
+static int counts_soft_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const void *lik, int64_t ld_lik,
+                              int lik_on_device, double *counts, int64_t n_counts, void *prob, double *log_evidence, bool f64) {
+    std::vector<double> log_max(log_evidence && n_rows > 0 ? static_cast<size_t>(n_rows) : 0);
+    const SoftLik soft = {true, lik, ld_lik, lik_on_device, log_evidence ? log_max.data() : nullptr};
+    const int rc = counts_host_common(P, ev, ld_ev, n_rows, counts, n_counts, prob, f64, soft);
+    if (rc == SBN_OK && log_evidence) add_log_max(prob, f64, log_max, log_evidence);
+    return rc;
+}
+
+int sbn_program_counts_soft_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
+                                 int64_t ld_lik, int lik_on_device, double *counts, int64_t n_counts, float *prob,
+                                 double *log_evidence) {
+    return counts_soft_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, counts, n_counts, prob, log_evidence, false);
+}
+
+int sbn_program_counts_soft_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
+                                     int64_t ld_lik, int lik_on_device, double *counts, int64_t n_counts, double *prob,
+                                     double *log_evidence) {
+    return counts_soft_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, counts, n_counts, prob, log_evidence, true);
 }
 
 int sbn_program_counts_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, int64_t n_counts,
@@ -1995,8 +2078,11 @@ int sbn_program_set_tables_f64(sbn_program *P, const double *tables, int64_t n_t
 // decoded codes of a chunk are the drawn-code buffer, the per-row output is P(observed) (sample) or max log P(x, e)
 // (MPE; max log P(x_MAP, e) for MAP).
 static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws, uint64_t seed,
-                              int64_t row_base, uint8_t *out, void *prob, bool f64, ProgramKind kind = kSample) {
-    int rc = check_rows(P, kind, ev, ld_ev, n_rows);
+                              int64_t row_base, uint8_t *out, void *prob, bool f64, ProgramKind kind = kSample,
+                              const SoftLik &soft = {}) {
+    int rc = check_rows(P, kind, ev, ld_ev, n_rows, soft.soft);
+    if (rc != SBN_OK) return rc;
+    rc = check_lik(P, soft);
     if (rc != SBN_OK) return rc;
     if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the sample call");
     if (n_draws <= 0 || n_draws > INT32_MAX) return fail(SBN_E_INVALID, "n_draws must be in 1 .. 2^31 - 1");
@@ -2039,7 +2125,11 @@ static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, 
         const uint32_t args[4] = {static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32), static_cast<uint32_t>(first),
                                   static_cast<uint32_t>(first >> 32)};
         if (!mpe) SBN_CUDA(cudaMemcpyAsync(P->d_sample_args, args, sizeof args, cudaMemcpyHostToDevice, P->stream));
-        const int rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream, dc);
+        int rc = stage_lik(P, soft, r0, rows);
+        if (rc != SBN_OK) return rc;
+        rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream, dc);
+        if (rc != SBN_OK) return rc;
+        rc = fetch_log_max(P, soft, r0, rows);
         if (rc != SBN_OK) return rc;
         if (P->n_sampled > 0)
             SBN_CUDA(cudaMemcpy2DAsync(out + r0, static_cast<size_t>(n_rows), P->d_drawn, static_cast<size_t>(dc.ld_drawn),
@@ -2052,6 +2142,7 @@ static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, 
             SBN_CUDA(cudaMemcpyAsync(prob, ps.ptr, elem, cudaMemcpyDeviceToHost, P->stream));
         return SBN_OK;
     });
+    P->lik = nullptr;  // a device pointer is the caller's: forget it
     if (rc != SBN_OK) return rc;
     SBN_CUDA(cudaStreamSynchronize(P->stream));
     if (mpe && !ps.batched) std::fill(static_cast<float *>(prob) + 1, static_cast<float *>(prob) + n_rows, *static_cast<float *>(prob));
@@ -2070,6 +2161,43 @@ int sbn_program_sample_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev
 
 int sbn_program_mpe_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, uint8_t *codes, float *log_prob) {
     return sample_host_common(P, ev, ld_ev, n_rows, 1, 0, 0, codes, log_prob, false, kMpe);
+}
+
+static int sample_soft_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const void *lik, int64_t ld_lik,
+                              int lik_on_device, int64_t n_draws, uint64_t seed, int64_t row_base, uint8_t *out, void *prob,
+                              double *log_evidence, bool f64) {
+    std::vector<double> log_max(log_evidence && n_rows > 0 ? static_cast<size_t>(n_rows) : 0);
+    const SoftLik soft = {true, lik, ld_lik, lik_on_device, log_evidence ? log_max.data() : nullptr};
+    const int rc = sample_host_common(P, ev, ld_ev, n_rows, n_draws, seed, row_base, out, prob, f64, kSample, soft);
+    if (rc == SBN_OK && log_evidence) add_log_max(prob, f64, log_max, log_evidence);
+    return rc;
+}
+
+int sbn_program_sample_soft_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
+                                 int64_t ld_lik, int lik_on_device, int64_t n_draws, uint64_t seed, int64_t row_base,
+                                 uint8_t *out, float *prob, double *log_evidence) {
+    return sample_soft_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, n_draws, seed, row_base, out, prob,
+                              log_evidence, false);
+}
+
+int sbn_program_sample_soft_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
+                                     int64_t ld_lik, int lik_on_device, int64_t n_draws, uint64_t seed, int64_t row_base,
+                                     uint8_t *out, double *prob, double *log_evidence) {
+    return sample_soft_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, n_draws, seed, row_base, out, prob,
+                              log_evidence, true);
+}
+
+int sbn_program_mpe_soft_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
+                              int64_t ld_lik, int lik_on_device, uint8_t *codes, double *log_prob) {
+    if (!log_prob) return fail(SBN_E_INVALID, "null output");
+    // the program's float32 max log P(x, e, lik / max), then the double sum log(max) added back
+    std::vector<float> lp(n_rows > 0 ? static_cast<size_t>(n_rows) : 0);
+    std::vector<double> log_max(lp.size());
+    const SoftLik soft = {true, lik, ld_lik, lik_on_device, log_max.data()};
+    const int rc = sample_host_common(P, ev, ld_ev, n_rows, 1, 0, 0, codes, lp.data(), false, kMpe, soft);
+    if (rc != SBN_OK) return rc;
+    for (size_t i = 0; i < lp.size(); ++i) log_prob[i] = static_cast<double>(lp[i]) + log_max[i];
+    return SBN_OK;
 }
 
 int sbn_program_profile(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out,

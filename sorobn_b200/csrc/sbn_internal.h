@@ -131,7 +131,7 @@ struct sbn_program {
     uint8_t *d_drawn = nullptr;   // sample program: drawn codes [n_sampled][n_draws][ld_drawn], then flags [ld_drawn]
     int64_t drawn_bytes = 0;
     uint32_t *d_sample_args = nullptr;  // seed lo, seed hi, row_base lo, row_base hi of the current chunk
-    // soft evidence (posterior and marginals programs, sbn_soft.cuh): (slot, card) of every likelihood, in
+    // soft evidence (any batched program, sbn_soft.cuh): (slot, card) of every likelihood, in
     // likelihood-column order; their pack descriptors; the staging buffer of host likelihoods [reserved][n_lik]
     // (double when f64) and sum log(max) [ld] of the last run; the likelihoods the next issue reads
     std::vector<std::pair<int, int>> soft;

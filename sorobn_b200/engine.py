@@ -16,7 +16,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libsorobn_
 _lib = None
 
 SBN_OK = 0
-ABI_VERSION = 14
+ABI_VERSION = 15
 
 
 class EngineError(RuntimeError):
@@ -78,6 +78,14 @@ def load():
         getattr(lib, name).restype = i32
         getattr(lib, name).argtypes = [vp, vp, i64, i64, vp, i64, i32, vp, i64, vp]
     lib.sbn_program_mpe_host.argtypes = [vp, vp, i64, i64, vp, vp]
+    for name in ("sbn_program_counts_soft_host", "sbn_program_counts_soft_host_f64"):
+        getattr(lib, name).restype = i32
+        getattr(lib, name).argtypes = [vp, vp, i64, i64, vp, i64, i32, vp, i64, vp, vp]
+    for name in ("sbn_program_sample_soft_host", "sbn_program_sample_soft_host_f64"):
+        getattr(lib, name).restype = i32
+        getattr(lib, name).argtypes = [vp, vp, i64, i64, vp, i64, i32, i64, c.c_uint64, i64, vp, vp, vp]
+    lib.sbn_program_mpe_soft_host.restype = i32
+    lib.sbn_program_mpe_soft_host.argtypes = [vp, vp, i64, i64, vp, i64, i32, vp, vp]
     lib.sbn_program_destroy.restype = None
     lib.sbn_program_destroy.argtypes = [vp]
     lib.sbn_program_reserve.restype = i32
@@ -122,7 +130,9 @@ EXPORTS = (
     "sbn_program_reserve", "sbn_program_run_host", "sbn_program_run_device", "sbn_program_profile",
     "sbn_program_step_roles", "sbn_program_counts_host", "sbn_program_counts_host_f64", "sbn_program_set_tables",
     "sbn_program_set_tables_f64", "sbn_program_sample_host", "sbn_program_sample_host_f64", "sbn_program_mpe_host",
-    "sbn_program_run_soft_host", "sbn_program_run_soft_host_f64",
+    "sbn_program_run_soft_host", "sbn_program_run_soft_host_f64", "sbn_program_counts_soft_host",
+    "sbn_program_counts_soft_host_f64", "sbn_program_sample_soft_host", "sbn_program_sample_soft_host_f64",
+    "sbn_program_mpe_soft_host",
     "sbn_program_info", "sbn_program_set_graph", "sbn_program_set_tiled", "sbn_gibbs_create", "sbn_gibbs_run_host",
     "sbn_sampler_run_host", "sbn_gibbs_conditional", "sbn_gibbs_destroy", "sbn_host_alloc", "sbn_host_free",
 )
@@ -264,7 +274,22 @@ class Program:
         in place, with no host round trip."""
         n_rows = int(n_rows)
         codes, ev_ptr = self._evidence(codes, n_rows)
+        lik, lik_args = self._likelihoods(lik, n_rows)
+        out = np.empty((self.Q, n_rows), dtype=self.dtype)
+        log_ev = np.empty(n_rows, dtype=np.float64) if log_evidence else None
+        _check(self._fn("sbn_program_run_soft_host")(self._h, ev_ptr, n_rows, n_rows, *lik_args, out.ctypes.data, n_rows,
+                                                      None if log_ev is None else log_ev.ctypes.data))
+        return (out, log_ev) if log_evidence else out
+
+    def _likelihoods(self, lik, n_rows):
+        """(the likelihoods [n_rows, n_lik], C-contiguous, and the call's (pointer, ld_lik, on-device flag)) of a
+        numpy array or a torch tensor; a CUDA tensor on the program's device is read in place, with no host round
+        trip.  ValueError for another shape or device.  Keep the first alive until the call returns.  The
+        likelihoods take the program's type, except that the float32 MPE and MAP programs take them in float64:
+        their pack takes the log of each ratio in double, and no float64 twin would rescue a row whose scale
+        float32 cannot hold."""
         n_lik = sum(int(self.plan._card[v]) for v in self.plan.soft)
+        f64 = self.f64 or self.plan.version in (8, 9)
         on_device = False
         if type(lik).__module__.startswith("torch"):
             if lik.is_cuda:
@@ -272,22 +297,16 @@ class Program:
 
                 if lik.device.index != self.device:
                     raise ValueError(f"likelihoods on cuda:{lik.device.index}; the program runs on cuda:{self.device}")
-                lik = lik.to(torch.float64 if self.f64 else torch.float32).contiguous()
+                lik = lik.to(torch.float64 if f64 else torch.float32).contiguous()
                 torch.cuda.current_stream(lik.device).synchronize()  # the program's stream reads it next
                 on_device = True
             else:
                 lik = lik.numpy()
         if not on_device:
-            lik = np.ascontiguousarray(lik, dtype=self.dtype)
+            lik = np.ascontiguousarray(lik, dtype=np.float64 if f64 else np.float32)
         if tuple(lik.shape) != (n_rows, n_lik):
             raise ValueError(f"likelihoods have shape {tuple(lik.shape)}, expected {(n_rows, n_lik)}")
-        out = np.empty((self.Q, n_rows), dtype=self.dtype)
-        log_ev = np.empty(n_rows, dtype=np.float64) if log_evidence else None
-        ptr = lik.data_ptr() if on_device else lik.ctypes.data
-        _check(self._fn("sbn_program_run_soft_host")(self._h, ev_ptr, n_rows, n_rows, ptr, n_lik, int(on_device),
-                                                      out.ctypes.data, n_rows,
-                                                      None if log_ev is None else log_ev.ctypes.data))
-        return (out, log_ev) if log_evidence else out
+        return lik, (lik.data_ptr() if on_device else lik.ctypes.data, n_lik, int(on_device))
 
     def evidence(self, codes: np.ndarray, n_rows: int) -> np.ndarray:
         """P(event) per evidence row (the normaliser of the posterior), host path."""
@@ -297,51 +316,78 @@ class Program:
         _check(self._fn("sbn_program_evidence_host")(self._h, ev_ptr, n_rows, n_rows, out.ctypes.data))
         return out
 
-    def counts(self, codes: np.ndarray, n_rows: int):
+    def counts(self, codes: np.ndarray, n_rows: int, lik=None, log_evidence: bool = False):
         """Counts programs (planner.build_counts_plan): (expected counts float64 [n_counts] summed over the
-        rows, P(observed) [n_rows], NaN for a row the float32 range rule flags), host path."""
+        rows, P(observed) [n_rows], NaN for a row the float32 range rule flags), host path.  A program with soft
+        evidence (planner.build_pattern_plan) takes likelihoods `lik` as `run_soft` does; P(observed) is then
+        P(observed, lik / max), and `log_evidence` appends log P(observed, lik) float64 [n_rows]."""
         n_rows = int(n_rows)
         codes, ev_ptr = self._evidence(codes, n_rows)
         counts = np.zeros(int(self.plan.n_counts), dtype=np.float64)
         prob = np.empty(n_rows, dtype=self.dtype)
-        _check(self._fn("sbn_program_counts_host")(self._h, ev_ptr, n_rows, n_rows, counts.ctypes.data, counts.size,
-                                                   prob.ctypes.data))
-        return counts, prob
+        if lik is None:
+            _check(self._fn("sbn_program_counts_host")(self._h, ev_ptr, n_rows, n_rows, counts.ctypes.data, counts.size,
+                                                       prob.ctypes.data))
+            return counts, prob
+        lik, lik_args = self._likelihoods(lik, n_rows)
+        log_ev = np.empty(n_rows, dtype=np.float64) if log_evidence else None
+        _check(self._fn("sbn_program_counts_soft_host")(self._h, ev_ptr, n_rows, n_rows, *lik_args, counts.ctypes.data,
+                                                        counts.size, prob.ctypes.data,
+                                                        None if log_ev is None else log_ev.ctypes.data))
+        return (counts, prob, log_ev) if log_evidence else (counts, prob)
 
     def set_tables(self, blob: np.ndarray):
         """Replace a counts program's tables (planner.refresh_tables gives the blob of new CPTs)."""
         blob = np.ascontiguousarray(blob, dtype=self.dtype)
         _check(self._fn("sbn_program_set_tables")(self._h, blob.ctypes.data, blob.size))
 
-    def sample(self, codes: np.ndarray, n_rows: int, n_draws: int, seed: int, row_base: int = 0):
+    def sample(self, codes: np.ndarray, n_rows: int, n_draws: int, seed: int, row_base: int = 0, lik=None,
+               log_evidence: bool = False):
         """Sample programs (planner.build_sample_plan): (drawn codes uint8 [n_sampled, n_draws, n_rows] in
         the order of `plan.sampled`, P(observed) [n_rows], NaN for a row the float32 range rule flags), host
-        path.  Row b's draws depend only on (seed, row_base + b, draw index)."""
+        path.  Row b's draws depend only on (seed, row_base + b, draw index).  `lik` and `log_evidence` are
+        those of `counts`, for a program with soft evidence."""
         n_rows, n_draws = int(n_rows), int(n_draws)
         codes, ev_ptr = self._evidence(codes, n_rows)
         out = np.empty((len(self.plan.sampled), n_draws, n_rows), dtype=np.uint8)
         prob = np.empty(n_rows, dtype=self.dtype)
-        _check(self._fn("sbn_program_sample_host")(self._h, ev_ptr, n_rows, n_rows, n_draws, int(seed) & (2**64 - 1),
-                                                   int(row_base), out.ctypes.data, prob.ctypes.data))
-        return out, prob
+        seed = int(seed) & (2**64 - 1)
+        if lik is None:
+            _check(self._fn("sbn_program_sample_host")(self._h, ev_ptr, n_rows, n_rows, n_draws, seed, int(row_base),
+                                                       out.ctypes.data, prob.ctypes.data))
+            return out, prob
+        lik, lik_args = self._likelihoods(lik, n_rows)
+        log_ev = np.empty(n_rows, dtype=np.float64) if log_evidence else None
+        _check(self._fn("sbn_program_sample_soft_host")(self._h, ev_ptr, n_rows, n_rows, *lik_args, n_draws, seed,
+                                                        int(row_base), out.ctypes.data, prob.ctypes.data,
+                                                        None if log_ev is None else log_ev.ctypes.data))
+        return (out, prob, log_ev) if log_evidence else (out, prob)
 
-    def mpe(self, codes: np.ndarray, n_rows: int):
+    def mpe(self, codes: np.ndarray, n_rows: int, lik=None):
         """MPE programs (planner.build_mpe_plan): (decoded codes uint8 [n_decoded, n_rows] in the order of
-        `plan.sampled`, max log P(x, e) float32 [n_rows], -inf for a row of probability zero), host path."""
+        `plan.sampled`, max log P(x, e) float32 [n_rows], -inf for a row of probability zero), host path.  A
+        program with soft evidence takes likelihoods `lik` as `run_soft` does; its max log P(x, e, lik) comes
+        back in float64, on the caller's scale of `lik`."""
         n_rows = int(n_rows)
         codes, ev_ptr = self._evidence(codes, n_rows)
         out = np.empty((len(self.plan.sampled), n_rows), dtype=np.uint8)
-        log_prob = np.empty(n_rows, dtype=np.float32)
-        _check(load().sbn_program_mpe_host(self._h, ev_ptr, n_rows, n_rows, out.ctypes.data, log_prob.ctypes.data))
+        if lik is None:
+            log_prob = np.empty(n_rows, dtype=np.float32)
+            _check(load().sbn_program_mpe_host(self._h, ev_ptr, n_rows, n_rows, out.ctypes.data, log_prob.ctypes.data))
+            return out, log_prob
+        lik, lik_args = self._likelihoods(lik, n_rows)
+        log_prob = np.empty(n_rows, dtype=np.float64)
+        _check(load().sbn_program_mpe_soft_host(self._h, ev_ptr, n_rows, n_rows, *lik_args, out.ctypes.data,
+                                                log_prob.ctypes.data))
         return out, log_prob
 
-    def map(self, codes: np.ndarray, n_rows: int):
+    def map(self, codes: np.ndarray, n_rows: int, lik=None):
         """Marginal MAP programs (planner.build_map_plan): (decoded codes uint8 [n_map, n_rows] of the MAP
         variables in the order of `plan.sampled`, max log P(x_MAP, e) float32 [n_rows], -inf for a row of
-        probability zero), host path.  The engine runs them through the MPE entry point."""
+        probability zero), host path.  The engine runs them through the MPE entry point, `lik` included."""
         if self.plan.version != 9:
             raise ValueError(f"a version-{self.plan.version} program is not a marginal MAP program")
-        return self.mpe(codes, n_rows)
+        return self.mpe(codes, n_rows, lik=lik)
 
     def run_device(self, d_ev: int, ld_ev: int, n_rows: int, d_out: int, ld_out: int, stream: int = 0):
         """Device path: raw device pointers, asynchronous on `stream`."""

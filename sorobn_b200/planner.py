@@ -29,7 +29,7 @@ oracle/program_interp.py (the CPU checker used in tests):
     header : MAGIC VERSION mode n_ev n_tables n_slots n_steps Q post_slot post_batched n_soft 0
     tables : (offset_floats, size) * n_tables         -- into the float table blob
     slots  : (batched, size_per_row) * n_slots        -- scratch buffers
-    soft   : (slot, card) * n_soft                    -- likelihood slots (versions 4 and 5 only)
+    soft   : (slot, card) * n_soft                    -- likelihood slots (header word 10 or 11, see below)
     steps  : kind n_in out_slot n_axes n_elim | cards[n_axes] | ecards[n_elim] |
              per input: is_slot id batched n_ev (col stride card)*n_ev estrides[n_elim] strides[n_axes]
 
@@ -46,13 +46,16 @@ input that spans both tile axes.
 1 = batched.  The posterior is produced by the last step into `post_slot`
 (`[Q]` or `[Q, B]`, unnormalised) and normalised per row by the engine.
 
-Soft evidence (`soft=` of `build_plan` and `build_marginals_plan`, batched versions 4 and 5 only): every
-soft variable v carries a per-row likelihood lambda_v over its states, one batched leaf factor over (v)
-in a slot no step writes.  The engine fills those slots before step 0 of every run (csrc/sbn_soft.cuh),
-each row divided by its maximum, from the caller's `[n_rows][ld_lik]` likelihood matrix whose columns are
-the soft variables sorted by name, states in domain order.  Header word 10 is `n_soft`, and the soft
-section lists `(slot, card)` per soft variable in that column order.  With `n_soft = 0` the words are
-those of a plan without soft evidence.
+Soft evidence (`soft=` of `build_plan`, `build_marginals_plan` and `build_pattern_plan`; batched plans
+only): every soft variable v carries a per-row likelihood lambda_v over its states, one batched leaf factor
+over (v) in a slot no step writes.  The engine fills those slots before step 0 of every run
+(csrc/sbn_soft.cuh), each row divided by its maximum, from the caller's `[n_rows][ld_lik]` likelihood
+matrix whose columns are the soft variables sorted by name, states in domain order.  The soft section lists
+`(slot, card)` per soft variable in that column order.  `n_soft` is header word 10 of versions 4 and 5 and
+word 11 of versions 6 to 9 (their word 10 holds `n_counts` / `n_sampled`).  The log-domain versions 8 and 9
+hold log(lambda_v / max lambda_v) in the slot, -inf for a zero entry.  A soft variable is unobserved: a
+counts plan gives its family's counts, sample and MPE plans draw or decode it, and a MAP plan sums it out
+unless it is a MAP variable.  With `n_soft = 0` the words are those of a plan without soft evidence.
 
 Marginals programs (`build_marginals_plan`, VERSION 5) answer P(t | e) for many targets t at
 once.  They use the same words, with two differences:
@@ -490,6 +493,35 @@ def build_map_plan(net: CompiledNet, evidence, map_vars, order=None, max_in=MAX_
         raise ValueError("nothing to compute: no MAP variable and no evidence")
     return _build(net, VERSION_MAP, evidence, targets=map_vars, order=order, max_in=max_in,
                   lift_evidence=lift_evidence, fuse_elims=fuse_elims)
+
+
+def build_pattern_plan(net: CompiledNet, kind, evidence, soft=(), map_vars=None, **kw) -> Plan:
+    """The plan of one missingness pattern with soft evidence: `kind` "counts", "sample", "mpe" or "map" (then
+    `map_vars` are the MAP variables), the observed columns `evidence` and the var ids `soft` whose per-row
+    likelihoods arrive at run time (see the module docstring).  A soft variable may not be evidence; it may be
+    a MAP variable.  With `soft=()` the plan is the one of the kind's own builder (`build_counts_plan`, ...),
+    word for word; `kw` are that builder's options."""
+    builders = {"counts": build_counts_plan, "sample": build_sample_plan, "mpe": build_mpe_plan, "map": build_map_plan}
+    if kind not in builders:
+        raise ValueError(f"kind must be one of {sorted(builders)}, not {kind!r}")
+    if (map_vars is not None) != (kind == "map"):
+        raise ValueError("map_vars go with kind 'map' only, and kind 'map' needs them")
+    evidence = tuple(evidence)
+    soft = _check_soft(net, evidence, soft, kw.get("mode", MODE_BATCHED))
+    if not soft:
+        return builders[kind](net, evidence, *(() if map_vars is None else (map_vars,)), **kw)
+    hidden = tuple(v for v in range(len(net.names)) if v not in set(evidence))
+    if kind == "counts":
+        return _build(net, VERSION_COUNTS, evidence, targets=hidden, soft=soft, **kw)
+    if kind in ("sample", "mpe"):
+        return _build(net, VERSION_SAMPLE if kind == "sample" else VERSION_MPE, evidence, targets=hidden, soft=soft, **kw)
+    map_vars = tuple(map_vars)
+    if len(set(map_vars)) != len(map_vars):
+        raise ValueError("duplicate MAP variable")
+    if set(map_vars) & set(evidence):
+        raise ValueError("A MAP variable cannot be part of the event")
+    # with soft evidence a plan that decodes nothing still has its log P(e, lik) to compute
+    return _build(net, VERSION_MAP, evidence, targets=map_vars, soft=soft, **kw)
 
 
 def count_layout(net: CompiledNet):
@@ -1295,6 +1327,8 @@ def _serialise(plan: Plan, table_arrays):
         post = [-1, 0]  # the readouts write the posterior themselves
     if plan.version in (VERSION, VERSION_MARGINALS):
         extra = [len(plan.soft), 0]
+    else:
+        extra[1] = len(plan.soft)
     w = [MAGIC, plan.version, plan.mode, len(plan.evidence), len(plan.tables), len(plan.slots), len(plan.steps),
          plan.Q, *post, *extra]
     assert len(w) == HEADER_WORDS
