@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SBN_ABI_VERSION 15
+#define SBN_ABI_VERSION 16
 
 #define SBN_OK 0
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
@@ -130,7 +130,7 @@ int sbn_program_counts_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev,
 int sbn_program_counts_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts,
                                 int64_t n_counts, double *prob);
 
-/* Replace a counts program's table blob in place (same size and layout: planner.refresh_tables) and
+/* Replace a counts or gradient program's table blob in place (same size and layout: planner.refresh_tables) and
  * re-run its evidence-independent launches; later runs, graph replays included, use the new values.
  * An EM loop plans once and calls this every iteration.  Other programs are refused: their paired
  * steps fold table products into coefficients built on the host. */
@@ -192,6 +192,33 @@ int sbn_program_sample_soft_host_f64(sbn_program *prog, const uint8_t *ev, int64
 int sbn_program_mpe_soft_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
                               int64_t ld_lik, int lik_on_device, uint8_t *codes /* [n_decoded][n_rows] */,
                               double *log_prob /* [n_rows] */);
+
+/* Gradients of log P(observed cells, lik) of a gradient program (planner.build_pattern_plan kind "grad",
+ * version 10; every other call refuses it, and these calls refuse every other program).  The program may have
+ * soft variables or none; with none, lik may be NULL.  `lik`, `ld_lik` and `lik_on_device` are those of
+ * sbn_program_run_soft_host.  prob[b] = P(observed, lik / max), NaN for a row below the float32 range (1e-30;
+ * 1e-290 for the float64 twin) or of probability zero: re-run it with the float64 program.
+ * Forward: prob and log_prob[b] = log P(observed, lik) (double; either may be NULL).  Only the launches
+ * P(observed) depends on run: no count step and no readout.
+ * Backward: `weights` [n_rows] double (host, or device memory of the program's device with weights_on_device);
+ * counts[e] += sum_b w_b * P(family entry e | observed, lik) (the layout of sbn_program_counts_host; a fully
+ * observed family adds w_b), which is sum_b w_b * theta_e * d log P_b / d theta_e; and
+ * deriv[j * ld_deriv + b] = d log P(observed, lik / max) / d (lik / max)_j of likelihood column j, which is
+ * max * d log P_b / d lik_j (divide by the row's maximum of that variable), exact where lik_j = 0.  A flagged
+ * row adds nothing and reads NaN.  The counts are reduced without floating-point atomics: two calls give
+ * bitwise the same results.  Large batches run in chunks. */
+int sbn_program_grad_forward_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
+                                  int64_t ld_lik, int lik_on_device, float *prob, double *log_prob);
+int sbn_program_grad_forward_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
+                                      const double *lik, int64_t ld_lik, int lik_on_device, double *prob,
+                                      double *log_prob);
+int sbn_program_grad_backward_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
+                                   int64_t ld_lik, int lik_on_device, const double *weights, int weights_on_device,
+                                   double *counts, int64_t n_counts, float *deriv, int64_t ld_deriv, float *prob);
+int sbn_program_grad_backward_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
+                                       const double *lik, int64_t ld_lik, int lik_on_device, const double *weights,
+                                       int weights_on_device, double *counts, int64_t n_counts, double *deriv,
+                                       int64_t ld_deriv, double *prob);
 
 /* Same with DEVICE buffers, asynchronous on `stream` (a cudaStream_t; NULL = default
  * stream).  n_rows must not exceed the reserved chunk size. */

@@ -476,9 +476,8 @@ class BayesNet:
             for r in runners:
                 r.close()
         self.em_log_likelihood_ = lls
+        self._write_cpts(cpts, keep=[f.reshape(-1) > 0 for f in fam])
         for v, node in enumerate(net.names):
-            table = pd.Series(cpts[v].reshape(-1), index=self._family_index(v))
-            self.P[node] = table[fam[v].reshape(-1) > 0]
             parents = self.parents.get(node)
             if parents:
                 tot = totals[v].reshape(-1)
@@ -488,6 +487,64 @@ class BayesNet:
                 self._P_sizes[node] = float(totals[v])
         self.prepare()
         return self
+
+    def _write_cpts(self, cpts, keep=None):
+        """Store dense CPTs (var id -> ndarray [*parents, v] over the compiled domains) in `P`, every entry or those
+        where keep[v] (flat) is set; the caller calls prepare()."""
+        for v, node in enumerate(self._compiled.names):
+            if cpts[v] is None:
+                continue
+            table = pd.Series(np.asarray(cpts[v], dtype=np.float64).reshape(-1), index=self._family_index(v))
+            self.P[node] = table if keep is None else table[keep[v]]
+
+    # ------------------------------------------------------------ gradients
+    def encode_rows(self, X: pd.DataFrame):
+        """The rows of `X` grouped by missingness pattern and encoded, once: `log_likelihood` takes the result in
+        place of `X`, which saves the encoding in a training loop that passes the same rows every step."""
+        from .autograd import EncodedRows
+
+        return EncodedRows(self._count_patterns(X), X.index, X.columns)
+
+    def log_likelihood(self, X, cpts: dict | None = None, likelihoods: dict | None = None):
+        """log P(observed cells of b, likelihoods of b) of every row of `X` (a frame as in `expected_counts`, or
+        `encode_rows(X)`), as a float64 torch tensor [n] on the network's device, computed on the GPU and
+        differentiable (DESIGN.md "Gradients of the log-likelihood").
+
+        cpts: {node: tensor [*parents, node]} over the compiled domains (`cpt_tensors()` gives the current ones
+        in that layout), used in place of the node's CPT; gradients flow into these tensors, e.g. the softmax of a
+        logits Parameter.  Every row must sum to 1 (within 1e-6), and a tensor that requires grad may have no zero
+        entry (parameterise through softmax).  likelihoods: soft evidence as in `expected_counts`; gradients flow
+        into its torch tensors.  Rows are grouped by missingness pattern, one gradient program per pattern; rows
+        the float32 program cannot hold re-run in float64.  A row of probability zero raises ValueError.  One
+        device only; second derivatives are not supported."""
+        from . import autograd
+
+        return autograd.log_likelihood(self, X, cpts, likelihoods)
+
+    def cpt_tensors(self) -> dict:
+        """{node: float64 torch tensor [*parents, node]}: the current dense CPTs over the compiled (sorted)
+        domains, in the layout `log_likelihood(cpts=...)` and `assign_cpts` take."""
+        import torch
+
+        net = self._net("reading the CPTs")
+        return {name: torch.tensor(net.cpt[v], dtype=torch.float64) for v, name in enumerate(net.names)}
+
+    def assign_cpts(self, cpts: dict) -> "BayesNet":
+        """Write dense CPTs {node: array or tensor [*parents, node]} (the layout of `cpt_tensors`) into `P`, every
+        entry kept, and prepare() the network."""
+        net = self._net("assigning CPTs")
+        dense = [None] * len(net.names)
+        for node, values in cpts.items():
+            if node not in net.index:
+                raise ValueError(f"a CPT for {node!r}, which is not a node of the network")
+            v = net.index[node]
+            arr = values.detach().cpu().numpy() if hasattr(values, "detach") else values
+            arr = np.asarray(arr, dtype=np.float64)
+            if arr.shape != net.cpt[v].shape:
+                raise ValueError(f"the CPT of {node!r} has shape {arr.shape}, expected {net.cpt[v].shape}")
+            dense[v] = arr
+        self._write_cpts(dense)
+        return self.prepare()
 
     def _family_index(self, v, parents_only=False):
         """Index of every combination of the compiled domains of [*parents, v] (or of the parents alone)."""
@@ -544,7 +601,7 @@ class BayesNet:
         plan is keyed by its MAP variables, sorted var ids, too), with the soft-evidence var ids `soft` (sorted
         by name; part of the key only when there are any)."""
         extra = (map_vars,) if kind == "map" else ()
-        if not soft:
+        if not soft and kind != "grad":  # there is no build_grad_plan
             build = getattr(_planner, f"build_{kind}_plan")
             return self._programs((kind, ev, *extra), lambda: build(self._compiled, ev, *extra))
         return self._programs((kind, ev, *extra, soft),

@@ -16,7 +16,7 @@ SOURCES = [os.path.join(HERE, f) for f in ("sbn_api.cu", "sbn_tiled_u0.cu", "sbn
                                             "sbn_chain.cu", "sbn_tma.cu", "sbn_pair.cu", "sbn_triple_rows.cu",
                                             "sbn_join.cu")]
 HEADERS = [os.path.join(HERE, h) for h in ("sbn_kernels.cuh", "sbn_gibbs.cuh", "sbn_chain.h", "sbn_tma.h", "sbn_pair.h", "sbn_join.h", "sbn_internal.h", "sbn_launch.h",
-                                            "sbn_launch_impl.cuh", "sbn_marginal.cuh", "sbn_count.cuh", "sbn_sample.cuh",
+                                            "sbn_launch_impl.cuh", "sbn_marginal.cuh", "sbn_count.cuh", "sbn_deriv.cuh", "sbn_sample.cuh",
                                             "sbn_mpe.cuh", "sbn_soft.cuh")] + [
     os.path.join(os.path.dirname(PKG), "include", "sorobn_b200.h")]
 OBJ_DIR = os.path.join(HERE, "build")

@@ -18,6 +18,7 @@
 
 #include "sbn_chain.h"
 #include "sbn_count.cuh"
+#include "sbn_deriv.cuh"
 #include "sbn_gibbs.cuh"
 #include "sbn_internal.h"
 #include "sbn_join.h"
@@ -61,8 +62,11 @@ constexpr int kVersionMpe = 8;        // planner.build_mpe_plan: log tables, max
                                       // max log P(x, e) in the posterior slot
 constexpr int kVersionMap = 9;        // planner.build_map_plan: version 8 plus a reduction word on kind-0 / 1 steps
                                       // (1 = log-sum-exp, 0 = max), max log P(x_MAP, e) in the posterior slot
+constexpr int kVersionGrad = 10;      // planner.build_pattern_plan(kind "grad"): version 6 with weighted count steps plus
+                                      // kind-6 derivative readouts, P(observed) in the posterior slot
 static_assert(kVersionMpe - kVersion == kMpe, "one program kind per header version, in order");
 static_assert(kVersionMap - kVersion == kMap, "one program kind per header version, in order");
+static_assert(kVersionGrad - kVersion == kGrad, "one program kind per header version, in order");
 constexpr int64_t kMarginalZoffMax = 1 << 24;  // int32 words of one readout's joint-state offset table
 constexpr int kMaxElim = 3;
 constexpr int kMaxZ = 256;
@@ -75,11 +79,13 @@ namespace {
 int parse(sbn_program *P, const int32_t *w, int64_t n) {
     if (n < kHeaderWords) return fail(SBN_E_INVALID, "program shorter than its header");
     if (w[0] != kMagic) return fail(SBN_E_INVALID, "bad program magic 0x%x", w[0]);
-    if (w[1] < kVersion || w[1] > kVersionMap)
-        return fail(SBN_E_INVALID, "program version %d, engine expects %d, %d, %d, %d, %d or %d", w[1], kVersion,
-                    kVersionMarginals, kVersionCounts, kVersionSample, kVersionMpe, kVersionMap);
+    if (w[1] < kVersion || w[1] > kVersionGrad)
+        return fail(SBN_E_INVALID, "program version %d, engine expects %d, %d, %d, %d, %d, %d or %d", w[1], kVersion,
+                    kVersionMarginals, kVersionCounts, kVersionSample, kVersionMpe, kVersionMap, kVersionGrad);
     P->kind = static_cast<ProgramKind>(w[1] - kVersion);
-    const bool marginals = P->kind == kMarginals, counts = P->kind == kCounts, mpe = sbn_log_domain(P->kind);
+    // a gradient program parses as a counts program plus its derivative readouts (kind 6)
+    const bool grad = P->kind == kGrad;
+    const bool marginals = P->kind == kMarginals, counts = P->kind == kCounts || grad, mpe = sbn_log_domain(P->kind);
     const bool map = P->kind == kMap;
     // sample, MPE and marginal MAP programs share the words of their last steps
     const bool decodes = P->kind == kSample || mpe;
@@ -94,7 +100,8 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         return fail(SBN_E_INVALID, "bad header counts");
     if (counts) {
         P->n_counts = w[10];
-        if (P->Q != 1 || P->n_counts <= 0) return fail(SBN_E_INVALID, "bad counts header");
+        if ((!grad && P->Q != 1) || P->n_counts <= 0 || P->mode != (grad ? 1 : P->mode))
+            return fail(SBN_E_INVALID, grad ? "bad gradient header" : "bad counts header");
     }
     if (decodes) {
         P->n_sampled = w[10];
@@ -124,7 +131,8 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         if (batched && P->mode == 0) return fail(SBN_E_INVALID, "batched slot in a flat program");
         P->slots.push_back({batched != 0, size, round_up(size, 4), nullptr});
     }
-    if (!marginals && ((P->slots[P->post_slot].batched ? 1 : 0) != P->post_batched || P->slots[P->post_slot].size < P->Q))
+    // (a gradient program's slot holds P(observed); its other output rows are written by the readouts)
+    if (!marginals && ((P->slots[P->post_slot].batched ? 1 : 0) != P->post_batched || P->slots[P->post_slot].size < (grad ? 1 : P->Q)))
         return fail(SBN_E_INVALID, "posterior slot mismatch");
     {
         // soft evidence: (slot, card) of every likelihood, filled before step 0 (sbn_soft.cuh); n_soft is word 10
@@ -143,7 +151,8 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             P->n_lik += card;
         }
     }
-    std::vector<int> written(marginals ? P->Q : 0, 0);  // posterior entries written by the readouts
+    if (grad && P->Q != 1 + P->n_lik) return fail(SBN_E_INVALID, "a gradient program writes 1 + %d rows, not %d", P->n_lik, P->Q);
+    std::vector<int> written(marginals || grad ? P->Q : 0, 0);  // posterior entries (gradient: output rows) written by the readouts
     for (int s = 0; s < n_steps; ++s) {
         if (!need(5)) return fail(SBN_E_INVALID, "truncated step %d", s);
         StepDesc st;
@@ -154,10 +163,10 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         const int n_elim = w[p + 4];
         st.cx = 1;
         p += 5;
-        const bool readout = st.kind == 2;
+        const bool readout = st.kind == 2 || (grad && st.kind == 6);  // kind 6: the layout of kind 2
         const bool count = st.kind == 3;
         const bool draw = decodes && st.kind == decode_kind;
-        if (st.kind != 0 && st.kind != 1 && !(readout && marginals) && !(count && counts) && !draw)
+        if (st.kind != 0 && st.kind != 1 && !(readout && (marginals || grad)) && !(count && counts) && !draw)
             return fail(SBN_E_INVALID, "step %d: bad kind", s);
         if (draw) {
             // the drawn variables are the step's `n_elim` axes; they fill the next drawn-code rows
@@ -241,7 +250,8 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         }
         p += n_elim;
         if (readout) {
-            if (st.q_offset < 0 || st.q_offset + st.n_out > P->Q) return fail(SBN_E_INVALID, "step %d: segment outside the posterior", s);
+            if (st.q_offset < (grad ? 1 : 0) || st.q_offset + st.n_out > P->Q)
+                return fail(SBN_E_INVALID, "step %d: segment outside the posterior", s);
             for (int64_t q = st.q_offset; q < st.q_offset + st.n_out; ++q) written[q]++;
         } else if (count) {
             if (static_cast<int64_t>(st.cx) * st.n_out >= (1LL << 31)) return fail(SBN_E_INVALID, "step %d: count step too large", s);
@@ -348,10 +358,11 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         for (int q = 0; q < P->Q; ++q)
             if (written[q] != 1) return fail(SBN_E_INVALID, "posterior entry %d is written %d times", q, written[q]);
     } else if (counts) {
-        // P(observed) is written before the first count step and not overwritten before the last one
+        // P(observed) is written before the first count step and not overwritten before the last one (the last
+        // derivative readout of a gradient program)
         int first = -1, last = -1, writer = -1;
         for (size_t i = 0; i < P->steps.size(); ++i) {
-            if (P->steps[i].kind == 3) {
+            if (P->steps[i].kind >= 2) {
                 if (first < 0) first = static_cast<int>(i);
                 last = static_cast<int>(i);
             } else if (P->steps[i].out_slot == P->post_slot) {
@@ -361,7 +372,28 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         if (first < 0) return fail(SBN_E_INVALID, "a counts program without a count step");
         if (writer < 0 || writer > first) return fail(SBN_E_INVALID, "P(observed) is not written before the count steps");
         for (int i = first; i <= last; ++i)
-            if (P->steps[i].kind != 3) return fail(SBN_E_INVALID, "step %d comes between the count steps", i);
+            if (P->steps[i].kind < 2) return fail(SBN_E_INVALID, "step %d comes between the count steps", i);
+        if (grad) {
+            for (int q = 1; q < P->Q; ++q)
+                if (written[q] != 1) return fail(SBN_E_INVALID, "output row %d is written %d times", q, written[q]);
+            // the forward run: the steps P(observed) depends on, through the last writer of every slot it reads
+            std::vector<int> last_writer(P->slots.size(), -1);
+            std::vector<std::vector<int>> deps(P->steps.size());
+            for (int i = 0; i < writer + 1; ++i) {
+                for (const InDesc &in : P->steps[i].in)
+                    if (in.is_slot && last_writer[in.id] >= 0) deps[i].push_back(last_writer[in.id]);
+                last_writer[P->steps[i].out_slot] = i;
+            }
+            P->forward.assign(P->steps.size(), 0);
+            std::vector<int> stack = {writer};
+            while (!stack.empty()) {
+                const int i = stack.back();
+                stack.pop_back();
+                if (P->forward[i]) continue;
+                P->forward[i] = 1;
+                for (int d : deps[i]) stack.push_back(d);
+            }
+        }
     } else if (P->steps.back().out_slot != P->post_slot) {
         return fail(SBN_E_INVALID, "last step does not write the posterior");
     }
@@ -584,7 +616,7 @@ void plan_tiles(sbn_program *P, std::vector<int32_t> *words) {
                 words->push_back(static_cast<int32_t>(off));
             }
         }
-        if (st.ecards.size() < 2 && st.kind != 2 && st.kind != 3 && st.kind != 4 && st.kind != 5) continue;
+        if (st.ecards.size() < 2 && st.kind < 2) continue;
         st.zoff_pos = static_cast<int64_t>(words->size());
         for (const InDesc &in : st.in) {
             for (int z = 0; z < st.cx; ++z) {
@@ -714,6 +746,7 @@ void drop_graphs(sbn_program *P) {
     // captured launches embed the kernel variants and pointers of the moment they were captured
     drop_graph(P->graph);
     drop_graph(P->pipe_graph);
+    drop_graph(P->forward_graph);
 }
 
 void free_scratch(sbn_program *P) {
@@ -724,6 +757,8 @@ void free_scratch(sbn_program *P) {
     cudaFree(P->d_total);
     cudaFree(P->d_lik);
     cudaFree(P->d_log_max);
+    cudaFree(P->d_weight);
+    P->d_weight = nullptr;
     P->d_lik = nullptr;
     P->d_log_max = nullptr;
     P->d_total = nullptr;
@@ -1044,8 +1079,40 @@ cudaError_t launch_count(sbn_program *P, const StepDesc &st, const uint8_t *ev, 
     const int64_t smem = bind_operands(P, st, c.in);
     c.smem_floats = static_cast<int32_t>(smem);
     double *counts = P->d_counts + st.q_offset;
-    if (P->f64) return sbn_count_launch<double>(c, grid, 0, counts, stream);
-    return sbn_count_launch<float>(c, grid, static_cast<size_t>(smem) * 4, counts, stream);
+    const double *weight = P->kind == kGrad ? P->weight : nullptr;  // a gradient program's counts are weighted
+    if (P->f64) return sbn_count_launch<double>(c, grid, 0, counts, stream, weight);
+    return sbn_count_launch<float>(c, grid, static_cast<size_t>(smem) * 4, counts, stream, weight);
+}
+
+// Derivative readout of a gradient program (kind 6): the soft variable's rows q_offset .. of the output, for rows
+// 0 .. n_rows - 1, divided by P(observed).
+cudaError_t launch_deriv(sbn_program *P, const StepDesc &st, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, float *d_out,
+                         int64_t ld_out, cudaStream_t stream) {
+    P->launches++;
+    SbnDeriv d;
+    memset(&d, 0, sizeof d);
+    SbnMarginal &m = d.m;
+    const size_t elem = P->f64 ? 8 : 4;
+    m.out = reinterpret_cast<char *>(d_out) + st.q_offset * ld_out * static_cast<int64_t>(elem);
+    m.ld_out = ld_out;
+    m.ev = ev;
+    m.ld_ev = ld_ev;
+    m.ld = P->ld;
+    m.zoff = P->d_tile_off + st.zoff_pos;
+    m.min_total = P->f64 ? 1e-290 : static_cast<double>(SBN_MIN_TOTAL_F32);
+    m.n_rows = static_cast<int32_t>(n_rows);
+    m.n_in = static_cast<int32_t>(st.in.size());
+    m.n_common = st.n_common;
+    m.card = st.cards[0];
+    m.cz = st.cx;
+    const int64_t smem = bind_operands(P, st, m.in);
+    for (size_t i = 0; i < st.in.size(); ++i) m.in[i].ts = st.in[i].strides[0];
+    m.smem_floats = static_cast<int32_t>(smem);
+    const Slot &ps = P->slots[P->post_slot];
+    d.prob = ps.ptr;
+    d.prob_batched = ps.batched ? 1 : 0;
+    if (P->f64) return sbn_deriv_launch<double>(d, 0, stream);
+    return sbn_deriv_launch<float>(d, static_cast<size_t>(smem) * 4, stream);
 }
 
 // The drawn-code buffer of a sample / MPE run (P->d_drawn): codes [n_sampled][n_draws][ld_drawn] (one draw for
@@ -1087,12 +1154,13 @@ cudaError_t launch_sample(sbn_program *P, const StepDesc &st, int k, const uint8
     return sbn_sample_launch<float>(m, static_cast<size_t>(smem) * 4, stream);
 }
 
-// A readout, count, sample or argmax step (kinds 2 .. 5) on its own launch; `k`: its index among the sample /
+// A readout, count, sample, argmax or derivative step (kinds 2 .. 6) on its own launch; `k`: its index among the sample /
 // argmax steps (Philox counter word 0 of a sample step)
 cudaError_t launch_kind_step(sbn_program *P, const StepDesc &st, int k, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
                              float *d_out, int64_t ld_out, const DrawnCodes &dc, cudaStream_t stream) {
     if (st.kind == 2) return launch_marginal(P, st, ev, ld_ev, n_rows, d_out, ld_out, stream);
     if (st.kind == 3) return launch_count(P, st, ev, ld_ev, n_rows, stream);
+    if (st.kind == 6) return launch_deriv(P, st, ev, ld_ev, n_rows, d_out, ld_out, stream);
     return launch_sample(P, st, k, ev, ld_ev, n_rows, dc, stream);
 }
 
@@ -1224,8 +1292,9 @@ int issue_all(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows
         if (events) SBN_CUDA(cudaEventRecord(events[k], stream));
         ++k;
         if (hoisted(P, st)) continue;  // computed once, when the program was created
+        if (P->forward_run && !P->forward[k - 1]) continue;  // a forward run of a gradient program: P(observed) only
         if (st.kind >= 2) {
-            const int decoded = st.kind >= 4 ? n_decoded++ : 0;
+            const int decoded = st.kind == 4 || st.kind == 5 ? n_decoded++ : 0;
             SBN_CUDA(launch_kind_step(P, st, decoded, d_ev, ld_ev, n_rows, d_out, ld_out, dc, stream));
             continue;
         }
@@ -1264,7 +1333,8 @@ int issue_all(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows
             if (!folded && !(chain_on(P) && P->segments.back()->ends_in_posterior))
                 SBN_CUDA(launch_normalise(P, d_out, ld_out, n_rows, stream));
             break;
-        case kCounts: SBN_CUDA(launch_prob(P, n_rows, d_out, nullptr, stream)); break;
+        case kCounts:
+        case kGrad: SBN_CUDA(launch_prob(P, n_rows, d_out, nullptr, stream)); break;
         case kSample: SBN_CUDA(launch_prob(P, n_rows, d_out, dc.flags(P), stream)); break;
         case kMarginals:  // the readouts normalise
         case kMpe:
@@ -1352,18 +1422,22 @@ int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n
 // The checks every run shares: the program is of the kind the entry point runs (kPosterior: the run, evidence
 // and profile calls, which take posterior and marginals programs), and the rows and their evidence are well formed
 int check_rows(const sbn_program *P, ProgramKind kind, const void *ev, int64_t ld_ev, int64_t n_rows, bool soft = false) {
-    static const char *const name[] = {"posterior", "marginals", "counts", "sample", "MPE", "MAP"};
+    static const char *const name[] = {"posterior", "marginals", "counts", "sample", "MPE", "MAP", "gradient"};
     static const char *const entry[] = {"sbn_program_run_*", "sbn_program_run_*", "sbn_program_counts_host",
-                                        "sbn_program_sample_host", "sbn_program_mpe_host", "sbn_program_mpe_host"};
+                                        "sbn_program_sample_host", "sbn_program_mpe_host", "sbn_program_mpe_host",
+                                        "sbn_program_grad_forward_host / sbn_program_grad_backward_host"};
     if (!P) return fail(SBN_E_INVALID, "null program");
-    if ((P->kind == kMarginals ? kPosterior : P->kind == kMap ? kMpe : P->kind) != kind)
-        return fail(SBN_E_INVALID, "a %s program runs through %s", name[P->kind], entry[P->kind]);
     static const char *const soft_entry[] = {"sbn_program_run_soft_host", "sbn_program_run_soft_host",
                                              "sbn_program_counts_soft_host", "sbn_program_sample_soft_host",
-                                             "sbn_program_mpe_soft_host", "sbn_program_mpe_soft_host"};
+                                             "sbn_program_mpe_soft_host", "sbn_program_mpe_soft_host", ""};
     static const char *const plain_entry[] = {"sbn_program_run_host", "sbn_program_run_host", "sbn_program_counts_host",
-                                              "sbn_program_sample_host", "sbn_program_mpe_host", "sbn_program_mpe_host"};
-    if (!P->soft.empty() && !soft)
+                                              "sbn_program_sample_host", "sbn_program_mpe_host", "sbn_program_mpe_host", ""};
+    if ((P->kind == kMarginals ? kPosterior : P->kind == kMap ? kMpe : P->kind) != kind)
+        return fail(SBN_E_INVALID, "a %s program%s runs through %s", name[P->kind],
+                    !P->soft.empty() && *soft_entry[P->kind] ? " with soft evidence" : "",
+                    !P->soft.empty() && *soft_entry[P->kind] ? soft_entry[P->kind] : entry[P->kind]);
+    if (kind == kGrad) {  // the gradient calls take programs with and without soft evidence
+    } else if (!P->soft.empty() && !soft)
         return fail(SBN_E_INVALID, "a %s program with soft evidence runs through %s", name[P->kind], soft_entry[P->kind]);
     if (P->soft.empty() && soft)
         return fail(SBN_E_INVALID, "a %s program without soft evidence runs through %s", name[P->kind], plain_entry[P->kind]);
@@ -1430,9 +1504,10 @@ int run_rows(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows,
     const bool short_chunk = (P->kind == kSample || sbn_log_domain(P->kind)) && n_rows < kSampleGraphMinRows;
     if (!P->use_graph || short_chunk) return issue_all(P, d_ev, ld_ev, n_rows, d_out, ld_out, stream, nullptr, dc);
     const GraphKey key = {d_ev, ld_ev, n_rows, d_out, ld_out, P->d_partial, P->d_drawn, dc.n_draws, dc.ld_drawn, P->lik,
-                          P->ld_lik};
+                          P->ld_lik, P->forward_run ? nullptr : P->weight};
     const bool branched = P->use_branches && P->kind <= kMarginals;
-    return replay(P, P->graph, key, P->stream, stream, [&] {
+    // a gradient program's forward run issues a subset of its launches: it keeps a graph of its own
+    return replay(P, P->forward_run ? P->forward_graph : P->graph, key, P->stream, stream, [&] {
         return branched ? issue_branched(P, d_ev, ld_ev, n_rows, d_out, ld_out, P->stream)
                         : issue_all(P, d_ev, ld_ev, n_rows, d_out, ld_out, P->stream, nullptr, dc);
     });
@@ -1604,13 +1679,14 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
             SBN_CUDA_P(sbn_triple_rows_set_attrs());
             SBN_CUDA_P(sbn_marginal_set_attrs());
             SBN_CUDA_P(sbn_count_set_attrs());
+            SBN_CUDA_P(sbn_deriv_set_attrs());
             SBN_CUDA_P(sbn_sample_set_attrs());
             SBN_CUDA_P(sbn_argmax_set_attrs());
             SBN_CUDA_P(sbn_batched_logdomain_set_attrs());
             done[device] = true;
         }
     }
-    if (P->kind == kCounts) {
+    if (P->kind == kCounts || P->kind == kGrad) {
         // the count table; the largest step's per-warp partial tables (count_grid caps them) are sized here and
         // allocated by each counts call only for its duration, so idle programs hold no partial tables
         for (const StepDesc &st : P->steps)
@@ -1675,7 +1751,8 @@ int sbn_program_reserve(sbn_program *P, int64_t max_rows) {
     const int64_t elem = P->f64 ? 8 : 4;
     // (+ a soft program's staged likelihoods and sum log(max))
     const int64_t per_row = batched_floats_per_row(P) * elem + P->n_ev + static_cast<int64_t>(P->Q) * elem + elem +
-                            (P->soft.empty() ? 0 : P->n_lik * static_cast<int64_t>(lik_elem(P)) + 8);
+                            (P->soft.empty() ? 0 : P->n_lik * static_cast<int64_t>(lik_elem(P)) + 8) +
+                            (P->kind == kGrad ? 8 : 0);  // (+ a gradient program's staged weights)
     size_t free_b = 0, total_b = 0;
     SBN_CUDA(cudaMemGetInfo(&free_b, &total_b));
     const int64_t budget = static_cast<int64_t>(free_b * 0.85);
@@ -1710,6 +1787,7 @@ int sbn_program_reserve(sbn_program *P, int64_t max_rows) {
         SBN_CUDA(cudaMalloc(&P->d_lik, static_cast<size_t>(ld) * P->n_lik * lik_elem(P)));
         SBN_CUDA(cudaMalloc(&P->d_log_max, static_cast<size_t>(ld) * 8));
     }
+    if (P->kind == kGrad) SBN_CUDA(cudaMalloc(&P->d_weight, static_cast<size_t>(ld) * 8));
     SBN_CUDA(cudaStreamSynchronize(P->stream));  // the memset must not race a caller's stream
     P->reserved_rows = rows;
     P->ld = ld;
@@ -2046,10 +2124,138 @@ int sbn_program_counts_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev
     return counts_host_common(P, ev, ld_ev, n_rows, counts, n_counts, prob, true);
 }
 
+// A gradient call (forward or backward) of rows 0 .. n_rows - 1, chunk by chunk: codes, likelihoods (when the
+// program has soft variables) and, backward, the row weights are staged (or read in place on the device); the
+// forward run issues the upward closure of P(observed) only.  Out: P(observed, lik / max) [n_rows] and log
+// P(observed, lik) [n_rows] (both optional); backward also the weighted counts added into `counts` and the
+// derivative readouts [n_lik][ld_deriv].
+struct GradArgs {
+    const void *lik = nullptr;
+    int64_t ld_lik = 0;
+    int lik_on_device = 0;
+    const double *weights = nullptr;  // null: a forward call
+    int weights_on_device = 0;
+    double *counts = nullptr;
+    int64_t n_counts = 0;
+    void *deriv = nullptr;
+    int64_t ld_deriv = 0;
+    void *prob = nullptr;
+    double *log_prob = nullptr;
+};
+
+static int grad_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const GradArgs &a, bool f64) {
+    int rc = check_rows(P, kGrad, ev, ld_ev, n_rows);
+    if (rc != SBN_OK) return rc;
+    if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the gradient call");
+    const bool backward = a.weights != nullptr;
+    const SoftLik soft = {P->n_lik > 0, a.lik, a.ld_lik, a.lik_on_device, nullptr};
+    rc = check_lik(P, soft);
+    if (rc != SBN_OK) return rc;
+    if (backward) {
+        if (!a.counts || (P->n_lik > 0 && !a.deriv)) return fail(SBN_E_INVALID, "null output");
+        if (a.n_counts != P->n_counts)
+            return fail(SBN_E_INVALID, "the count table has %lld entries, not %lld", (long long)P->n_counts, (long long)a.n_counts);
+        if (P->n_lik > 0 && a.ld_deriv < n_rows) return fail(SBN_E_INVALID, "ld_deriv < n_rows");
+    }
+    rc = reserve_rows(P, n_rows);
+    if (rc != SBN_OK) return rc;
+    if (backward) {
+        const cudaError_t e = cudaMalloc(&P->d_partial, static_cast<size_t>(std::max<int64_t>(1, P->partial_doubles)) * 8);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            P->d_partial = nullptr;
+            return fail(SBN_E_NOMEM, "cudaMalloc of %lld bytes of partial count tables failed: %s",
+                        (long long)(P->partial_doubles * 8), cudaGetErrorString(e));
+        }
+        SBN_CUDA(cudaMemsetAsync(P->d_counts, 0, static_cast<size_t>(P->n_counts) * 8, P->stream));
+    }
+    P->forward_run = !backward;
+    const size_t elem = f64 ? 8 : 4;
+    std::vector<char> prob(static_cast<size_t>(P->reserved_rows) * elem);
+    std::vector<double> log_max(static_cast<size_t>(P->reserved_rows), 0.0);
+    rc = for_each_chunk(P, ev, ld_ev, n_rows, P->reserved_rows, [&](int64_t r0, int64_t rows) -> int {
+        int rc = stage_lik(P, soft, r0, rows);
+        if (rc != SBN_OK) return rc;
+        if (backward && a.weights_on_device) {
+            P->weight = a.weights + r0;
+        } else if (backward) {
+            SBN_CUDA(cudaMemcpyAsync(P->d_weight, a.weights + r0, static_cast<size_t>(rows) * 8, cudaMemcpyHostToDevice, P->stream));
+            P->weight = P->d_weight;
+        }
+        rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
+        if (rc != SBN_OK) return rc;
+        SBN_CUDA(cudaMemcpyAsync(prob.data(), P->d_out, static_cast<size_t>(rows) * elem, cudaMemcpyDeviceToHost, P->stream));
+        if (P->n_lik > 0) {
+            SBN_CUDA(cudaMemcpyAsync(log_max.data(), P->d_log_max, static_cast<size_t>(rows) * 8, cudaMemcpyDeviceToHost, P->stream));
+            if (backward)
+                SBN_CUDA(cudaMemcpy2DAsync(static_cast<char *>(a.deriv) + r0 * elem, static_cast<size_t>(a.ld_deriv) * elem,
+                                           reinterpret_cast<char *>(P->d_out) + P->ld * elem, static_cast<size_t>(P->ld) * elem,
+                                           static_cast<size_t>(rows) * elem, static_cast<size_t>(P->n_lik),
+                                           cudaMemcpyDeviceToHost, P->stream));
+        }
+        SBN_CUDA(cudaStreamSynchronize(P->stream));
+        for (int64_t i = 0; i < rows; ++i) {
+            const double p = f64 ? reinterpret_cast<const double *>(prob.data())[i] : reinterpret_cast<const float *>(prob.data())[i];
+            if (a.prob) memcpy(static_cast<char *>(a.prob) + (r0 + i) * elem, prob.data() + i * elem, elem);
+            if (a.log_prob) a.log_prob[r0 + i] = std::log(p) + log_max[static_cast<size_t>(i)];  // NaN where flagged
+        }
+        return SBN_OK;
+    });
+    if (rc == SBN_OK && backward) {
+        std::vector<double> h(static_cast<size_t>(P->n_counts));
+        cudaError_t e = cudaMemcpyAsync(h.data(), P->d_counts, h.size() * 8, cudaMemcpyDeviceToHost, P->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(P->stream);
+        if (e != cudaSuccess) rc = fail(SBN_E_CUDA, "reading the count table failed: %s", cudaGetErrorString(e));
+        for (int64_t i = 0; rc == SBN_OK && i < P->n_counts; ++i) a.counts[i] += h[static_cast<size_t>(i)];
+    }
+    cudaStreamSynchronize(P->stream);  // nothing may still read the partial tables
+    cudaFree(P->d_partial);
+    P->d_partial = nullptr;
+    P->forward_run = false;
+    P->lik = nullptr;  // device pointers are the caller's: forget them
+    P->weight = nullptr;
+    return rc;
+}
+
+int sbn_program_grad_forward_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
+                                  int64_t ld_lik, int lik_on_device, float *prob, double *log_prob) {
+    GradArgs a;
+    a.lik = lik, a.ld_lik = ld_lik, a.lik_on_device = lik_on_device, a.prob = prob, a.log_prob = log_prob;
+    return grad_common(P, ev, ld_ev, n_rows, a, false);
+}
+
+int sbn_program_grad_forward_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
+                                      int64_t ld_lik, int lik_on_device, double *prob, double *log_prob) {
+    GradArgs a;
+    a.lik = lik, a.ld_lik = ld_lik, a.lik_on_device = lik_on_device, a.prob = prob, a.log_prob = log_prob;
+    return grad_common(P, ev, ld_ev, n_rows, a, true);
+}
+
+int sbn_program_grad_backward_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
+                                   int64_t ld_lik, int lik_on_device, const double *weights, int weights_on_device,
+                                   double *counts, int64_t n_counts, float *deriv, int64_t ld_deriv, float *prob) {
+    if (!weights) return fail(SBN_E_INVALID, "null weights");
+    GradArgs a;
+    a.lik = lik, a.ld_lik = ld_lik, a.lik_on_device = lik_on_device, a.weights = weights, a.weights_on_device = weights_on_device;
+    a.counts = counts, a.n_counts = n_counts, a.deriv = deriv, a.ld_deriv = ld_deriv, a.prob = prob;
+    return grad_common(P, ev, ld_ev, n_rows, a, false);
+}
+
+int sbn_program_grad_backward_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
+                                       int64_t ld_lik, int lik_on_device, const double *weights, int weights_on_device,
+                                       double *counts, int64_t n_counts, double *deriv, int64_t ld_deriv, double *prob) {
+    if (!weights) return fail(SBN_E_INVALID, "null weights");
+    GradArgs a;
+    a.lik = lik, a.ld_lik = ld_lik, a.lik_on_device = lik_on_device, a.weights = weights, a.weights_on_device = weights_on_device;
+    a.counts = counts, a.n_counts = n_counts, a.deriv = deriv, a.ld_deriv = ld_deriv, a.prob = prob;
+    return grad_common(P, ev, ld_ev, n_rows, a, true);
+}
+
 static int set_tables_common(sbn_program *P, const void *tables, int64_t n, bool f64) {
     if (!P) return fail(SBN_E_INVALID, "null program");
-    if (P->kind != kCounts)
-        return fail(SBN_E_INVALID, "only counts programs take new tables (other programs fold table products into their launches)");
+    if (P->kind != kCounts && P->kind != kGrad)
+        return fail(SBN_E_INVALID, "only counts and gradient programs take new tables (other programs fold table products into "
+                                   "their launches)");
     if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the table call");
     if (n != P->n_table_floats || (n > 0 && !tables))
         return fail(SBN_E_INVALID, "the table blob has %lld entries, not %lld", (long long)P->n_table_floats, (long long)n);

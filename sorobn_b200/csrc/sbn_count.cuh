@@ -21,6 +21,10 @@
 //     butterfly, also fixed, when all 32 share the key) and the group's lowest lane adds the sum to
 //     the warp's own partial table in global memory.  `sbn_count_reduce` then adds the partial
 //     tables into the count table, in partial-table order.
+//
+// `sbn_count_weighted_step` is the same step with a per-row double weight w_b (gradient programs,
+// planner.py KIND_COUNT of version 10): each contribution is multiplied by w_b / P_b, and a fully
+// observed family adds w_b.  Weights may be negative; the reduction order is the unweighted one.
 #pragma once
 #include "sbn_kernels.cuh"
 #include "sbn_marginal.cuh"
@@ -81,8 +85,9 @@ __device__ __forceinline__ double sbn_group_sum(double v, unsigned grp) {
     return s;
 }
 
-template <typename T, int C>
-__global__ void __launch_bounds__(SBN_COUNT_THREADS) sbn_count_step(const __grid_constant__ SbnCount p) {
+// The body of both count kernels; W: rows weighted by weight[b]
+template <typename T, int C, bool W>
+__device__ __forceinline__ void sbn_count_body(const SbnCount &p, const double *__restrict__ weight) {
     extern __shared__ __align__(16) float s_tab[];
     __shared__ __align__(8) uint64_t s_bar;
     sbn_pdl_entry();
@@ -116,10 +121,16 @@ __global__ void __launch_bounds__(SBN_COUNT_THREADS) sbn_count_step(const __grid
         const int64_t b = blk * SBN_COUNT_THREADS + threadIdx.x;
         int key = -1;  // -1: no contribution (past the last row, or out of range)
         double inv = 0.0;
+        double one = 1.0;  // what a fully observed family adds
         if (b < p.n_rows) {
             const double pr = static_cast<double>(static_cast<const T *>(p.prob)[p.prob_batched ? b : 0]);
             if (pr >= p.min_total) {  // false for NaN too
-                inv = 1.0 / pr;
+                if constexpr (W) {
+                    one = weight[b];
+                    inv = one / pr;
+                } else {
+                    inv = 1.0 / pr;
+                }
                 key = 0;
                 for (int k = 0; k < p.n_key; ++k)
                     key += min(static_cast<int>(p.ev[static_cast<int64_t>(p.key_col[k]) * p.ld_ev + b]), p.key_card[k] - 1) *
@@ -130,7 +141,7 @@ __global__ void __launch_bounds__(SBN_COUNT_THREADS) sbn_count_step(const __grid
         const bool lead = key >= 0 && lane == __ffs(grp) - 1;
 
         if (n_in == 0) {  // a histogram of the keys
-            const double v = sbn_group_sum(key >= 0 ? 1.0 : 0.0, grp);
+            const double v = sbn_group_sum(key >= 0 ? one : 0.0, grp);
             if (lead) part[key] += v;
             __syncwarp();
             continue;
@@ -207,6 +218,17 @@ __global__ void __launch_bounds__(SBN_COUNT_THREADS) sbn_count_step(const __grid
     }
 }
 
+template <typename T, int C>
+__global__ void __launch_bounds__(SBN_COUNT_THREADS) sbn_count_step(const __grid_constant__ SbnCount p) {
+    sbn_count_body<T, C, false>(p, nullptr);
+}
+
+template <typename T, int C>
+__global__ void __launch_bounds__(SBN_COUNT_THREADS) sbn_count_weighted_step(const __grid_constant__ SbnCount p,
+                                                                              const double *__restrict__ weight) {
+    sbn_count_body<T, C, true>(p, weight);
+}
+
 // count[e] += sum over the partial tables, in partial-table order
 __global__ void sbn_count_reduce(const double *__restrict__ partial, int64_t n_parts, int32_t n_entries,
                                  double *__restrict__ counts) {
@@ -227,11 +249,18 @@ __global__ void sbn_count_prob(const T *__restrict__ prob, int32_t prob_batched,
     out[b] = static_cast<double>(v) >= min_total ? v : static_cast<T>(__int_as_float(0x7fc00000));
 }
 
+// `weight` non-null: the weighted step (gradient programs)
 template <typename T>
-inline cudaError_t sbn_count_launch(const SbnCount &c, int64_t grid, size_t smem, double *counts, cudaStream_t stream) {
-    if (c.cs <= 2) sbn_count_step<T, 2><<<static_cast<unsigned>(grid), SBN_COUNT_THREADS, smem, stream>>>(c);
-    else if (c.cs <= 4) sbn_count_step<T, 4><<<static_cast<unsigned>(grid), SBN_COUNT_THREADS, smem, stream>>>(c);
-    else sbn_count_step<T, 8><<<static_cast<unsigned>(grid), SBN_COUNT_THREADS, smem, stream>>>(c);
+inline cudaError_t sbn_count_launch(const SbnCount &c, int64_t grid, size_t smem, double *counts, cudaStream_t stream,
+                                    const double *weight = nullptr) {
+    const unsigned g = static_cast<unsigned>(grid);
+    if (weight) {
+        if (c.cs <= 2) sbn_count_weighted_step<T, 2><<<g, SBN_COUNT_THREADS, smem, stream>>>(c, weight);
+        else if (c.cs <= 4) sbn_count_weighted_step<T, 4><<<g, SBN_COUNT_THREADS, smem, stream>>>(c, weight);
+        else sbn_count_weighted_step<T, 8><<<g, SBN_COUNT_THREADS, smem, stream>>>(c, weight);
+    } else if (c.cs <= 2) sbn_count_step<T, 2><<<g, SBN_COUNT_THREADS, smem, stream>>>(c);
+    else if (c.cs <= 4) sbn_count_step<T, 4><<<g, SBN_COUNT_THREADS, smem, stream>>>(c);
+    else sbn_count_step<T, 8><<<g, SBN_COUNT_THREADS, smem, stream>>>(c);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     const int threads = 256;
@@ -244,5 +273,8 @@ inline cudaError_t sbn_count_set_attrs() {
     cudaError_t e = cudaFuncSetAttribute(sbn_count_step<float, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, SBN_SMEM_BUDGET);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(sbn_count_step<float, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, SBN_SMEM_BUDGET);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(sbn_count_step<float, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, SBN_SMEM_BUDGET);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(sbn_count_weighted_step<float, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, SBN_SMEM_BUDGET);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(sbn_count_weighted_step<float, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, SBN_SMEM_BUDGET);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(sbn_count_weighted_step<float, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, SBN_SMEM_BUDGET);
     return e;
 }

@@ -78,7 +78,7 @@ inline int64_t round_up(int64_t v, int64_t m) { return (v + m - 1) / m * m; }
 struct SbnSegment;  // sbn_chain.h
 struct SbnPair;     // sbn_pair.h
 
-// What a program computes, fixed by its header version (4 .. 9 in this order)
+// What a program computes, fixed by its header version (4 .. 10 in this order)
 enum ProgramKind {
     kPosterior,  // kind-0 / 1 steps, then the normalised posterior slot
     kMarginals,  // kind-2 readouts write the posterior, already normalised; no posterior slot
@@ -88,6 +88,8 @@ enum ProgramKind {
                  // one draw, post_slot holds max log P(x, e)
     kMap,        // marginal MAP: an MPE program whose kind-0 / 1 steps each sum out (log-sum-exp) or maximise,
                  // post_slot holds max log P(x_MAP, e); it runs through the MPE entry point
+    kGrad,       // gradient: a counts program whose kind-3 steps are weighted per row, plus kind-6 derivative
+                 // readouts written to rows 1 .. of the output; row 0 and post_slot hold P(observed)
 };
 
 // Programs on log tables (MPE and marginal MAP): float32 only, the log-domain step kernels only
@@ -104,10 +106,11 @@ struct GraphKey {
     int64_t n_draws = 0, ld_drawn = 0;
     const void *lik = nullptr;      // soft-evidence program: the likelihoods the pack reads, and their pitch
     int64_t ld_lik = 0;
+    const void *weight = nullptr;   // gradient program: the row weights of the count steps
     bool operator==(const GraphKey &o) const {
         return ev == o.ev && out == o.out && ld_ev == o.ld_ev && n_rows == o.n_rows && ld_out == o.ld_out &&
                partial == o.partial && drawn == o.drawn && n_draws == o.n_draws && ld_drawn == o.ld_drawn &&
-               lik == o.lik && ld_lik == o.ld_lik;
+               lik == o.lik && ld_lik == o.ld_lik && weight == o.weight;
     }
 };
 struct CachedGraph {
@@ -141,6 +144,14 @@ struct sbn_program {
     double *d_log_max = nullptr;
     const void *lik = nullptr;
     int64_t ld_lik = 0;
+    // gradient program: per step, whether P(observed) depends on it (the steps a forward run issues); the staging
+    // buffer of host weights [reserved]; the weights the next backward issue reads; whether the next issue is a
+    // forward run, and the forward run's own graph
+    std::vector<char> forward;
+    double *d_weight = nullptr;
+    const double *weight = nullptr;
+    bool forward_run = false;
+    CachedGraph forward_graph;
     std::vector<std::pair<int64_t, int64_t>> tables;  // (offset, size) in floats
     std::vector<int64_t> table_padded;
     float *d_tables = nullptr;

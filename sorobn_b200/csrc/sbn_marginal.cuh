@@ -64,8 +64,12 @@ struct SbnMarginal {
     SbnMargIn in[SBN_MAX_IN];
 };
 
-template <typename T, int C>
-__global__ void __launch_bounds__(SBN_MARG_THREADS) sbn_marginal_step(const __grid_constant__ SbnMarginal p) {
+// The body of the marginals readout and of the derivative readout of gradient programs (sbn_deriv.cuh).
+// D = false: the segment is normalised (above).  D = true: each entry is divided by the row's P(observed),
+// prob[b] (prob_batched) or prob[0], in double, and rounded to T once; a row whose P(observed) is below
+// min_total (or zero / NaN) is written NaN.
+template <typename T, int C, bool D>
+__device__ __forceinline__ void sbn_readout_body(const SbnMarginal &p, const void *prob, int32_t prob_batched) {
     extern __shared__ __align__(16) float s_tab[];
     __shared__ __align__(8) uint64_t s_bar;
     sbn_pdl_entry();
@@ -122,7 +126,14 @@ __global__ void __launch_bounds__(SBN_MARG_THREADS) sbn_marginal_step(const __gr
     const int n_in = p.n_in, n_common = p.n_common, cz = p.cz, card = p.card;
     // float: runs of SBN_MARG_PART joint states; double: one run (the partial sum is the sum)
     constexpr int kRun = std::is_same<T, float>::value ? SBN_MARG_PART : (1 << 30);
-    double total = 0.0, lo = p.min_total;
+    double total = 0.0, lo = p.min_total;  // D: `total` holds the row's P(observed)
+    if constexpr (D) {
+        total = static_cast<double>(static_cast<const T *>(prob)[prob_batched ? b : 0]);
+        if (!(total >= p.min_total)) {  // out of range, zero or NaN
+            for (int s = 0; s < card; ++s) out[static_cast<int64_t>(s) * p.ld_out] = static_cast<T>(__int_as_float(0x7fc00000));
+            return;
+        }
+    }
     double acc[C];  // after the last pass: its sums (all of them when card <= C)
     for (int s0 = 0; s0 < card; s0 += C) {
 #pragma unroll
@@ -155,27 +166,41 @@ __global__ void __launch_bounds__(SBN_MARG_THREADS) sbn_marginal_step(const __gr
 #pragma unroll
             for (int s = 0; s < C; ++s) acc[s] += static_cast<double>(part[s]);
         }
+        if constexpr (D) {
 #pragma unroll
-        for (int s = 0; s < C; ++s) {
-            if (s0 + s < card) {
-                total += acc[s];
-                if (acc[s] > 0.0 && acc[s] < lo) lo = acc[s];
-                if (card > C) out[static_cast<int64_t>(s0 + s) * p.ld_out] = static_cast<T>(acc[s]);
+            for (int s = 0; s < C; ++s)
+                if (s0 + s < card) out[static_cast<int64_t>(s0 + s) * p.ld_out] = static_cast<T>(acc[s] / total);
+        } else {
+#pragma unroll
+            for (int s = 0; s < C; ++s) {
+                if (s0 + s < card) {
+                    total += acc[s];
+                    if (acc[s] > 0.0 && acc[s] < lo) lo = acc[s];
+                    if (card > C) out[static_cast<int64_t>(s0 + s) * p.ld_out] = static_cast<T>(acc[s]);
+                }
             }
         }
     }
-    const bool ok = total >= p.min_total && lo >= p.min_total;  // false for NaN too
-    const T nan = static_cast<T>(__int_as_float(0x7fc00000));
-    if (card <= C) {
+    if constexpr (!D) {
+        // false for NaN too (in this order the shared body compiles to the standalone kernel's instructions)
+        const bool ok = lo >= p.min_total && total >= p.min_total;
+        const T nan = static_cast<T>(__int_as_float(0x7fc00000));
+        if (card <= C) {
 #pragma unroll
-        for (int s = 0; s < C; ++s)
-            if (s < card) out[static_cast<int64_t>(s) * p.ld_out] = ok ? static_cast<T>(acc[s] / total) : nan;
-    } else {
-        for (int s = 0; s < card; ++s) {
-            T *o = out + static_cast<int64_t>(s) * p.ld_out;
-            *o = ok ? static_cast<T>(static_cast<double>(*o) / total) : nan;
+            for (int s = 0; s < C; ++s)
+                if (s < card) out[static_cast<int64_t>(s) * p.ld_out] = ok ? static_cast<T>(acc[s] / total) : nan;
+        } else {
+            for (int s = 0; s < card; ++s) {
+                T *o = out + static_cast<int64_t>(s) * p.ld_out;
+                *o = ok ? static_cast<T>(static_cast<double>(*o) / total) : nan;
+            }
         }
     }
+}
+
+template <typename T, int C>
+__global__ void __launch_bounds__(SBN_MARG_THREADS) sbn_marginal_step(const __grid_constant__ SbnMarginal p) {
+    sbn_readout_body<T, C, false>(p, nullptr, 0);
 }
 
 // C = the smallest instantiated accumulator count that covers the target (8 and passes beyond)

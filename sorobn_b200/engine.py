@@ -16,7 +16,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libsorobn_
 _lib = None
 
 SBN_OK = 0
-ABI_VERSION = 15
+ABI_VERSION = 16
 
 
 class EngineError(RuntimeError):
@@ -86,6 +86,12 @@ def load():
         getattr(lib, name).argtypes = [vp, vp, i64, i64, vp, i64, i32, i64, c.c_uint64, i64, vp, vp, vp]
     lib.sbn_program_mpe_soft_host.restype = i32
     lib.sbn_program_mpe_soft_host.argtypes = [vp, vp, i64, i64, vp, i64, i32, vp, vp]
+    for name in ("sbn_program_grad_forward_host", "sbn_program_grad_forward_host_f64"):
+        getattr(lib, name).restype = i32
+        getattr(lib, name).argtypes = [vp, vp, i64, i64, vp, i64, i32, vp, vp]
+    for name in ("sbn_program_grad_backward_host", "sbn_program_grad_backward_host_f64"):
+        getattr(lib, name).restype = i32
+        getattr(lib, name).argtypes = [vp, vp, i64, i64, vp, i64, i32, vp, i32, vp, i64, vp, i64, vp]
     lib.sbn_program_destroy.restype = None
     lib.sbn_program_destroy.argtypes = [vp]
     lib.sbn_program_reserve.restype = i32
@@ -132,7 +138,8 @@ EXPORTS = (
     "sbn_program_set_tables_f64", "sbn_program_sample_host", "sbn_program_sample_host_f64", "sbn_program_mpe_host",
     "sbn_program_run_soft_host", "sbn_program_run_soft_host_f64", "sbn_program_counts_soft_host",
     "sbn_program_counts_soft_host_f64", "sbn_program_sample_soft_host", "sbn_program_sample_soft_host_f64",
-    "sbn_program_mpe_soft_host",
+    "sbn_program_mpe_soft_host", "sbn_program_grad_forward_host", "sbn_program_grad_forward_host_f64",
+    "sbn_program_grad_backward_host", "sbn_program_grad_backward_host_f64",
     "sbn_program_info", "sbn_program_set_graph", "sbn_program_set_tiled", "sbn_gibbs_create", "sbn_gibbs_run_host",
     "sbn_sampler_run_host", "sbn_gibbs_conditional", "sbn_gibbs_destroy", "sbn_host_alloc", "sbn_host_free",
 )
@@ -336,8 +343,65 @@ class Program:
                                                         None if log_ev is None else log_ev.ctypes.data))
         return (counts, prob, log_ev) if log_evidence else (counts, prob)
 
+    def _grad_lik(self, lik, n_rows):
+        """`_likelihoods` of a gradient program, which may have no soft variable: then `lik` must be None."""
+        if not self.plan.soft:
+            if lik is not None:
+                raise ValueError("likelihoods given to a gradient program without soft variables")
+            return None, (None, 0, 0)
+        if lik is None:
+            raise ValueError("a gradient program with soft variables needs their likelihoods")
+        return self._likelihoods(lik, n_rows)
+
+    def grad_forward(self, codes: np.ndarray, n_rows: int, lik=None):
+        """Gradient programs (planner.build_pattern_plan kind "grad"): (P(observed, lik / max) [n_rows], NaN for a
+        row the float32 range rule flags; log P(observed, lik) float64 [n_rows]).  Only the launches P(observed)
+        depends on run.  `lik` as in `run_soft`, for a program with soft variables."""
+        n_rows = int(n_rows)
+        codes, ev_ptr = self._evidence(codes, n_rows)
+        lik, lik_args = self._grad_lik(lik, n_rows)
+        prob = np.empty(n_rows, dtype=self.dtype)
+        log_prob = np.empty(n_rows, dtype=np.float64)
+        _check(self._fn("sbn_program_grad_forward_host")(self._h, ev_ptr, n_rows, n_rows, *lik_args, prob.ctypes.data,
+                                                         log_prob.ctypes.data))
+        return prob, log_prob
+
+    def grad_backward(self, codes: np.ndarray, n_rows: int, weights, lik=None):
+        """Gradient programs: (weighted counts float64 [n_counts] = sum_b w_b * P(family entry | observed, lik),
+        derivative readouts [n_lik, n_rows] = d log P(observed, lik / max) / d (lik / max), P(observed, lik / max)
+        [n_rows]), NaN readouts and P(observed) for a flagged row, which adds nothing.  `weights` [n_rows] is a
+        numpy array or a torch tensor; a CUDA tensor on the program's device is read in place, as `lik` is."""
+        n_rows = int(n_rows)
+        codes, ev_ptr = self._evidence(codes, n_rows)
+        lik, lik_args = self._grad_lik(lik, n_rows)
+        on_device = False
+        if type(weights).__module__.startswith("torch"):
+            if weights.is_cuda:
+                import torch
+
+                if weights.device.index != self.device:
+                    raise ValueError(f"weights on cuda:{weights.device.index}; the program runs on cuda:{self.device}")
+                weights = weights.to(torch.float64).contiguous()
+                torch.cuda.current_stream(weights.device).synchronize()
+                on_device = True
+            else:
+                weights = weights.detach().numpy()
+        if not on_device:
+            weights = np.ascontiguousarray(weights, dtype=np.float64)
+        if tuple(weights.shape) != (n_rows,):
+            raise ValueError(f"weights have shape {tuple(weights.shape)}, expected {(n_rows,)}")
+        n_lik = self.Q - 1
+        counts = np.zeros(int(self.plan.n_counts), dtype=np.float64)
+        deriv = np.empty((n_lik, n_rows), dtype=self.dtype)
+        prob = np.empty(n_rows, dtype=self.dtype)
+        _check(self._fn("sbn_program_grad_backward_host")(
+            self._h, ev_ptr, n_rows, n_rows, *lik_args, weights.data_ptr() if on_device else weights.ctypes.data,
+            int(on_device), counts.ctypes.data, counts.size, deriv.ctypes.data if n_lik else None, n_rows,
+            prob.ctypes.data))
+        return counts, deriv, prob
+
     def set_tables(self, blob: np.ndarray):
-        """Replace a counts program's tables (planner.refresh_tables gives the blob of new CPTs)."""
+        """Replace a counts or gradient program's tables (planner.refresh_tables gives the blob of new CPTs)."""
         blob = np.ascontiguousarray(blob, dtype=self.dtype)
         _check(self._fn("sbn_program_set_tables")(self._h, blob.ctypes.data, blob.size))
 

@@ -143,6 +143,23 @@ as in version 8 (a bucket of MAP variables, and every product-only step).  No la
 Argmax steps (kind 5, the words of version 8) decode the MAP buckets only: their separators hold MAP and
 observed variables alone, because every summed variable is gone by then.  `p_slot` holds
 max_{x_MAP} log P(x_MAP, e).
+
+Gradient programs (`build_pattern_plan(net, "grad", ...)`, VERSION 10) give the derivatives of
+log P(observed cells, lik) of every row (DESIGN.md "Gradients of the log-likelihood").  They are counts
+programs plus one derivative readout (kind 6) per soft variable s:
+
+    header : MAGIC 10 1 n_ev n_tables n_slots n_steps Q p_slot p_batched n_counts n_soft
+    kind 6 : 6 n_in -1 1 n_elim q_offset | card_s | ecards[n_elim] | inputs as above
+
+Q = 1 + the likelihood columns.  The count steps add each row's family posterior times a per-row weight
+w_b given at run time (a fully observed family adds w_b), which is sum_b w_b * theta * d log P_b / d theta.
+A kind-6 step reads the bucket k that lambda_s entered, with every input of that bucket except lambda_s:
+
+    D_s(x, b) = sum_{U_k - s} pi_k * prod_{f in F_k, f != lambda_s} f  /  P(observed)
+
+written at rows `q_offset ..` (1 + the soft variable's first likelihood column) of the run's output; row 0 is
+P(observed).  D_s is d log P / d lambda_s, exact where lambda_s(x) = 0.  `Plan.forward_steps` lists the steps
+P(observed) depends on (the upward pass): a forward run issues only those.
 """
 from __future__ import annotations
 
@@ -181,6 +198,8 @@ SAMPLE_MAX_TERMS = 16  # gathered (col stride card) terms per input of a sample 
 KIND_ARGMAX = 5  # decode one bucket's eliminated variables given the decoded separator (MPE programs only)
 VERSION_MPE = 8
 VERSION_MAP = 9  # marginal MAP: the MPE words plus a reduction word on kind-0 / kind-1 steps
+KIND_DERIV = 6  # derivative of P(observed) by one soft variable's likelihood, over P(observed) (gradient programs only)
+VERSION_GRAD = 10
 REDUCE_MAX, REDUCE_LOGSUMEXP = 0, 1
 HEADER_WORDS = 12
 
@@ -276,6 +295,9 @@ class Plan:
     sampled: tuple = ()  # sample / MPE plans: the var id of every drawn (decoded) code row, in drawing order
     soft: tuple = ()  # soft-evidence var ids, sorted by name (== likelihood column order)
     soft_slots: tuple = ()  # the slot of every soft variable's likelihood, in `soft` order
+    # gradient plans: indices of the steps P(observed) depends on, in program order.  The engine derives the same set
+    # from the slot words (csrc/sbn_api.cu parse); the CPU replay reads this one, and a GPU test checks the two agree
+    forward_steps: tuple = ()
 
     # ---- cost model (DESIGN.md "algorithmic bytes") -------------------------------
     def bytes_per_row(self, n_draws=1):
@@ -500,14 +522,22 @@ def build_pattern_plan(net: CompiledNet, kind, evidence, soft=(), map_vars=None,
     `map_vars` are the MAP variables), the observed columns `evidence` and the var ids `soft` whose per-row
     likelihoods arrive at run time (see the module docstring).  A soft variable may not be evidence; it may be
     a MAP variable.  With `soft=()` the plan is the one of the kind's own builder (`build_counts_plan`, ...),
-    word for word; `kw` are that builder's options."""
+    word for word; `kw` are that builder's options.
+
+    `kind` "grad" plans the gradient program of the pattern (version 10, soft evidence or not): the counts
+    program's steps with weighted counts, plus one derivative readout per soft variable."""
     builders = {"counts": build_counts_plan, "sample": build_sample_plan, "mpe": build_mpe_plan, "map": build_map_plan}
-    if kind not in builders:
-        raise ValueError(f"kind must be one of {sorted(builders)}, not {kind!r}")
+    if kind not in builders and kind != "grad":
+        raise ValueError(f"kind must be one of {sorted([*builders, 'grad'])}, not {kind!r}")
     if (map_vars is not None) != (kind == "map"):
         raise ValueError("map_vars go with kind 'map' only, and kind 'map' needs them")
     evidence = tuple(evidence)
     soft = _check_soft(net, evidence, soft, kw.get("mode", MODE_BATCHED))
+    if kind == "grad":
+        if kw.get("mode", MODE_BATCHED) != MODE_BATCHED:
+            raise ValueError("a gradient program is batched")
+        hidden = tuple(v for v in range(len(net.names)) if v not in set(evidence))
+        return _build(net, VERSION_GRAD, evidence, targets=hidden, soft=soft, **kw)
     if not soft:
         return builders[kind](net, evidence, *(() if map_vars is None else (map_vars,)), **kw)
     hidden = tuple(v for v in range(len(net.names)) if v not in set(evidence))
@@ -875,8 +905,8 @@ def _build(net, version, evidence, query=(), targets=(), mode=MODE_BATCHED, orde
 
     if version == VERSION_MARGINALS:
         return _marginals_passes(b, buckets, factors, targets)
-    if version == VERSION_COUNTS:
-        return _counts_passes(b, buckets, factors)
+    if version in (VERSION_COUNTS, VERSION_GRAD):
+        return _counts_passes(b, buckets, factors, grad=version == VERSION_GRAD)
     if version in (VERSION_SAMPLE, VERSION_MPE, VERSION_MAP):
         return _sample_passes(b, buckets, factors, version)
 
@@ -922,17 +952,21 @@ def _marginals_passes(b, buckets, leftovers, targets):
     return b.finish(VERSION_MARGINALS, None, q, targets=t_sorted)
 
 
-def _counts_passes(b, buckets, leftovers):
+def _counts_passes(b, buckets, leftovers, grad=False):
     """Downward pass and count steps of a counts plan (DESIGN.md "Expected counts and EM").
 
     The unobserved members M_v of v's family are read from the smallest bucket k with M_v in U_k (the
     bucket the CPT of v entered has them all):
         counts_v(M_v; key(row)) += sum_{U_k - M_v} pi_k * prod_{f in F_k} f / P(observed),
-    where P(observed) is the product of every leftover scalar of the upward pass, computed once."""
+    where P(observed) is the product of every leftover scalar of the upward pass, computed once.
+
+    grad=True: a gradient plan (version 10), whose derivative readouts (`_deriv_steps`) follow the count
+    steps on the same downward messages."""
     card, names, ev_col = b.card, b.net.names, b.ev_col
     members = {v: [u for u in b.net.scope(v) if u not in ev_col] for v in range(len(names))}
     read = {v: _smallest_bucket(b, buckets, set(M)) for v, M in members.items() if M}
-    pi = _downward(b, buckets, leftovers, read.values())
+    deriv = _deriv_buckets(b, buckets) if grad else {}
+    pi = _downward(b, buckets, leftovers, [*read.values(), *deriv.values()])
     prob = b.emit(b.fold(leftovers), (), [], may_lift=False)
 
     c_offsets, n_counts = count_layout(b.net)
@@ -955,8 +989,60 @@ def _counts_passes(b, buckets, leftovers):
                              f"{MARGINAL_MAX_Z}, their product below 2^31)")
         b.steps.append(Step(KIND_COUNT, ins, -1, out_vars, tuple(int(card[u]) for u in out_vars), elims, ecards,
                             q_offset=c_offsets[v], key=key, cstrides=tuple(stride[u] for u in out_vars), norm=prob))
+    if not grad:
+        b.steps = _prune_dead(b.steps)
+        return b.finish(VERSION_COUNTS, prob, 1, n_counts=n_counts, count_offsets=c_offsets)
+    q = _deriv_steps(b, buckets, pi, deriv, prob)
     b.steps = _prune_dead(b.steps)
-    return b.finish(VERSION_COUNTS, prob, 1, n_counts=n_counts, count_offsets=c_offsets)
+    forward = _closure(b.steps, prob.buf)
+    return b.finish(VERSION_GRAD, prob, q, n_counts=n_counts, count_offsets=c_offsets, forward_steps=forward)
+
+
+def _deriv_buckets(b, buckets):
+    """{soft var id: the bucket its likelihood entered}; ValueError for a likelihood that was folded into another
+    factor first, which leaves no bucket holding it as an input of its own."""
+    out = {}
+    for v, lid in b.soft:
+        k = next((k for k, (F, _, _, _) in enumerate(buckets) if any(f.is_slot and f.buf == lid for f in F)), None)
+        if k is None:
+            raise ValueError(f"the likelihood of {b.net.names[v]!r} was folded into another factor before its bucket: "
+                             "no derivative readout can leave it out")
+        out[v] = k
+    return out
+
+
+def _deriv_steps(b, buckets, pi, deriv, prob):
+    """The derivative readouts of a gradient plan, soft variables in likelihood-column order: s is read from the
+    bucket its likelihood entered, every input but the likelihood, summed over the rest of the bucket.  Returns
+    the rows of the run's output (1 + the likelihood columns)."""
+    card, names = b.card, b.net.names
+    q = 1
+    for v, lid in b.soft:
+        k = deriv[v]
+        F_k, X, _, lam = buckets[k]
+        F = [f for f in F_k if not (f.is_slot and f.buf == lid)]
+        U = set().union(*[f.vars for f in F], *([pi[k].vars] if pi[k] is not None else []))
+        ins, elims, ecards = _bucket_read(b, (F, X, U, lam), pi[k], (v,))
+        cz = b.size(elims)
+        if cz > MARGINAL_MAX_Z or cz * int(card[v]) >= 2**31:
+            raise ValueError(f"the bucket read for the likelihood of {names[v]!r} is too large for a readout: {cz} "
+                             f"joint states summed out (at most {MARGINAL_MAX_Z}) x {int(card[v])} states (below 2^31)")
+        b.steps.append(Step(KIND_DERIV, ins, -1, (v,), (int(card[v]),), elims, ecards, q_offset=q, norm=prob))
+        q += int(card[v])
+    return q
+
+
+def _closure(steps, lid):
+    """Indices of the steps the factor of logical id `lid` depends on, in program order."""
+    by_id = {st.out_id: st for st in steps if st.kind in (KIND_FLAT, KIND_BATCHED)}
+    need, stack = set(), [lid]
+    while stack:
+        i = stack.pop()
+        if i in need or i not in by_id:  # a likelihood has no producer
+            continue
+        need.add(i)
+        stack.extend(f.buf for f, _, _ in by_id[i].inputs if f.is_slot)
+    return tuple(i for i, st in enumerate(steps) if st.kind in (KIND_FLAT, KIND_BATCHED) and st.out_id in need)
 
 
 def _sample_passes(b, buckets, leftovers, version):
@@ -1073,7 +1159,7 @@ def _prune_dead(steps):
     """Drop the launches nothing reads (the root buckets' own messages when no other root needs them)."""
     used, keep = set(), []
     for st in reversed(steps):
-        if st.kind in (KIND_MARGINAL, KIND_COUNT) or st.out_id in used:
+        if st.kind in (KIND_MARGINAL, KIND_COUNT, KIND_DERIV) or st.out_id in used:
             keep.append(st)
             used.update(f.buf for f, _, _ in st.inputs if f.is_slot)
             if st.norm is not None:
@@ -1317,9 +1403,9 @@ def _serialise(plan: Plan, table_arrays):
     plan.table_offsets = offsets
 
     extra = [0, 0]
-    if plan.version in (VERSION, VERSION_COUNTS, VERSION_SAMPLE, VERSION_MPE, VERSION_MAP):
+    if plan.version in (VERSION, VERSION_COUNTS, VERSION_SAMPLE, VERSION_MPE, VERSION_MAP, VERSION_GRAD):
         post = [plan.post_slot, int(plan.slots[plan.post_slot][0])]
-        if plan.version == VERSION_COUNTS:
+        if plan.version in (VERSION_COUNTS, VERSION_GRAD):
             extra = [plan.n_counts, 0]
         elif plan.version in (VERSION_SAMPLE, VERSION_MPE, VERSION_MAP):
             extra = [len(plan.sampled), 0]
@@ -1340,7 +1426,7 @@ def _serialise(plan: Plan, table_arrays):
         w += [s, int(plan._card[v])]
     for st in plan.steps:
         w += [st.kind, len(st.inputs), st.out_slot, len(st.cards), len(st.ecards)]
-        if st.kind == KIND_MARGINAL:
+        if st.kind in (KIND_MARGINAL, KIND_DERIV):
             w.append(st.q_offset)
         elif st.kind == KIND_COUNT:
             w += [st.q_offset, len(st.key)]
