@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SBN_ABI_VERSION 16
+#define SBN_ABI_VERSION 17
 
 #define SBN_OK 0
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
@@ -219,6 +219,19 @@ int sbn_program_grad_backward_host_f64(sbn_program *prog, const uint8_t *ev, int
                                        const double *lik, int64_t ld_lik, int lik_on_device, const double *weights,
                                        int weights_on_device, double *counts, int64_t n_counts, double *deriv,
                                        int64_t ld_deriv, double *prob);
+
+/* Per-row joint posteriors of a joint program (planner.build_joint_plan / build_pattern_plan kind "joint",
+ * version 11; every other call refuses it, and these calls refuse every other program).  `lik` is NULL exactly
+ * when the program has no soft variables; otherwise `lik`, `ld_lik` and `lik_on_device` are those of
+ * sbn_program_run_soft_host.  out[q * ld_out + b] = row q of the program's output for row b: the joint posterior
+ * of each group's unobserved members at its rows (planner: Plan.group_rows; the first member fastest), given
+ * the row's observed cells and likelihoods.  prob[b] = P(observed, lik / max).  A row below the float32 range
+ * (1e-30; 1e-290 for the float64 twin) or of probability zero reads NaN throughout: re-run it with the float64
+ * program.  No atomics: two calls give bitwise the same results.  Large batches run in chunks. */
+int sbn_program_joint_host(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
+                           int64_t ld_lik, int lik_on_device, float *out, int64_t ld_out, float *prob);
+int sbn_program_joint_host_f64(sbn_program *prog, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
+                               int64_t ld_lik, int lik_on_device, double *out, int64_t ld_out, double *prob);
 
 /* Same with DEVICE buffers, asynchronous on `stream` (a cudaStream_t; NULL = default
  * stream).  n_rows must not exceed the reserved chunk size. */

@@ -29,7 +29,8 @@ samples of the missing cells and latent nodes, one sample program per pattern
 explanation, one log-domain max-sum program per pattern (planner.build_mpe_plan, csrc/sbn_mpe.cuh).
 `map_many` / `map` find the marginal MAP state of chosen variables (by default the missing cells), the
 other unobserved variables summed out: one log-sum-exp, then max-sum program per pattern
-(planner.build_map_plan).
+(planner.build_map_plan).  `joint_marginals_many` returns, for every row, the joint posterior of every CPT
+family or of chosen groups of variables, one joint program per pattern (planner.build_joint_plan).
 """
 from __future__ import annotations
 
@@ -418,6 +419,88 @@ class BayesNet:
             size = int(np.prod(net.cpt[v].shape))
             out[name] = pd.Series(counts[offsets[v]:offsets[v] + size], index=self._family_index(v), name=name)
         return out
+
+    def joint_marginals_many(self, X: pd.DataFrame, groups=None, likelihoods: dict | None = None) -> dict:
+        """For every row of `X`, the joint posterior of every CPT family, or of chosen groups of variables, given
+        the row's observed cells (and likelihoods), computed on the GPU.
+
+        Missing data follows `expected_counts`: the columns of `X` are observed cells, None or NaN is a missing
+        cell, a node without a column is latent, and `likelihoods` is soft evidence.  `groups` lists the entries
+        to return: a node name gives that node's family with axes [*parents, node] (the dense CPT order of
+        `cpt_tensors`); a tuple of node names gives that group, in the given order.  Default: every node's family.
+        A single name or tuple is one entry.
+
+        Returns {entry: DataFrame} indexed like `X`, with one column per joint state of the group (a MultiIndex
+        with one level per member, states sorted); each row sums to 1.  An observed member is a one-hot on the
+        row's observed state, so the frame's shape does not depend on the row's missingness.  A row whose observed
+        cells and likelihoods have probability zero is NaN in every frame.  Raises ValueError for a value outside
+        its variable's domain, an unknown node and a duplicate member.
+
+        Summed over the rows, the family frames are `expected_counts(X)`.  Rows are grouped by missingness pattern;
+        each pattern is one joint program (planner.build_joint_plan): the counts program's upward and downward
+        passes with a per-row readout of every group in place of the count steps (csrc/sbn_count.cuh
+        `sbn_joint_step`).  Rows the float32 program cannot hold re-run in float64."""
+        net = self._net("computing joint posteriors")
+        if groups is None:
+            groups = list(net.names)
+        elif isinstance(groups, (str, tuple)):
+            groups = [groups]
+        entries, gids = [], []
+        for g in groups:
+            members = (g,) if isinstance(g, str) else tuple(g)
+            unknown = [m for m in members if m not in net.index]
+            if unknown:
+                raise ValueError(f"group {g!r}: {unknown[:5]} are not nodes of the network")
+            if isinstance(g, str):
+                ids = tuple(net.scope(net.index[g]))
+            else:
+                ids = tuple(net.index[m] for m in members)
+                if not ids or len(set(ids)) != len(ids):
+                    raise ValueError(f"group {g!r} is empty or has a duplicate member")
+            if g not in entries:
+                entries.append(g)
+                gids.append(ids)
+        gids = tuple(gids)
+        pattern_groups = self._count_patterns(X)
+        soft, lik = self._pattern_soft(likelihoods, X)
+        n = len(X.index)
+        dense = [np.zeros((n, int(np.prod([int(net.card[u]) for u in ids])))) for ids in gids]
+        for ev, rows, codes in pattern_groups:
+            col = {v: i for i, v in enumerate(ev)}
+            if all(u in col for ids in gids for u in ids):
+                # nothing to read out: P(observed) alone decides the rows, from the pattern's counts program
+                runner = self._pattern_runner("counts", ev, soft=soft)
+                run = (lambda p, c, r: (None, p.counts(c, len(r))[1])) if lik is None else \
+                    (lambda p, c, r: (None, p.counts(c, len(r), lik=_lik_rows(lik, r))[1]))
+            else:
+                # fetched right before it runs, as in `sample_many`
+                runner = self._programs(("joint", ev, gids, soft), lambda: _planner.build_pattern_plan(
+                    net, "joint", ev, soft=soft, groups=gids))
+                run = lambda p, c, r: p.joint(c, len(r), lik=None if lik is None else _lik_rows(lik, r))  # noqa: E731
+            out, prob, flagged, again = self._run_pattern(runner, run, codes, rows)
+            bad = np.isnan(prob)
+            for k, ids in enumerate(gids):
+                cards = [int(net.card[u]) for u in ids]
+                strides = [int(np.prod(cards[j + 1:], dtype=np.int64)) for j in range(len(ids))]
+                base = np.zeros(len(rows), dtype=np.int64)
+                for u, s in zip(ids, strides):
+                    if u in col:
+                        base += codes[col[u]].astype(np.int64) * s
+                M = [(int(net.card[u]), s) for u, s in zip(ids, strides) if u not in col]
+                if not M:
+                    dense[k][rows, base] = 1.0
+                else:
+                    uoff = np.zeros(1, dtype=np.int64)
+                    for c, s in M:  # each later member slower: the first one fastest
+                        uoff = (uoff[None, :] + np.arange(c, dtype=np.int64)[:, None] * s).reshape(-1)
+                    q0 = runner.plan.group_rows[k]
+                    block = out[q0:q0 + len(uoff)].astype(np.float64)
+                    if again is not None:
+                        block[:, flagged] = again[q0:q0 + len(uoff)]
+                    dense[k][rows[:, None], base[:, None] + uoff[None, :]] = block.T
+                dense[k][rows[bad]] = np.nan
+        return {g: pd.DataFrame(d, index=X.index, columns=pd.MultiIndex.from_product(
+            [net.domains[u] for u in ids], names=[net.names[u] for u in ids])) for g, ids, d in zip(entries, gids, dense)}
 
     def fit_em(self, X: pd.DataFrame, max_iter: int = 100, tol: float = 1e-6,
                likelihoods: dict | None = None) -> "BayesNet":

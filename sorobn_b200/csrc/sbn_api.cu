@@ -66,7 +66,10 @@ constexpr int kVersionGrad = 10;      // planner.build_pattern_plan(kind "grad")
                                       // kind-6 derivative readouts, P(observed) in the posterior slot
 static_assert(kVersionMpe - kVersion == kMpe, "one program kind per header version, in order");
 static_assert(kVersionMap - kVersion == kMap, "one program kind per header version, in order");
+constexpr int kVersionJoint = 11;     // planner.build_joint_plan: version 6 with kind-7 per-row joint readouts in place of
+                                      // the count steps, P(observed) in the posterior slot
 static_assert(kVersionGrad - kVersion == kGrad, "one program kind per header version, in order");
+static_assert(kVersionJoint - kVersion == kJoint, "one program kind per header version, in order");
 constexpr int64_t kMarginalZoffMax = 1 << 24;  // int32 words of one readout's joint-state offset table
 constexpr int kMaxElim = 3;
 constexpr int kMaxZ = 256;
@@ -79,14 +82,16 @@ namespace {
 int parse(sbn_program *P, const int32_t *w, int64_t n) {
     if (n < kHeaderWords) return fail(SBN_E_INVALID, "program shorter than its header");
     if (w[0] != kMagic) return fail(SBN_E_INVALID, "bad program magic 0x%x", w[0]);
-    if (w[1] < kVersion || w[1] > kVersionGrad)
-        return fail(SBN_E_INVALID, "program version %d, engine expects %d, %d, %d, %d, %d, %d or %d", w[1], kVersion,
-                    kVersionMarginals, kVersionCounts, kVersionSample, kVersionMpe, kVersionMap, kVersionGrad);
+    if (w[1] < kVersion || w[1] > kVersionJoint)
+        return fail(SBN_E_INVALID, "program version %d, engine expects %d, %d, %d, %d, %d, %d, %d or %d", w[1], kVersion,
+                    kVersionMarginals, kVersionCounts, kVersionSample, kVersionMpe, kVersionMap, kVersionGrad, kVersionJoint);
     P->kind = static_cast<ProgramKind>(w[1] - kVersion);
     // a gradient program parses as a counts program plus its derivative readouts (kind 6)
     const bool grad = P->kind == kGrad;
     const bool marginals = P->kind == kMarginals, counts = P->kind == kCounts || grad, mpe = sbn_log_domain(P->kind);
     const bool map = P->kind == kMap;
+    // a joint program: the counts program's passes with kind-7 readouts in place of the count steps
+    const bool joint = P->kind == kJoint;
     // sample, MPE and marginal MAP programs share the words of their last steps
     const bool decodes = P->kind == kSample || mpe;
     P->mode = w[2];
@@ -103,6 +108,7 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         if ((!grad && P->Q != 1) || P->n_counts <= 0 || P->mode != (grad ? 1 : P->mode))
             return fail(SBN_E_INVALID, grad ? "bad gradient header" : "bad counts header");
     }
+    if (joint && (w[10] != 0 || P->mode != 1)) return fail(SBN_E_INVALID, "bad joint header");
     if (decodes) {
         P->n_sampled = w[10];
         if (P->Q != 1 || P->mode != 1 || P->n_sampled < 0)
@@ -132,7 +138,7 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         P->slots.push_back({batched != 0, size, round_up(size, 4), nullptr});
     }
     // (a gradient program's slot holds P(observed); its other output rows are written by the readouts)
-    if (!marginals && ((P->slots[P->post_slot].batched ? 1 : 0) != P->post_batched || P->slots[P->post_slot].size < (grad ? 1 : P->Q)))
+    if (!marginals && ((P->slots[P->post_slot].batched ? 1 : 0) != P->post_batched || P->slots[P->post_slot].size < (grad || joint ? 1 : P->Q)))
         return fail(SBN_E_INVALID, "posterior slot mismatch");
     {
         // soft evidence: (slot, card) of every likelihood, filled before step 0 (sbn_soft.cuh); n_soft is word 10
@@ -152,7 +158,7 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         }
     }
     if (grad && P->Q != 1 + P->n_lik) return fail(SBN_E_INVALID, "a gradient program writes 1 + %d rows, not %d", P->n_lik, P->Q);
-    std::vector<int> written(marginals || grad ? P->Q : 0, 0);  // posterior entries (gradient: output rows) written by the readouts
+    std::vector<int> written(marginals || grad || joint ? P->Q : 0, 0);  // posterior entries (gradient: output rows) written by the readouts
     for (int s = 0; s < n_steps; ++s) {
         if (!need(5)) return fail(SBN_E_INVALID, "truncated step %d", s);
         StepDesc st;
@@ -166,7 +172,8 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         const bool readout = st.kind == 2 || (grad && st.kind == 6);  // kind 6: the layout of kind 2
         const bool count = st.kind == 3;
         const bool draw = decodes && st.kind == decode_kind;
-        if (st.kind != 0 && st.kind != 1 && !(readout && (marginals || grad)) && !(count && counts) && !draw)
+        const bool jread = joint && st.kind == 7;  // the layout of kind 2, any number of output axes
+        if (st.kind != 0 && st.kind != 1 && !(readout && (marginals || grad)) && !(count && counts) && !draw && !jread)
             return fail(SBN_E_INVALID, "step %d: bad kind", s);
         if (draw) {
             // the drawn variables are the step's `n_elim` axes; they fill the next drawn-code rows
@@ -216,6 +223,13 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
                 return fail(SBN_E_INVALID, "step %d: count-table entries outside the table", s);
             st.span = span;
         }
+        if (jread) {
+            // the group's unobserved members are the output axes, written at output rows q_offset .. q_offset + n_out - 1
+            if (!need(1)) return fail(SBN_E_INVALID, "truncated step %d", s);
+            st.q_offset = w[p++];
+            if (st.out_slot != -1 || n_axes < 1 || n_axes > SBN_MAX_AXES || n_elim < 0 || n_elim > 64 || n_in < 1)
+                return fail(SBN_E_INVALID, "step %d: bad joint readout", s);
+        }
         if (readout) {
             // one output axis (the target), written at posterior rows q_offset .. q_offset + card - 1
             if (!need(1)) return fail(SBN_E_INVALID, "truncated step %d", s);
@@ -226,7 +240,7 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         if (st.kind == 1 && P->mode == 0) return fail(SBN_E_INVALID, "step %d: batched step in a flat program", s);
         if (n_in < (count ? 0 : 1) || n_in > SBN_MAX_IN) return fail(SBN_E_INVALID, "step %d: %d inputs", s, n_in);
         if (n_axes < 0 || n_axes > SBN_MAX_AXES) return fail(SBN_E_INVALID, "step %d: %d axes", s, n_axes);
-        const bool writes_slot = !readout && !count && !draw;
+        const bool writes_slot = !readout && !count && !draw && !jread;
         if (writes_slot && (n_elim < 0 || n_elim > kMaxElim)) return fail(SBN_E_INVALID, "step %d: %d eliminated axes", s, n_elim);
         if (writes_slot && (st.out_slot < 0 || st.out_slot >= n_slots)) return fail(SBN_E_INVALID, "step %d: out slot", s);
         if (!need(n_axes + n_elim)) return fail(SBN_E_INVALID, "truncated step %d", s);
@@ -235,7 +249,7 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             const int c = w[p + j];
             if (c < 1) return fail(SBN_E_INVALID, "step %d: axis card %d", s, c);
             st.n_out *= c;
-            if (st.n_out >= (1LL << 31) || (count && st.n_out > kMarginalZoffMax / SBN_MAX_IN))
+            if (st.n_out >= (1LL << 31) || ((count || jread) && st.n_out > kMarginalZoffMax / SBN_MAX_IN))
                 return fail(SBN_E_INVALID, "step %d: output too large", s);
             st.cards.push_back(c);
         }
@@ -243,7 +257,7 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
         for (int k = 0; k < n_elim; ++k) {
             const int c = w[p + k];
             if (c < 1 || (draw && c > 256)) return fail(SBN_E_INVALID, "step %d: eliminated card %d", s, c);
-            if (static_cast<int64_t>(st.cx) * c > (readout || count ? kMarginalZoffMax / SBN_MAX_IN : kMaxZ))
+            if (static_cast<int64_t>(st.cx) * c > (readout || count || jread ? kMarginalZoffMax / SBN_MAX_IN : kMaxZ))
                 return fail(SBN_E_INVALID, "step %d: too many eliminated states", s);
             st.cx *= c;
             st.ecards.push_back(c);
@@ -255,12 +269,16 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             for (int64_t q = st.q_offset; q < st.q_offset + st.n_out; ++q) written[q]++;
         } else if (count) {
             if (static_cast<int64_t>(st.cx) * st.n_out >= (1LL << 31)) return fail(SBN_E_INVALID, "step %d: count step too large", s);
+        } else if (jread) {
+            if (static_cast<int64_t>(st.cx) * st.n_out >= (1LL << 31)) return fail(SBN_E_INVALID, "step %d: joint readout too large", s);
+            if (st.q_offset < 0 || st.q_offset + st.n_out > P->Q) return fail(SBN_E_INVALID, "step %d: rows outside the output", s);
+            for (int64_t q = st.q_offset; q < st.q_offset + st.n_out; ++q) written[q]++;
         } else if (!draw) {
             const Slot &os = P->slots[st.out_slot];
             if (os.batched != (st.kind == 1)) return fail(SBN_E_INVALID, "step %d: out slot kind mismatch", s);
             if (os.size < st.n_out) return fail(SBN_E_INVALID, "step %d: out slot too small", s);
         }
-        const bool per_row = st.kind == 1 || ((readout || count || draw) && P->mode == 1);  // batched operands allowed
+        const bool per_row = st.kind == 1 || ((readout || count || draw || jread) && P->mode == 1);  // batched operands allowed
         for (int i = 0; i < n_in; ++i) {
             if (!need(4)) return fail(SBN_E_INVALID, "truncated step %d input %d", s, i);
             InDesc in;
@@ -319,7 +337,7 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
             if (max_off >= size) return fail(SBN_E_INVALID, "step %d input %d: reads past its buffer", s, i);
             st.in.push_back(std::move(in));
         }
-        if (count) {  // inputs without any family axis first: loaded once per joint state z
+        if (count || jread) {  // inputs without any family (group) axis first: loaded once per joint state z
             auto no_axis = [](const InDesc &in) { return std::all_of(in.strides.begin(), in.strides.end(), [](int v) { return v == 0; }); };
             std::stable_partition(st.in.begin(), st.in.end(), no_axis);
             st.n_common = static_cast<int>(std::count_if(st.in.begin(), st.in.end(), no_axis));
@@ -357,9 +375,9 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
     } else if (marginals) {
         for (int q = 0; q < P->Q; ++q)
             if (written[q] != 1) return fail(SBN_E_INVALID, "posterior entry %d is written %d times", q, written[q]);
-    } else if (counts) {
+    } else if (counts || joint) {
         // P(observed) is written before the first count step and not overwritten before the last one (the last
-        // derivative readout of a gradient program)
+        // derivative readout of a gradient program; the last joint readout)
         int first = -1, last = -1, writer = -1;
         for (size_t i = 0; i < P->steps.size(); ++i) {
             if (P->steps[i].kind >= 2) {
@@ -369,7 +387,10 @@ int parse(sbn_program *P, const int32_t *w, int64_t n) {
                 writer = static_cast<int>(i);
             }
         }
-        if (first < 0) return fail(SBN_E_INVALID, "a counts program without a count step");
+        if (first < 0) return fail(SBN_E_INVALID, joint ? "a joint program without a readout" : "a counts program without a count step");
+        if (joint)
+            for (int q = 0; q < P->Q; ++q)
+                if (written[q] != 1) return fail(SBN_E_INVALID, "output row %d is written %d times", q, written[q]);
         if (writer < 0 || writer > first) return fail(SBN_E_INVALID, "P(observed) is not written before the count steps");
         for (int i = first; i <= last; ++i)
             if (P->steps[i].kind < 2) return fail(SBN_E_INVALID, "step %d comes between the count steps", i);
@@ -594,8 +615,9 @@ void plan_tiles(sbn_program *P, std::vector<int32_t> *words) {
     // zoff[i][z] = sum_k digit_k(z) * estride_i[k], first eliminated variable fastest
     for (StepDesc &st : P->steps) {
         st.zoff_pos = -1;
-        if (st.kind == 3) {
-            // count step: soff[i][s] = sum_j digit_j(s) * strides_i[j], coff[s] = sum_j digit_j(s) * cstrides[j]
+        if (st.kind == 3 || st.kind == 7) {
+            // count step and joint readout: soff[i][s] = sum_j digit_j(s) * strides_i[j]; count step:
+            // coff[s] = sum_j digit_j(s) * cstrides[j]
             st.soff_pos = static_cast<int64_t>(words->size());
             for (const InDesc &in : st.in)
                 for (int64_t s = 0; s < st.n_out; ++s) {
@@ -606,6 +628,8 @@ void plan_tiles(sbn_program *P, std::vector<int32_t> *words) {
                     }
                     words->push_back(static_cast<int32_t>(off));
                 }
+        }
+        if (st.kind == 3) {
             st.coff_pos = static_cast<int64_t>(words->size());
             for (int64_t s = 0; s < st.n_out; ++s) {
                 int64_t r = s, off = 0;
@@ -1084,6 +1108,34 @@ cudaError_t launch_count(sbn_program *P, const StepDesc &st, const uint8_t *ev, 
     return sbn_count_launch<float>(c, grid, static_cast<size_t>(smem) * 4, counts, stream, weight);
 }
 
+// Joint readout of a joint program (kind 7): the group's rows q_offset .. of the output, for rows 0 .. n_rows - 1,
+// divided by P(observed)
+cudaError_t launch_joint(sbn_program *P, const StepDesc &st, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, float *d_out,
+                         int64_t ld_out, cudaStream_t stream) {
+    P->launches++;
+    SbnCount c;
+    memset(&c, 0, sizeof c);
+    c.ev = ev;
+    c.ld_ev = ld_ev;
+    c.ld = P->ld;
+    const Slot &ps = P->slots[P->post_slot];
+    c.prob = ps.ptr;
+    c.prob_batched = ps.batched ? 1 : 0;
+    c.zoff = st.zoff_pos >= 0 ? P->d_tile_off + st.zoff_pos : nullptr;
+    c.soff = P->d_tile_off + st.soff_pos;
+    c.min_total = P->f64 ? 1e-290 : static_cast<double>(SBN_MIN_TOTAL_F32);
+    c.n_rows = static_cast<int32_t>(n_rows);
+    c.n_in = static_cast<int32_t>(st.in.size());
+    c.n_common = st.n_common;
+    c.cs = static_cast<int32_t>(st.n_out);
+    c.cz = st.cx;
+    const int64_t smem = bind_operands(P, st, c.in);
+    c.smem_floats = static_cast<int32_t>(smem);
+    const int64_t first = st.q_offset * ld_out;
+    if (P->f64) return sbn_joint_launch<double>(c, 0, reinterpret_cast<double *>(d_out) + first, ld_out, stream);
+    return sbn_joint_launch<float>(c, static_cast<size_t>(smem) * 4, d_out + first, ld_out, stream);
+}
+
 // Derivative readout of a gradient program (kind 6): the soft variable's rows q_offset .. of the output, for rows
 // 0 .. n_rows - 1, divided by P(observed).
 cudaError_t launch_deriv(sbn_program *P, const StepDesc &st, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, float *d_out,
@@ -1154,13 +1206,14 @@ cudaError_t launch_sample(sbn_program *P, const StepDesc &st, int k, const uint8
     return sbn_sample_launch<float>(m, static_cast<size_t>(smem) * 4, stream);
 }
 
-// A readout, count, sample, argmax or derivative step (kinds 2 .. 6) on its own launch; `k`: its index among the sample /
+// A readout, count, sample, argmax, derivative or joint step (kinds 2 .. 7) on its own launch; `k`: its index among the sample /
 // argmax steps (Philox counter word 0 of a sample step)
 cudaError_t launch_kind_step(sbn_program *P, const StepDesc &st, int k, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
                              float *d_out, int64_t ld_out, const DrawnCodes &dc, cudaStream_t stream) {
     if (st.kind == 2) return launch_marginal(P, st, ev, ld_ev, n_rows, d_out, ld_out, stream);
     if (st.kind == 3) return launch_count(P, st, ev, ld_ev, n_rows, stream);
     if (st.kind == 6) return launch_deriv(P, st, ev, ld_ev, n_rows, d_out, ld_out, stream);
+    if (st.kind == 7) return launch_joint(P, st, ev, ld_ev, n_rows, d_out, ld_out, stream);
     return launch_sample(P, st, k, ev, ld_ev, n_rows, dc, stream);
 }
 
@@ -1336,6 +1389,7 @@ int issue_all(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows
         case kCounts:
         case kGrad: SBN_CUDA(launch_prob(P, n_rows, d_out, nullptr, stream)); break;
         case kSample: SBN_CUDA(launch_prob(P, n_rows, d_out, dc.flags(P), stream)); break;
+        case kJoint: SBN_CUDA(launch_prob(P, n_rows, P->d_total, nullptr, stream)); break;  // d_out holds the readouts
         case kMarginals:  // the readouts normalise
         case kMpe:
         case kMap: break;
@@ -1422,21 +1476,23 @@ int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n
 // The checks every run shares: the program is of the kind the entry point runs (kPosterior: the run, evidence
 // and profile calls, which take posterior and marginals programs), and the rows and their evidence are well formed
 int check_rows(const sbn_program *P, ProgramKind kind, const void *ev, int64_t ld_ev, int64_t n_rows, bool soft = false) {
-    static const char *const name[] = {"posterior", "marginals", "counts", "sample", "MPE", "MAP", "gradient"};
+    static const char *const name[] = {"posterior", "marginals", "counts", "sample", "MPE", "MAP", "gradient", "joint"};
     static const char *const entry[] = {"sbn_program_run_*", "sbn_program_run_*", "sbn_program_counts_host",
                                         "sbn_program_sample_host", "sbn_program_mpe_host", "sbn_program_mpe_host",
-                                        "sbn_program_grad_forward_host / sbn_program_grad_backward_host"};
+                                        "sbn_program_grad_forward_host / sbn_program_grad_backward_host",
+                                        "sbn_program_joint_host"};
     if (!P) return fail(SBN_E_INVALID, "null program");
     static const char *const soft_entry[] = {"sbn_program_run_soft_host", "sbn_program_run_soft_host",
                                              "sbn_program_counts_soft_host", "sbn_program_sample_soft_host",
-                                             "sbn_program_mpe_soft_host", "sbn_program_mpe_soft_host", ""};
+                                             "sbn_program_mpe_soft_host", "sbn_program_mpe_soft_host", "", ""};
     static const char *const plain_entry[] = {"sbn_program_run_host", "sbn_program_run_host", "sbn_program_counts_host",
-                                              "sbn_program_sample_host", "sbn_program_mpe_host", "sbn_program_mpe_host", ""};
+                                              "sbn_program_sample_host", "sbn_program_mpe_host", "sbn_program_mpe_host", "",
+                                              ""};
     if ((P->kind == kMarginals ? kPosterior : P->kind == kMap ? kMpe : P->kind) != kind)
         return fail(SBN_E_INVALID, "a %s program%s runs through %s", name[P->kind],
                     !P->soft.empty() && *soft_entry[P->kind] ? " with soft evidence" : "",
                     !P->soft.empty() && *soft_entry[P->kind] ? soft_entry[P->kind] : entry[P->kind]);
-    if (kind == kGrad) {  // the gradient calls take programs with and without soft evidence
+    if (kind == kGrad || kind == kJoint) {  // the gradient and joint calls take programs with and without soft evidence
     } else if (!P->soft.empty() && !soft)
         return fail(SBN_E_INVALID, "a %s program with soft evidence runs through %s", name[P->kind], soft_entry[P->kind]);
     if (P->soft.empty() && soft)
@@ -1680,6 +1736,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
             SBN_CUDA_P(sbn_marginal_set_attrs());
             SBN_CUDA_P(sbn_count_set_attrs());
             SBN_CUDA_P(sbn_deriv_set_attrs());
+            SBN_CUDA_P(sbn_joint_set_attrs());
             SBN_CUDA_P(sbn_sample_set_attrs());
             SBN_CUDA_P(sbn_argmax_set_attrs());
             SBN_CUDA_P(sbn_batched_logdomain_set_attrs());
@@ -2249,6 +2306,54 @@ int sbn_program_grad_backward_host_f64(sbn_program *P, const uint8_t *ev, int64_
     a.lik = lik, a.ld_lik = ld_lik, a.lik_on_device = lik_on_device, a.weights = weights, a.weights_on_device = weights_on_device;
     a.counts = counts, a.n_counts = n_counts, a.deriv = deriv, a.ld_deriv = ld_deriv, a.prob = prob;
     return grad_common(P, ev, ld_ev, n_rows, a, true);
+}
+
+// A joint call of rows 0 .. n_rows - 1, chunk by chunk: codes and (when the program has soft variables) likelihoods
+// are staged, or read in place on the device; each chunk's readouts [Q][ld] and P(observed) come back.
+static int joint_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const void *lik, int64_t ld_lik,
+                        int lik_on_device, void *out_, int64_t ld_out, void *prob_, bool f64) {
+    int rc = check_rows(P, kJoint, ev, ld_ev, n_rows);
+    if (rc != SBN_OK) return rc;
+    if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the joint call");
+    if (!P->soft.empty() && !lik)
+        return fail(SBN_E_INVALID, "a joint program with soft evidence needs its likelihoods: pass lik to %s",
+                    f64 ? "sbn_program_joint_host_f64" : "sbn_program_joint_host");
+    if (P->soft.empty() && lik)
+        return fail(SBN_E_INVALID, "a joint program without soft evidence takes no likelihoods: pass lik = NULL to %s",
+                    f64 ? "sbn_program_joint_host_f64" : "sbn_program_joint_host");
+    const SoftLik soft = {!P->soft.empty(), lik, ld_lik, lik_on_device, nullptr};
+    rc = check_lik(P, soft);
+    if (rc != SBN_OK) return rc;
+    if (!out_ || !prob_) return fail(SBN_E_INVALID, "null output");
+    if (ld_out < n_rows) return fail(SBN_E_INVALID, "ld_out < n_rows");
+    rc = reserve_rows(P, n_rows);
+    if (rc != SBN_OK) return rc;
+    const size_t elem = f64 ? 8 : 4;
+    char *out = static_cast<char *>(out_), *prob = static_cast<char *>(prob_);
+    rc = for_each_chunk(P, ev, ld_ev, n_rows, P->reserved_rows, [&](int64_t r0, int64_t rows) -> int {
+        int rc = stage_lik(P, soft, r0, rows);
+        if (rc != SBN_OK) return rc;
+        rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
+        if (rc != SBN_OK) return rc;
+        SBN_CUDA(cudaMemcpy2DAsync(out + r0 * elem, static_cast<size_t>(ld_out) * elem, P->d_out, static_cast<size_t>(P->ld) * elem,
+                                   static_cast<size_t>(rows) * elem, static_cast<size_t>(P->Q), cudaMemcpyDeviceToHost, P->stream));
+        SBN_CUDA(cudaMemcpyAsync(prob + r0 * elem, P->d_total, static_cast<size_t>(rows) * elem, cudaMemcpyDeviceToHost, P->stream));
+        return SBN_OK;
+    });
+    P->lik = nullptr;  // a device pointer is the caller's: forget it
+    if (rc != SBN_OK) return rc;
+    SBN_CUDA(cudaStreamSynchronize(P->stream));
+    return SBN_OK;
+}
+
+int sbn_program_joint_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
+                           int64_t ld_lik, int lik_on_device, float *out, int64_t ld_out, float *prob) {
+    return joint_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, out, ld_out, prob, false);
+}
+
+int sbn_program_joint_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
+                               int64_t ld_lik, int lik_on_device, double *out, int64_t ld_out, double *prob) {
+    return joint_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, out, ld_out, prob, true);
 }
 
 static int set_tables_common(sbn_program *P, const void *tables, int64_t n, bool f64) {

@@ -25,6 +25,17 @@
 // `sbn_count_weighted_step` is the same step with a per-row double weight w_b (gradient programs,
 // planner.py KIND_COUNT of version 10): each contribution is multiplied by w_b / P_b, and a fully
 // observed family adds w_b.  Weights may be negative; the reduction order is the unweighted one.
+//
+// `sbn_joint_step` (joint programs, planner.py KIND_JOINT = 7) is the same per-row computation with an epilogue
+// that stores instead of reducing: for ONE group of variables,
+//
+//     out[s * ld_out + b] = sum_z prod_i in_i[ zoff_i(z) + soff_i(s) + evoff_i(b) ] / P_b
+//
+// over the group's unobserved members s (their compact joint index, the first member fastest), rows innermost
+// so that a warp's stores coalesce.  The division is in double and the result is rounded to T once; a row whose
+// P_b is below `min_total` (or zero / NaN) is written NaN.  A group of more than C joint states runs in passes
+// of C: the normaliser is known up front, so each pass stores its entries and nothing is re-read.  There is no
+// key, no partial table and no atomic: two runs are bitwise equal.
 #pragma once
 #include "sbn_kernels.cuh"
 #include "sbn_marginal.cuh"
@@ -85,16 +96,19 @@ __device__ __forceinline__ double sbn_group_sum(double v, unsigned grp) {
     return s;
 }
 
-// The body of both count kernels; W: rows weighted by weight[b]
-template <typename T, int C, bool W>
-__device__ __forceinline__ void sbn_count_body(const SbnCount &p, const double *__restrict__ weight) {
+// The body of the count kernels and of the joint readout; W: rows weighted by weight[b]; J: the joint readout,
+// which stores each row's entries at out[s * ld_out + b] instead of adding them to the warp's partial table
+template <typename T, int C, bool W, bool J = false>
+__device__ __forceinline__ void sbn_count_body(const SbnCount &p, const double *__restrict__ weight,
+                                               T *__restrict__ out = nullptr, int64_t ld_out = 0) {
     extern __shared__ __align__(16) float s_tab[];
     __shared__ __align__(8) uint64_t s_bar;
     sbn_pdl_entry();
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    double *const part = p.partial + (static_cast<int64_t>(blockIdx.x) * SBN_COUNT_WARPS + warp) * p.n_entries;
-    for (int e = lane; e < p.n_entries; e += 32) part[e] = 0.0;
+    double *const part = J ? nullptr : p.partial + (static_cast<int64_t>(blockIdx.x) * SBN_COUNT_WARPS + warp) * p.n_entries;
+    if constexpr (!J)
+        for (int e = lane; e < p.n_entries; e += 32) part[e] = 0.0;
 
     const bool staged = p.smem_floats > 0;
     if (staged) {
@@ -121,11 +135,13 @@ __device__ __forceinline__ void sbn_count_body(const SbnCount &p, const double *
         const int64_t b = blk * SBN_COUNT_THREADS + threadIdx.x;
         int key = -1;  // -1: no contribution (past the last row, or out of range)
         double inv = 0.0;
-        double one = 1.0;  // what a fully observed family adds
+        double one = 1.0;  // what a fully observed family adds (joint readout: P_b)
         if (b < p.n_rows) {
             const double pr = static_cast<double>(static_cast<const T *>(p.prob)[p.prob_batched ? b : 0]);
             if (pr >= p.min_total) {  // false for NaN too
-                if constexpr (W) {
+                if constexpr (J) {
+                    one = pr;
+                } else if constexpr (W) {
                     one = weight[b];
                     inv = one / pr;
                 } else {
@@ -137,10 +153,10 @@ __device__ __forceinline__ void sbn_count_body(const SbnCount &p, const double *
                            p.key_stride[k];
             }
         }
-        const unsigned grp = __match_any_sync(0xffffffffu, key);
+        const unsigned grp = J ? 0u : __match_any_sync(0xffffffffu, key);
         const bool lead = key >= 0 && lane == __ffs(grp) - 1;
 
-        if (n_in == 0) {  // a histogram of the keys
+        if (!J && n_in == 0) {  // a histogram of the keys
             const double v = sbn_group_sum(key >= 0 ? one : 0.0, grp);
             if (lead) part[key] += v;
             __syncwarp();
@@ -206,6 +222,16 @@ __device__ __forceinline__ void sbn_count_body(const SbnCount &p, const double *
                     for (int s = 0; s < C; ++s) acc[s] += static_cast<double>(part_s[s]);
                 }
             }
+            if constexpr (J) {
+                if (b < p.n_rows) {
+#pragma unroll
+                    for (int s = 0; s < C; ++s)
+                        if (s0 + s < cs)
+                            out[static_cast<int64_t>(s0 + s) * ld_out + b] =
+                                key >= 0 ? static_cast<T>(acc[s] / one) : static_cast<T>(__int_as_float(0x7fc00000));
+                }
+                continue;
+            }
 #pragma unroll
             for (int s = 0; s < C; ++s) {
                 if (s0 + s < cs) {  // warp-uniform
@@ -227,6 +253,13 @@ template <typename T, int C>
 __global__ void __launch_bounds__(SBN_COUNT_THREADS) sbn_count_weighted_step(const __grid_constant__ SbnCount p,
                                                                               const double *__restrict__ weight) {
     sbn_count_body<T, C, true>(p, weight);
+}
+
+// `out` is the group's first output row; p.partial, p.coff and the key are unused
+template <typename T, int C>
+__global__ void __launch_bounds__(SBN_COUNT_THREADS) sbn_joint_step(const __grid_constant__ SbnCount p, T *__restrict__ out,
+                                                                     int64_t ld_out) {
+    sbn_count_body<T, C, false, true>(p, nullptr, out, ld_out);
 }
 
 // count[e] += sum over the partial tables, in partial-table order
@@ -267,6 +300,24 @@ inline cudaError_t sbn_count_launch(const SbnCount &c, int64_t grid, size_t smem
     sbn_count_reduce<<<static_cast<unsigned>((c.n_entries + threads - 1) / threads), threads, 0, stream>>>(
         c.partial, grid * SBN_COUNT_WARPS, c.n_entries, counts);
     return cudaGetLastError();
+}
+
+// One CTA per SBN_COUNT_THREADS rows; C = the smallest instantiated accumulator count that covers the group (8 and
+// passes beyond)
+template <typename T>
+inline cudaError_t sbn_joint_launch(const SbnCount &c, size_t smem, T *out, int64_t ld_out, cudaStream_t stream) {
+    const unsigned g = static_cast<unsigned>((static_cast<int64_t>(c.n_rows) + SBN_COUNT_THREADS - 1) / SBN_COUNT_THREADS);
+    if (c.cs <= 2) sbn_joint_step<T, 2><<<g, SBN_COUNT_THREADS, smem, stream>>>(c, out, ld_out);
+    else if (c.cs <= 4) sbn_joint_step<T, 4><<<g, SBN_COUNT_THREADS, smem, stream>>>(c, out, ld_out);
+    else sbn_joint_step<T, 8><<<g, SBN_COUNT_THREADS, smem, stream>>>(c, out, ld_out);
+    return cudaGetLastError();
+}
+
+inline cudaError_t sbn_joint_set_attrs() {
+    cudaError_t e = cudaFuncSetAttribute(sbn_joint_step<float, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, SBN_SMEM_BUDGET);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(sbn_joint_step<float, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, SBN_SMEM_BUDGET);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(sbn_joint_step<float, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, SBN_SMEM_BUDGET);
+    return e;
 }
 
 inline cudaError_t sbn_count_set_attrs() {

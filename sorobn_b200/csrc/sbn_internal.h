@@ -78,7 +78,7 @@ inline int64_t round_up(int64_t v, int64_t m) { return (v + m - 1) / m * m; }
 struct SbnSegment;  // sbn_chain.h
 struct SbnPair;     // sbn_pair.h
 
-// What a program computes, fixed by its header version (4 .. 10 in this order)
+// What a program computes, fixed by its header version (4 .. 11 in this order)
 enum ProgramKind {
     kPosterior,  // kind-0 / 1 steps, then the normalised posterior slot
     kMarginals,  // kind-2 readouts write the posterior, already normalised; no posterior slot
@@ -90,6 +90,8 @@ enum ProgramKind {
                  // post_slot holds max log P(x_MAP, e); it runs through the MPE entry point
     kGrad,       // gradient: a counts program whose kind-3 steps are weighted per row, plus kind-6 derivative
                  // readouts written to rows 1 .. of the output; row 0 and post_slot hold P(observed)
+    kJoint,      // joint: a counts program whose steps are kind-7 per-row readouts of groups of variables into the
+                 // output [Q][ld]; post_slot holds P(observed), the run's per-row P(observed) goes to d_total
 };
 
 // Programs on log tables (MPE and marginal MAP): float32 only, the log-domain step kernels only

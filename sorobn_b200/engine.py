@@ -16,7 +16,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libsorobn_
 _lib = None
 
 SBN_OK = 0
-ABI_VERSION = 16
+ABI_VERSION = 17
 
 
 class EngineError(RuntimeError):
@@ -92,6 +92,9 @@ def load():
     for name in ("sbn_program_grad_backward_host", "sbn_program_grad_backward_host_f64"):
         getattr(lib, name).restype = i32
         getattr(lib, name).argtypes = [vp, vp, i64, i64, vp, i64, i32, vp, i32, vp, i64, vp, i64, vp]
+    for name in ("sbn_program_joint_host", "sbn_program_joint_host_f64"):
+        getattr(lib, name).restype = i32
+        getattr(lib, name).argtypes = [vp, vp, i64, i64, vp, i64, i32, vp, i64, vp]
     lib.sbn_program_destroy.restype = None
     lib.sbn_program_destroy.argtypes = [vp]
     lib.sbn_program_reserve.restype = i32
@@ -139,7 +142,8 @@ EXPORTS = (
     "sbn_program_run_soft_host", "sbn_program_run_soft_host_f64", "sbn_program_counts_soft_host",
     "sbn_program_counts_soft_host_f64", "sbn_program_sample_soft_host", "sbn_program_sample_soft_host_f64",
     "sbn_program_mpe_soft_host", "sbn_program_grad_forward_host", "sbn_program_grad_forward_host_f64",
-    "sbn_program_grad_backward_host", "sbn_program_grad_backward_host_f64",
+    "sbn_program_grad_backward_host", "sbn_program_grad_backward_host_f64", "sbn_program_joint_host",
+    "sbn_program_joint_host_f64",
     "sbn_program_info", "sbn_program_set_graph", "sbn_program_set_tiled", "sbn_gibbs_create", "sbn_gibbs_run_host",
     "sbn_sampler_run_host", "sbn_gibbs_conditional", "sbn_gibbs_destroy", "sbn_host_alloc", "sbn_host_free",
 )
@@ -399,6 +403,27 @@ class Program:
             int(on_device), counts.ctypes.data, counts.size, deriv.ctypes.data if n_lik else None, n_rows,
             prob.ctypes.data))
         return counts, deriv, prob
+
+    def joint(self, codes: np.ndarray, n_rows: int, lik=None):
+        """Joint programs (planner.build_joint_plan): (output [Q, n_rows], whose rows `plan.group_rows[k] ..` hold
+        the joint posterior of group k's unobserved members (the first one fastest); P(observed, lik / max)
+        [n_rows]), NaN throughout for a row the float32 range rule flags, host path.  `lik` as in `run_soft`, for
+        a program with soft variables (and None otherwise)."""
+        n_rows = int(n_rows)
+        codes, ev_ptr = self._evidence(codes, n_rows)
+        if self.plan.soft:
+            if lik is None:
+                raise ValueError("a joint program with soft variables needs their likelihoods")
+            lik, lik_args = self._likelihoods(lik, n_rows)
+        elif lik is not None:
+            raise ValueError("likelihoods given to a joint program without soft variables")
+        else:
+            lik_args = (None, 0, 0)
+        out = np.empty((self.Q, n_rows), dtype=self.dtype)
+        prob = np.empty(n_rows, dtype=self.dtype)
+        _check(self._fn("sbn_program_joint_host")(self._h, ev_ptr, n_rows, n_rows, *lik_args, out.ctypes.data, n_rows,
+                                                  prob.ctypes.data))
+        return out, prob
 
     def set_tables(self, blob: np.ndarray):
         """Replace a counts or gradient program's tables (planner.refresh_tables gives the blob of new CPTs)."""

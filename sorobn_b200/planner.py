@@ -160,6 +160,25 @@ A kind-6 step reads the bucket k that lambda_s entered, with every input of that
 written at rows `q_offset ..` (1 + the soft variable's first likelihood column) of the run's output; row 0 is
 P(observed).  D_s is d log P / d lambda_s, exact where lambda_s(x) = 0.  `Plan.forward_steps` lists the steps
 P(observed) depends on (the upward pass): a forward run issues only those.
+
+Joint programs (`build_joint_plan`, `build_pattern_plan(net, "joint", ...)`, VERSION 11) give, for every row,
+the joint posterior of chosen groups of variables (by default every CPT family) given the row's observed cells
+and likelihoods.  They are counts programs whose count steps are per-row readouts (kind 7):
+
+    header : MAGIC 11 1 n_ev n_tables n_slots n_steps Q p_slot p_batched 0 n_soft
+    kind 7 : 7 n_in -1 n_axes n_elim q_offset | cards[n_axes] | ecards[n_elim] | inputs as above
+
+`p_slot` holds P(observed, lik / max) of every row, as in version 6.  A kind-7 step reads the unobserved
+members M_g of group g (its output axes, in the group's order, the first one fastest) from the smallest bucket
+that holds them, and writes
+
+    sum_{U_k - M_g} pi_k * prod_{f in F_k} f / P(observed)
+
+at rows `q_offset .. q_offset + |M_g| - 1` of the run's `[Q][ld]` output; Q is the sum of those sizes over the
+groups.  A group the pattern observes completely has no step (its posterior is a one-hot on the observed
+codes).  A family lies in the bucket its CPT entered; a group that lies in no CPT's scope gets a constant table
+of ones over M_g, entered with the CPTs, so that elimination builds a bucket holding it (`Plan.ones`).  Those
+tables follow the CPTs' in the table section.
 """
 from __future__ import annotations
 
@@ -200,6 +219,8 @@ VERSION_MPE = 8
 VERSION_MAP = 9  # marginal MAP: the MPE words plus a reduction word on kind-0 / kind-1 steps
 KIND_DERIV = 6  # derivative of P(observed) by one soft variable's likelihood, over P(observed) (gradient programs only)
 VERSION_GRAD = 10
+KIND_JOINT = 7  # per-row joint posterior of one group of variables (joint programs only)
+VERSION_JOINT = 11
 REDUCE_MAX, REDUCE_LOGSUMEXP = 0, 1
 HEADER_WORDS = 12
 
@@ -298,6 +319,9 @@ class Plan:
     # gradient plans: indices of the steps P(observed) depends on, in program order.  The engine derives the same set
     # from the slot words (csrc/sbn_api.cu parse); the CPU replay reads this one, and a GPU test checks the two agree
     forward_steps: tuple = ()
+    groups: tuple = ()  # joint plans: the var ids of every group, in call order
+    group_rows: tuple = ()  # joint plans: each group's first output row, -1 for a group the pattern observes completely
+    ones: tuple = ()  # joint plans: the unobserved members of every group given a table of ones, in table order
 
     # ---- cost model (DESIGN.md "algorithmic bytes") -------------------------------
     def bytes_per_row(self, n_draws=1):
@@ -315,7 +339,7 @@ class Plan:
                         total += 4 * nd * int(np.prod([c for c, s in zip(st.ecards, es) if s], dtype=np.int64))
                 total += nd * len(st.elims)
                 continue
-            if st.kind not in (KIND_BATCHED, KIND_MARGINAL, KIND_COUNT):
+            if st.kind not in (KIND_BATCHED, KIND_MARGINAL, KIND_COUNT, KIND_JOINT):
                 continue
             for f, _, _ in st.inputs:
                 if f.batched:
@@ -328,7 +352,7 @@ class Plan:
             # normalise: read unnormalised posterior, write posterior (a marginals program's
             # readouts write their segments normalised, counted above)
             total += 8 * self.Q
-        elif self.version in (VERSION_COUNTS, VERSION_SAMPLE, VERSION_MPE, VERSION_MAP):
+        elif self.version in (VERSION_COUNTS, VERSION_SAMPLE, VERSION_MPE, VERSION_MAP, VERSION_JOINT):
             total += 4  # P(observed) (max log P(x, e)) out
         total += len(self.evidence)  # uint8 codes
         if self.soft:
@@ -517,7 +541,31 @@ def build_map_plan(net: CompiledNet, evidence, map_vars, order=None, max_in=MAX_
                   lift_evidence=lift_evidence, fuse_elims=fuse_elims)
 
 
-def build_pattern_plan(net: CompiledNet, kind, evidence, soft=(), map_vars=None, **kw) -> Plan:
+def build_joint_plan(net: CompiledNet, evidence, groups=None, soft=(), order=None, max_in=MAX_IN, lift_evidence=True,
+                     fuse_elims=None) -> Plan:
+    """Plan the joint posterior of every group of `groups` for each row of one missingness pattern (a version-11
+    program, see the module docstring): `groups` are tuples of var ids (default: every CPT family, in
+    [*parents, v] order), `evidence` the observed columns and `soft` the var ids with per-row likelihoods.
+    `Plan.group_rows` gives each group's first output row (-1: observed completely).  ValueError for a
+    duplicate member, and when no group has an unobserved member (the program would output nothing)."""
+    evidence = tuple(evidence)
+    soft = _check_soft(net, evidence, soft, MODE_BATCHED)
+    if groups is None:
+        groups = [net.scope(v) for v in range(len(net.names))]
+    groups = tuple(tuple(int(u) for u in g) for g in groups)
+    for g in groups:
+        if not g or len(set(g)) != len(g):
+            raise ValueError(f"group {[net.names[u] for u in g]} is empty or has a duplicate member")
+        if any(u < 0 or u >= len(net.names) for u in g):
+            raise ValueError(f"group {g} names a variable the network does not have")
+    if not any(u not in set(evidence) for g in groups for u in g):
+        raise ValueError("every group is observed completely: a joint program would output nothing")
+    hidden = tuple(v for v in range(len(net.names)) if v not in set(evidence))
+    return _build(net, VERSION_JOINT, evidence, targets=hidden, order=order, max_in=max_in, lift_evidence=lift_evidence,
+                  fuse_elims=fuse_elims, soft=soft, groups=groups)
+
+
+def build_pattern_plan(net: CompiledNet, kind, evidence, soft=(), map_vars=None, groups=None, **kw) -> Plan:
     """The plan of one missingness pattern with soft evidence: `kind` "counts", "sample", "mpe" or "map" (then
     `map_vars` are the MAP variables), the observed columns `evidence` and the var ids `soft` whose per-row
     likelihoods arrive at run time (see the module docstring).  A soft variable may not be evidence; it may be
@@ -525,12 +573,20 @@ def build_pattern_plan(net: CompiledNet, kind, evidence, soft=(), map_vars=None,
     word for word; `kw` are that builder's options.
 
     `kind` "grad" plans the gradient program of the pattern (version 10, soft evidence or not): the counts
-    program's steps with weighted counts, plus one derivative readout per soft variable."""
+    program's steps with weighted counts, plus one derivative readout per soft variable.  `kind` "joint" plans
+    the joint posteriors of `groups` (version 11, soft evidence or not; `build_joint_plan`)."""
     builders = {"counts": build_counts_plan, "sample": build_sample_plan, "mpe": build_mpe_plan, "map": build_map_plan}
-    if kind not in builders and kind != "grad":
-        raise ValueError(f"kind must be one of {sorted([*builders, 'grad'])}, not {kind!r}")
+    if kind not in builders and kind not in ("grad", "joint"):
+        raise ValueError(f"kind must be one of {sorted([*builders, 'grad', 'joint'])}, not {kind!r}")
     if (map_vars is not None) != (kind == "map"):
         raise ValueError("map_vars go with kind 'map' only, and kind 'map' needs them")
+    if groups is not None and kind != "joint":
+        raise ValueError("groups go with kind 'joint' only")
+    if kind == "joint":
+        if kw.get("mode", MODE_BATCHED) != MODE_BATCHED:
+            raise ValueError("a joint program is batched")
+        kw.pop("mode", None)
+        return build_joint_plan(net, evidence, groups, soft=soft, **kw)
     evidence = tuple(evidence)
     soft = _check_soft(net, evidence, soft, kw.get("mode", MODE_BATCHED))
     if kind == "grad":
@@ -803,12 +859,13 @@ def _dense_strides(cards):
 
 
 def _build(net, version, evidence, query=(), targets=(), mode=MODE_BATCHED, order=None, max_in=MAX_IN,
-           lift_evidence=True, fuse_elims=None, merge_sum_outs=None, soft=()):
+           lift_evidence=True, fuse_elims=None, merge_sum_outs=None, soft=(), groups=None):
     """A plan of program `version` (VERSION, VERSION_MARGINALS, ...): the upward pass of variable
     elimination, then the kind's tail.  `targets` are kept relevant besides the query and the evidence:
     a marginals plan reads them out, and counts, sample and MPE plans pass every unobserved variable.
     `soft` (sorted by name) adds one batched likelihood factor per variable, read from a slot no step
-    writes; it enters the variable's bucket, or the final product of a queried variable."""
+    writes; it enters the variable's bucket, or the final product of a queried variable.  `groups` (joint plans)
+    are the var-id tuples whose joint posteriors the plan reads out."""
     if fuse_elims is None:
         fuse_elims = os.environ.get("SOROBN_B200_FUSE", "1") == "1"
     if len(set(evidence)) != len(evidence):
@@ -847,6 +904,19 @@ def _build(net, version, evidence, query=(), targets=(), mode=MODE_BATCHED, orde
         if len(ev) > MAX_EV:
             raise ValueError(f"CPT of {net.names[v]!r} has {len(ev)} evidence axes; the kernel supports {MAX_EV}")
         factors.append(_Factor(False, t, tuple(u for u, _ in free), tuple(s for _, s in free), ev, False))
+    ones = []
+    if version == VERSION_JOINT:
+        # a group whose unobserved members lie in no CPT's scope gets a table of ones over them: elimination then
+        # builds a bucket that holds the group, and no value changes
+        for g in groups:
+            M = tuple(u for u in g if u not in ev_col)
+            if len(M) < 2 or M in ones or any(set(M) <= set(net.scope(v)) for v in range(len(net.names))):
+                continue
+            shape = [int(card[u]) for u in M]
+            b.table_arrays.append(np.ones(shape, dtype=np.float64))
+            b.table_axes.append(list(M))
+            factors.append(_Factor(False, len(b.table_arrays) - 1, M, _dense_strides(shape[::-1])[::-1], (), False))
+            ones.append(M)
     # the likelihoods: batched leaf factors over one variable each, under logical ids no step produces
     b.soft = tuple((v, b.next_id + k) for k, v in enumerate(soft))
     b.next_id += len(soft)
@@ -907,6 +977,8 @@ def _build(net, version, evidence, query=(), targets=(), mode=MODE_BATCHED, orde
         return _marginals_passes(b, buckets, factors, targets)
     if version in (VERSION_COUNTS, VERSION_GRAD):
         return _counts_passes(b, buckets, factors, grad=version == VERSION_GRAD)
+    if version == VERSION_JOINT:
+        return _counts_passes(b, buckets, factors, groups=groups, ones=tuple(ones))
     if version in (VERSION_SAMPLE, VERSION_MPE, VERSION_MAP):
         return _sample_passes(b, buckets, factors, version)
 
@@ -952,7 +1024,7 @@ def _marginals_passes(b, buckets, leftovers, targets):
     return b.finish(VERSION_MARGINALS, None, q, targets=t_sorted)
 
 
-def _counts_passes(b, buckets, leftovers, grad=False):
+def _counts_passes(b, buckets, leftovers, grad=False, groups=None, ones=()):
     """Downward pass and count steps of a counts plan (DESIGN.md "Expected counts and EM").
 
     The unobserved members M_v of v's family are read from the smallest bucket k with M_v in U_k (the
@@ -961,13 +1033,21 @@ def _counts_passes(b, buckets, leftovers, grad=False):
     where P(observed) is the product of every leftover scalar of the upward pass, computed once.
 
     grad=True: a gradient plan (version 10), whose derivative readouts (`_deriv_steps`) follow the count
-    steps on the same downward messages."""
+    steps on the same downward messages.
+
+    groups: a joint plan (version 11): the members M_g of every group g (unobserved, in the group's order) are
+    read the same way, each into rows of the output (`_joint_steps`), in place of the count steps."""
     card, names, ev_col = b.card, b.net.names, b.ev_col
-    members = {v: [u for u in b.net.scope(v) if u not in ev_col] for v in range(len(names))}
+    if groups is None:
+        members = {v: [u for u in b.net.scope(v) if u not in ev_col] for v in range(len(names))}
+    else:
+        members = {k: [u for u in g if u not in ev_col] for k, g in enumerate(groups)}
     read = {v: _smallest_bucket(b, buckets, set(M)) for v, M in members.items() if M}
     deriv = _deriv_buckets(b, buckets) if grad else {}
     pi = _downward(b, buckets, leftovers, [*read.values(), *deriv.values()])
     prob = b.emit(b.fold(leftovers), (), [], may_lift=False)
+    if groups is not None:
+        return _joint_steps(b, buckets, pi, read, members, groups, ones, prob)
 
     c_offsets, n_counts = count_layout(b.net)
     for v, M in members.items():
@@ -996,6 +1076,30 @@ def _counts_passes(b, buckets, leftovers, grad=False):
     b.steps = _prune_dead(b.steps)
     forward = _closure(b.steps, prob.buf)
     return b.finish(VERSION_GRAD, prob, q, n_counts=n_counts, count_offsets=c_offsets, forward_steps=forward)
+
+
+def _joint_steps(b, buckets, pi, read, members, groups, ones, prob):
+    """The readouts of a joint plan, groups in call order: group k's members M (first one fastest) from bucket
+    read[k], summed over the rest of the bucket and divided by P(observed), at the next |M| output rows."""
+    card, names = b.card, b.net.names
+    q, rows = 0, []
+    for k, g in enumerate(groups):
+        M = tuple(members[k])
+        if not M:
+            rows.append(-1)
+            continue
+        ins, elims, ecards = _bucket_read(b, buckets[read[k]], pi[read[k]], M)
+        cz, cs = b.size(elims), b.size(M)
+        if cz > MARGINAL_MAX_Z or cs > MARGINAL_MAX_Z or cz * cs >= 2**31:
+            raise ValueError(f"the bucket read for the group {[names[u] for u in g]} is too large for a joint readout: "
+                             f"{cz} joint states summed out and {cs} group states (each at most {MARGINAL_MAX_Z}, "
+                             "their product below 2^31)")
+        b.steps.append(Step(KIND_JOINT, ins, -1, M, tuple(int(card[u]) for u in M), elims, ecards, q_offset=q,
+                            norm=prob))
+        rows.append(q)
+        q += cs
+    b.steps = _prune_dead(b.steps)
+    return b.finish(VERSION_JOINT, prob, q, groups=tuple(groups), group_rows=tuple(rows), ones=ones)
 
 
 def _deriv_buckets(b, buckets):
@@ -1159,7 +1263,7 @@ def _prune_dead(steps):
     """Drop the launches nothing reads (the root buckets' own messages when no other root needs them)."""
     used, keep = set(), []
     for st in reversed(steps):
-        if st.kind in (KIND_MARGINAL, KIND_COUNT, KIND_DERIV) or st.out_id in used:
+        if st.kind in (KIND_MARGINAL, KIND_COUNT, KIND_DERIV, KIND_JOINT) or st.out_id in used:
             keep.append(st)
             used.update(f.buf for f, _, _ in st.inputs if f.is_slot)
             if st.norm is not None:
@@ -1403,7 +1507,7 @@ def _serialise(plan: Plan, table_arrays):
     plan.table_offsets = offsets
 
     extra = [0, 0]
-    if plan.version in (VERSION, VERSION_COUNTS, VERSION_SAMPLE, VERSION_MPE, VERSION_MAP, VERSION_GRAD):
+    if plan.version in (VERSION, VERSION_COUNTS, VERSION_SAMPLE, VERSION_MPE, VERSION_MAP, VERSION_GRAD, VERSION_JOINT):
         post = [plan.post_slot, int(plan.slots[plan.post_slot][0])]
         if plan.version in (VERSION_COUNTS, VERSION_GRAD):
             extra = [plan.n_counts, 0]
@@ -1415,7 +1519,7 @@ def _serialise(plan: Plan, table_arrays):
         extra = [len(plan.soft), 0]
     else:
         extra[1] = len(plan.soft)
-    w = [MAGIC, plan.version, plan.mode, len(plan.evidence), len(plan.tables), len(plan.slots), len(plan.steps),
+    w = [MAGIC, plan.version, plan.mode, len(plan.evidence), len(offsets), len(plan.slots), len(plan.steps),
          plan.Q, *post, *extra]
     assert len(w) == HEADER_WORDS
     for o, s in offsets:
@@ -1426,7 +1530,7 @@ def _serialise(plan: Plan, table_arrays):
         w += [s, int(plan._card[v])]
     for st in plan.steps:
         w += [st.kind, len(st.inputs), st.out_slot, len(st.cards), len(st.ecards)]
-        if st.kind in (KIND_MARGINAL, KIND_DERIV):
+        if st.kind in (KIND_MARGINAL, KIND_DERIV, KIND_JOINT):
             w.append(st.q_offset)
         elif st.kind == KIND_COUNT:
             w += [st.q_offset, len(st.key)]
