@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SBN_ABI_VERSION 17
+#define SBN_ABI_VERSION 18
 
 #define SBN_OK 0
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
@@ -311,6 +311,39 @@ int sbn_gibbs_conditional(sbn_sampler *sampler, int32_t var, const uint8_t *join
 #define SBN_ALGO_GIBBS_GENERIC 3  /* Gibbs through the generic kernel even when the straight-line one applies (tests) */
 int sbn_sampler_run_host(sbn_sampler *sampler, int algo, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
                          int64_t n_iterations, uint64_t seed, float *out, int64_t ld_out);
+
+/* ------------------------------------------------------------------ structure learning
+ * A tally is a complete discrete data set resident on one device, for the counting passes of score-based
+ * structure learning (sorobn_b200/structure.py).  `codes` is host memory, uint8 state codes
+ * codes[v * ld + b] (v < n_vars, b < n_rows: one row of codes per column, rows innermost, as the evidence
+ * layout), every code below cards[v] (1 <= cards[v] <= 256; checked); it is uploaded once, at creation.
+ * A data set that does not fit the device fails with SBN_E_NOMEM.
+ *
+ * A batch of families is given by `words`: per family k, then its k distinct member columns, the child first
+ * and its parents after it.  Family f's contingency table has T_f = prod cards entries, at most
+ * SBN_TALLY_MAX_TABLE, laid out [parent k-1] .. [parent 1][child] with the child fastest (entry
+ * sum_i code_i * prod_{l < i} cards[member l]); the tables of a batch are concatenated in family order.
+ * Families whose tables fit SBN_TALLY_SMEM_BINS together are counted in shared memory, each code byte read
+ * once per such group; a family with a larger table counts with global atomics.  Counts are exact.
+ *
+ * sbn_tally_counts: every table of the batch, counts[n_counts] (n_counts = sum_f T_f).
+ * sbn_tally_scores: scores[f], the decomposable score of family f in double, with N = n_rows, N_jk the count of
+ * child state k under parent configuration j (q = T_f / r configurations, r = cards[child], seen or not) and
+ * N_j = sum_k N_jk:
+ *   SBN_SCORE_BIC:  sum_jk N_jk ln(N_jk / N_j) - ln(N) q (r - 1) / 2, with 0 ln 0 = 0;
+ *   SBN_SCORE_BDEU: sum_j [lgamma(a/q) - lgamma(N_j + a/q) + sum_k (lgamma(N_jk + a/(q r)) - lgamma(a/(q r)))],
+ *                   a = ess > 0, the equivalent sample size (ignored by BIC). */
+typedef struct sbn_tally sbn_tally;
+#define SBN_TALLY_MAX_TABLE (1 << 22)  /* entries of one family's table                         */
+#define SBN_TALLY_SMEM_BINS 32768      /* shared-memory bins of one group; larger tables go global */
+#define SBN_SCORE_BIC 0
+#define SBN_SCORE_BDEU 1
+int sbn_tally_create(int device, const uint8_t *codes, int64_t ld, int32_t n_vars, int64_t n_rows, const int32_t *cards,
+                     sbn_tally **out);
+int sbn_tally_counts(sbn_tally *tally, const int32_t *words, int64_t n_words, uint64_t *counts, int64_t n_counts);
+int sbn_tally_scores(sbn_tally *tally, const int32_t *words, int64_t n_words, int kind, double ess, double *scores,
+                     int64_t n_families);
+void sbn_tally_destroy(sbn_tally *tally);
 
 /* Pinned host memory for evidence / posterior staging buffers. */
 int sbn_host_alloc(void **ptr, int64_t bytes);

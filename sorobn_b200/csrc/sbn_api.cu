@@ -35,13 +35,17 @@ namespace {
 
 thread_local std::string g_err;
 
-int fail(int code, const char *fmt, ...) {
+void set_error(const char *fmt, va_list ap) {
     char buf[512];
+    vsnprintf(buf, sizeof buf, fmt, ap);
+    g_err = buf;
+}
+
+int fail(int code, const char *fmt, ...) {
     va_list ap;
     va_start(ap, fmt);
-    vsnprintf(buf, sizeof buf, fmt, ap);
+    set_error(fmt, ap);
     va_end(ap);
-    g_err = buf;
     return code;
 }
 
@@ -76,6 +80,14 @@ constexpr int kMaxZ = 256;
 constexpr int kHeaderWords = 12;
 
 }  // namespace
+
+int sbn_fail(int code, const char *fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    set_error(fmt, ap);
+    va_end(ap);
+    return code;
+}
 
 namespace {
 

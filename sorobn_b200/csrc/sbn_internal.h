@@ -75,6 +75,10 @@ struct Slot {
 
 inline int64_t round_up(int64_t v, int64_t m) { return (v + m - 1) / m * m; }
 
+// Record the message sbn_last_error returns (printf format) and return `code`: the error convention of every
+// entry point, for the translation units outside sbn_api.cu
+int sbn_fail(int code, const char *fmt, ...);
+
 struct SbnSegment;  // sbn_chain.h
 struct SbnPair;     // sbn_pair.h
 

@@ -16,7 +16,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libsorobn_
 _lib = None
 
 SBN_OK = 0
-ABI_VERSION = 17
+ABI_VERSION = 18
 
 
 class EngineError(RuntimeError):
@@ -123,6 +123,14 @@ def load():
     lib.sbn_gibbs_conditional.argtypes = [vp, i32, vp, vp]
     lib.sbn_gibbs_destroy.restype = None
     lib.sbn_gibbs_destroy.argtypes = [vp]
+    lib.sbn_tally_create.restype = i32
+    lib.sbn_tally_create.argtypes = [i32, vp, i64, i32, i64, vp, c.POINTER(vp)]
+    lib.sbn_tally_counts.restype = i32
+    lib.sbn_tally_counts.argtypes = [vp, vp, i64, vp, i64]
+    lib.sbn_tally_scores.restype = i32
+    lib.sbn_tally_scores.argtypes = [vp, vp, i64, i32, c.c_double, vp, i64]
+    lib.sbn_tally_destroy.restype = None
+    lib.sbn_tally_destroy.argtypes = [vp]
     lib.sbn_host_alloc.restype = i32
     lib.sbn_host_alloc.argtypes = [c.POINTER(vp), i64]
     lib.sbn_host_free.restype = i32
@@ -145,7 +153,8 @@ EXPORTS = (
     "sbn_program_grad_backward_host", "sbn_program_grad_backward_host_f64", "sbn_program_joint_host",
     "sbn_program_joint_host_f64",
     "sbn_program_info", "sbn_program_set_graph", "sbn_program_set_tiled", "sbn_gibbs_create", "sbn_gibbs_run_host",
-    "sbn_sampler_run_host", "sbn_gibbs_conditional", "sbn_gibbs_destroy", "sbn_host_alloc", "sbn_host_free",
+    "sbn_sampler_run_host", "sbn_gibbs_conditional", "sbn_gibbs_destroy", "sbn_tally_create", "sbn_tally_counts",
+    "sbn_tally_scores", "sbn_tally_destroy", "sbn_host_alloc", "sbn_host_free",
 )
 
 
@@ -561,6 +570,69 @@ class GibbsSampler:
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:
             load().sbn_gibbs_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+TALLY_MAX_TABLE = 1 << 22     # SBN_TALLY_MAX_TABLE: entries of one family's table
+TALLY_SMEM_BINS = 32768       # SBN_TALLY_SMEM_BINS: a larger table counts with global atomics
+
+
+class Tally:
+    """A complete discrete data set resident on one GPU, and the counting passes of structure learning over it
+    (csrc/sbn_tally.cu).  `codes` is uint8 [n_vars, n_rows], every code of column v below `cards[v]`; it is
+    uploaded once.  A family is a sequence of column ids, the child first and its parents after it."""
+
+    SCORES = {"bic": 0, "bdeu": 1}
+
+    def __init__(self, codes, cards, device: int | None = None):
+        lib = load()
+        self.device = default_device() if device is None else int(device)
+        codes = np.ascontiguousarray(codes, dtype=np.uint8)
+        if codes.ndim != 2:
+            raise ValueError(f"codes have shape {codes.shape}, expected [n_vars, n_rows]")
+        self.cards = np.ascontiguousarray(cards, dtype=np.int32)
+        if self.cards.shape != (codes.shape[0],):
+            raise ValueError(f"{self.cards.size} cardinalities for {codes.shape[0]} columns")
+        self.n_vars, self.n_rows = codes.shape
+        self._h = ctypes.c_void_p()
+        _check(lib.sbn_tally_create(self.device, codes.ctypes.data, self.n_rows, self.n_vars, self.n_rows,
+                                    self.cards.ctypes.data, ctypes.byref(self._h)))
+
+    @staticmethod
+    def _words(families):
+        words = []
+        for fam in families:
+            words.append(len(fam))
+            words.extend(int(v) for v in fam)
+        return np.ascontiguousarray(words, dtype=np.int32)
+
+    def counts(self, families) -> list:
+        """The contingency table of every family, exact: uint64 [prod of the members' cards] each, the child
+        fastest, then the first parent, and so on."""
+        sizes = [int(np.prod([int(self.cards[v]) for v in fam])) for fam in families]
+        words = self._words(families)
+        out = np.zeros(sum(sizes), dtype=np.uint64)
+        _check(load().sbn_tally_counts(self._h, words.ctypes.data, words.size, out.ctypes.data, out.size))
+        return np.split(out, np.cumsum(sizes)[:-1])
+
+    def scores(self, families, kind: str = "bic", ess: float = 1.0) -> np.ndarray:
+        """The decomposable score ("bic" or "bdeu" with equivalent sample size `ess`) of every family, float64;
+        only the scores leave the device."""
+        words = self._words(families)
+        out = np.empty(len(families), dtype=np.float64)
+        _check(load().sbn_tally_scores(self._h, words.ctypes.data, words.size, self.SCORES[kind], float(ess),
+                                       out.ctypes.data, out.size))
+        return out
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h.value:
+            load().sbn_tally_destroy(self._h)
             self._h = None
 
     def __del__(self):
