@@ -1083,13 +1083,29 @@ int64_t count_grid(const sbn_program *P, const StepDesc &st, int64_t n_rows) {
     return std::max<int64_t>(1, std::min<int64_t>({blocks, 4LL * P->n_sms, cap}));
 }
 
+// What one run reads and writes beyond its codes and output, for one host call only (the caller's device pointers
+// live here, never on the program): the drawn-code buffer's draws and pitch (sample / MPE run: P->d_drawn holds
+// codes [n_sampled][n_draws][ld_drawn], one draw for MPE, then one flag byte per row), the likelihoods the pack
+// reads and their pitch (soft evidence), the row weights of a gradient program's count steps, whether the run is a
+// gradient program's forward run (P(observed) only), and the per-warp partial count tables (counts / backward run).
+struct RunInputs {
+    int64_t n_draws = 1, ld_drawn = 0;
+    const void *lik = nullptr;
+    int64_t ld_lik = 0;
+    const double *weight = nullptr;
+    bool forward = false;
+    double *partial = nullptr;
+    uint8_t *flags(const sbn_program *P) const { return P->d_drawn + static_cast<int64_t>(P->n_sampled) * n_draws * ld_drawn; }
+};
+
 // Count step (kind 3): adds the family's expected counts of rows 0 .. n_rows - 1 into P->d_counts.
-cudaError_t launch_count(sbn_program *P, const StepDesc &st, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, cudaStream_t stream) {
+cudaError_t launch_count(sbn_program *P, const StepDesc &st, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
+                         const RunInputs &in, cudaStream_t stream) {
     P->launches += 2;
     SbnCount c;
     memset(&c, 0, sizeof c);
     const int64_t grid = count_grid(P, st, n_rows);
-    c.partial = P->d_partial;
+    c.partial = in.partial;
     c.ev = ev;
     c.ld_ev = ld_ev;
     c.ld = P->ld;
@@ -1115,7 +1131,7 @@ cudaError_t launch_count(sbn_program *P, const StepDesc &st, const uint8_t *ev, 
     const int64_t smem = bind_operands(P, st, c.in);
     c.smem_floats = static_cast<int32_t>(smem);
     double *counts = P->d_counts + st.q_offset;
-    const double *weight = P->kind == kGrad ? P->weight : nullptr;  // a gradient program's counts are weighted
+    const double *weight = P->kind == kGrad ? in.weight : nullptr;  // a gradient program's counts are weighted
     if (P->f64) return sbn_count_launch<double>(c, grid, 0, counts, stream, weight);
     return sbn_count_launch<float>(c, grid, static_cast<size_t>(smem) * 4, counts, stream, weight);
 }
@@ -1179,31 +1195,24 @@ cudaError_t launch_deriv(sbn_program *P, const StepDesc &st, const uint8_t *ev, 
     return sbn_deriv_launch<float>(d, static_cast<size_t>(smem) * 4, stream);
 }
 
-// The drawn-code buffer of a sample / MPE run (P->d_drawn): codes [n_sampled][n_draws][ld_drawn] (one draw for
-// MPE), then one flag byte per row
-struct DrawnCodes {
-    int64_t n_draws = 1, ld_drawn = 0;
-    uint8_t *flags(const sbn_program *P) const { return P->d_drawn + static_cast<int64_t>(P->n_sampled) * n_draws * ld_drawn; }
-};
-
 // Sample step (kind 4): draws its variables for rows 0 .. n_rows - 1 and draws 0 .. n_draws - 1 (`k`: its index
 // among the sample steps).  Argmax step of an MPE program (kind 5, n_draws = 1): decodes them.
 cudaError_t launch_sample(sbn_program *P, const StepDesc &st, int k, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
-                          const DrawnCodes &dc, cudaStream_t stream) {
+                          const RunInputs &in, cudaStream_t stream) {
     P->launches++;
     SbnSample m;
     memset(&m, 0, sizeof m);
     m.ev = ev;
     m.ld_ev = ld_ev;
     m.drawn = P->d_drawn;
-    m.ld_drawn = dc.ld_drawn;
+    m.ld_drawn = in.ld_drawn;
     m.ld = P->ld;
     m.zoff = P->d_tile_off + st.zoff_pos;
     m.args = P->d_sample_args;
-    m.flag = dc.flags(P);
+    m.flag = in.flags(P);
     m.min_total = P->f64 ? 1e-290 : static_cast<double>(SBN_MIN_TOTAL_F32);
     m.n_rows = static_cast<int32_t>(n_rows);
-    m.n_draws = static_cast<int32_t>(dc.n_draws);
+    m.n_draws = static_cast<int32_t>(in.n_draws);
     m.n_ev = P->n_ev;
     m.n_in = static_cast<int32_t>(st.in.size());
     m.cz = st.cx;
@@ -1221,12 +1230,12 @@ cudaError_t launch_sample(sbn_program *P, const StepDesc &st, int k, const uint8
 // A readout, count, sample, argmax, derivative or joint step (kinds 2 .. 7) on its own launch; `k`: its index among the sample /
 // argmax steps (Philox counter word 0 of a sample step)
 cudaError_t launch_kind_step(sbn_program *P, const StepDesc &st, int k, const uint8_t *ev, int64_t ld_ev, int64_t n_rows,
-                             float *d_out, int64_t ld_out, const DrawnCodes &dc, cudaStream_t stream) {
+                             float *d_out, int64_t ld_out, const RunInputs &in, cudaStream_t stream) {
     if (st.kind == 2) return launch_marginal(P, st, ev, ld_ev, n_rows, d_out, ld_out, stream);
-    if (st.kind == 3) return launch_count(P, st, ev, ld_ev, n_rows, stream);
+    if (st.kind == 3) return launch_count(P, st, ev, ld_ev, n_rows, in, stream);
     if (st.kind == 6) return launch_deriv(P, st, ev, ld_ev, n_rows, d_out, ld_out, stream);
     if (st.kind == 7) return launch_joint(P, st, ev, ld_ev, n_rows, d_out, ld_out, stream);
-    return launch_sample(P, st, k, ev, ld_ev, n_rows, dc, stream);
+    return launch_sample(P, st, k, ev, ld_ev, n_rows, in, stream);
 }
 
 // The per-row output of a counts or sample run: P(observed) out of the posterior slot, NaN where it is out of
@@ -1272,22 +1281,22 @@ cudaError_t launch_normalise(sbn_program *P, float *d_out, int64_t ld_out, int64
 // pass through float32 first)
 inline size_t lik_elem(const sbn_program *P) { return P->f64 || sbn_log_domain(P->kind) ? 8 : 4; }
 
-// Soft-evidence program: fill the likelihood slots from P->lik (pitch P->ld_lik) and sum log(max) per row; the
+// Soft-evidence program: fill the likelihood slots from in.lik (pitch in.ld_lik) and sum log(max) per row; the
 // log-domain kinds store log(lik / max)
-cudaError_t launch_soft_pack(sbn_program *P, int64_t n_rows, cudaStream_t stream) {
+cudaError_t launch_soft_pack(sbn_program *P, int64_t n_rows, const RunInputs &in, cudaStream_t stream) {
     P->launches++;
     const int threads = 256;
     const unsigned grid = static_cast<unsigned>((n_rows + threads - 1) / threads);
     const int32_t rows = static_cast<int32_t>(n_rows), n_soft = static_cast<int32_t>(P->soft.size());
     if (sbn_log_domain(P->kind))  // MPE / MAP: log(lik / max) into the slots of a max-sum / log-sum-exp program
-        sbn_soft_pack_log<<<grid, threads, 0, stream>>>(static_cast<const double *>(P->lik), P->ld_lik, rows, n_soft,
+        sbn_soft_pack_log<<<grid, threads, 0, stream>>>(static_cast<const double *>(in.lik), in.ld_lik, rows, n_soft,
                                                         P->d_soft, P->d_arena, P->ld, P->d_log_max);
     else if (P->f64)
-        sbn_soft_pack<double><<<grid, threads, 0, stream>>>(static_cast<const double *>(P->lik), P->ld_lik, rows, n_soft,
+        sbn_soft_pack<double><<<grid, threads, 0, stream>>>(static_cast<const double *>(in.lik), in.ld_lik, rows, n_soft,
                                                             P->d_soft, reinterpret_cast<double *>(P->d_arena), P->ld,
                                                             P->d_log_max);
     else
-        sbn_soft_pack<float><<<grid, threads, 0, stream>>>(static_cast<const float *>(P->lik), P->ld_lik, rows, n_soft,
+        sbn_soft_pack<float><<<grid, threads, 0, stream>>>(static_cast<const float *>(in.lik), in.ld_lik, rows, n_soft,
                                                            P->d_soft, P->d_arena, P->ld, P->d_log_max);
     return cudaGetLastError();
 }
@@ -1344,10 +1353,10 @@ inline bool fold_normalise(const sbn_program *P, const StepDesc &st, const SbnSt
 // run; an MPE run leaves max log P(x, e) in the posterior slot.  `events` (profiling): one record per step, one
 // after the steps, one after the epilogue.
 int issue_all(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out, int64_t ld_out,
-              cudaStream_t stream, cudaEvent_t *events, const DrawnCodes &dc = {}) {
+              cudaStream_t stream, cudaEvent_t *events, const RunInputs &in = {}) {
     // the flags of the sample steps start clear in every run, captured graph or not
-    if (P->kind == kSample) SBN_CUDA(cudaMemsetAsync(dc.flags(P), 0, static_cast<size_t>(n_rows), stream));
-    if (!P->soft.empty()) SBN_CUDA(launch_soft_pack(P, n_rows, stream));
+    if (P->kind == kSample) SBN_CUDA(cudaMemsetAsync(in.flags(P), 0, static_cast<size_t>(n_rows), stream));
+    if (!P->soft.empty()) SBN_CUDA(launch_soft_pack(P, n_rows, in, stream));
     SbnStep q;
     int k = 0;
     int n_decoded = 0;  // sample / argmax steps issued so far
@@ -1357,10 +1366,10 @@ int issue_all(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows
         if (events) SBN_CUDA(cudaEventRecord(events[k], stream));
         ++k;
         if (hoisted(P, st)) continue;  // computed once, when the program was created
-        if (P->forward_run && !P->forward[k - 1]) continue;  // a forward run of a gradient program: P(observed) only
+        if (in.forward && !P->forward[k - 1]) continue;  // a forward run of a gradient program: P(observed) only
         if (st.kind >= 2) {
             const int decoded = st.kind == 4 || st.kind == 5 ? n_decoded++ : 0;
-            SBN_CUDA(launch_kind_step(P, st, decoded, d_ev, ld_ev, n_rows, d_out, ld_out, dc, stream));
+            SBN_CUDA(launch_kind_step(P, st, decoded, d_ev, ld_ev, n_rows, d_out, ld_out, in, stream));
             continue;
         }
         const int seg = chain_on(P) ? P->seg_first[k - 1] : -1;
@@ -1400,7 +1409,7 @@ int issue_all(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows
             break;
         case kCounts:
         case kGrad: SBN_CUDA(launch_prob(P, n_rows, d_out, nullptr, stream)); break;
-        case kSample: SBN_CUDA(launch_prob(P, n_rows, d_out, dc.flags(P), stream)); break;
+        case kSample: SBN_CUDA(launch_prob(P, n_rows, d_out, in.flags(P), stream)); break;
         case kJoint: SBN_CUDA(launch_prob(P, n_rows, P->d_total, nullptr, stream)); break;  // d_out holds the readouts
         case kMarginals:  // the readouts normalise
         case kMpe:
@@ -1418,14 +1427,14 @@ int issue_all(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows
 // A step runs on the stream of the producer of its largest slot input (chains stay on one
 // stream, no event needed); leaves take the branch streams round-robin.
 int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out, int64_t ld_out,
-                   cudaStream_t origin) {
+                   cudaStream_t origin, const RunInputs &in) {
     const int n_steps = static_cast<int>(P->steps.size());
     const int n_slots = static_cast<int>(P->slots.size());
     std::vector<int> last_writer(n_slots, -1);
     std::vector<std::vector<int>> readers(n_slots);
     std::vector<int> stream_of(n_steps, 0);
     cudaEvent_t fork = P->step_done[n_steps];  // reused as the fork event before any step
-    if (!P->soft.empty()) SBN_CUDA(launch_soft_pack(P, n_rows, origin));  // every branch forks after it
+    if (!P->soft.empty()) SBN_CUDA(launch_soft_pack(P, n_rows, in, origin));  // every branch forks after it
     SBN_CUDA(cudaEventRecord(fork, origin));
     bool joined[sbn_program::kBranches] = {false, false, false, false};
     int rr = 0;
@@ -1463,7 +1472,7 @@ int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n
         for (int d : deps)
             if (stream_of[d] != k) SBN_CUDA(cudaStreamWaitEvent(stream, P->step_done[d], 0));
         if (readout) {
-            SBN_CUDA(launch_kind_step(P, st, 0, d_ev, ld_ev, n_rows, d_out, ld_out, {}, stream));
+            SBN_CUDA(launch_kind_step(P, st, 0, d_ev, ld_ev, n_rows, d_out, ld_out, in, stream));
         } else {
             build_params(P, st, d_ev, ld_ev, n_rows, &q);
             SBN_CUDA(launch_step(P, st, q, stream));
@@ -1485,30 +1494,36 @@ int issue_branched(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n
     return SBN_OK;
 }
 
-// The checks every run shares: the program is of the kind the entry point runs (kPosterior: the run, evidence
-// and profile calls, which take posterior and marginals programs), and the rows and their evidence are well formed
+// Per program kind: its name, and the host call of its programs without and with soft evidence
+struct KindCalls {
+    const char *name, *plain, *soft;
+};
+constexpr const char *kGradCalls = "sbn_program_grad_forward_host / sbn_program_grad_backward_host";
+constexpr KindCalls kKindCalls[] = {
+    {"posterior", "sbn_program_run_host", "sbn_program_run_soft_host"},
+    {"marginals", "sbn_program_run_host", "sbn_program_run_soft_host"},
+    {"counts", "sbn_program_counts_host", "sbn_program_counts_soft_host"},
+    {"sample", "sbn_program_sample_host", "sbn_program_sample_soft_host"},
+    {"MPE", "sbn_program_mpe_host", "sbn_program_mpe_soft_host"},
+    {"MAP", "sbn_program_mpe_host", "sbn_program_mpe_soft_host"},
+    {"gradient", kGradCalls, kGradCalls},
+    {"joint", "sbn_program_joint_host", "sbn_program_joint_host"},
+};
+
+// The checks every run shares: the program is of the kind the entry point runs (kPosterior: the run, evidence and
+// profile calls, which take posterior and marginals programs; kMpe: MPE and MAP programs) and has soft evidence
+// exactly when the call is the kind's soft-evidence call (the gradient and joint calls take both), and the rows
+// and their evidence are well formed
 int check_rows(const sbn_program *P, ProgramKind kind, const void *ev, int64_t ld_ev, int64_t n_rows, bool soft = false) {
-    static const char *const name[] = {"posterior", "marginals", "counts", "sample", "MPE", "MAP", "gradient", "joint"};
-    static const char *const entry[] = {"sbn_program_run_*", "sbn_program_run_*", "sbn_program_counts_host",
-                                        "sbn_program_sample_host", "sbn_program_mpe_host", "sbn_program_mpe_host",
-                                        "sbn_program_grad_forward_host / sbn_program_grad_backward_host",
-                                        "sbn_program_joint_host"};
     if (!P) return fail(SBN_E_INVALID, "null program");
-    static const char *const soft_entry[] = {"sbn_program_run_soft_host", "sbn_program_run_soft_host",
-                                             "sbn_program_counts_soft_host", "sbn_program_sample_soft_host",
-                                             "sbn_program_mpe_soft_host", "sbn_program_mpe_soft_host", "", ""};
-    static const char *const plain_entry[] = {"sbn_program_run_host", "sbn_program_run_host", "sbn_program_counts_host",
-                                              "sbn_program_sample_host", "sbn_program_mpe_host", "sbn_program_mpe_host", "",
-                                              ""};
+    const KindCalls &calls = kKindCalls[P->kind];
+    const bool has_soft = !P->soft.empty();
+    const char *own = has_soft ? calls.soft : calls.plain;
     if ((P->kind == kMarginals ? kPosterior : P->kind == kMap ? kMpe : P->kind) != kind)
-        return fail(SBN_E_INVALID, "a %s program%s runs through %s", name[P->kind],
-                    !P->soft.empty() && *soft_entry[P->kind] ? " with soft evidence" : "",
-                    !P->soft.empty() && *soft_entry[P->kind] ? soft_entry[P->kind] : entry[P->kind]);
-    if (kind == kGrad || kind == kJoint) {  // the gradient and joint calls take programs with and without soft evidence
-    } else if (!P->soft.empty() && !soft)
-        return fail(SBN_E_INVALID, "a %s program with soft evidence runs through %s", name[P->kind], soft_entry[P->kind]);
-    if (P->soft.empty() && soft)
-        return fail(SBN_E_INVALID, "a %s program without soft evidence runs through %s", name[P->kind], plain_entry[P->kind]);
+        return fail(SBN_E_INVALID, "a %s program%s runs through %s", calls.name, has_soft ? " with soft evidence" : "", own);
+    if (kind != kGrad && kind != kJoint && has_soft != soft)
+        return fail(SBN_E_INVALID, "a %s program %s soft evidence runs through %s", calls.name, has_soft ? "with" : "without",
+                    own);
     if (n_rows <= 0) return fail(SBN_E_INVALID, "n_rows must be positive");
     if (P->n_ev > 0 && !ev) return fail(SBN_E_INVALID, "null evidence");
     if (P->n_ev > 1 && ld_ev < n_rows) return fail(SBN_E_INVALID, "ld_ev < n_rows");
@@ -1531,6 +1546,14 @@ int check_run_args(const sbn_program *P, const void *ev, int64_t ld_ev, int64_t 
 int reserve_rows(sbn_program *P, int64_t n_rows) {
     SBN_CUDA(cudaSetDevice(P->device));
     return n_rows > P->reserved_rows ? sbn_program_reserve(P, n_rows) : SBN_OK;
+}
+
+// Rows per chunk of a host call: the reservation, capped by SOROBN_B200_CHUNK_ROWS (rounded down to a multiple of 32,
+// at least 32) when it is set, so that a test can run a batch in several chunks.  Read on every call.
+int64_t chunk_rows(const sbn_program *P) {
+    const char *e = getenv("SOROBN_B200_CHUNK_ROWS");
+    if (!e || !*e) return P->reserved_rows;
+    return std::min(P->reserved_rows, std::max<int64_t>(32, atoll(e) / 32 * 32));
 }
 
 // Replay `g` on `stream`.  When `key` differs from the key it was captured for, capture it first: `issue()` issues
@@ -1566,18 +1589,18 @@ constexpr int64_t kSampleGraphMinRows = 4096;
 // One run of rows already on the device: a replay of the program's graph (captured on the program's stream) when
 // graphs are on, else plain launches on `stream`
 int run_rows(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out, int64_t ld_out,
-             cudaStream_t stream, const DrawnCodes &dc = {}) {
+             cudaStream_t stream, const RunInputs &in = {}) {
     // a short sample / MPE chunk runs as plain launches: capturing and instantiating a graph costs more than it
     // saves, and the short runs of a pattern whose rows are scattered through a frame come in many lengths
     const bool short_chunk = (P->kind == kSample || sbn_log_domain(P->kind)) && n_rows < kSampleGraphMinRows;
-    if (!P->use_graph || short_chunk) return issue_all(P, d_ev, ld_ev, n_rows, d_out, ld_out, stream, nullptr, dc);
-    const GraphKey key = {d_ev, ld_ev, n_rows, d_out, ld_out, P->d_partial, P->d_drawn, dc.n_draws, dc.ld_drawn, P->lik,
-                          P->ld_lik, P->forward_run ? nullptr : P->weight};
+    if (!P->use_graph || short_chunk) return issue_all(P, d_ev, ld_ev, n_rows, d_out, ld_out, stream, nullptr, in);
+    const GraphKey key = {d_ev, ld_ev, n_rows, d_out, ld_out, in.partial, P->d_drawn, in.n_draws, in.ld_drawn, in.lik,
+                          in.ld_lik, in.forward ? nullptr : in.weight};
     const bool branched = P->use_branches && P->kind <= kMarginals;
     // a gradient program's forward run issues a subset of its launches: it keeps a graph of its own
-    return replay(P, P->forward_run ? P->forward_graph : P->graph, key, P->stream, stream, [&] {
-        return branched ? issue_branched(P, d_ev, ld_ev, n_rows, d_out, ld_out, P->stream)
-                        : issue_all(P, d_ev, ld_ev, n_rows, d_out, ld_out, P->stream, nullptr, dc);
+    return replay(P, in.forward ? P->forward_graph : P->graph, key, P->stream, stream, [&] {
+        return branched ? issue_branched(P, d_ev, ld_ev, n_rows, d_out, ld_out, P->stream, in)
+                        : issue_all(P, d_ev, ld_ev, n_rows, d_out, ld_out, P->stream, nullptr, in);
     });
 }
 
@@ -1593,6 +1616,311 @@ int for_each_chunk(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_r
                                        P->stream));
         const int rc = body(r0, rows);
         if (rc != SBN_OK) return rc;
+    }
+    return SBN_OK;
+}
+
+// Whether a posterior run of n_rows host rows in chunks of `cap` goes through run_pipelined
+bool pipelined(const sbn_program *P, int64_t n_rows, int64_t cap, size_t elem) {
+    // Transfer-bound programs (a handful of launches for megabytes of codes in and posteriors
+    // out: Asia is ONE batched launch for 4 MB + 8 MB per million rows) are pipelined: the batch is
+    // cut into column ranges of the same staging buffers, H2D / kernels / D2H run on three streams
+    // chained by events, so a range's posteriors drain while the next range computes and the one
+    // after uploads -- PCIe is full duplex.  Launch-heavy programs (the grid: 48 launches per run,
+    // 5 MB of copies against milliseconds of kernels) keep the single CUDA-graph replay.
+    int64_t launches_per_run = 1;
+    for (size_t k = 0; k < P->steps.size(); ++k)
+        if (!hoisted(P, P->steps[k])) ++launches_per_run;
+    const int64_t bytes = n_rows * (P->n_ev + static_cast<int64_t>(P->Q) * static_cast<int64_t>(elem));
+    static const int pipe_env = [] {
+        const char *e = getenv("SOROBN_B200_PIPELINE");
+        return e ? atoi(e) : 1;
+    }();
+    return pipe_env && n_rows <= cap && launches_per_run <= 8 && bytes >= (int64_t(2) << 20) && n_rows >= 4 * 32768;
+}
+
+// One posterior run of a whole host batch (n_rows <= the reservation), pipelined over column ranges
+int run_pipelined(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, char *out, int64_t ld_out, size_t elem) {
+    constexpr int kMaxRanges = 8;
+    static const int kRanges = [] {
+        const char *e = getenv("SOROBN_B200_PIPE_RANGES");
+        // few ranges: each range adds copies and launches, and the copies are the bound
+        const int v = e ? atoi(e) : 3;
+        return v >= 2 && v <= kMaxRanges ? v : 3;
+    }();
+    if (P->pipe_events.empty()) {
+        P->pipe_events.resize(3 + 2 * kMaxRanges);
+        for (auto &e : P->pipe_events) SBN_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    }
+    cudaStream_t s_in = P->branch[0], s_run = P->stream, s_out = P->branch[1];
+    const int64_t range = round_up((n_rows + kRanges - 1) / kRanges, 32);
+    // the side streams fork from s_run and join back into it; a few plain launches per range, nothing to
+    // amortise inside
+    auto issue_ranges = [&]() -> int {
+        cudaEvent_t fork = P->pipe_events[0], j_in = P->pipe_events[1 + 2 * kMaxRanges], j_out = P->pipe_events[2 + 2 * kMaxRanges];
+        SBN_CUDA(cudaEventRecord(fork, s_run));
+        SBN_CUDA(cudaStreamWaitEvent(s_in, fork, 0));
+        SBN_CUDA(cudaStreamWaitEvent(s_out, fork, 0));
+        for (int64_t r0 = 0, k = 0; r0 < n_rows; r0 += range, ++k) {
+            const int64_t rows = std::min(range, n_rows - r0);
+            cudaEvent_t up = P->pipe_events[1 + 2 * k], done = P->pipe_events[2 + 2 * k];
+            if (P->n_ev > 0) {
+                SBN_CUDA(cudaMemcpy2DAsync(P->d_ev + r0, static_cast<size_t>(P->ld), ev + r0, static_cast<size_t>(ld_ev),
+                                           static_cast<size_t>(rows), static_cast<size_t>(P->n_ev), cudaMemcpyHostToDevice, s_in));
+                SBN_CUDA(cudaEventRecord(up, s_in));
+                SBN_CUDA(cudaStreamWaitEvent(s_run, up, 0));
+            }
+            char *d_out = reinterpret_cast<char *>(P->d_out) + r0 * elem;
+            const int rc = issue_all(P, P->d_ev + r0, P->ld, rows, reinterpret_cast<float *>(d_out), P->ld, s_run, nullptr);
+            if (rc != SBN_OK) return rc;
+            SBN_CUDA(cudaEventRecord(done, s_run));
+            SBN_CUDA(cudaStreamWaitEvent(s_out, done, 0));
+            SBN_CUDA(cudaMemcpy2DAsync(out + r0 * elem, static_cast<size_t>(ld_out) * elem, d_out, static_cast<size_t>(P->ld) * elem,
+                                       static_cast<size_t>(rows) * elem, static_cast<size_t>(P->Q), cudaMemcpyDeviceToHost, s_out));
+        }
+        SBN_CUDA(cudaEventRecord(j_in, s_in));
+        SBN_CUDA(cudaStreamWaitEvent(s_run, j_in, 0));
+        SBN_CUDA(cudaEventRecord(j_out, s_out));
+        SBN_CUDA(cudaStreamWaitEvent(s_run, j_out, 0));
+        return SBN_OK;
+    };
+    // the whole fan-out is replayed as ONE graph launch when the host buffers are pinned (a dozen copies,
+    // launches and event edges cost CPU time of the order of what they overlap); the graph is kept for the
+    // (buffers, rows) it was built for
+    auto pinned = [](const void *ptr) {
+        cudaPointerAttributes a;
+        if (cudaPointerGetAttributes(&a, ptr) != cudaSuccess) {
+            cudaGetLastError();
+            return false;
+        }
+        return a.type == cudaMemoryTypeHost;
+    };
+    int rc;
+    if (P->use_graph && pinned(out) && (P->n_ev == 0 || pinned(ev)))
+        rc = replay(P, P->pipe_graph, {ev, ld_ev, n_rows, out, ld_out}, s_run, s_run, issue_ranges);
+    else
+        rc = issue_ranges();
+    if (rc != SBN_OK) {  // the side streams may not have joined s_run
+        cudaStreamSynchronize(s_in);
+        cudaStreamSynchronize(s_out);
+    }
+    const cudaError_t e = cudaStreamSynchronize(s_run);
+    if (rc != SBN_OK) return rc;
+    SBN_CUDA(e);
+    return SBN_OK;
+}
+
+// One host call: the program kind it takes (as check_rows), whether it is the kind's soft-evidence call, its
+// precision, the caller's rows and where each output goes.  The caller's pointers are read and written during the
+// call only.
+struct HostCall {
+    HostCall(ProgramKind kind, bool f64, const uint8_t *ev, int64_t ld_ev, int64_t n_rows)
+        : kind(kind), f64(f64), ev(ev), ld_ev(ld_ev), n_rows(n_rows) {}
+    ProgramKind kind;
+    bool soft = false;
+    bool f64;
+    const uint8_t *ev;  // codes [n_ev][ld_ev]
+    int64_t ld_ev, n_rows;
+    const void *lik = nullptr;  // soft evidence: [n_rows][ld_lik], host or (lik_on_device) device memory
+    int64_t ld_lik = 0;
+    int lik_on_device = 0;
+    const double *weights = nullptr;  // gradient program: the row weights of a backward call (null: a forward call)
+    int weights_on_device = 0;
+    int64_t n_draws = 1;  // sample program: draws per row, seed, the caller's index of row 0
+    uint64_t seed = 0;
+    int64_t row_base = 0;
+    // the readouts [Q][ld_out] of a posterior or joint run, the derivative readouts [n_lik][ld_out] of a backward
+    // run, the drawn / decoded codes [n_sampled][n_draws][n_rows] of a sample / MPE run
+    void *out = nullptr;
+    int64_t ld_out = 0;
+    // per row, in the program's type: P(event) of a posterior run, P(observed) of a counts, sample, gradient or
+    // joint run, max log P of an MPE run
+    void *prob = nullptr;
+    double *log_prob = nullptr;  // per row: log of prob (MPE: prob) + sum log(max) of a soft-evidence row
+    double *counts = nullptr;    // counts program / backward call: the count table [n_counts], added into
+    int64_t n_counts = 0;
+};
+
+// Every host call but the pipelined posterior run: the checks, the reservation, the call's buffers, then per chunk
+// the staged rows, one run and its downloads, and after one final sync the count table and log P of the batch.
+int host_call(sbn_program *P, const HostCall &c) {
+    int rc = check_rows(P, c.kind, c.ev, c.ld_ev, c.n_rows, c.soft);
+    if (rc != SBN_OK) return rc;
+    if (P->f64 != c.f64) return fail(SBN_E_INVALID, "program precision does not match the call");
+    const int64_t n_rows = c.n_rows;
+    const bool soft = !P->soft.empty(), mpe = c.kind == kMpe, decodes = mpe || c.kind == kSample;
+    const bool backward = c.kind == kGrad && c.weights, counting = c.kind == kCounts || backward;
+    const char *joint_call = c.f64 ? "sbn_program_joint_host_f64" : "sbn_program_joint_host";
+    if (c.kind == kJoint && soft && !c.lik)
+        return fail(SBN_E_INVALID, "a joint program with soft evidence needs its likelihoods: pass lik to %s", joint_call);
+    if (c.kind == kJoint && !soft && c.lik)
+        return fail(SBN_E_INVALID, "a joint program without soft evidence takes no likelihoods: pass lik = NULL to %s", joint_call);
+    if (soft && !c.lik) return fail(SBN_E_INVALID, "null likelihoods");
+    if (soft && c.ld_lik < P->n_lik)
+        return fail(SBN_E_INVALID, "ld_lik %lld < the %d likelihood columns", (long long)c.ld_lik, P->n_lik);
+    switch (c.kind) {  // the outputs
+        case kPosterior:
+            if (!c.out && !c.prob) return fail(SBN_E_INVALID, "null output");
+            if (c.out && P->Q > 1 && c.ld_out < n_rows) return fail(SBN_E_INVALID, "ld_out < n_rows");
+            if (P->kind == kMarginals && (c.prob || c.log_prob))
+                return fail(SBN_E_INVALID, "a marginals program has no single normaliser; P(event) and log P(e, lik) come "
+                                           "from a posterior program");
+            break;
+        case kJoint:
+            if (!c.out || !c.prob) return fail(SBN_E_INVALID, "null output");
+            if (c.ld_out < n_rows) return fail(SBN_E_INVALID, "ld_out < n_rows");
+            break;
+        case kSample:
+            if (c.n_draws <= 0 || c.n_draws > INT32_MAX) return fail(SBN_E_INVALID, "n_draws must be in 1 .. 2^31 - 1");
+            if (c.row_base < 0) return fail(SBN_E_INVALID, "row_base must not be negative");
+            if ((P->n_sampled > 0 && !c.out) || !c.prob) return fail(SBN_E_INVALID, "null output");
+            break;
+        case kMpe:
+            if ((P->n_sampled > 0 && !c.out) || (!c.prob && !c.log_prob)) return fail(SBN_E_INVALID, "null output");
+            break;
+        case kCounts:
+            if (!c.counts || !c.prob) return fail(SBN_E_INVALID, "null output");
+            break;
+        case kGrad:
+            if (backward && (!c.counts || (P->n_lik > 0 && !c.out))) return fail(SBN_E_INVALID, "null output");
+            if (backward && P->n_lik > 0 && c.ld_out < n_rows) return fail(SBN_E_INVALID, "ld_deriv < n_rows");
+            break;
+        default: break;
+    }
+    if (counting && c.n_counts != P->n_counts)
+        return fail(SBN_E_INVALID, "the count table has %lld entries, not %lld", (long long)P->n_counts, (long long)c.n_counts);
+    // the chunk capacity follows the largest batch seen so far (a program first used for one row must not answer a
+    // later million-row batch one row at a time)
+    rc = reserve_rows(P, n_rows);
+    if (rc != SBN_OK) return rc;
+    int64_t cap = chunk_rows(P);
+    const size_t elem = c.f64 ? 8 : 4;
+    if (c.kind == kPosterior && c.out && !soft && pipelined(P, n_rows, cap, elem))
+        return run_pipelined(P, c.ev, c.ld_ev, n_rows, static_cast<char *>(c.out), c.ld_out, elem);
+
+    // from here on every return leaves nothing running on the program's stream and frees the partial tables
+    struct Finish {
+        sbn_program *P;
+        double *partial;
+        ~Finish() {
+            cudaStreamSynchronize(P->stream);
+            if (partial) cudaFree(partial);
+        }
+    } finish = {P, nullptr};
+    RunInputs in;
+    in.forward = c.kind == kGrad && !backward;
+    if (counting) {
+        // the per-warp partial tables live for this call only: a program that is not running holds none of them
+        const cudaError_t e = cudaMalloc(&finish.partial, static_cast<size_t>(std::max<int64_t>(1, P->partial_doubles)) * 8);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            finish.partial = nullptr;
+            return fail(SBN_E_NOMEM, "cudaMalloc of %lld bytes of partial count tables failed: %s",
+                        (long long)(P->partial_doubles * 8), cudaGetErrorString(e));
+        }
+        in.partial = finish.partial;
+        SBN_CUDA(cudaMemsetAsync(P->d_counts, 0, static_cast<size_t>(P->n_counts) * 8, P->stream));
+    }
+    if (decodes) {
+        // the drawn codes of a chunk ([n_sampled][n_draws] bytes + one flag byte per row) take at most half of the
+        // free device memory: larger batches run in more chunks
+        const int64_t per_row = static_cast<int64_t>(P->n_sampled) * c.n_draws + 1;
+        if (round_up(std::min(cap, n_rows), 32) * per_row > P->drawn_bytes) {  // the buffer of an earlier call may do
+            size_t free_b = 0, total_b = 0;
+            SBN_CUDA(cudaMemGetInfo(&free_b, &total_b));
+            const int64_t budget = static_cast<int64_t>(free_b / 2) + P->drawn_bytes;
+            if (round_up(cap, 32) * per_row > budget) cap = std::max<int64_t>(32, budget / per_row / 32 * 32);
+        }
+        in.n_draws = c.n_draws;
+        in.ld_drawn = round_up(std::min(cap, n_rows), 32);
+        const int64_t bytes = in.ld_drawn * per_row;
+        if (bytes > P->drawn_bytes) {
+            SBN_CUDA(cudaStreamSynchronize(P->stream));
+            cudaFree(P->d_drawn);
+            P->d_drawn = nullptr;
+            P->drawn_bytes = 0;
+            const cudaError_t e = cudaMalloc(&P->d_drawn, static_cast<size_t>(bytes));
+            if (e != cudaSuccess) {
+                cudaGetLastError();
+                P->d_drawn = nullptr;
+                return fail(SBN_E_NOMEM, "cudaMalloc of %lld bytes of drawn codes failed: %s", (long long)bytes, cudaGetErrorString(e));
+            }
+            P->drawn_bytes = bytes;
+        }
+        if (!mpe && !P->d_sample_args) SBN_CUDA(cudaMalloc(&P->d_sample_args, 4 * sizeof(uint32_t)));
+    }
+    // a chunk's readouts: rows first .. first + n_readouts - 1 of d_out (a gradient program's derivatives follow
+    // its P(observed) row)
+    const int64_t first = c.kind == kGrad ? 1 : 0;
+    const int64_t n_readouts = !c.out || decodes ? 0 : c.kind == kGrad ? P->n_lik : P->Q;
+    // a chunk's per-row value: the normaliser of a posterior or joint run, the maximum in the posterior slot of an
+    // MPE run ([1][ld], or one value for every row), P(observed) in d_out otherwise; into the caller's prob, or into
+    // a batch buffer of the call's own when only its log is asked for
+    const bool one_value = mpe && !P->slots[P->post_slot].batched;
+    const void *value = c.kind == kPosterior || c.kind == kJoint ? static_cast<const void *>(P->d_total)
+                        : mpe                                    ? P->slots[P->post_slot].ptr
+                                                                 : P->d_out;
+    std::vector<char> own(!c.prob && c.log_prob ? static_cast<size_t>(n_rows) * elem : 0);
+    char *prob = c.prob ? static_cast<char *>(c.prob) : own.empty() ? nullptr : own.data();
+    std::vector<double> log_max(c.log_prob ? static_cast<size_t>(n_rows) : 0, 0.0);
+    const size_t lik_bytes = lik_elem(P);
+    rc = for_each_chunk(P, c.ev, c.ld_ev, n_rows, cap, [&](int64_t r0, int64_t rows) -> int {
+        // the chunk's likelihoods and weights: device rows read in place, host rows staged on the program's stream
+        const char *lik = static_cast<const char *>(c.lik) + r0 * c.ld_lik * static_cast<int64_t>(lik_bytes);
+        if (soft && c.lik_on_device) {
+            in.lik = lik;
+            in.ld_lik = c.ld_lik;
+        } else if (soft) {
+            SBN_CUDA(cudaMemcpy2DAsync(P->d_lik, static_cast<size_t>(P->n_lik) * lik_bytes, lik, static_cast<size_t>(c.ld_lik) * lik_bytes,
+                                       static_cast<size_t>(P->n_lik) * lik_bytes, static_cast<size_t>(rows), cudaMemcpyHostToDevice,
+                                       P->stream));
+            in.lik = P->d_lik;
+            in.ld_lik = P->n_lik;
+        }
+        if (backward && c.weights_on_device) {
+            in.weight = c.weights + r0;
+        } else if (backward) {
+            SBN_CUDA(cudaMemcpyAsync(P->d_weight, c.weights + r0, static_cast<size_t>(rows) * 8, cudaMemcpyHostToDevice, P->stream));
+            in.weight = P->d_weight;
+        }
+        if (c.kind == kSample) {
+            // read by the sample steps at run time, so that one captured graph serves every seed and chunk
+            const uint64_t first_row = static_cast<uint64_t>(c.row_base + r0);
+            const uint32_t args[4] = {static_cast<uint32_t>(c.seed), static_cast<uint32_t>(c.seed >> 32),
+                                      static_cast<uint32_t>(first_row), static_cast<uint32_t>(first_row >> 32)};
+            SBN_CUDA(cudaMemcpyAsync(P->d_sample_args, args, sizeof args, cudaMemcpyHostToDevice, P->stream));
+        }
+        // the graph reads the tables and the count table by address, so it replays the values sbn_program_set_tables uploads
+        const int rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream, in);
+        if (rc != SBN_OK) return rc;
+        if (decodes && P->n_sampled > 0)
+            SBN_CUDA(cudaMemcpy2DAsync(static_cast<uint8_t *>(c.out) + r0, static_cast<size_t>(n_rows), P->d_drawn,
+                                       static_cast<size_t>(in.ld_drawn), static_cast<size_t>(rows),
+                                       static_cast<size_t>(P->n_sampled * c.n_draws), cudaMemcpyDeviceToHost, P->stream));
+        if (n_readouts > 0)
+            SBN_CUDA(cudaMemcpy2DAsync(static_cast<char *>(c.out) + r0 * elem, static_cast<size_t>(c.ld_out) * elem,
+                                       reinterpret_cast<char *>(P->d_out) + first * P->ld * elem, static_cast<size_t>(P->ld) * elem,
+                                       static_cast<size_t>(rows) * elem, static_cast<size_t>(n_readouts), cudaMemcpyDeviceToHost,
+                                       P->stream));
+        if (prob && !one_value)
+            SBN_CUDA(cudaMemcpyAsync(prob + r0 * elem, value, static_cast<size_t>(rows) * elem, cudaMemcpyDeviceToHost, P->stream));
+        else if (prob && r0 == 0)
+            SBN_CUDA(cudaMemcpyAsync(prob, value, elem, cudaMemcpyDeviceToHost, P->stream));
+        if (soft && c.log_prob)
+            SBN_CUDA(cudaMemcpyAsync(log_max.data() + r0, P->d_log_max, static_cast<size_t>(rows) * 8, cudaMemcpyDeviceToHost, P->stream));
+        return SBN_OK;
+    });
+    if (rc != SBN_OK) return rc;
+    std::vector<double> table(counting ? static_cast<size_t>(P->n_counts) : 0);
+    if (counting) SBN_CUDA(cudaMemcpyAsync(table.data(), P->d_counts, table.size() * 8, cudaMemcpyDeviceToHost, P->stream));
+    SBN_CUDA(cudaStreamSynchronize(P->stream));
+    for (size_t i = 0; i < table.size(); ++i) c.counts[i] += table[i];
+    if (one_value && prob) std::fill(reinterpret_cast<float *>(prob) + 1, reinterpret_cast<float *>(prob) + n_rows, *reinterpret_cast<float *>(prob));
+    // log P(observed, lik) = log P(observed, lik / max) + sum log(max) of the row, NaN where the row is flagged; an
+    // MPE run's maximum is a log already
+    for (int64_t i = 0; c.log_prob && i < n_rows; ++i) {
+        const double p = c.f64 ? reinterpret_cast<const double *>(prob)[i] : reinterpret_cast<const float *>(prob)[i];
+        c.log_prob[i] = (mpe ? p : std::log(p)) + log_max[static_cast<size_t>(i)];
     }
     return SBN_OK;
 }
@@ -1793,7 +2121,6 @@ void sbn_program_destroy(sbn_program *P) {
     sbn_pair_free(P);
     cudaFree(P->d_shared);
     cudaFree(P->d_counts);
-    cudaFree(P->d_partial);
     cudaFree(P->d_drawn);
     cudaFree(P->d_sample_args);
     cudaFree(P->d_soft);
@@ -1877,495 +2204,133 @@ int sbn_program_run_device(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, i
     return run_rows(P, d_ev, ld_ev, n_rows, d_out, ld_out, static_cast<cudaStream_t>(stream_));
 }
 
-static int run_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, void *out_, int64_t ld_out,
-                           bool f64, bool want_totals = false) {
-    int rc = check_run_args(P, ev, ld_ev, n_rows, out_, want_totals ? n_rows : ld_out);
-    if (rc != SBN_OK) return rc;
-    if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the run call");
-    if (want_totals && P->kind == kMarginals)
-        return fail(SBN_E_INVALID, "a marginals program has no single normaliser; P(event) comes from a program without targets");
-    const size_t elem = f64 ? 8 : 4;
-    char *out = static_cast<char *>(out_);
-    // the chunk capacity follows the largest batch seen so far (a program first used for one row must not answer a
-    // later million-row batch one row at a time)
-    rc = reserve_rows(P, n_rows);
-    if (rc != SBN_OK) return rc;
-    const int64_t cap = P->reserved_rows;
-    // Transfer-bound programs (a handful of launches for megabytes of codes in and posteriors
-    // out: Asia is ONE batched launch for 4 MB + 8 MB per million rows) are pipelined: the batch is
-    // cut into column ranges of the same staging buffers, H2D / kernels / D2H run on three streams
-    // chained by events, so a range's posteriors drain while the next range computes and the one
-    // after uploads -- PCIe is full duplex.  Launch-heavy programs (the grid: 48 launches per run,
-    // 5 MB of copies against milliseconds of kernels) keep the single CUDA-graph replay.
-    int64_t launches_per_run = 1;
-    for (size_t k = 0; k < P->steps.size(); ++k)
-        if (!hoisted(P, P->steps[k])) ++launches_per_run;
-    const int64_t bytes = n_rows * (P->n_ev + static_cast<int64_t>(want_totals ? 1 : P->Q) * static_cast<int64_t>(elem));
-    static const int pipe_env = [] {
-        const char *e = getenv("SOROBN_B200_PIPELINE");
-        return e ? atoi(e) : 1;
-    }();
-    if (pipe_env && !want_totals && n_rows <= cap && launches_per_run <= 8 && bytes >= (int64_t(2) << 20) && n_rows >= 4 * 32768) {
-        constexpr int kMaxRanges = 8;
-        static const int kRanges = [] {
-            const char *e = getenv("SOROBN_B200_PIPE_RANGES");
-            // few ranges: each range adds copies and launches, and the copies are the bound
-            const int v = e ? atoi(e) : 3;
-            return v >= 2 && v <= kMaxRanges ? v : 3;
-        }();
-        if (P->pipe_events.empty()) {
-            P->pipe_events.resize(3 + 2 * kMaxRanges);
-            for (auto &e : P->pipe_events) SBN_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        }
-        cudaStream_t s_in = P->branch[0], s_run = P->stream, s_out = P->branch[1];
-        const int64_t range = round_up((n_rows + kRanges - 1) / kRanges, 32);
-        // the side streams fork from s_run and join back into it; a few plain launches per range, nothing to
-        // amortise inside
-        auto issue_ranges = [&]() -> int {
-            cudaEvent_t fork = P->pipe_events[0], j_in = P->pipe_events[1 + 2 * kMaxRanges], j_out = P->pipe_events[2 + 2 * kMaxRanges];
-            SBN_CUDA(cudaEventRecord(fork, s_run));
-            SBN_CUDA(cudaStreamWaitEvent(s_in, fork, 0));
-            SBN_CUDA(cudaStreamWaitEvent(s_out, fork, 0));
-            for (int64_t r0 = 0, k = 0; r0 < n_rows; r0 += range, ++k) {
-                const int64_t rows = std::min(range, n_rows - r0);
-                cudaEvent_t up = P->pipe_events[1 + 2 * k], done = P->pipe_events[2 + 2 * k];
-                if (P->n_ev > 0) {
-                    SBN_CUDA(cudaMemcpy2DAsync(P->d_ev + r0, static_cast<size_t>(P->ld), ev + r0, static_cast<size_t>(ld_ev),
-                                               static_cast<size_t>(rows), static_cast<size_t>(P->n_ev), cudaMemcpyHostToDevice, s_in));
-                    SBN_CUDA(cudaEventRecord(up, s_in));
-                    SBN_CUDA(cudaStreamWaitEvent(s_run, up, 0));
-                }
-                char *d_out = reinterpret_cast<char *>(P->d_out) + r0 * elem;
-                const int rc = issue_all(P, P->d_ev + r0, P->ld, rows, reinterpret_cast<float *>(d_out), P->ld, s_run, nullptr);
-                if (rc != SBN_OK) return rc;
-                SBN_CUDA(cudaEventRecord(done, s_run));
-                SBN_CUDA(cudaStreamWaitEvent(s_out, done, 0));
-                SBN_CUDA(cudaMemcpy2DAsync(out + r0 * elem, static_cast<size_t>(ld_out) * elem, d_out, static_cast<size_t>(P->ld) * elem,
-                                           static_cast<size_t>(rows) * elem, static_cast<size_t>(P->Q), cudaMemcpyDeviceToHost, s_out));
-            }
-            SBN_CUDA(cudaEventRecord(j_in, s_in));
-            SBN_CUDA(cudaStreamWaitEvent(s_run, j_in, 0));
-            SBN_CUDA(cudaEventRecord(j_out, s_out));
-            SBN_CUDA(cudaStreamWaitEvent(s_run, j_out, 0));
-            return SBN_OK;
-        };
-        // the whole fan-out is replayed as ONE graph launch when the host buffers are pinned (a dozen copies,
-        // launches and event edges cost CPU time of the order of what they overlap); the graph is kept for the
-        // (buffers, rows) it was built for
-        auto pinned = [](const void *ptr) {
-            cudaPointerAttributes a;
-            if (cudaPointerGetAttributes(&a, ptr) != cudaSuccess) {
-                cudaGetLastError();
-                return false;
-            }
-            return a.type == cudaMemoryTypeHost;
-        };
-        if (P->use_graph && pinned(out) && (P->n_ev == 0 || pinned(ev)))
-            rc = replay(P, P->pipe_graph, {ev, ld_ev, n_rows, out, ld_out}, s_run, s_run, issue_ranges);
-        else
-            rc = issue_ranges();
-        if (rc != SBN_OK) {  // the side streams may not have joined s_run
-            cudaStreamSynchronize(s_in);
-            cudaStreamSynchronize(s_out);
-        }
-        const cudaError_t e = cudaStreamSynchronize(s_run);
-        if (rc != SBN_OK) return rc;
-        SBN_CUDA(e);
-        return SBN_OK;
-    }
-    rc = for_each_chunk(P, ev, ld_ev, n_rows, cap, [&](int64_t r0, int64_t rows) -> int {
-        const int rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
-        if (rc != SBN_OK) return rc;
-        if (want_totals)
-            SBN_CUDA(cudaMemcpyAsync(out + r0 * elem, P->d_total, static_cast<size_t>(rows) * elem,
-                                     cudaMemcpyDeviceToHost, P->stream));
-        else
-            SBN_CUDA(cudaMemcpy2DAsync(out + r0 * elem, static_cast<size_t>(ld_out) * elem, P->d_out,
-                                       static_cast<size_t>(P->ld) * elem, static_cast<size_t>(rows) * elem,
-                                       static_cast<size_t>(P->Q), cudaMemcpyDeviceToHost, P->stream));
-        return SBN_OK;
-    });
-    if (rc != SBN_OK) return rc;
-    SBN_CUDA(cudaStreamSynchronize(P->stream));
-    return SBN_OK;
-}
-
 int sbn_program_run_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, float *out, int64_t ld_out) {
-    return run_host_common(P, ev, ld_ev, n_rows, out, ld_out, false);
+    HostCall c(kPosterior, false, ev, ld_ev, n_rows);
+    c.out = out, c.ld_out = ld_out;
+    return host_call(P, c);
 }
 
 int sbn_program_run_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *out,
                              int64_t ld_out) {
-    return run_host_common(P, ev, ld_ev, n_rows, out, ld_out, true);
+    HostCall c(kPosterior, true, ev, ld_ev, n_rows);
+    c.out = out, c.ld_out = ld_out;
+    return host_call(P, c);
 }
 
 int sbn_program_evidence_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, float *prob) {
-    return run_host_common(P, ev, ld_ev, n_rows, prob, n_rows, false, true);
+    HostCall c(kPosterior, false, ev, ld_ev, n_rows);
+    c.prob = prob;
+    return host_call(P, c);
 }
 
 int sbn_program_evidence_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *prob) {
-    return run_host_common(P, ev, ld_ev, n_rows, prob, n_rows, true, true);
+    HostCall c(kPosterior, true, ev, ld_ev, n_rows);
+    c.prob = prob;
+    return host_call(P, c);
 }
 
-// The caller's likelihoods of a soft-evidence call ([n_rows][ld_lik], host memory or, with `on_device`, device memory
-// of the program's device) and, when `log_max` is set, where sum log(max) of every row goes (host, [n_rows])
-struct SoftLik {
-    bool soft = false;  // false: a call without soft evidence
-    const void *lik = nullptr;
-    int64_t ld_lik = 0;
-    int on_device = 0;
-    double *log_max = nullptr;
-};
-
-static int check_lik(const sbn_program *P, const SoftLik &s) {
-    if (!s.soft) return SBN_OK;
-    if (!s.lik) return fail(SBN_E_INVALID, "null likelihoods");
-    if (s.ld_lik < P->n_lik) return fail(SBN_E_INVALID, "ld_lik %lld < the %d likelihood columns", (long long)s.ld_lik, P->n_lik);
-    return SBN_OK;
-}
-
-// Point the next issue at rows [r0, r0 + rows) of the likelihoods: a device pointer in place, host rows copied into
-// the staging buffer (on the program's stream, ahead of the run)
-static int stage_lik(sbn_program *P, const SoftLik &s, int64_t r0, int64_t rows) {
-    if (!s.soft) return SBN_OK;
-    const size_t elem = lik_elem(P);
-    const char *chunk = static_cast<const char *>(s.lik) + r0 * s.ld_lik * static_cast<int64_t>(elem);
-    if (s.on_device) {
-        P->lik = chunk;
-        P->ld_lik = s.ld_lik;
-    } else {
-        SBN_CUDA(cudaMemcpy2DAsync(P->d_lik, static_cast<size_t>(P->n_lik) * elem, chunk, static_cast<size_t>(s.ld_lik) * elem,
-                                   static_cast<size_t>(P->n_lik) * elem, static_cast<size_t>(rows), cudaMemcpyHostToDevice,
-                                   P->stream));
-        P->lik = P->d_lik;
-        P->ld_lik = P->n_lik;
-    }
-    return SBN_OK;
-}
-
-// After a chunk's run: its rows' sum log(max), when the caller asked for them
-static int fetch_log_max(sbn_program *P, const SoftLik &s, int64_t r0, int64_t rows) {
-    if (s.soft && s.log_max)
-        SBN_CUDA(cudaMemcpyAsync(s.log_max + r0, P->d_log_max, static_cast<size_t>(rows) * 8, cudaMemcpyDeviceToHost, P->stream));
-    return SBN_OK;
-}
-
-// A posterior or marginals program with soft evidence: per chunk, the codes and (host) likelihoods are staged,
-// the pack fills the likelihood slots inside the run (captured graph or not), the posterior comes back, and
-// with `log_evidence` log P(e, lik) = log(normaliser) + sum log(max).  Never pipelined.
-static int run_soft_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const void *lik,
-                           int64_t ld_lik, int lik_on_device, void *out_, int64_t ld_out, double *log_evidence, bool f64) {
-    int rc = check_run_args(P, ev, ld_ev, n_rows, out_, ld_out, true);
-    if (rc != SBN_OK) return rc;
-    if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the run call");
-    const SoftLik soft = {true, lik, ld_lik, lik_on_device, nullptr};
-    rc = check_lik(P, soft);
-    if (rc != SBN_OK) return rc;
-    if (log_evidence && P->kind == kMarginals)
-        return fail(SBN_E_INVALID, "a marginals program has no single normaliser; log P(e, lik) comes from a posterior program");
-    const size_t elem = f64 ? 8 : 4;
-    char *out = static_cast<char *>(out_);
-    rc = reserve_rows(P, n_rows);
-    if (rc != SBN_OK) return rc;
-    const int64_t cap = P->reserved_rows;
-    std::vector<char> total(log_evidence ? static_cast<size_t>(cap) * elem : 0);
-    std::vector<double> log_max(log_evidence ? static_cast<size_t>(cap) : 0);
-    rc = for_each_chunk(P, ev, ld_ev, n_rows, cap, [&](int64_t r0, int64_t rows) -> int {
-        int rc = stage_lik(P, soft, r0, rows);
-        if (rc != SBN_OK) return rc;
-        rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
-        if (rc != SBN_OK) return rc;
-        SBN_CUDA(cudaMemcpy2DAsync(out + r0 * elem, static_cast<size_t>(ld_out) * elem, P->d_out, static_cast<size_t>(P->ld) * elem,
-                                   static_cast<size_t>(rows) * elem, static_cast<size_t>(P->Q), cudaMemcpyDeviceToHost, P->stream));
-        if (!log_evidence) return SBN_OK;
-        SBN_CUDA(cudaMemcpyAsync(total.data(), P->d_total, static_cast<size_t>(rows) * elem, cudaMemcpyDeviceToHost, P->stream));
-        SBN_CUDA(cudaMemcpyAsync(log_max.data(), P->d_log_max, static_cast<size_t>(rows) * 8, cudaMemcpyDeviceToHost, P->stream));
-        SBN_CUDA(cudaStreamSynchronize(P->stream));
-        for (int64_t i = 0; i < rows; ++i) {
-            const double t = f64 ? reinterpret_cast<const double *>(total.data())[i] : reinterpret_cast<const float *>(total.data())[i];
-            log_evidence[r0 + i] = std::log(t) + log_max[i];  // NaN where the normaliser is flagged
-        }
-        return SBN_OK;
-    });
-    P->lik = nullptr;  // a device pointer is the caller's: forget it
-    if (rc != SBN_OK) return rc;
-    SBN_CUDA(cudaStreamSynchronize(P->stream));
-    return SBN_OK;
-}
-
+// A posterior or marginals program with soft evidence: the pack fills the likelihood slots inside each chunk's run
+// (captured graph or not); with `log_evidence`, log P(e, lik) = log(normaliser) + sum log(max).  Never pipelined.
 int sbn_program_run_soft_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
                               int64_t ld_lik, int lik_on_device, float *out, int64_t ld_out, double *log_evidence) {
-    return run_soft_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, out, ld_out, log_evidence, false);
+    HostCall c(kPosterior, false, ev, ld_ev, n_rows);
+    c.soft = true, c.lik = lik, c.ld_lik = ld_lik, c.lik_on_device = lik_on_device;
+    c.out = out, c.ld_out = ld_out, c.log_prob = log_evidence;
+    return host_call(P, c);
 }
 
 int sbn_program_run_soft_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
                                   int64_t ld_lik, int lik_on_device, double *out, int64_t ld_out, double *log_evidence) {
-    return run_soft_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, out, ld_out, log_evidence, true);
-}
-
-// The chunks of a counts call: P(observed) per chunk, then the batch's counts added into `counts`
-static int add_expected_counts(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, void *prob,
-                               size_t elem, const SoftLik &soft) {
-    SBN_CUDA(cudaMemsetAsync(P->d_counts, 0, static_cast<size_t>(P->n_counts) * 8, P->stream));
-    const int rc = for_each_chunk(P, ev, ld_ev, n_rows, P->reserved_rows, [&](int64_t r0, int64_t rows) -> int {
-        int rc = stage_lik(P, soft, r0, rows);
-        if (rc != SBN_OK) return rc;
-        // the graph reads the tables and the count table by address, so it replays the values sbn_program_set_tables uploads
-        rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
-        if (rc != SBN_OK) return rc;
-        SBN_CUDA(cudaMemcpyAsync(static_cast<char *>(prob) + r0 * elem, P->d_out, static_cast<size_t>(rows) * elem,
-                                 cudaMemcpyDeviceToHost, P->stream));
-        return fetch_log_max(P, soft, r0, rows);
-    });
-    if (rc != SBN_OK) return rc;
-    std::vector<double> h(static_cast<size_t>(P->n_counts));
-    SBN_CUDA(cudaMemcpyAsync(h.data(), P->d_counts, h.size() * 8, cudaMemcpyDeviceToHost, P->stream));
-    SBN_CUDA(cudaStreamSynchronize(P->stream));
-    for (int64_t i = 0; i < P->n_counts; ++i) counts[i] += h[static_cast<size_t>(i)];
-    return SBN_OK;
-}
-
-static int counts_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, int64_t n_counts,
-                              void *prob, bool f64, const SoftLik &soft = {}) {
-    int rc = check_rows(P, kCounts, ev, ld_ev, n_rows, soft.soft);
-    if (rc != SBN_OK) return rc;
-    rc = check_lik(P, soft);
-    if (rc != SBN_OK) return rc;
-    if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the counts call");
-    if (!counts || !prob) return fail(SBN_E_INVALID, "null output");
-    if (n_counts != P->n_counts) return fail(SBN_E_INVALID, "the count table has %lld entries, not %lld", (long long)P->n_counts, (long long)n_counts);
-    rc = reserve_rows(P, n_rows);
-    if (rc != SBN_OK) return rc;
-    // the per-warp partial tables live for this call only: a program that is not running holds none of them
-    {
-        const cudaError_t e = cudaMalloc(&P->d_partial, static_cast<size_t>(std::max<int64_t>(1, P->partial_doubles)) * 8);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            P->d_partial = nullptr;
-            return fail(SBN_E_NOMEM, "cudaMalloc of %lld bytes of partial count tables failed: %s",
-                        (long long)(P->partial_doubles * 8), cudaGetErrorString(e));
-        }
-    }
-    rc = add_expected_counts(P, ev, ld_ev, n_rows, counts, prob, f64 ? 8 : 4, soft);
-    cudaStreamSynchronize(P->stream);  // nothing may still read the partial tables
-    cudaFree(P->d_partial);
-    P->d_partial = nullptr;
-    P->lik = nullptr;  // a device pointer is the caller's: forget it
-    return rc;
-}
-
-// log P(observed, lik) = log P(observed, lik / max) + sum log(max) of every row: NaN where `prob` is flagged
-static void add_log_max(const void *prob, bool f64, const std::vector<double> &log_max, double *log_evidence) {
-    for (size_t i = 0; i < log_max.size(); ++i) {
-        const double p = f64 ? static_cast<const double *>(prob)[i] : static_cast<const float *>(prob)[i];
-        log_evidence[i] = std::log(p) + log_max[i];
-    }
-}
-
-static int counts_soft_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const void *lik, int64_t ld_lik,
-                              int lik_on_device, double *counts, int64_t n_counts, void *prob, double *log_evidence, bool f64) {
-    std::vector<double> log_max(log_evidence && n_rows > 0 ? static_cast<size_t>(n_rows) : 0);
-    const SoftLik soft = {true, lik, ld_lik, lik_on_device, log_evidence ? log_max.data() : nullptr};
-    const int rc = counts_host_common(P, ev, ld_ev, n_rows, counts, n_counts, prob, f64, soft);
-    if (rc == SBN_OK && log_evidence) add_log_max(prob, f64, log_max, log_evidence);
-    return rc;
+    HostCall c(kPosterior, true, ev, ld_ev, n_rows);
+    c.soft = true, c.lik = lik, c.ld_lik = ld_lik, c.lik_on_device = lik_on_device;
+    c.out = out, c.ld_out = ld_out, c.log_prob = log_evidence;
+    return host_call(P, c);
 }
 
 int sbn_program_counts_soft_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
                                  int64_t ld_lik, int lik_on_device, double *counts, int64_t n_counts, float *prob,
                                  double *log_evidence) {
-    return counts_soft_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, counts, n_counts, prob, log_evidence, false);
+    HostCall c(kCounts, false, ev, ld_ev, n_rows);
+    c.soft = true, c.lik = lik, c.ld_lik = ld_lik, c.lik_on_device = lik_on_device;
+    c.counts = counts, c.n_counts = n_counts, c.prob = prob, c.log_prob = log_evidence;
+    return host_call(P, c);
 }
 
 int sbn_program_counts_soft_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
                                      int64_t ld_lik, int lik_on_device, double *counts, int64_t n_counts, double *prob,
                                      double *log_evidence) {
-    return counts_soft_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, counts, n_counts, prob, log_evidence, true);
+    HostCall c(kCounts, true, ev, ld_ev, n_rows);
+    c.soft = true, c.lik = lik, c.ld_lik = ld_lik, c.lik_on_device = lik_on_device;
+    c.counts = counts, c.n_counts = n_counts, c.prob = prob, c.log_prob = log_evidence;
+    return host_call(P, c);
 }
 
 int sbn_program_counts_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts, int64_t n_counts,
                             float *prob) {
-    return counts_host_common(P, ev, ld_ev, n_rows, counts, n_counts, prob, false);
+    HostCall c(kCounts, false, ev, ld_ev, n_rows);
+    c.counts = counts, c.n_counts = n_counts, c.prob = prob;
+    return host_call(P, c);
 }
 
 int sbn_program_counts_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, double *counts,
                                 int64_t n_counts, double *prob) {
-    return counts_host_common(P, ev, ld_ev, n_rows, counts, n_counts, prob, true);
+    HostCall c(kCounts, true, ev, ld_ev, n_rows);
+    c.counts = counts, c.n_counts = n_counts, c.prob = prob;
+    return host_call(P, c);
 }
 
-// A gradient call (forward or backward) of rows 0 .. n_rows - 1, chunk by chunk: codes, likelihoods (when the
-// program has soft variables) and, backward, the row weights are staged (or read in place on the device); the
-// forward run issues the upward closure of P(observed) only.  Out: P(observed, lik / max) [n_rows] and log
-// P(observed, lik) [n_rows] (both optional); backward also the weighted counts added into `counts` and the
-// derivative readouts [n_lik][ld_deriv].
-struct GradArgs {
-    const void *lik = nullptr;
-    int64_t ld_lik = 0;
-    int lik_on_device = 0;
-    const double *weights = nullptr;  // null: a forward call
-    int weights_on_device = 0;
-    double *counts = nullptr;
-    int64_t n_counts = 0;
-    void *deriv = nullptr;
-    int64_t ld_deriv = 0;
-    void *prob = nullptr;
-    double *log_prob = nullptr;
-};
-
-static int grad_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const GradArgs &a, bool f64) {
-    int rc = check_rows(P, kGrad, ev, ld_ev, n_rows);
-    if (rc != SBN_OK) return rc;
-    if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the gradient call");
-    const bool backward = a.weights != nullptr;
-    const SoftLik soft = {P->n_lik > 0, a.lik, a.ld_lik, a.lik_on_device, nullptr};
-    rc = check_lik(P, soft);
-    if (rc != SBN_OK) return rc;
-    if (backward) {
-        if (!a.counts || (P->n_lik > 0 && !a.deriv)) return fail(SBN_E_INVALID, "null output");
-        if (a.n_counts != P->n_counts)
-            return fail(SBN_E_INVALID, "the count table has %lld entries, not %lld", (long long)P->n_counts, (long long)a.n_counts);
-        if (P->n_lik > 0 && a.ld_deriv < n_rows) return fail(SBN_E_INVALID, "ld_deriv < n_rows");
-    }
-    rc = reserve_rows(P, n_rows);
-    if (rc != SBN_OK) return rc;
-    if (backward) {
-        const cudaError_t e = cudaMalloc(&P->d_partial, static_cast<size_t>(std::max<int64_t>(1, P->partial_doubles)) * 8);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            P->d_partial = nullptr;
-            return fail(SBN_E_NOMEM, "cudaMalloc of %lld bytes of partial count tables failed: %s",
-                        (long long)(P->partial_doubles * 8), cudaGetErrorString(e));
-        }
-        SBN_CUDA(cudaMemsetAsync(P->d_counts, 0, static_cast<size_t>(P->n_counts) * 8, P->stream));
-    }
-    P->forward_run = !backward;
-    const size_t elem = f64 ? 8 : 4;
-    std::vector<char> prob(static_cast<size_t>(P->reserved_rows) * elem);
-    std::vector<double> log_max(static_cast<size_t>(P->reserved_rows), 0.0);
-    rc = for_each_chunk(P, ev, ld_ev, n_rows, P->reserved_rows, [&](int64_t r0, int64_t rows) -> int {
-        int rc = stage_lik(P, soft, r0, rows);
-        if (rc != SBN_OK) return rc;
-        if (backward && a.weights_on_device) {
-            P->weight = a.weights + r0;
-        } else if (backward) {
-            SBN_CUDA(cudaMemcpyAsync(P->d_weight, a.weights + r0, static_cast<size_t>(rows) * 8, cudaMemcpyHostToDevice, P->stream));
-            P->weight = P->d_weight;
-        }
-        rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
-        if (rc != SBN_OK) return rc;
-        SBN_CUDA(cudaMemcpyAsync(prob.data(), P->d_out, static_cast<size_t>(rows) * elem, cudaMemcpyDeviceToHost, P->stream));
-        if (P->n_lik > 0) {
-            SBN_CUDA(cudaMemcpyAsync(log_max.data(), P->d_log_max, static_cast<size_t>(rows) * 8, cudaMemcpyDeviceToHost, P->stream));
-            if (backward)
-                SBN_CUDA(cudaMemcpy2DAsync(static_cast<char *>(a.deriv) + r0 * elem, static_cast<size_t>(a.ld_deriv) * elem,
-                                           reinterpret_cast<char *>(P->d_out) + P->ld * elem, static_cast<size_t>(P->ld) * elem,
-                                           static_cast<size_t>(rows) * elem, static_cast<size_t>(P->n_lik),
-                                           cudaMemcpyDeviceToHost, P->stream));
-        }
-        SBN_CUDA(cudaStreamSynchronize(P->stream));
-        for (int64_t i = 0; i < rows; ++i) {
-            const double p = f64 ? reinterpret_cast<const double *>(prob.data())[i] : reinterpret_cast<const float *>(prob.data())[i];
-            if (a.prob) memcpy(static_cast<char *>(a.prob) + (r0 + i) * elem, prob.data() + i * elem, elem);
-            if (a.log_prob) a.log_prob[r0 + i] = std::log(p) + log_max[static_cast<size_t>(i)];  // NaN where flagged
-        }
-        return SBN_OK;
-    });
-    if (rc == SBN_OK && backward) {
-        std::vector<double> h(static_cast<size_t>(P->n_counts));
-        cudaError_t e = cudaMemcpyAsync(h.data(), P->d_counts, h.size() * 8, cudaMemcpyDeviceToHost, P->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(P->stream);
-        if (e != cudaSuccess) rc = fail(SBN_E_CUDA, "reading the count table failed: %s", cudaGetErrorString(e));
-        for (int64_t i = 0; rc == SBN_OK && i < P->n_counts; ++i) a.counts[i] += h[static_cast<size_t>(i)];
-    }
-    cudaStreamSynchronize(P->stream);  // nothing may still read the partial tables
-    cudaFree(P->d_partial);
-    P->d_partial = nullptr;
-    P->forward_run = false;
-    P->lik = nullptr;  // device pointers are the caller's: forget them
-    P->weight = nullptr;
-    return rc;
-}
-
+// A gradient call: codes, likelihoods (when the program has soft variables) and, backward, the row weights are
+// staged or read in place on the device; the forward run issues the upward closure of P(observed) only.  Out:
+// P(observed, lik / max) and log P(observed, lik) [n_rows] (forward, both optional); backward the weighted counts
+// added into `counts`, the derivative readouts [n_lik][ld_deriv] and P(observed, lik / max) (optional).
 int sbn_program_grad_forward_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
                                   int64_t ld_lik, int lik_on_device, float *prob, double *log_prob) {
-    GradArgs a;
-    a.lik = lik, a.ld_lik = ld_lik, a.lik_on_device = lik_on_device, a.prob = prob, a.log_prob = log_prob;
-    return grad_common(P, ev, ld_ev, n_rows, a, false);
+    HostCall c(kGrad, false, ev, ld_ev, n_rows);
+    c.lik = lik, c.ld_lik = ld_lik, c.lik_on_device = lik_on_device, c.prob = prob, c.log_prob = log_prob;
+    return host_call(P, c);
 }
 
 int sbn_program_grad_forward_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
                                       int64_t ld_lik, int lik_on_device, double *prob, double *log_prob) {
-    GradArgs a;
-    a.lik = lik, a.ld_lik = ld_lik, a.lik_on_device = lik_on_device, a.prob = prob, a.log_prob = log_prob;
-    return grad_common(P, ev, ld_ev, n_rows, a, true);
+    HostCall c(kGrad, true, ev, ld_ev, n_rows);
+    c.lik = lik, c.ld_lik = ld_lik, c.lik_on_device = lik_on_device, c.prob = prob, c.log_prob = log_prob;
+    return host_call(P, c);
 }
 
 int sbn_program_grad_backward_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
                                    int64_t ld_lik, int lik_on_device, const double *weights, int weights_on_device,
                                    double *counts, int64_t n_counts, float *deriv, int64_t ld_deriv, float *prob) {
     if (!weights) return fail(SBN_E_INVALID, "null weights");
-    GradArgs a;
-    a.lik = lik, a.ld_lik = ld_lik, a.lik_on_device = lik_on_device, a.weights = weights, a.weights_on_device = weights_on_device;
-    a.counts = counts, a.n_counts = n_counts, a.deriv = deriv, a.ld_deriv = ld_deriv, a.prob = prob;
-    return grad_common(P, ev, ld_ev, n_rows, a, false);
+    HostCall c(kGrad, false, ev, ld_ev, n_rows);
+    c.lik = lik, c.ld_lik = ld_lik, c.lik_on_device = lik_on_device, c.weights = weights, c.weights_on_device = weights_on_device;
+    c.counts = counts, c.n_counts = n_counts, c.out = deriv, c.ld_out = ld_deriv, c.prob = prob;
+    return host_call(P, c);
 }
 
 int sbn_program_grad_backward_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
                                        int64_t ld_lik, int lik_on_device, const double *weights, int weights_on_device,
                                        double *counts, int64_t n_counts, double *deriv, int64_t ld_deriv, double *prob) {
     if (!weights) return fail(SBN_E_INVALID, "null weights");
-    GradArgs a;
-    a.lik = lik, a.ld_lik = ld_lik, a.lik_on_device = lik_on_device, a.weights = weights, a.weights_on_device = weights_on_device;
-    a.counts = counts, a.n_counts = n_counts, a.deriv = deriv, a.ld_deriv = ld_deriv, a.prob = prob;
-    return grad_common(P, ev, ld_ev, n_rows, a, true);
+    HostCall c(kGrad, true, ev, ld_ev, n_rows);
+    c.lik = lik, c.ld_lik = ld_lik, c.lik_on_device = lik_on_device, c.weights = weights, c.weights_on_device = weights_on_device;
+    c.counts = counts, c.n_counts = n_counts, c.out = deriv, c.ld_out = ld_deriv, c.prob = prob;
+    return host_call(P, c);
 }
 
-// A joint call of rows 0 .. n_rows - 1, chunk by chunk: codes and (when the program has soft variables) likelihoods
-// are staged, or read in place on the device; each chunk's readouts [Q][ld] and P(observed) come back.
-static int joint_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const void *lik, int64_t ld_lik,
-                        int lik_on_device, void *out_, int64_t ld_out, void *prob_, bool f64) {
-    int rc = check_rows(P, kJoint, ev, ld_ev, n_rows);
-    if (rc != SBN_OK) return rc;
-    if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the joint call");
-    if (!P->soft.empty() && !lik)
-        return fail(SBN_E_INVALID, "a joint program with soft evidence needs its likelihoods: pass lik to %s",
-                    f64 ? "sbn_program_joint_host_f64" : "sbn_program_joint_host");
-    if (P->soft.empty() && lik)
-        return fail(SBN_E_INVALID, "a joint program without soft evidence takes no likelihoods: pass lik = NULL to %s",
-                    f64 ? "sbn_program_joint_host_f64" : "sbn_program_joint_host");
-    const SoftLik soft = {!P->soft.empty(), lik, ld_lik, lik_on_device, nullptr};
-    rc = check_lik(P, soft);
-    if (rc != SBN_OK) return rc;
-    if (!out_ || !prob_) return fail(SBN_E_INVALID, "null output");
-    if (ld_out < n_rows) return fail(SBN_E_INVALID, "ld_out < n_rows");
-    rc = reserve_rows(P, n_rows);
-    if (rc != SBN_OK) return rc;
-    const size_t elem = f64 ? 8 : 4;
-    char *out = static_cast<char *>(out_), *prob = static_cast<char *>(prob_);
-    rc = for_each_chunk(P, ev, ld_ev, n_rows, P->reserved_rows, [&](int64_t r0, int64_t rows) -> int {
-        int rc = stage_lik(P, soft, r0, rows);
-        if (rc != SBN_OK) return rc;
-        rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream);
-        if (rc != SBN_OK) return rc;
-        SBN_CUDA(cudaMemcpy2DAsync(out + r0 * elem, static_cast<size_t>(ld_out) * elem, P->d_out, static_cast<size_t>(P->ld) * elem,
-                                   static_cast<size_t>(rows) * elem, static_cast<size_t>(P->Q), cudaMemcpyDeviceToHost, P->stream));
-        SBN_CUDA(cudaMemcpyAsync(prob + r0 * elem, P->d_total, static_cast<size_t>(rows) * elem, cudaMemcpyDeviceToHost, P->stream));
-        return SBN_OK;
-    });
-    P->lik = nullptr;  // a device pointer is the caller's: forget it
-    if (rc != SBN_OK) return rc;
-    SBN_CUDA(cudaStreamSynchronize(P->stream));
-    return SBN_OK;
-}
-
+// A joint call: codes and (when the program has soft variables) likelihoods are staged, or read in place on the
+// device; each chunk's readouts [Q][ld] and P(observed) come back.
 int sbn_program_joint_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
                            int64_t ld_lik, int lik_on_device, float *out, int64_t ld_out, float *prob) {
-    return joint_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, out, ld_out, prob, false);
+    HostCall c(kJoint, false, ev, ld_ev, n_rows);
+    c.lik = lik, c.ld_lik = ld_lik, c.lik_on_device = lik_on_device, c.out = out, c.ld_out = ld_out, c.prob = prob;
+    return host_call(P, c);
 }
 
 int sbn_program_joint_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
                                int64_t ld_lik, int lik_on_device, double *out, int64_t ld_out, double *prob) {
-    return joint_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, out, ld_out, prob, true);
+    HostCall c(kJoint, true, ev, ld_ev, n_rows);
+    c.lik = lik, c.ld_lik = ld_lik, c.lik_on_device = lik_on_device, c.out = out, c.ld_out = ld_out, c.prob = prob;
+    return host_call(P, c);
 }
 
 static int set_tables_common(sbn_program *P, const void *tables, int64_t n, bool f64) {
@@ -2397,130 +2362,53 @@ int sbn_program_set_tables_f64(sbn_program *P, const double *tables, int64_t n_t
     return set_tables_common(P, tables, n_table_doubles, true);
 }
 
-// The host path of sample programs and (kind = kMpe, one draw, no seed) of MPE and marginal MAP programs: the
-// decoded codes of a chunk are the drawn-code buffer, the per-row output is P(observed) (sample) or max log P(x, e)
-// (MPE; max log P(x_MAP, e) for MAP).
-static int sample_host_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws, uint64_t seed,
-                              int64_t row_base, uint8_t *out, void *prob, bool f64, ProgramKind kind = kSample,
-                              const SoftLik &soft = {}) {
-    int rc = check_rows(P, kind, ev, ld_ev, n_rows, soft.soft);
-    if (rc != SBN_OK) return rc;
-    rc = check_lik(P, soft);
-    if (rc != SBN_OK) return rc;
-    if (P->f64 != f64) return fail(SBN_E_INVALID, "program precision does not match the sample call");
-    if (n_draws <= 0 || n_draws > INT32_MAX) return fail(SBN_E_INVALID, "n_draws must be in 1 .. 2^31 - 1");
-    if (row_base < 0) return fail(SBN_E_INVALID, "row_base must not be negative");
-    if ((P->n_sampled > 0 && !out) || !prob) return fail(SBN_E_INVALID, "null output");
-    rc = reserve_rows(P, n_rows);
-    if (rc != SBN_OK) return rc;
-    // the drawn codes of a chunk ([n_sampled][n_draws] bytes + one flag byte per row) take at most half of the
-    // free device memory: larger batches run in more chunks
-    const int64_t per_row = static_cast<int64_t>(P->n_sampled) * n_draws + 1;
-    int64_t cap = P->reserved_rows;
-    if (round_up(std::min(cap, n_rows), 32) * per_row > P->drawn_bytes) {  // the buffer of an earlier call may do
-        size_t free_b = 0, total_b = 0;
-        SBN_CUDA(cudaMemGetInfo(&free_b, &total_b));
-        const int64_t budget = static_cast<int64_t>(free_b / 2) + P->drawn_bytes;
-        if (round_up(cap, 32) * per_row > budget) cap = std::max<int64_t>(32, budget / per_row / 32 * 32);
-    }
-    const DrawnCodes dc = {n_draws, round_up(std::min(cap, n_rows), 32)};
-    const int64_t bytes = dc.ld_drawn * per_row;
-    if (bytes > P->drawn_bytes) {
-        SBN_CUDA(cudaStreamSynchronize(P->stream));
-        cudaFree(P->d_drawn);
-        P->d_drawn = nullptr;
-        P->drawn_bytes = 0;
-        const cudaError_t e = cudaMalloc(&P->d_drawn, static_cast<size_t>(bytes));
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            P->d_drawn = nullptr;
-            return fail(SBN_E_NOMEM, "cudaMalloc of %lld bytes of drawn codes failed: %s", (long long)bytes, cudaGetErrorString(e));
-        }
-        P->drawn_bytes = bytes;
-    }
-    const bool mpe = kind == kMpe;
-    if (!mpe && !P->d_sample_args) SBN_CUDA(cudaMalloc(&P->d_sample_args, 4 * sizeof(uint32_t)));
-    const size_t elem = f64 ? 8 : 4;
-    const Slot &ps = P->slots[P->post_slot];  // MPE program: max log P(x, e), [1][ld] or one value for every row
-    rc = for_each_chunk(P, ev, ld_ev, n_rows, cap, [&](int64_t r0, int64_t rows) -> int {
-        // read by the sample steps at run time, so that one captured graph serves every seed and chunk
-        const uint64_t first = static_cast<uint64_t>(row_base + r0);
-        const uint32_t args[4] = {static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32), static_cast<uint32_t>(first),
-                                  static_cast<uint32_t>(first >> 32)};
-        if (!mpe) SBN_CUDA(cudaMemcpyAsync(P->d_sample_args, args, sizeof args, cudaMemcpyHostToDevice, P->stream));
-        int rc = stage_lik(P, soft, r0, rows);
-        if (rc != SBN_OK) return rc;
-        rc = run_rows(P, P->d_ev, P->ld, rows, P->d_out, P->ld, P->stream, dc);
-        if (rc != SBN_OK) return rc;
-        rc = fetch_log_max(P, soft, r0, rows);
-        if (rc != SBN_OK) return rc;
-        if (P->n_sampled > 0)
-            SBN_CUDA(cudaMemcpy2DAsync(out + r0, static_cast<size_t>(n_rows), P->d_drawn, static_cast<size_t>(dc.ld_drawn),
-                                       static_cast<size_t>(rows), static_cast<size_t>(P->n_sampled * n_draws),
-                                       cudaMemcpyDeviceToHost, P->stream));
-        if (!mpe || ps.batched)
-            SBN_CUDA(cudaMemcpyAsync(static_cast<char *>(prob) + r0 * elem, mpe ? ps.ptr : P->d_out,
-                                     static_cast<size_t>(rows) * elem, cudaMemcpyDeviceToHost, P->stream));
-        else if (r0 == 0)
-            SBN_CUDA(cudaMemcpyAsync(prob, ps.ptr, elem, cudaMemcpyDeviceToHost, P->stream));
-        return SBN_OK;
-    });
-    P->lik = nullptr;  // a device pointer is the caller's: forget it
-    if (rc != SBN_OK) return rc;
-    SBN_CUDA(cudaStreamSynchronize(P->stream));
-    if (mpe && !ps.batched) std::fill(static_cast<float *>(prob) + 1, static_cast<float *>(prob) + n_rows, *static_cast<float *>(prob));
-    return SBN_OK;
-}
-
+// The host path of sample programs and (kMpe, one draw, no seed) of MPE and marginal MAP programs: the decoded
+// codes of a chunk are the drawn-code buffer, the per-row output is P(observed) (sample) or max log P(x, e) (MPE;
+// max log P(x_MAP, e) for MAP).
 int sbn_program_sample_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws, uint64_t seed,
                             int64_t row_base, uint8_t *out, float *prob) {
-    return sample_host_common(P, ev, ld_ev, n_rows, n_draws, seed, row_base, out, prob, false);
+    HostCall c(kSample, false, ev, ld_ev, n_rows);
+    c.n_draws = n_draws, c.seed = seed, c.row_base = row_base, c.out = out, c.prob = prob;
+    return host_call(P, c);
 }
 
 int sbn_program_sample_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int64_t n_draws,
                                 uint64_t seed, int64_t row_base, uint8_t *out, double *prob) {
-    return sample_host_common(P, ev, ld_ev, n_rows, n_draws, seed, row_base, out, prob, true);
+    HostCall c(kSample, true, ev, ld_ev, n_rows);
+    c.n_draws = n_draws, c.seed = seed, c.row_base = row_base, c.out = out, c.prob = prob;
+    return host_call(P, c);
 }
 
 int sbn_program_mpe_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, uint8_t *codes, float *log_prob) {
-    return sample_host_common(P, ev, ld_ev, n_rows, 1, 0, 0, codes, log_prob, false, kMpe);
-}
-
-static int sample_soft_common(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const void *lik, int64_t ld_lik,
-                              int lik_on_device, int64_t n_draws, uint64_t seed, int64_t row_base, uint8_t *out, void *prob,
-                              double *log_evidence, bool f64) {
-    std::vector<double> log_max(log_evidence && n_rows > 0 ? static_cast<size_t>(n_rows) : 0);
-    const SoftLik soft = {true, lik, ld_lik, lik_on_device, log_evidence ? log_max.data() : nullptr};
-    const int rc = sample_host_common(P, ev, ld_ev, n_rows, n_draws, seed, row_base, out, prob, f64, kSample, soft);
-    if (rc == SBN_OK && log_evidence) add_log_max(prob, f64, log_max, log_evidence);
-    return rc;
+    HostCall c(kMpe, false, ev, ld_ev, n_rows);
+    c.out = codes, c.prob = log_prob;
+    return host_call(P, c);
 }
 
 int sbn_program_sample_soft_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const float *lik,
                                  int64_t ld_lik, int lik_on_device, int64_t n_draws, uint64_t seed, int64_t row_base,
                                  uint8_t *out, float *prob, double *log_evidence) {
-    return sample_soft_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, n_draws, seed, row_base, out, prob,
-                              log_evidence, false);
+    HostCall c(kSample, false, ev, ld_ev, n_rows);
+    c.soft = true, c.lik = lik, c.ld_lik = ld_lik, c.lik_on_device = lik_on_device;
+    c.n_draws = n_draws, c.seed = seed, c.row_base = row_base, c.out = out, c.prob = prob, c.log_prob = log_evidence;
+    return host_call(P, c);
 }
 
 int sbn_program_sample_soft_host_f64(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
                                      int64_t ld_lik, int lik_on_device, int64_t n_draws, uint64_t seed, int64_t row_base,
                                      uint8_t *out, double *prob, double *log_evidence) {
-    return sample_soft_common(P, ev, ld_ev, n_rows, lik, ld_lik, lik_on_device, n_draws, seed, row_base, out, prob,
-                              log_evidence, true);
+    HostCall c(kSample, true, ev, ld_ev, n_rows);
+    c.soft = true, c.lik = lik, c.ld_lik = ld_lik, c.lik_on_device = lik_on_device;
+    c.n_draws = n_draws, c.seed = seed, c.row_base = row_base, c.out = out, c.prob = prob, c.log_prob = log_evidence;
+    return host_call(P, c);
 }
 
+// The program's float32 max log P(x, e, lik / max), then the double sum log(max) added back
 int sbn_program_mpe_soft_host(sbn_program *P, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, const double *lik,
                               int64_t ld_lik, int lik_on_device, uint8_t *codes, double *log_prob) {
-    if (!log_prob) return fail(SBN_E_INVALID, "null output");
-    // the program's float32 max log P(x, e, lik / max), then the double sum log(max) added back
-    std::vector<float> lp(n_rows > 0 ? static_cast<size_t>(n_rows) : 0);
-    std::vector<double> log_max(lp.size());
-    const SoftLik soft = {true, lik, ld_lik, lik_on_device, log_max.data()};
-    const int rc = sample_host_common(P, ev, ld_ev, n_rows, 1, 0, 0, codes, lp.data(), false, kMpe, soft);
-    if (rc != SBN_OK) return rc;
-    for (size_t i = 0; i < lp.size(); ++i) log_prob[i] = static_cast<double>(lp[i]) + log_max[i];
-    return SBN_OK;
+    HostCall c(kMpe, false, ev, ld_ev, n_rows);
+    c.soft = true, c.lik = lik, c.ld_lik = ld_lik, c.lik_on_device = lik_on_device, c.out = codes, c.log_prob = log_prob;
+    return host_call(P, c);
 }
 
 int sbn_program_profile(sbn_program *P, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows, float *d_out,

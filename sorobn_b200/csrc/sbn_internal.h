@@ -134,29 +134,23 @@ struct sbn_program {
     int64_t n_counts = 0;    // counts program: entries of the count table
     int64_t n_table_floats = 0;  // size of the table blob (sbn_program_set_tables replaces it in place)
     double *d_counts = nullptr;   // counts program: the run's count table [n_counts]
-    double *d_partial = nullptr;  // counts program: per-warp partial tables of one count step (during a counts call only)
-    int64_t partial_doubles = 0;
+    int64_t partial_doubles = 0;  // counts / gradient program: doubles of the per-warp partial tables a call allocates
     int n_sampled = 0;            // sample / MPE program: drawn-code rows (one per unobserved variable)
     uint8_t *d_drawn = nullptr;   // sample program: drawn codes [n_sampled][n_draws][ld_drawn], then flags [ld_drawn]
     int64_t drawn_bytes = 0;
     uint32_t *d_sample_args = nullptr;  // seed lo, seed hi, row_base lo, row_base hi of the current chunk
     // soft evidence (any batched program, sbn_soft.cuh): (slot, card) of every likelihood, in
     // likelihood-column order; their pack descriptors; the staging buffer of host likelihoods [reserved][n_lik]
-    // (double when f64) and sum log(max) [ld] of the last run; the likelihoods the next issue reads
+    // (double when f64) and sum log(max) [ld] of the last run
     std::vector<std::pair<int, int>> soft;
     int n_lik = 0;
     int32_t *d_soft = nullptr;
     void *d_lik = nullptr;
     double *d_log_max = nullptr;
-    const void *lik = nullptr;
-    int64_t ld_lik = 0;
     // gradient program: per step, whether P(observed) depends on it (the steps a forward run issues); the staging
-    // buffer of host weights [reserved]; the weights the next backward issue reads; whether the next issue is a
-    // forward run, and the forward run's own graph
+    // buffer of host weights [reserved]; the forward run's own graph
     std::vector<char> forward;
     double *d_weight = nullptr;
-    const double *weight = nullptr;
-    bool forward_run = false;
     CachedGraph forward_graph;
     std::vector<std::pair<int64_t, int64_t>> tables;  // (offset, size) in floats
     std::vector<int64_t> table_padded;

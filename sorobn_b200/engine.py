@@ -301,32 +301,45 @@ class Program:
                                                       None if log_ev is None else log_ev.ctypes.data))
         return (out, log_ev) if log_evidence else out
 
+    def _array(self, a, dtype, shape, what):
+        """(the array argument `a` as a C-contiguous `dtype` array, to keep alive until the call returns; its
+        pointer; whether it is on the device) of a numpy array or a torch tensor.  A CUDA tensor on the program's
+        device is read in place, with no host round trip.  ValueError for another `shape` or device; `what` names
+        the argument."""
+        on_device = type(a).__module__.startswith("torch") and a.is_cuda
+        if on_device:
+            import torch
+
+            if a.device.index != self.device:
+                raise ValueError(f"{what} on cuda:{a.device.index}; the program runs on cuda:{self.device}")
+            a = a.to(torch.float64 if dtype == np.float64 else torch.float32).contiguous()
+            torch.cuda.current_stream(a.device).synchronize()  # the program's stream reads it next
+        else:
+            a = np.ascontiguousarray(a.detach().numpy() if type(a).__module__.startswith("torch") else a, dtype=dtype)
+        if tuple(a.shape) != shape:
+            raise ValueError(f"{what} have shape {tuple(a.shape)}, expected {shape}")
+        return a, a.data_ptr() if on_device else a.ctypes.data, on_device
+
     def _likelihoods(self, lik, n_rows):
-        """(the likelihoods [n_rows, n_lik], C-contiguous, and the call's (pointer, ld_lik, on-device flag)) of a
-        numpy array or a torch tensor; a CUDA tensor on the program's device is read in place, with no host round
-        trip.  ValueError for another shape or device.  Keep the first alive until the call returns.  The
-        likelihoods take the program's type, except that the float32 MPE and MAP programs take them in float64:
-        their pack takes the log of each ratio in double, and no float64 twin would rescue a row whose scale
-        float32 cannot hold."""
+        """(the likelihoods [n_rows, n_lik] as `_array` keeps them, and the call's (pointer, ld_lik, on-device
+        flag)).  The likelihoods take the program's type, except that the float32 MPE and MAP programs take them in
+        float64: their pack takes the log of each ratio in double, and no float64 twin would rescue a row whose
+        scale float32 cannot hold."""
         n_lik = sum(int(self.plan._card[v]) for v in self.plan.soft)
         f64 = self.f64 or self.plan.version in (8, 9)
-        on_device = False
-        if type(lik).__module__.startswith("torch"):
-            if lik.is_cuda:
-                import torch
+        lik, ptr, on_device = self._array(lik, np.float64 if f64 else np.float32, (n_rows, n_lik), "likelihoods")
+        return lik, (ptr, n_lik, int(on_device))
 
-                if lik.device.index != self.device:
-                    raise ValueError(f"likelihoods on cuda:{lik.device.index}; the program runs on cuda:{self.device}")
-                lik = lik.to(torch.float64 if f64 else torch.float32).contiguous()
-                torch.cuda.current_stream(lik.device).synchronize()  # the program's stream reads it next
-                on_device = True
-            else:
-                lik = lik.numpy()
-        if not on_device:
-            lik = np.ascontiguousarray(lik, dtype=np.float64 if f64 else np.float32)
-        if tuple(lik.shape) != (n_rows, n_lik):
-            raise ValueError(f"likelihoods have shape {tuple(lik.shape)}, expected {(n_rows, n_lik)}")
-        return lik, (lik.data_ptr() if on_device else lik.ctypes.data, n_lik, int(on_device))
+    def _program_likelihoods(self, lik, n_rows, kind):
+        """`_likelihoods` of a call that takes programs with and without soft variables (`kind` "gradient" or
+        "joint"): the first need their likelihoods, the second take none."""
+        if not self.plan.soft:
+            if lik is not None:
+                raise ValueError(f"likelihoods given to a {kind} program without soft variables")
+            return None, (None, 0, 0)
+        if lik is None:
+            raise ValueError(f"a {kind} program with soft variables needs their likelihoods")
+        return self._likelihoods(lik, n_rows)
 
     def evidence(self, codes: np.ndarray, n_rows: int) -> np.ndarray:
         """P(event) per evidence row (the normaliser of the posterior), host path."""
@@ -356,23 +369,13 @@ class Program:
                                                         None if log_ev is None else log_ev.ctypes.data))
         return (counts, prob, log_ev) if log_evidence else (counts, prob)
 
-    def _grad_lik(self, lik, n_rows):
-        """`_likelihoods` of a gradient program, which may have no soft variable: then `lik` must be None."""
-        if not self.plan.soft:
-            if lik is not None:
-                raise ValueError("likelihoods given to a gradient program without soft variables")
-            return None, (None, 0, 0)
-        if lik is None:
-            raise ValueError("a gradient program with soft variables needs their likelihoods")
-        return self._likelihoods(lik, n_rows)
-
     def grad_forward(self, codes: np.ndarray, n_rows: int, lik=None):
         """Gradient programs (planner.build_pattern_plan kind "grad"): (P(observed, lik / max) [n_rows], NaN for a
         row the float32 range rule flags; log P(observed, lik) float64 [n_rows]).  Only the launches P(observed)
         depends on run.  `lik` as in `run_soft`, for a program with soft variables."""
         n_rows = int(n_rows)
         codes, ev_ptr = self._evidence(codes, n_rows)
-        lik, lik_args = self._grad_lik(lik, n_rows)
+        lik, lik_args = self._program_likelihoods(lik, n_rows, "gradient")
         prob = np.empty(n_rows, dtype=self.dtype)
         log_prob = np.empty(n_rows, dtype=np.float64)
         _check(self._fn("sbn_program_grad_forward_host")(self._h, ev_ptr, n_rows, n_rows, *lik_args, prob.ctypes.data,
@@ -386,31 +389,15 @@ class Program:
         numpy array or a torch tensor; a CUDA tensor on the program's device is read in place, as `lik` is."""
         n_rows = int(n_rows)
         codes, ev_ptr = self._evidence(codes, n_rows)
-        lik, lik_args = self._grad_lik(lik, n_rows)
-        on_device = False
-        if type(weights).__module__.startswith("torch"):
-            if weights.is_cuda:
-                import torch
-
-                if weights.device.index != self.device:
-                    raise ValueError(f"weights on cuda:{weights.device.index}; the program runs on cuda:{self.device}")
-                weights = weights.to(torch.float64).contiguous()
-                torch.cuda.current_stream(weights.device).synchronize()
-                on_device = True
-            else:
-                weights = weights.detach().numpy()
-        if not on_device:
-            weights = np.ascontiguousarray(weights, dtype=np.float64)
-        if tuple(weights.shape) != (n_rows,):
-            raise ValueError(f"weights have shape {tuple(weights.shape)}, expected {(n_rows,)}")
+        lik, lik_args = self._program_likelihoods(lik, n_rows, "gradient")
+        weights, w_ptr, w_on_device = self._array(weights, np.float64, (n_rows,), "weights")
         n_lik = self.Q - 1
         counts = np.zeros(int(self.plan.n_counts), dtype=np.float64)
         deriv = np.empty((n_lik, n_rows), dtype=self.dtype)
         prob = np.empty(n_rows, dtype=self.dtype)
         _check(self._fn("sbn_program_grad_backward_host")(
-            self._h, ev_ptr, n_rows, n_rows, *lik_args, weights.data_ptr() if on_device else weights.ctypes.data,
-            int(on_device), counts.ctypes.data, counts.size, deriv.ctypes.data if n_lik else None, n_rows,
-            prob.ctypes.data))
+            self._h, ev_ptr, n_rows, n_rows, *lik_args, w_ptr, int(w_on_device), counts.ctypes.data, counts.size,
+            deriv.ctypes.data if n_lik else None, n_rows, prob.ctypes.data))
         return counts, deriv, prob
 
     def joint(self, codes: np.ndarray, n_rows: int, lik=None):
@@ -420,14 +407,7 @@ class Program:
         a program with soft variables (and None otherwise)."""
         n_rows = int(n_rows)
         codes, ev_ptr = self._evidence(codes, n_rows)
-        if self.plan.soft:
-            if lik is None:
-                raise ValueError("a joint program with soft variables needs their likelihoods")
-            lik, lik_args = self._likelihoods(lik, n_rows)
-        elif lik is not None:
-            raise ValueError("likelihoods given to a joint program without soft variables")
-        else:
-            lik_args = (None, 0, 0)
+        lik, lik_args = self._program_likelihoods(lik, n_rows, "joint")
         out = np.empty((self.Q, n_rows), dtype=self.dtype)
         prob = np.empty(n_rows, dtype=self.dtype)
         _check(self._fn("sbn_program_joint_host")(self._h, ev_ptr, n_rows, n_rows, *lik_args, out.ctypes.data, n_rows,
