@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SBN_ABI_VERSION 18
+#define SBN_ABI_VERSION 19
 
 #define SBN_OK 0
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
@@ -344,6 +344,24 @@ int sbn_tally_counts(sbn_tally *tally, const int32_t *words, int64_t n_words, ui
 int sbn_tally_scores(sbn_tally *tally, const int32_t *words, int64_t n_words, int kind, double ess, double *scores,
                      int64_t n_families);
 void sbn_tally_destroy(sbn_tally *tally);
+
+/* ------------------------------------------------------------------ loopy belief propagation
+ * Approximate posterior marginals of networks too wide to eliminate exactly: sum-product message passing on the
+ * factor graph of the CPT families, synchronous flooding with damping (the algorithm, its zero and underflow
+ * rules and the word layout: sorobn_b200/bp.py).  `words` and `tables` come from bp.compile_graph; every word is
+ * bounds-checked here.  One thread runs one evidence row through every sweep; larger batches run in chunks, and a
+ * row's result does not depend on the chunking.
+ * sbn_bp_run_host: `ev` uint8 codes [n_ev][ld_ev] (host; a code past its variable's states reads as the last);
+ * out[q * ld_out + b] = the belief of row b in state q of the targets' output (float, host); iterations[b] = the
+ * sweep at which row b converged (its largest damped-message change fell below tol) or met a zero sum (its
+ * beliefs are then NaN), or n_iterations + 1 when it did not converge.  1 <= n_iterations < 2^31 - 1,
+ * 0 <= damping < 1, tol >= 0 (tol = 0 runs exactly n_iterations sweeps). */
+typedef struct sbn_bp sbn_bp;
+int sbn_bp_create(int device, const int32_t *words, int64_t n_words, const float *tables, int64_t n_table_floats,
+                  sbn_bp **out);
+int sbn_bp_run_host(sbn_bp *bp, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int32_t n_iterations, float damping,
+                    float tol, float *out, int64_t ld_out, int32_t *iterations);
+void sbn_bp_destroy(sbn_bp *bp);
 
 /* Pinned host memory for evidence / posterior staging buffers. */
 int sbn_host_alloc(void **ptr, int64_t bytes);

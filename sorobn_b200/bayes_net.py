@@ -31,6 +31,8 @@ explanation, one log-domain max-sum program per pattern (planner.build_mpe_plan,
 other unobserved variables summed out: one log-sum-exp, then max-sum program per pattern
 (planner.build_map_plan).  `joint_marginals_many` returns, for every row, the joint posterior of every CPT
 family or of chosen groups of variables, one joint program per pattern (planner.build_joint_plan).
+`marginals_many(..., algorithm="bp")` approximates every marginal by loopy belief propagation on the device, one
+row per thread (sorobn_b200/bp.py, csrc/sbn_bp.cu), for networks too wide to eliminate exactly.
 """
 from __future__ import annotations
 
@@ -38,11 +40,13 @@ import graphlib
 import random
 import threading
 import typing
+import warnings
 from collections import OrderedDict, defaultdict
 
 import numpy as np
 import pandas as pd
 
+from . import bp as _bp
 from . import planner as _planner
 
 __all__ = ["BayesNet"]
@@ -1078,6 +1082,9 @@ class BayesNet:
             codes, bad = self._encode_events(pd.DataFrame({v: [event[v]] for v in ev_vars}, index=[0]), ev_vars)
             post = None if bad[0] else entry.f64().run_soft(codes, lik, 1)[:, 0]
             return _posterior_series(post, index, name)
+        if algorithm == "bp":
+            post = self._bp_query(query, pd.DataFrame({v: [event[v]] for v in event}, index=[0]), n_iterations)
+            return _posterior_series(post[:, 0], self._states_index([self._compiled.index[query[0]]]), name)
         if algorithm in ("gibbs", "likelihood", "rejection"):
             events = pd.DataFrame({v: [event[v]] for v in event}, index=[0])
             freq, index = self._sample_query(algorithm, query, events, n_iterations)
@@ -1087,7 +1094,7 @@ class BayesNet:
             answer = pd.Series(values, index=index, name=name)
             return answer[answer > 0]  # the reference only lists the states that were sampled
         if algorithm != "exact":
-            raise ValueError("Unknown algorithm, must be one of: exact, gibbs, likelihood, rejection")
+            raise ValueError("Unknown algorithm, must be one of: exact, gibbs, likelihood, rejection, bp")
 
         ev_vars = tuple(event)
         plan, program = self._plan(query, ev_vars, _planner.MODE_FLAT)
@@ -1162,11 +1169,16 @@ class BayesNet:
             soft, lik = self._soft_matrix(likelihoods, len(events.index), ev_vars)
             plan = self._soft_programs(query, ev_vars, soft, marginals=False).plan
             return self._soft_frame(query, events, soft, lik, self._answer_index(plan), marginals=False)
+        if algorithm == "bp":
+            if devices is not None:
+                raise ValueError("algorithm='bp' runs on one device: devices=[...] is not supported")
+            post = self._bp_query(query, events, n_iterations)
+            return pd.DataFrame(post.T, index=events.index, columns=self._states_index([self._compiled.index[query[0]]]))
         if algorithm in ("gibbs", "likelihood", "rejection"):
             freq, index = self._sample_query(algorithm, query, events, n_iterations)
             return pd.DataFrame(freq.T.astype(np.float64), index=events.index, columns=index)
         if algorithm != "exact":
-            raise ValueError("Unknown algorithm, must be one of: exact, gibbs, likelihood, rejection")
+            raise ValueError("Unknown algorithm, must be one of: exact, gibbs, likelihood, rejection, bp")
         plan, _ = self._plan(query, ev_vars, _planner.MODE_BATCHED, device=None if devices is None else devices[0])
         return self._posterior_frame(query, events, self._answer_index(plan), devices=devices)
 
@@ -1338,7 +1350,8 @@ class BayesNet:
             raise ValueError("At least one query variable has to be specified")
         return tuple(sorted(set(variables)))
 
-    def marginals_many(self, events: pd.DataFrame, variables=None, likelihoods: dict | None = None) -> pd.DataFrame:
+    def marginals_many(self, events: pd.DataFrame, variables=None, likelihoods: dict | None = None, algorithm="exact",
+                       n_iterations=100, damping=0.5, tol=1e-5) -> pd.DataFrame:
         """The posterior marginal of every variable in `variables` (default: every variable that is not
         a column of `events`), for every row of `events`, from ONE device program: an upward and a
         downward pass over the bucket tree of the elimination, then one readout per variable
@@ -1347,16 +1360,75 @@ class BayesNet:
         Returns one row per evidence row; the columns are a MultiIndex of (variable, state), variables
         sorted by name, states sorted.  Zero-probability states stay (as 0.0); impossible rows and rows
         with a value outside its variable's domain are NaN.  `likelihoods`: soft evidence, as in
-        `query_many`; a soft node may be a target."""
+        `query_many`; a soft node may be a target.
+
+        algorithm="bp": loopy belief propagation on the device instead of elimination, for networks whose induced
+        width the exact planner refuses (sorobn_b200/bp.py defines it).  Sum-product messages on the factor graph of
+        the CPT families are swept synchronously, each factor-to-variable message damped as (1 - damping) * new +
+        damping * old, until the largest change of any message of the row falls below `tol` or `n_iterations`
+        sweeps have run (tol=0 runs exactly n_iterations).  Deterministic, exact on polytrees, approximate on loopy
+        networks, where it may also miss impossible evidence.  Same frame as the exact path; rows that did not
+        converge keep their last beliefs and raise one RuntimeWarning with their count.  ValueError unless
+        0 <= damping < 1, n_iterations >= 1 and tol >= 0.  No soft evidence."""
+        if algorithm not in ("exact", "bp"):
+            raise ValueError("Unknown algorithm, must be one of: exact, bp")
+        if likelihoods is not None:
+            self._check_soft_call(algorithm, None)
+        if algorithm == "bp":
+            _bp.check_arguments(n_iterations, damping, tol)
         ev_vars = tuple(events.columns)
         targets = self._targets(variables, ev_vars)
         net = self._compiled
         columns = pd.MultiIndex.from_tuples([(t, s) for t in targets for s in net.domains[net.index[t]]],
                                             names=["variable", "state"])
+        if algorithm == "bp":
+            return pd.DataFrame(self._bp_run(targets, events, n_iterations, damping, tol).T, index=events.index,
+                                columns=columns)
         if likelihoods is not None:
             soft, lik = self._soft_matrix(likelihoods, len(events.index), ev_vars)
             return self._soft_frame(targets, events, soft, lik, columns, marginals=True)
         return self._posterior_frame(targets, events, columns, marginals=True)
+
+    def _bp_run(self, targets, events, n_iterations, damping, tol):
+        """Loopy belief propagation (bp.py) of the sorted `targets` for every row of `events`: beliefs float64
+        [Q, n] in the targets' column order, NaN for a row that met a zero sum or has a value outside its
+        variable's domain.  One RuntimeWarning counts the rows that did not converge."""
+        from . import engine
+
+        net = self._net("querying")
+        ev_vars = tuple(events.columns)
+        for name in (*targets, *ev_vars):
+            if name not in net.index:
+                raise KeyError(name)
+
+        def build():
+            g = _bp.compile_graph(net, [net.index[e] for e in ev_vars], [net.index[t] for t in targets])
+            return engine.BeliefPropagation(g.words, g.tables, device=self.device)
+
+        runner = self._cached(("bp", tuple(targets), ev_vars), build)
+        n = len(events.index)
+        if n == 0:
+            return np.zeros((runner.Q, 0))
+        codes, bad = self._encode_events(events, ev_vars)
+        out, iters = runner.run(codes, n, n_iterations, damping, tol)
+        out = out.astype(np.float64)
+        out[:, bad] = np.nan
+        stuck = int(np.count_nonzero((iters > n_iterations) & ~bad))
+        if stuck:
+            warnings.warn(f"belief propagation: {stuck} of {n} rows did not converge to tol={tol:g} in {n_iterations} "
+                          "sweeps; they keep the beliefs of their last sweep", RuntimeWarning, stacklevel=3)
+        return out
+
+    def _bp_query(self, query, events, n_iterations):
+        """`query` / `query_many` with algorithm="bp": one query variable, the default damping and tol."""
+        if len(query) != 1:
+            raise ValueError("algorithm='bp' answers one query variable at a time: belief propagation gives no joint "
+                             "over variables of different families")
+        _bp.check_arguments(n_iterations, 0.5, 1e-5)
+        ev_vars = tuple(events.columns)
+        if query[0] not in self._net("querying").index:
+            raise KeyError(query[0])
+        return self._bp_run(self._targets(query, ev_vars), events, n_iterations, 0.5, 1e-5)
 
     def marginals(self, event: dict, variables=None) -> dict:
         """`marginals_many` for one event, in float64 (as `query`): {variable: Series}, each Series equal to

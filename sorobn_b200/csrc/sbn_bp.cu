@@ -1,0 +1,462 @@
+// sorobn_b200 -- loopy belief propagation, one evidence row per thread (sorobn_b200/bp.py defines the algorithm
+// and the words; DESIGN.md "Loopy belief propagation").
+//
+// Rows are independent fixed-point problems, so one thread runs one row through every sweep inside one launch,
+// with no grid-wide synchronisation (the shape of sbn_gibbs.cuh):
+//   * the compiled words are staged in shared memory: every thread of a warp walks the same records, so control
+//     flow and the word reads are uniform (broadcast);
+//   * the factor tables are staged in shared memory when they fit beside the words, else read through the
+//     read-only path;
+//   * the per-row message state lives in a device scratch laid out [message entry][row], so the 32 rows of a warp
+//     read and write 128 consecutive bytes of each entry; offsets are 64-bit;
+//   * a row that converged (or met a zero) leaves its loop.
+// Both directions of every message are stored (mu at entries [0, E), nu at [E, 2E)): step 1 reads nu and writes
+// mu, step 2 reads mu and writes nu, so every entry is updated in place.  Storing only mu and forming nu on the
+// fly would halve the state but multiply step 1's reads by the variable degrees.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cmath>
+#include <cstdlib>
+#include <vector>
+
+#include "sbn_internal.h"
+
+namespace {
+
+constexpr int32_t kMagic = 0x53424250;  // "SBBP" (bp.MAGIC)
+constexpr int kHeader = 12;
+constexpr int kThreads = 128;
+constexpr int kMaxCard = 256;  // bp.MAX_CARD
+constexpr int kSmemLimit = 200 * 1024;
+constexpr int64_t kScratchBudget = 1LL << 30;  // bytes of message state per chunk
+constexpr double kTiny = 0x1p-32;             // the rescale of sbn_gibbs.cuh
+constexpr double kRescale = 0x1p64;
+
+// The states loop of a message: unrolled over the MAXC registers of the narrow kernel (each state guarded by
+// x < c), or bounded by the card c in the wide kernel, whose arrays live in local memory.
+#define BP_XN (MAXC <= 8 ? MAXC : c)
+
+struct BpArgs {
+    const int32_t *words;
+    int n_words;
+    const float *tables;
+    int n_table_floats;
+    int tables_in_smem;
+    const uint8_t *ev;  // [n_ev][ld]
+    float *msg;         // [2E][ld]
+    float *out;         // [Q][ld]
+    int32_t *iters;     // [ld]
+    int64_t ld, n_rows;
+    int n_iterations;
+    float damping, tol;
+};
+
+// Product of the mu of a variable's edges except `skip` (-1: all of them) into p[], rescaled against underflow;
+// returns the sum of p[0 .. c).  The product runs in double: the rescale keeps its largest state in range, but with
+// many neighbours a smaller state can fall more than 2^126 below the largest before later factors bring it back
+// (60 disagreeing children of one variable do), and in float32 it would lose its digits in the subnormals.
+template <int MAXC>
+__device__ __forceinline__ double bp_product(const int32_t *edges, int deg, int skip, int c, const float *mu,
+                                             int64_t ld, double (&p)[MAXC]) {
+#pragma unroll
+    for (int x = 0; x < BP_XN; ++x) p[x] = 1.0;
+    for (int k = 0; k < deg; ++k) {
+        if (k == skip) continue;
+        const float *m = mu + static_cast<int64_t>(edges[k]) * ld;
+        double top = 0.0;
+#pragma unroll
+        for (int x = 0; x < BP_XN; ++x)
+            if (x < c) {
+                p[x] *= static_cast<double>(m[static_cast<int64_t>(x) * ld]);
+                top = fmax(top, p[x]);
+            }
+        if (top < kTiny) {
+#pragma unroll
+            for (int x = 0; x < BP_XN; ++x) p[x] *= kRescale;
+        }
+    }
+    double s = 0.0;
+#pragma unroll
+    for (int x = 0; x < BP_XN; ++x)
+        if (x < c) s += p[x];
+    return s;
+}
+
+}  // namespace
+
+template <int MAXC>
+__global__ void __launch_bounds__(kThreads) sbn_bp_kernel(const __grid_constant__ BpArgs a) {
+    extern __shared__ __align__(16) uint8_t s_raw[];
+    int32_t *w = reinterpret_cast<int32_t *>(s_raw);
+    float *s_tab = reinterpret_cast<float *>(s_raw + ((a.n_words * 4 + 15) & ~15));
+    for (int i = threadIdx.x; i < a.n_words; i += blockDim.x) w[i] = a.words[i];
+    if (a.tables_in_smem)
+        for (int i = threadIdx.x; i < a.n_table_floats; i += blockDim.x) s_tab[i] = a.tables[i];
+    __syncthreads();
+    const int64_t row = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (row >= a.n_rows) return;
+    const bool tsm = a.tables_in_smem != 0;
+    const float *__restrict__ gtab = a.tables;
+    auto table = [&](int e) -> float { return tsm ? s_tab[e] : __ldg(gtab + e); };
+
+    const int n_fac = w[3], n_var = w[4], E = w[5], n_tgt = w[6], Q = w[7];
+    const int fac_pos = w[9], var_pos = w[10], tgt_pos = w[11];
+    const int64_t ld = a.ld;
+    float *mu = a.msg + row;
+    float *nu = a.msg + static_cast<int64_t>(E) * ld + row;
+    const uint8_t *ev = a.ev + row;
+    const float lam = a.damping, keep = 1.f - a.damping;
+
+    // uniform start: every edge's mu and nu
+    for (int f = 0, p = fac_pos; f < n_fac; ++f) {
+        const int n_mem = w[p + 2], n_evax = w[p + 3];
+        for (int i = 0; i < n_mem; ++i) {
+            const int c = w[p + 4 + 3 * i], e = w[p + 6 + 3 * i];
+            const float u = 1.f / static_cast<float>(c);
+            for (int x = 0; x < c; ++x) {
+                mu[static_cast<int64_t>(e + x) * ld] = u;
+                nu[static_cast<int64_t>(e + x) * ld] = u;
+            }
+        }
+        p += 4 + 3 * n_mem + 3 * n_evax;
+    }
+
+    int recorded = a.n_iterations + 1;
+    bool dead = false;
+    for (int t = 1; t <= a.n_iterations; ++t) {
+        // ---- step 1: every factor-to-variable message, damped, and the residual
+        float r = 0.f;
+        for (int f = 0, p = fac_pos; f < n_fac; ++f) {
+            const int n_mem = w[p + 2], n_evax = w[p + 3];
+            const int32_t *mem = w + p + 4;
+            const int32_t *ax = mem + 3 * n_mem;
+            int base = w[p + 1];
+            for (int k = 0; k < n_evax; ++k) {
+                const int code = min(static_cast<int>(ev[static_cast<int64_t>(ax[3 * k]) * ld]), ax[3 * k + 2] - 1);
+                base += code * ax[3 * k + 1];
+            }
+            int T = 1;
+            for (int i = 0; i < n_mem; ++i) T *= mem[3 * i];
+            for (int i = 0; i < n_mem; ++i) {
+                const int c = mem[3 * i], si = mem[3 * i + 1], e = mem[3 * i + 2];
+                const int n_other = T / c;
+                float s[MAXC];
+#pragma unroll
+                for (int x = 0; x < BP_XN; ++x) s[x] = 0.f;
+                for (int j = 0; j < n_other; ++j) {
+                    // decode j over the other members (first fastest): their states, table offset and nu product
+                    int rem = j, idx = base;
+                    float prod = 1.f;
+                    for (int u = 0; u < n_mem; ++u) {
+                        if (u == i) continue;
+                        const int cu = mem[3 * u];
+                        const int xu = rem % cu;
+                        rem /= cu;
+                        idx += xu * mem[3 * u + 1];
+                        prod *= nu[static_cast<int64_t>(mem[3 * u + 2] + xu) * ld];
+                    }
+#pragma unroll
+                    for (int x = 0; x < BP_XN; ++x)
+                        if (x < c) s[x] += table(idx + x * si) * prod;
+                }
+                float S = 0.f;
+#pragma unroll
+                for (int x = 0; x < BP_XN; ++x)
+                    if (x < c) S += s[x];
+                // divide (not multiply by 1 / S): the sum of the other members' nu products is not rescaled and
+                // may be subnormal, where 1 / S overflows while every ratio s[x] / S is finite
+                if (!(S > 0.f)) dead = true;
+                float *m = mu + static_cast<int64_t>(e) * ld;
+#pragma unroll
+                for (int x = 0; x < BP_XN; ++x)
+                    if (x < c) {
+                        const float old = m[static_cast<int64_t>(x) * ld];
+                        const float v = keep * (s[x] / S) + lam * old;
+                        r = fmaxf(r, fabsf(v - old));
+                        m[static_cast<int64_t>(x) * ld] = v;
+                    }
+            }
+            p += 4 + 3 * n_mem + 3 * n_evax;
+        }
+        if (dead) {
+            recorded = t;
+            break;
+        }
+        // ---- step 2: every variable-to-factor message from the new mu
+        for (int v = 0, p = var_pos; v < n_var && !dead; ++v) {
+            const int c = w[p + 1], deg = w[p + 2];
+            const int32_t *edges = w + p + 3;
+            for (int k = 0; k < deg; ++k) {
+                double q[MAXC];
+                const double S = bp_product<MAXC>(edges, deg, k, c, mu, ld, q);
+                if (!(S > 0.0)) dead = true;
+                float *n = nu + static_cast<int64_t>(edges[k]) * ld;
+#pragma unroll
+                for (int x = 0; x < BP_XN; ++x)
+                    if (x < c) n[static_cast<int64_t>(x) * ld] = static_cast<float>(q[x] / S);
+            }
+            p += 3 + deg;
+        }
+        if (dead) {
+            recorded = t;
+            break;
+        }
+        if (r < a.tol) {
+            recorded = t;
+            break;
+        }
+    }
+    a.iters[row] = recorded;
+    // ---- beliefs of the targets from the last sweep's mu
+    for (int k = 0; k < n_tgt && !dead; ++k) {
+        const int p = w[tgt_pos + 2 * k];
+        const int c = w[p + 1], deg = w[p + 2];
+        double q[MAXC];
+        const double S = bp_product<MAXC>(w + p + 3, deg, -1, c, mu, ld, q);
+        if (!(S > 0.0)) {
+            dead = true;
+            break;
+        }
+        float *o = a.out + static_cast<int64_t>(w[tgt_pos + 2 * k + 1]) * ld + row;
+#pragma unroll
+        for (int x = 0; x < BP_XN; ++x)
+            if (x < c) o[static_cast<int64_t>(x) * ld] = static_cast<float>(q[x] / S);
+    }
+    if (dead)
+        for (int q = 0; q < Q; ++q) a.out[static_cast<int64_t>(q) * ld + row] = __int_as_float(0x7fc00000);
+}
+
+struct sbn_bp {
+    int device = 0;
+    std::vector<int32_t> words;
+    int n_table_floats = 0;
+    int n_ev = 0, E = 0, Q = 0, max_card = 1;
+    int smem = 0;
+    bool tables_in_smem = false;
+    int32_t *d_words = nullptr;
+    float *d_tables = nullptr;
+    int64_t cap = 0;  // rows per chunk
+    uint8_t *d_ev = nullptr;
+    float *d_msg = nullptr, *d_out = nullptr;
+    int32_t *d_iters = nullptr;
+    cudaStream_t stream = nullptr;
+};
+
+namespace {
+
+#define SBN_BP_CUDA(call)                                                                                        \
+    do {                                                                                                       \
+        cudaError_t e_ = (call);                                                                               \
+        if (e_ != cudaSuccess)                                                                                 \
+            return sbn_fail(e_ == cudaErrorMemoryAllocation ? SBN_E_NOMEM : SBN_E_CUDA, "%s failed: %s (%s:%d)", \
+                            #call, cudaGetErrorString(e_), __FILE__, __LINE__);                                \
+    } while (0)
+
+// Bounds-check every word (bp.py layout); fills n_ev, E, Q and the widest message.
+int validate(const int32_t *w, int64_t n, int64_t n_tables, sbn_bp &b) {
+    if (n < kHeader) return sbn_fail(SBN_E_INVALID, "bp words: %lld words, the header has %d", static_cast<long long>(n), kHeader);
+    if (n >= (1LL << 30)) return sbn_fail(SBN_E_INVALID, "bp words: %lld words", static_cast<long long>(n));
+    if (w[0] != kMagic || w[1] != 1) return sbn_fail(SBN_E_INVALID, "bp words: bad magic or version %d", w[1]);
+    const int n_ev = w[2], n_fac = w[3], n_var = w[4], E = w[5], n_tgt = w[6], Q = w[7];
+    if (n_ev < 0 || n_fac < 1 || n_var < 1 || E < 1 || n_tgt < 1 || Q < 1 || w[8] != n_tables)
+        return sbn_fail(SBN_E_INVALID, "bp words: bad header (n_ev %d, factors %d, variables %d, E %d, targets %d, Q %d, "
+                        "table floats %d of %lld)", n_ev, n_fac, n_var, E, n_tgt, Q, w[8], static_cast<long long>(n_tables));
+    if (w[9] != kHeader || w[10] < w[9] || w[11] < w[10] || static_cast<int64_t>(w[11]) + 2LL * n_tgt != n)
+        return sbn_fail(SBN_E_INVALID, "bp words: bad section positions %d %d %d", w[9], w[10], w[11]);
+    int64_t p = w[9];
+    int64_t edge_end = 0;
+    int max_card = 1;
+    for (int f = 0; f < n_fac; ++f) {
+        if (p + 4 > w[10]) return sbn_fail(SBN_E_INVALID, "bp words: factor %d runs past its section", f);
+        const int64_t off = w[p + 1];
+        const int n_mem = w[p + 2], n_evax = w[p + 3];
+        if (n_mem < 1 || n_evax < 0 || p + 4 + 3LL * (n_mem + n_evax) > w[10])
+            return sbn_fail(SBN_E_INVALID, "bp words: factor %d has %d members and %d evidence axes", f, n_mem, n_evax);
+        int64_t span = 1;  // entries the factor's table spans
+        for (int i = 0; i < n_mem; ++i) {
+            const int c = w[p + 4 + 3 * i], s = w[p + 5 + 3 * i], e = w[p + 6 + 3 * i];
+            if (c < 1 || c > kMaxCard || s != span || e < 0 || static_cast<int64_t>(e) + c > E)
+                return sbn_fail(SBN_E_INVALID, "bp words: factor %d member %d (card %d, stride %d, edge %d)", f, i, c, s, e);
+            span *= c;
+            edge_end = std::max<int64_t>(edge_end, static_cast<int64_t>(e) + c);
+            max_card = std::max(max_card, c);
+            if (span >= (1LL << 31)) return sbn_fail(SBN_E_INVALID, "bp words: factor %d is too large", f);
+        }
+        for (int k = 0; k < n_evax; ++k) {
+            const int32_t *ax = w + p + 4 + 3 * n_mem + 3 * k;
+            if (ax[0] < 0 || ax[0] >= n_ev || ax[1] != span || ax[2] < 1 || ax[2] > 256)
+                return sbn_fail(SBN_E_INVALID, "bp words: factor %d evidence axis %d (col %d, stride %d, card %d)", f, k,
+                                ax[0], ax[1], ax[2]);
+            span *= ax[2];
+            if (span >= (1LL << 31)) return sbn_fail(SBN_E_INVALID, "bp words: factor %d is too large", f);
+        }
+        if (off < 0 || off + span > n_tables)
+            return sbn_fail(SBN_E_INVALID, "bp words: factor %d table [%lld, +%lld) outside %lld floats", f,
+                            static_cast<long long>(off), static_cast<long long>(span), static_cast<long long>(n_tables));
+        p += 4 + 3 * (n_mem + n_evax);
+    }
+    if (p != w[10] || edge_end != E) return sbn_fail(SBN_E_INVALID, "bp words: factor section does not end at its edges");
+    std::vector<int> var_at(n, -1);
+    for (int v = 0; v < n_var; ++v) {
+        if (p + 3 > w[11]) return sbn_fail(SBN_E_INVALID, "bp words: variable %d runs past its section", v);
+        const int c = w[p + 1], deg = w[p + 2];
+        if (c < 1 || c > kMaxCard || deg < 1 || p + 3 + deg > w[11])
+            return sbn_fail(SBN_E_INVALID, "bp words: variable %d (card %d, degree %d)", v, c, deg);
+        for (int k = 0; k < deg; ++k) {
+            const int e = w[p + 3 + k];
+            if (e < 0 || static_cast<int64_t>(e) + c > E)
+                return sbn_fail(SBN_E_INVALID, "bp words: variable %d edge %d at %d", v, k, e);
+        }
+        var_at[p] = c;
+        p += 3 + deg;
+    }
+    if (p != w[11]) return sbn_fail(SBN_E_INVALID, "bp words: variable section does not end at the targets");
+    for (int k = 0; k < n_tgt; ++k) {
+        const int vp = w[p + 2 * k], q = w[p + 2 * k + 1];
+        if (vp < 0 || vp >= n || var_at[vp] < 0 || q < 0 || q + var_at[vp] > Q)
+            return sbn_fail(SBN_E_INVALID, "bp words: target %d (record %d, q_offset %d)", k, vp, q);
+    }
+    b.n_ev = n_ev;
+    b.E = E;
+    b.Q = Q;
+    b.max_card = max_card;
+    return SBN_OK;
+}
+
+int reserve(sbn_bp *b, int64_t rows) {
+    if (rows <= b->cap) return SBN_OK;
+    const int64_t per_row = 2LL * b->E * 4;
+    int64_t cap = std::max<int64_t>(kThreads, kScratchBudget / per_row / kThreads * kThreads);
+    cap = std::min(cap, round_up(rows, kThreads));
+    if (cap <= b->cap) return SBN_OK;
+    cudaFree(b->d_ev);
+    cudaFree(b->d_msg);
+    cudaFree(b->d_out);
+    cudaFree(b->d_iters);
+    b->d_ev = nullptr;
+    b->d_msg = b->d_out = nullptr;
+    b->d_iters = nullptr;
+    b->cap = 0;
+    SBN_BP_CUDA(cudaMalloc(&b->d_ev, std::max<int64_t>(1, b->n_ev) * cap));
+    SBN_BP_CUDA(cudaMalloc(&b->d_msg, 2LL * b->E * cap * 4));
+    SBN_BP_CUDA(cudaMalloc(&b->d_out, static_cast<int64_t>(b->Q) * cap * 4));
+    SBN_BP_CUDA(cudaMalloc(&b->d_iters, cap * 4));
+    b->cap = cap;
+    return SBN_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sbn_bp_create(int device, const int32_t *words, int64_t n_words, const float *tables, int64_t n_table_floats,
+                  sbn_bp **out) {
+    if (!words || !out || (n_table_floats > 0 && !tables)) return sbn_fail(SBN_E_INVALID, "null argument");
+    *out = nullptr;
+    sbn_bp probe;
+    int rc = validate(words, n_words, n_table_floats, probe);
+    if (rc != SBN_OK) return rc;
+    const int64_t words_bytes = (n_words * 4 + 15) & ~15LL;
+    if (words_bytes > kSmemLimit)
+        return sbn_fail(SBN_E_INVALID, "bp words: %lld words do not fit the kernel's shared memory",
+                        static_cast<long long>(n_words));
+    int n_dev = 0;
+    if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) return sbn_fail(SBN_E_NODEVICE, "no CUDA device available");
+    if (device < 0 || device >= n_dev) return sbn_fail(SBN_E_NODEVICE, "device %d out of range (%d visible)", device, n_dev);
+    sbn_bp *b = new sbn_bp();
+    b->device = device;
+    b->words.assign(words, words + n_words);
+    b->n_table_floats = static_cast<int>(n_table_floats);
+    b->n_ev = probe.n_ev;
+    b->E = probe.E;
+    b->Q = probe.Q;
+    b->max_card = probe.max_card;
+    b->tables_in_smem = words_bytes + n_table_floats * 4 <= kSmemLimit;
+    b->smem = static_cast<int>(words_bytes + (b->tables_in_smem ? n_table_floats * 4 : 0));
+    auto bail = [&](int code) {
+        sbn_bp_destroy(b);
+        return code;
+    };
+#define SBN_BP_CUDA_B(call)                                                                                             \
+    do {                                                                                                              \
+        cudaError_t e_ = (call);                                                                                      \
+        if (e_ != cudaSuccess)                                                                                        \
+            return bail(sbn_fail(e_ == cudaErrorMemoryAllocation ? SBN_E_NOMEM : SBN_E_CUDA, "%s failed: %s (%s:%d)", \
+                                 #call, cudaGetErrorString(e_), __FILE__, __LINE__));                                 \
+    } while (0)
+    SBN_BP_CUDA_B(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    SBN_BP_CUDA_B(cudaGetDeviceProperties(&prop, device));
+    if (prop.major != 9 || prop.minor != 0)
+        return bail(sbn_fail(SBN_E_NODEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", device,
+                             prop.major, prop.minor));
+    SBN_BP_CUDA_B(cudaFuncSetAttribute(sbn_bp_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+    SBN_BP_CUDA_B(cudaFuncSetAttribute(sbn_bp_kernel<kMaxCard>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+    SBN_BP_CUDA_B(cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking));
+    SBN_BP_CUDA_B(cudaMalloc(&b->d_words, n_words * 4));
+    SBN_BP_CUDA_B(cudaMemcpy(b->d_words, words, n_words * 4, cudaMemcpyHostToDevice));
+    if (n_table_floats > 0) {
+        SBN_BP_CUDA_B(cudaMalloc(&b->d_tables, n_table_floats * 4));
+        SBN_BP_CUDA_B(cudaMemcpy(b->d_tables, tables, n_table_floats * 4, cudaMemcpyHostToDevice));
+    }
+#undef SBN_BP_CUDA_B
+    *out = b;
+    return SBN_OK;
+}
+
+int sbn_bp_run_host(sbn_bp *b, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int32_t n_iterations, float damping,
+                    float tol, float *out, int64_t ld_out, int32_t *iterations) {
+    if (!b || !out || !iterations || (b->n_ev > 0 && !ev)) return sbn_fail(SBN_E_INVALID, "null argument");
+    if (n_rows < 0 || ld_ev < n_rows || ld_out < n_rows)
+        return sbn_fail(SBN_E_INVALID, "bad shape: %lld rows, pitches %lld / %lld", static_cast<long long>(n_rows),
+                        static_cast<long long>(ld_ev), static_cast<long long>(ld_out));
+    if (n_iterations < 1 || n_iterations == 0x7fffffff)
+        return sbn_fail(SBN_E_INVALID, "n_iterations must be in [1, 2^31 - 2], not %d", n_iterations);
+    if (!(damping >= 0.f && damping < 1.f)) return sbn_fail(SBN_E_INVALID, "damping must be in [0, 1), not %g", damping);
+    if (!(tol >= 0.f) || std::isinf(tol)) return sbn_fail(SBN_E_INVALID, "tol must be finite and >= 0, not %g", tol);
+    if (n_rows == 0) return SBN_OK;
+    SBN_BP_CUDA(cudaSetDevice(b->device));
+    int64_t want = n_rows;
+    if (const char *s = std::getenv("SOROBN_B200_CHUNK_ROWS")) {
+        const long long cap = std::atoll(s);
+        if (cap > 0) want = std::min<int64_t>(want, cap);
+    }
+    int rc = reserve(b, want);
+    if (rc != SBN_OK) return rc;
+    const int64_t chunk = std::min(b->cap, want);
+    for (int64_t r0 = 0; r0 < n_rows; r0 += chunk) {
+        const int64_t n = std::min(chunk, n_rows - r0);
+        if (b->n_ev > 0)
+            SBN_BP_CUDA(cudaMemcpy2DAsync(b->d_ev, b->cap, ev + r0, ld_ev, n, b->n_ev, cudaMemcpyHostToDevice, b->stream));
+        BpArgs a{b->d_words, static_cast<int>(b->words.size()), b->d_tables, b->n_table_floats, b->tables_in_smem ? 1 : 0,
+                 b->d_ev, b->d_msg, b->d_out, b->d_iters, b->cap, n, n_iterations, damping, tol};
+        const unsigned grid = static_cast<unsigned>((n + kThreads - 1) / kThreads);
+        if (b->max_card <= 8)
+            sbn_bp_kernel<8><<<grid, kThreads, b->smem, b->stream>>>(a);
+        else
+            sbn_bp_kernel<kMaxCard><<<grid, kThreads, b->smem, b->stream>>>(a);
+        SBN_BP_CUDA(cudaGetLastError());
+        SBN_BP_CUDA(cudaMemcpy2DAsync(out + r0, ld_out * 4, b->d_out, b->cap * 4, n * 4, b->Q, cudaMemcpyDeviceToHost,
+                                      b->stream));
+        SBN_BP_CUDA(cudaMemcpyAsync(iterations + r0, b->d_iters, n * 4, cudaMemcpyDeviceToHost, b->stream));
+    }
+    SBN_BP_CUDA(cudaStreamSynchronize(b->stream));
+    return SBN_OK;
+}
+
+void sbn_bp_destroy(sbn_bp *b) {
+    if (!b) return;
+    cudaSetDevice(b->device);
+    if (b->stream) cudaStreamSynchronize(b->stream);
+    cudaFree(b->d_words);
+    cudaFree(b->d_tables);
+    cudaFree(b->d_ev);
+    cudaFree(b->d_msg);
+    cudaFree(b->d_out);
+    cudaFree(b->d_iters);
+    if (b->stream) cudaStreamDestroy(b->stream);
+    delete b;
+}
+
+}  // extern "C"
