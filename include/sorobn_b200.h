@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SBN_ABI_VERSION 19
+#define SBN_ABI_VERSION 20
 
 #define SBN_OK 0
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
@@ -355,12 +355,20 @@ void sbn_tally_destroy(sbn_tally *tally);
  * out[q * ld_out + b] = the belief of row b in state q of the targets' output (float, host); iterations[b] = the
  * sweep at which row b converged (its largest damped-message change fell below tol) or met a zero sum (its
  * beliefs are then NaN), or n_iterations + 1 when it did not converge.  1 <= n_iterations < 2^31 - 1,
- * 0 <= damping < 1, tol >= 0 (tol = 0 runs exactly n_iterations sweeps). */
+ * 0 <= damping < 1, tol >= 0 (tol = 0 runs exactly n_iterations sweeps).
+ * sbn_bp_mpe_host: max-product words of bp.compile_mpe_graph (version 2; sbn_bp_create takes either version, and
+ * each run call refuses the other's words): the same sweep with a max in place of the sum, then, per row,
+ * codes[k * ld_codes + b] = the decoded state of the k-th unobserved variable (var id order; codes may be NULL when
+ * there is none), log_p[b] = log P(decode, observed cells) in double (-inf for a decode of probability 0, NaN for
+ * a row that met a zero sum, whose codes are 0) and iterations[b] as above (0 when every node is observed).
+ * Same argument rules as sbn_bp_run_host. */
 typedef struct sbn_bp sbn_bp;
 int sbn_bp_create(int device, const int32_t *words, int64_t n_words, const float *tables, int64_t n_table_floats,
                   sbn_bp **out);
 int sbn_bp_run_host(sbn_bp *bp, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int32_t n_iterations, float damping,
                     float tol, float *out, int64_t ld_out, int32_t *iterations);
+int sbn_bp_mpe_host(sbn_bp *bp, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int32_t n_iterations,
+                    float damping, float tol, uint8_t *codes, int64_t ld_codes, double *log_p, int32_t *iterations);
 void sbn_bp_destroy(sbn_bp *bp);
 
 /* Pinned host memory for evidence / posterior staging buffers. */

@@ -32,7 +32,8 @@ other unobserved variables summed out: one log-sum-exp, then max-sum program per
 (planner.build_map_plan).  `joint_marginals_many` returns, for every row, the joint posterior of every CPT
 family or of chosen groups of variables, one joint program per pattern (planner.build_joint_plan).
 `marginals_many(..., algorithm="bp")` approximates every marginal by loopy belief propagation on the device, one
-row per thread (sorobn_b200/bp.py, csrc/sbn_bp.cu), for networks too wide to eliminate exactly.
+row per thread (sorobn_b200/bp.py, csrc/sbn_bp.cu), for networks too wide to eliminate exactly, and
+`mpe_many(..., algorithm="bp")` decodes every row by max-product belief propagation there.
 """
 from __future__ import annotations
 
@@ -787,7 +788,8 @@ class BayesNet:
                                           names=[events.index.name, "draw"])
         return self._codes_frame(codes.reshape(len(net.names), -1), index)
 
-    def mpe_many(self, events: pd.DataFrame, return_log_proba: bool = False, likelihoods: dict | None = None):
+    def mpe_many(self, events: pd.DataFrame, return_log_proba: bool = False, likelihoods: dict | None = None,
+                 algorithm="exact", n_iterations=100, damping=0.5, tol=1e-5):
         """The most probable explanation of every row of `events`, computed on the GPU: the joint state of
         every unobserved variable that maximises P(unobserved, the row's observed cells).
 
@@ -807,21 +809,93 @@ class BayesNet:
 
         likelihoods: soft evidence, as in `expected_counts` (noisy observations: Viterbi-style decoding).  The
         soft nodes are decoded too, and the log probability is log P(explanation, observed cells, likelihoods)
-        on the scale of the given likelihoods."""
-        return self._mpe_frame(events, return_log_proba, likelihoods)
+        on the scale of the given likelihoods.
 
-    def mpe(self, event: dict, likelihoods: dict | None = None) -> pd.Series:
+        algorithm="bp": max-product loopy belief propagation on the device instead of elimination, for networks
+        whose induced width the exact planner refuses (sorobn_b200/bp.py, "Max-product", defines it).  Every CPT is
+        a factor and every unobserved node a variable; max-product messages are swept synchronously, each
+        factor-to-variable message damped as (1 - damping) * new + damping * old, until the largest change of any
+        message of the row falls below `tol` or `n_iterations` sweeps have run.  Each variable then takes the first
+        state of its largest belief, and the row's log P(explanation, observed cells) is summed over the CPTs in
+        float64.  Exact on polytrees whose MPE is unique; on loopy networks an approximation whose log P is that
+        of the assignment returned, never above the exact MPE's, and on grids often far below it (DESIGN.md,
+        "Max-product belief propagation", gives measured gaps).  Rows are grouped by missingness pattern, one
+        compiled graph per pattern; the frame and the log P Series are those of the exact path.  A row whose
+        messages or beliefs sum to zero, or whose observed cells alone hit a CPT entry of zero, raises the exact
+        path's ValueError: any assignment of positive probability keeps every message non-zero, so its observed
+        cells are impossible.  A row whose decode has probability zero (the per-variable decode can combine tied
+        states of different maximisers, and loopy messages are approximate) is returned with log P = -inf, and one
+        RuntimeWarning gives their count; rows that did not converge keep the decode of their last sweep and raise one
+        RuntimeWarning with their count.  ValueError for `likelihoods` (no soft evidence) and unless 0 <= damping < 1, n_iterations >= 1 and
+        tol >= 0."""
+        return self._mpe_frame(events, return_log_proba, likelihoods, algorithm=algorithm, n_iterations=n_iterations,
+                               damping=damping, tol=tol)
+
+    def mpe(self, event: dict, likelihoods: dict | None = None, algorithm="exact", n_iterations=100, damping=0.5,
+            tol=1e-5) -> pd.Series:
         """The most probable explanation of one event: `mpe_many(pd.DataFrame([event])).iloc[0]`, a Series
         indexed by node name.  likelihoods: soft evidence of the event, {node: a vector over the node's sorted
-        domain, or a {state: weight} dict}, as in `query`."""
-        return self._mpe_frame(pd.DataFrame([event]), False, likelihoods, single=True).iloc[0]
+        domain, or a {state: weight} dict}, as in `query`.  algorithm, n_iterations, damping, tol: as in
+        `mpe_many`."""
+        return self._mpe_frame(pd.DataFrame([event]), False, likelihoods, single=True, algorithm=algorithm,
+                               n_iterations=n_iterations, damping=damping, tol=tol).iloc[0]
 
-    def _mpe_frame(self, events, return_log_proba, likelihoods, single=False):
+    def _mpe_frame(self, events, return_log_proba, likelihoods, single=False, algorithm="exact", n_iterations=100,
+                   damping=0.5, tol=1e-5):
+        if algorithm not in ("exact", "bp"):
+            raise ValueError("Unknown algorithm, must be one of: exact, bp")
+        if algorithm == "bp":
+            if likelihoods is not None:
+                self._check_soft_call(algorithm, None)
+            _bp.check_arguments(n_iterations, damping, tol)
         groups = self._count_patterns(events)
-        soft = self._pattern_soft(likelihoods, events, single)
-        codes, _, log_p = self._decode(events, groups, "mpe", "they have nothing to explain", soft=soft)
+        if algorithm == "bp":
+            codes, log_p = self._bp_decode(events, groups, n_iterations, damping, tol)
+        else:
+            soft = self._pattern_soft(likelihoods, events, single)
+            codes, _, log_p = self._decode(events, groups, "mpe", "they have nothing to explain", soft=soft)
         frame = self._codes_frame(codes, events.index)
         return (frame, pd.Series(log_p, index=events.index)) if return_log_proba else frame
+
+    def _bp_decode(self, events, groups, n_iterations, damping, tol):
+        """(codes [n_nodes, n], log P [n]) of max-product belief propagation (bp.compile_mpe_graph) over the pattern
+        groups of `events`, one cached graph per pattern: the observed codes copied through, the decoded ones in
+        var id order.  Dead rows raise; one RuntimeWarning each counts the rows whose decode has probability zero
+        and the rows that did not converge."""
+        from . import engine
+
+        net = self._compiled
+        n_rows = len(events.index)
+        codes = np.zeros((len(net.names), n_rows), dtype=np.uint8)
+        log_p = np.zeros(n_rows, dtype=np.float64)
+        zero = stuck = 0
+        for ev, rows, ev_codes in groups:
+            for i, v in enumerate(ev):
+                codes[v][rows] = ev_codes[i]
+
+            def build(ev=ev):
+                g = _bp.compile_mpe_graph(net, ev)
+                return engine.BeliefPropagation(g.words, g.tables, device=self.device)
+
+            # fetched right before it runs, as in `sample_many`
+            runner = self._cached(("bp_mpe", ev), build)
+            decoded, lp, iters = runner.mpe(ev_codes, len(rows), n_iterations, damping, tol)
+            _check_possible(events.index, rows, np.isnan(lp), "they have nothing to explain")
+            observed = set(ev)
+            hidden = [v for v in range(len(net.names)) if v not in observed]
+            for j, v in enumerate(hidden):
+                codes[v][rows] = decoded[j]
+            log_p[rows] = lp
+            zero += int(np.count_nonzero(lp == -np.inf))
+            stuck += int(np.count_nonzero(iters > n_iterations))
+        if zero:
+            warnings.warn(f"belief propagation: {zero} of {n_rows} rows decoded an explanation of probability zero "
+                          "(log P = -inf)", RuntimeWarning, stacklevel=4)
+        if stuck:
+            warnings.warn(f"belief propagation: {stuck} of {n_rows} rows did not converge to tol={tol:g} in "
+                          f"{n_iterations} sweeps; they keep the decode of their last sweep", RuntimeWarning,
+                          stacklevel=4)
+        return codes, log_p
 
     def map_many(self, events: pd.DataFrame, variables=None, return_log_proba: bool = False,
                  likelihoods: dict | None = None):

@@ -41,6 +41,31 @@ invisible after normalisation wherever nothing underflowed.  Double keeps the sm
 disagreeing neighbours a state can fall more than 2^126 below the largest on the way, past float32's range.  Every
 normalisation divides by the sum (a subnormal sum still gives finite ratios).
 
+Max-product (the most probable explanation; `compile_mpe_graph`, `BayesNet.mpe_many(algorithm="bp")`)
+--------------------------------------------------------------------------------------------------
+Factor graph.  Every unobserved node is a variable and nothing is pruned: in max-product a barren leaf sends
+max_x P(x | pa), which depends on its parents (P(A=0) = 0.6, B | A=0 = (0.5, 0.5), B | A=1 = (0.9, 0.1): the MPE
+is A=1, B=0 at 0.36 > 0.30, and without B the decode would give A=0).  There is one factor per CPT of the
+network, its evidence axes indexed by the row's codes; a factor whose members are all observed is kept with 0
+members: the sweep skips it and the score reads it.  Before the first sweep, a 0-member factor whose entry at the
+row's codes is 0 makes the row dead (its observed cells are impossible, and no message would show it): it runs no
+sweep and records 0.
+
+Sweep.  The sweep above, except that step 1 maximises:
+    mu'_{f->v}(x) = max_{x_f \\ v} f(x_f, e) prod_{u != v} nu_{u->f}(x_u)   (the max starting at 0),
+then normalised to sum 1 and damped as in sum-product.  Step 2, the residual, tol, the n_iterations + 1 record, the
+zero rule and the double products with their rescale are unchanged.
+
+Decode.  After the row's last sweep, each variable's belief product prod_{f ∋ v} mu_{f->v} is formed in double (as
+the beliefs above, before normalisation); its code is the first state with the largest product (x walked upwards,
+strict >).  A belief that sums to 0 makes the row dead.
+
+Score.  log P(x̂, e) = sum over every factor, 0-member ones included, of log(double(table entry at x̂ and the row's
+codes)), in double.  It may be -inf for a live row: the per-variable decode can combine tied states of different
+maximisers (even on a polytree: A uniform and B = not A decode A=0, B=0), and loopy messages are approximate.  A
+dead row reports NaN and codes 0.  A pattern that observes every node has 0 variables and 0 edges: it runs no sweep,
+records 0 and returns only its score.
+
 Words (int32; `sbn_bp_create` bounds-checks every one)
 ------------------------------------------------------
     header : MAGIC 1 n_ev n_factors n_vars E n_targets Q n_table_floats fac_pos var_pos tgt_pos
@@ -54,6 +79,10 @@ table in the blob has its unobserved members innermost, dense, member 0 fastest 
 evidence axes outside them: the entry of a row is table offset + sum_k min(code_k, card_k - 1) * stride_k +
 sum_i x_i * stride_i.  Factors follow the variable order (topological), members the CPT's axis order [*parents, v],
 variables their ids; targets are sorted by name, each at rows q_offset .. q_offset + card of the output.
+
+Version 2 (max-product) has the same layout, with three differences: a factor record may have n_mem = 0; n_vars
+and E may be 0; the target section lists every variable record in variable order, with q_offset = its position,
+its row of the codes output (Q = n_vars).
 """
 from __future__ import annotations
 
@@ -62,7 +91,8 @@ from dataclasses import dataclass
 import numpy as np
 
 MAGIC = 0x53424250  # "SBBP"
-VERSION = 1
+VERSION = 1  # sum-product (compile_graph)
+VERSION_MPE = 2  # max-product (compile_mpe_graph)
 HEADER_WORDS = 12
 MAX_CARD = 256  # states of an unobserved variable (the kernel's widest message)
 
@@ -117,18 +147,32 @@ def compile_graph(net, evidence, targets) -> Graph:
     """The factor graph of `net` (planner.CompiledNet) given the evidence var ids (the columns of the codes, in
     order) and the target var ids, as words and a table blob (module docstring)."""
     evidence, targets = [int(e) for e in evidence], [int(t) for t in targets]
-    if len(set(evidence)) != len(evidence):
-        raise ValueError("duplicate evidence variable")
     if not targets:
         raise ValueError("at least one target is needed")
     if set(targets) & set(evidence):
         raise ValueError("a target cannot be an evidence variable")
+    return _compile(net, evidence, relevant_set(net, evidence, targets), targets, VERSION)
+
+
+def compile_mpe_graph(net, evidence) -> Graph:
+    """The max-product factor graph of `net` given the evidence var ids (module docstring, "Max-product"): every
+    CPT a factor, every unobserved node a variable and a target, as version-2 words and a table blob."""
+    evidence = [int(e) for e in evidence]
+    observed = set(evidence)
+    variables = [v for v in range(len(net.names)) if v not in observed]
+    return _compile(net, evidence, set(range(len(net.names))), variables, VERSION_MPE)
+
+
+def _compile(net, evidence, relevant, targets, version) -> Graph:
+    """Words and blob of the factors of the `relevant` CPTs (version 1 drops those with every member observed);
+    version 1 targets are sorted by name and span their cards, version 2 targets are every variable in order."""
+    if len(set(evidence)) != len(evidence):
+        raise ValueError("duplicate evidence variable")
     card = [int(c) for c in net.card]
     for v in evidence:
         if card[v] > 255:
             raise ValueError(f"evidence variable {net.names[v]!r} has {card[v]} states; state codes are uint8")
     ev_col = {v: k for k, v in enumerate(evidence)}
-    relevant = relevant_set(net, evidence, targets)
     variables = [v for v in sorted(relevant) if v not in ev_col]
     for v in variables:
         if card[v] > MAX_CARD:
@@ -141,7 +185,7 @@ def compile_graph(net, evidence, targets) -> Graph:
     for v in sorted(relevant):
         scope = list(net.scope(v))
         members = [u for u in scope if u not in ev_col]
-        if not members:
+        if not members and version == VERSION:
             continue
         evax = [u for u in scope if u in ev_col]
         T = int(np.prod([card[u] for u in members]))
@@ -169,12 +213,13 @@ def compile_graph(net, evidence, targets) -> Graph:
         rec = [v, card[v], len(edges_of[v]), *edges_of[v]]
         var_words.append(rec)
         pos += len(rec)
-    names = {t: net.names[t] for t in targets}
-    targets = sorted(set(targets), key=lambda t: names[t])
+    if version == VERSION:
+        names = {t: net.names[t] for t in targets}
+        targets = sorted(set(targets), key=lambda t: names[t])
     q_offsets, Q = [], 0
     for t in targets:
         q_offsets.append(Q)
-        Q += card[t]
+        Q += card[t] if version == VERSION else 1
 
     fac_flat = [w for rec in fac_words for w in rec]
     var_flat = [w for rec in var_words for w in rec]
@@ -185,7 +230,7 @@ def compile_graph(net, evidence, targets) -> Graph:
     for t, q in zip(targets, q_offsets):
         tgt_flat += [var_pos + var_rel[t], q]
     tables64 = np.concatenate(blobs) if blobs else np.zeros(0)
-    header = [MAGIC, VERSION, len(evidence), len(fac_words), len(variables), E, len(targets), Q, tables64.size,
+    header = [MAGIC, version, len(evidence), len(fac_words), len(variables), E, len(targets), Q, tables64.size,
               fac_pos, var_pos, tgt_pos]
     words = np.asarray(header + fac_flat + var_flat + tgt_flat, dtype=np.int64)
     if words.max(initial=0) >= 2**31 or tables64.size >= 2**31:

@@ -13,6 +13,8 @@
 // Both directions of every message are stored (mu at entries [0, E), nu at [E, 2E)): step 1 reads nu and writes
 // mu, step 2 reads mu and writes nu, so every entry is updated in place.  Storing only mu and forming nu on the
 // fly would halve the state but multiply step 1's reads by the variable degrees.
+// The max-product instantiations (version-2 words, the most probable explanation) run the same sweep with a max in
+// step 1, then decode every variable and score the decode in the same thread.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -50,6 +52,8 @@ struct BpArgs {
     int64_t ld, n_rows;
     int n_iterations;
     float damping, tol;
+    uint8_t *codes;  // max-product: [n_var][ld]
+    double *log_p;   // max-product: [ld]
 };
 
 // Product of the mu of a variable's edges except `skip` (-1: all of them) into p[], rescaled against underflow;
@@ -85,7 +89,9 @@ __device__ __forceinline__ double bp_product(const int32_t *edges, int deg, int 
 
 }  // namespace
 
-template <int MAXC>
+// MAX = false: sum-product, version-1 words, beliefs of the targets; MAX = true: max-product, version-2 words,
+// codes and log P of the decode (bp.py "Max-product").
+template <int MAXC, bool MAX>
 __global__ void __launch_bounds__(kThreads) sbn_bp_kernel(const __grid_constant__ BpArgs a) {
     extern __shared__ __align__(16) uint8_t s_raw[];
     int32_t *w = reinterpret_cast<int32_t *>(s_raw);
@@ -122,13 +128,36 @@ __global__ void __launch_bounds__(kThreads) sbn_bp_kernel(const __grid_constant_
         p += 4 + 3 * n_mem + 3 * n_evax;
     }
 
-    int recorded = a.n_iterations + 1;
     bool dead = false;
-    for (int t = 1; t <= a.n_iterations; ++t) {
+    if constexpr (MAX) {
+        // a family whose members are all observed, at an entry of probability 0: the row's evidence is impossible,
+        // and no message would ever see it (the sweep skips such factors)
+        for (int f = 0, p = fac_pos; f < n_fac; ++f) {
+            const int n_mem = w[p + 2], n_evax = w[p + 3];
+            if (n_mem == 0) {
+                int idx = w[p + 1];
+                for (int k = 0; k < n_evax; ++k) {
+                    const int32_t *ax = w + p + 4 + 3 * k;
+                    idx += min(static_cast<int>(ev[static_cast<int64_t>(ax[0]) * ld]), ax[2] - 1) * ax[1];
+                }
+                if (!(table(idx) > 0.f)) dead = true;
+            }
+            p += 4 + 3 * n_mem + 3 * n_evax;
+        }
+    }
+    // max-product: a pattern that observes every node has nothing to decode, and a row dead before its first sweep
+    // runs none; both record 0
+    const int sweeps = MAX && (n_var == 0 || dead) ? 0 : a.n_iterations;
+    int recorded = MAX && (n_var == 0 || dead) ? 0 : a.n_iterations + 1;
+    for (int t = 1; t <= sweeps; ++t) {
         // ---- step 1: every factor-to-variable message, damped, and the residual
         float r = 0.f;
         for (int f = 0, p = fac_pos; f < n_fac; ++f) {
             const int n_mem = w[p + 2], n_evax = w[p + 3];
+            if (MAX && n_mem == 0) {  // an all-observed family: only the score reads it
+                p += 4 + 3 * n_evax;
+                continue;
+            }
             const int32_t *mem = w + p + 4;
             const int32_t *ax = mem + 3 * n_mem;
             int base = w[p + 1];
@@ -158,7 +187,12 @@ __global__ void __launch_bounds__(kThreads) sbn_bp_kernel(const __grid_constant_
                     }
 #pragma unroll
                     for (int x = 0; x < BP_XN; ++x)
-                        if (x < c) s[x] += table(idx + x * si) * prod;
+                        if (x < c) {
+                            if constexpr (MAX)
+                                s[x] = fmaxf(s[x], table(idx + x * si) * prod);
+                            else
+                                s[x] += table(idx + x * si) * prod;
+                        }
                 }
                 float S = 0.f;
 #pragma unroll
@@ -208,29 +242,77 @@ __global__ void __launch_bounds__(kThreads) sbn_bp_kernel(const __grid_constant_
         }
     }
     a.iters[row] = recorded;
-    // ---- beliefs of the targets from the last sweep's mu
-    for (int k = 0; k < n_tgt && !dead; ++k) {
-        const int p = w[tgt_pos + 2 * k];
-        const int c = w[p + 1], deg = w[p + 2];
-        double q[MAXC];
-        const double S = bp_product<MAXC>(w + p + 3, deg, -1, c, mu, ld, q);
-        if (!(S > 0.0)) {
-            dead = true;
-            break;
-        }
-        float *o = a.out + static_cast<int64_t>(w[tgt_pos + 2 * k + 1]) * ld + row;
+    if constexpr (MAX) {
+        // ---- decode: every variable's first state of largest belief product, from the last sweep's mu.  The code
+        // is left in the first nu entry of each of the variable's edges (no sweep reads nu any more), where the
+        // score finds it through the factor's member records.
+        for (int k = 0; k < n_tgt && !dead; ++k) {
+            const int p = w[tgt_pos + 2 * k];
+            const int c = w[p + 1], deg = w[p + 2];
+            double q[MAXC];
+            const double S = bp_product<MAXC>(w + p + 3, deg, -1, c, mu, ld, q);
+            if (!(S > 0.0)) {
+                dead = true;
+                break;
+            }
+            int best = 0;
+            double top = q[0];
 #pragma unroll
-        for (int x = 0; x < BP_XN; ++x)
-            if (x < c) o[static_cast<int64_t>(x) * ld] = static_cast<float>(q[x] / S);
+            for (int x = 1; x < BP_XN; ++x)
+                if (x < c && q[x] > top) {
+                    top = q[x];
+                    best = x;
+                }
+            a.codes[static_cast<int64_t>(w[tgt_pos + 2 * k + 1]) * ld + row] = static_cast<uint8_t>(best);
+            for (int j = 0; j < deg; ++j) nu[static_cast<int64_t>(w[p + 3 + j]) * ld] = static_cast<float>(best);
+        }
+        // ---- score: log P(decode, e) over every factor, 0-member ones included
+        double lp = 0.0;
+        for (int f = 0, p = fac_pos; f < n_fac && !dead; ++f) {
+            const int n_mem = w[p + 2], n_evax = w[p + 3];
+            const int32_t *mem = w + p + 4;
+            const int32_t *ax = mem + 3 * n_mem;
+            int idx = w[p + 1];
+            for (int i = 0; i < n_mem; ++i)
+                idx += static_cast<int>(nu[static_cast<int64_t>(mem[3 * i + 2]) * ld]) * mem[3 * i + 1];
+            for (int k = 0; k < n_evax; ++k) {
+                const int code = min(static_cast<int>(ev[static_cast<int64_t>(ax[3 * k]) * ld]), ax[3 * k + 2] - 1);
+                idx += code * ax[3 * k + 1];
+            }
+            lp += log(static_cast<double>(table(idx)));
+            p += 4 + 3 * n_mem + 3 * n_evax;
+        }
+        if (dead) {
+            lp = __longlong_as_double(0x7ff8000000000000LL);
+            for (int k = 0; k < n_tgt; ++k) a.codes[static_cast<int64_t>(w[tgt_pos + 2 * k + 1]) * ld + row] = 0;
+        }
+        a.log_p[row] = lp;
+    } else {
+        // ---- beliefs of the targets from the last sweep's mu
+        for (int k = 0; k < n_tgt && !dead; ++k) {
+            const int p = w[tgt_pos + 2 * k];
+            const int c = w[p + 1], deg = w[p + 2];
+            double q[MAXC];
+            const double S = bp_product<MAXC>(w + p + 3, deg, -1, c, mu, ld, q);
+            if (!(S > 0.0)) {
+                dead = true;
+                break;
+            }
+            float *o = a.out + static_cast<int64_t>(w[tgt_pos + 2 * k + 1]) * ld + row;
+#pragma unroll
+            for (int x = 0; x < BP_XN; ++x)
+                if (x < c) o[static_cast<int64_t>(x) * ld] = static_cast<float>(q[x] / S);
+        }
+        if (dead)
+            for (int q = 0; q < Q; ++q) a.out[static_cast<int64_t>(q) * ld + row] = __int_as_float(0x7fc00000);
     }
-    if (dead)
-        for (int q = 0; q < Q; ++q) a.out[static_cast<int64_t>(q) * ld + row] = __int_as_float(0x7fc00000);
 }
 
 struct sbn_bp {
     int device = 0;
     std::vector<int32_t> words;
     int n_table_floats = 0;
+    int version = 1;
     int n_ev = 0, E = 0, Q = 0, max_card = 1;
     int smem = 0;
     bool tables_in_smem = false;
@@ -240,6 +322,8 @@ struct sbn_bp {
     uint8_t *d_ev = nullptr;
     float *d_msg = nullptr, *d_out = nullptr;
     int32_t *d_iters = nullptr;
+    uint8_t *d_codes = nullptr;  // version 2
+    double *d_log_p = nullptr;
     cudaStream_t stream = nullptr;
 };
 
@@ -253,13 +337,19 @@ namespace {
                             #call, cudaGetErrorString(e_), __FILE__, __LINE__);                                \
     } while (0)
 
-// Bounds-check every word (bp.py layout); fills n_ev, E, Q and the widest message.
+// Bounds-check every word (bp.py layout); fills the version, n_ev, E, Q and the widest message.  Version 2
+// (max-product) allows factors of 0 members and 0 variables and edges, and its targets must be every variable
+// record in order at q_offset k, each member edge of a factor exactly one variable's: the score finds the decoded
+// codes through them.
 int validate(const int32_t *w, int64_t n, int64_t n_tables, sbn_bp &b) {
     if (n < kHeader) return sbn_fail(SBN_E_INVALID, "bp words: %lld words, the header has %d", static_cast<long long>(n), kHeader);
     if (n >= (1LL << 30)) return sbn_fail(SBN_E_INVALID, "bp words: %lld words", static_cast<long long>(n));
-    if (w[0] != kMagic || w[1] != 1) return sbn_fail(SBN_E_INVALID, "bp words: bad magic or version %d", w[1]);
+    if (w[0] != kMagic || (w[1] != 1 && w[1] != 2)) return sbn_fail(SBN_E_INVALID, "bp words: bad magic or version %d", w[1]);
+    const bool mpe = w[1] == 2;
+    const int lo = mpe ? 0 : 1;  // the least n_var, E, targets, Q and members of a factor
     const int n_ev = w[2], n_fac = w[3], n_var = w[4], E = w[5], n_tgt = w[6], Q = w[7];
-    if (n_ev < 0 || n_fac < 1 || n_var < 1 || E < 1 || n_tgt < 1 || Q < 1 || w[8] != n_tables)
+    if (n_ev < 0 || n_fac < 1 || n_var < lo || E < lo || n_tgt < lo || Q < lo || w[8] != n_tables ||
+        (mpe && (n_tgt != n_var || Q != n_var)))
         return sbn_fail(SBN_E_INVALID, "bp words: bad header (n_ev %d, factors %d, variables %d, E %d, targets %d, Q %d, "
                         "table floats %d of %lld)", n_ev, n_fac, n_var, E, n_tgt, Q, w[8], static_cast<long long>(n_tables));
     if (w[9] != kHeader || w[10] < w[9] || w[11] < w[10] || static_cast<int64_t>(w[11]) + 2LL * n_tgt != n)
@@ -271,7 +361,7 @@ int validate(const int32_t *w, int64_t n, int64_t n_tables, sbn_bp &b) {
         if (p + 4 > w[10]) return sbn_fail(SBN_E_INVALID, "bp words: factor %d runs past its section", f);
         const int64_t off = w[p + 1];
         const int n_mem = w[p + 2], n_evax = w[p + 3];
-        if (n_mem < 1 || n_evax < 0 || p + 4 + 3LL * (n_mem + n_evax) > w[10])
+        if (n_mem < lo || n_evax < 0 || p + 4 + 3LL * (n_mem + n_evax) > w[10])
             return sbn_fail(SBN_E_INVALID, "bp words: factor %d has %d members and %d evidence axes", f, n_mem, n_evax);
         int64_t span = 1;  // entries the factor's table spans
         for (int i = 0; i < n_mem; ++i) {
@@ -297,7 +387,11 @@ int validate(const int32_t *w, int64_t n, int64_t n_tables, sbn_bp &b) {
         p += 4 + 3 * (n_mem + n_evax);
     }
     if (p != w[10] || edge_end != E) return sbn_fail(SBN_E_INVALID, "bp words: factor section does not end at its edges");
-    std::vector<int> var_at(n, -1);
+    // version 2: the card of the factor member whose edge starts at e (E is now bounded by the checked records)
+    std::vector<int> member_card(mpe ? E : 0, 0);
+    for (int64_t q = w[9]; mpe && q < w[10]; q += 4 + 3 * (w[q + 2] + w[q + 3]))
+        for (int i = 0; i < w[q + 2]; ++i) member_card[w[q + 6 + 3 * i]] = w[q + 4 + 3 * i];
+    std::vector<int> var_at(n, -1), var_pos;
     for (int v = 0; v < n_var; ++v) {
         if (p + 3 > w[11]) return sbn_fail(SBN_E_INVALID, "bp words: variable %d runs past its section", v);
         const int c = w[p + 1], deg = w[p + 2];
@@ -305,18 +399,24 @@ int validate(const int32_t *w, int64_t n, int64_t n_tables, sbn_bp &b) {
             return sbn_fail(SBN_E_INVALID, "bp words: variable %d (card %d, degree %d)", v, c, deg);
         for (int k = 0; k < deg; ++k) {
             const int e = w[p + 3 + k];
-            if (e < 0 || static_cast<int64_t>(e) + c > E)
+            if (e < 0 || static_cast<int64_t>(e) + c > E || (mpe && member_card[e] != c))
                 return sbn_fail(SBN_E_INVALID, "bp words: variable %d edge %d at %d", v, k, e);
+            if (mpe) member_card[e] = 0;  // claimed
         }
         var_at[p] = c;
+        var_pos.push_back(static_cast<int>(p));
         p += 3 + deg;
     }
     if (p != w[11]) return sbn_fail(SBN_E_INVALID, "bp words: variable section does not end at the targets");
+    if (mpe && std::any_of(member_card.begin(), member_card.end(), [](int c) { return c != 0; }))
+        return sbn_fail(SBN_E_INVALID, "bp words: a factor member's edge belongs to no variable");
     for (int k = 0; k < n_tgt; ++k) {
         const int vp = w[p + 2 * k], q = w[p + 2 * k + 1];
-        if (vp < 0 || vp >= n || var_at[vp] < 0 || q < 0 || q + var_at[vp] > Q)
+        if (vp < 0 || vp >= n || var_at[vp] < 0 || q < 0 || q + (mpe ? 1 : var_at[vp]) > Q ||
+            (mpe && (vp != var_pos[k] || q != k)))
             return sbn_fail(SBN_E_INVALID, "bp words: target %d (record %d, q_offset %d)", k, vp, q);
     }
+    b.version = w[1];
     b.n_ev = n_ev;
     b.E = E;
     b.Q = Q;
@@ -324,9 +424,57 @@ int validate(const int32_t *w, int64_t n, int64_t n_tables, sbn_bp &b) {
     return SBN_OK;
 }
 
+template <bool MAX>
+void launch(const BpArgs &a, int max_card, unsigned grid, int smem, cudaStream_t stream) {
+    if (max_card <= 8)
+        sbn_bp_kernel<8, MAX><<<grid, kThreads, smem, stream>>>(a);
+    else
+        sbn_bp_kernel<kMaxCard, MAX><<<grid, kThreads, smem, stream>>>(a);
+}
+
+int reserve(sbn_bp *b, int64_t rows);
+
+// The argument checks, the reservation and the chunk loop of both run calls: upload a chunk's codes, run it,
+// download its iterations, and queue the download of its outputs by `fetch(r0, n)`; one synchronise at the end.
+template <bool MAX, typename Fetch>
+int run_rows(sbn_bp *b, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int32_t n_iterations, float damping, float tol,
+             int64_t ld_out, int32_t *iterations, Fetch fetch) {
+    if (n_rows < 0 || ld_ev < n_rows || ld_out < n_rows)
+        return sbn_fail(SBN_E_INVALID, "bad shape: %lld rows, pitches %lld / %lld", static_cast<long long>(n_rows),
+                        static_cast<long long>(ld_ev), static_cast<long long>(ld_out));
+    if (n_iterations < 1 || n_iterations == 0x7fffffff)
+        return sbn_fail(SBN_E_INVALID, "n_iterations must be in [1, 2^31 - 2], not %d", n_iterations);
+    if (!(damping >= 0.f && damping < 1.f)) return sbn_fail(SBN_E_INVALID, "damping must be in [0, 1), not %g", damping);
+    if (!(tol >= 0.f) || std::isinf(tol)) return sbn_fail(SBN_E_INVALID, "tol must be finite and >= 0, not %g", tol);
+    if (n_rows == 0) return SBN_OK;
+    SBN_BP_CUDA(cudaSetDevice(b->device));
+    int64_t want = n_rows;
+    if (const char *s = std::getenv("SOROBN_B200_CHUNK_ROWS")) {
+        const long long cap = std::atoll(s);
+        if (cap > 0) want = std::min<int64_t>(want, cap);
+    }
+    int rc = reserve(b, want);
+    if (rc != SBN_OK) return rc;
+    const int64_t chunk = std::min(b->cap, want);
+    for (int64_t r0 = 0; r0 < n_rows; r0 += chunk) {
+        const int64_t n = std::min(chunk, n_rows - r0);
+        if (b->n_ev > 0)
+            SBN_BP_CUDA(cudaMemcpy2DAsync(b->d_ev, b->cap, ev + r0, ld_ev, n, b->n_ev, cudaMemcpyHostToDevice, b->stream));
+        BpArgs a{b->d_words, static_cast<int>(b->words.size()), b->d_tables, b->n_table_floats, b->tables_in_smem ? 1 : 0,
+                 b->d_ev, b->d_msg, b->d_out, b->d_iters, b->cap, n, n_iterations, damping, tol, b->d_codes, b->d_log_p};
+        launch<MAX>(a, b->max_card, static_cast<unsigned>((n + kThreads - 1) / kThreads), b->smem, b->stream);
+        SBN_BP_CUDA(cudaGetLastError());
+        rc = fetch(r0, n);
+        if (rc != SBN_OK) return rc;
+        SBN_BP_CUDA(cudaMemcpyAsync(iterations + r0, b->d_iters, n * 4, cudaMemcpyDeviceToHost, b->stream));
+    }
+    SBN_BP_CUDA(cudaStreamSynchronize(b->stream));
+    return SBN_OK;
+}
+
 int reserve(sbn_bp *b, int64_t rows) {
     if (rows <= b->cap) return SBN_OK;
-    const int64_t per_row = 2LL * b->E * 4;
+    const int64_t per_row = std::max<int64_t>(1, 2LL * b->E * 4);  // E = 0: a max-product pattern with nothing to decode
     int64_t cap = std::max<int64_t>(kThreads, kScratchBudget / per_row / kThreads * kThreads);
     cap = std::min(cap, round_up(rows, kThreads));
     if (cap <= b->cap) return SBN_OK;
@@ -334,14 +482,23 @@ int reserve(sbn_bp *b, int64_t rows) {
     cudaFree(b->d_msg);
     cudaFree(b->d_out);
     cudaFree(b->d_iters);
+    cudaFree(b->d_codes);
+    cudaFree(b->d_log_p);
     b->d_ev = nullptr;
     b->d_msg = b->d_out = nullptr;
     b->d_iters = nullptr;
+    b->d_codes = nullptr;
+    b->d_log_p = nullptr;
     b->cap = 0;
     SBN_BP_CUDA(cudaMalloc(&b->d_ev, std::max<int64_t>(1, b->n_ev) * cap));
-    SBN_BP_CUDA(cudaMalloc(&b->d_msg, 2LL * b->E * cap * 4));
-    SBN_BP_CUDA(cudaMalloc(&b->d_out, static_cast<int64_t>(b->Q) * cap * 4));
+    SBN_BP_CUDA(cudaMalloc(&b->d_msg, std::max<int64_t>(1, 2LL * b->E) * cap * 4));
     SBN_BP_CUDA(cudaMalloc(&b->d_iters, cap * 4));
+    if (b->version == 2) {
+        SBN_BP_CUDA(cudaMalloc(&b->d_codes, std::max<int64_t>(1, b->Q) * cap));
+        SBN_BP_CUDA(cudaMalloc(&b->d_log_p, cap * 8));
+    } else {
+        SBN_BP_CUDA(cudaMalloc(&b->d_out, static_cast<int64_t>(b->Q) * cap * 4));
+    }
     b->cap = cap;
     return SBN_OK;
 }
@@ -368,6 +525,7 @@ int sbn_bp_create(int device, const int32_t *words, int64_t n_words, const float
     b->device = device;
     b->words.assign(words, words + n_words);
     b->n_table_floats = static_cast<int>(n_table_floats);
+    b->version = probe.version;
     b->n_ev = probe.n_ev;
     b->E = probe.E;
     b->Q = probe.Q;
@@ -391,8 +549,12 @@ int sbn_bp_create(int device, const int32_t *words, int64_t n_words, const float
     if (prop.major != 9 || prop.minor != 0)
         return bail(sbn_fail(SBN_E_NODEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", device,
                              prop.major, prop.minor));
-    SBN_BP_CUDA_B(cudaFuncSetAttribute(sbn_bp_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
-    SBN_BP_CUDA_B(cudaFuncSetAttribute(sbn_bp_kernel<kMaxCard>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+    SBN_BP_CUDA_B(cudaFuncSetAttribute(sbn_bp_kernel<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+    SBN_BP_CUDA_B(cudaFuncSetAttribute(sbn_bp_kernel<kMaxCard, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       kSmemLimit));
+    SBN_BP_CUDA_B(cudaFuncSetAttribute(sbn_bp_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+    SBN_BP_CUDA_B(cudaFuncSetAttribute(sbn_bp_kernel<kMaxCard, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       kSmemLimit));
     SBN_BP_CUDA_B(cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking));
     SBN_BP_CUDA_B(cudaMalloc(&b->d_words, n_words * 4));
     SBN_BP_CUDA_B(cudaMemcpy(b->d_words, words, n_words * 4, cudaMemcpyHostToDevice));
@@ -408,41 +570,26 @@ int sbn_bp_create(int device, const int32_t *words, int64_t n_words, const float
 int sbn_bp_run_host(sbn_bp *b, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int32_t n_iterations, float damping,
                     float tol, float *out, int64_t ld_out, int32_t *iterations) {
     if (!b || !out || !iterations || (b->n_ev > 0 && !ev)) return sbn_fail(SBN_E_INVALID, "null argument");
-    if (n_rows < 0 || ld_ev < n_rows || ld_out < n_rows)
-        return sbn_fail(SBN_E_INVALID, "bad shape: %lld rows, pitches %lld / %lld", static_cast<long long>(n_rows),
-                        static_cast<long long>(ld_ev), static_cast<long long>(ld_out));
-    if (n_iterations < 1 || n_iterations == 0x7fffffff)
-        return sbn_fail(SBN_E_INVALID, "n_iterations must be in [1, 2^31 - 2], not %d", n_iterations);
-    if (!(damping >= 0.f && damping < 1.f)) return sbn_fail(SBN_E_INVALID, "damping must be in [0, 1), not %g", damping);
-    if (!(tol >= 0.f) || std::isinf(tol)) return sbn_fail(SBN_E_INVALID, "tol must be finite and >= 0, not %g", tol);
-    if (n_rows == 0) return SBN_OK;
-    SBN_BP_CUDA(cudaSetDevice(b->device));
-    int64_t want = n_rows;
-    if (const char *s = std::getenv("SOROBN_B200_CHUNK_ROWS")) {
-        const long long cap = std::atoll(s);
-        if (cap > 0) want = std::min<int64_t>(want, cap);
-    }
-    int rc = reserve(b, want);
-    if (rc != SBN_OK) return rc;
-    const int64_t chunk = std::min(b->cap, want);
-    for (int64_t r0 = 0; r0 < n_rows; r0 += chunk) {
-        const int64_t n = std::min(chunk, n_rows - r0);
-        if (b->n_ev > 0)
-            SBN_BP_CUDA(cudaMemcpy2DAsync(b->d_ev, b->cap, ev + r0, ld_ev, n, b->n_ev, cudaMemcpyHostToDevice, b->stream));
-        BpArgs a{b->d_words, static_cast<int>(b->words.size()), b->d_tables, b->n_table_floats, b->tables_in_smem ? 1 : 0,
-                 b->d_ev, b->d_msg, b->d_out, b->d_iters, b->cap, n, n_iterations, damping, tol};
-        const unsigned grid = static_cast<unsigned>((n + kThreads - 1) / kThreads);
-        if (b->max_card <= 8)
-            sbn_bp_kernel<8><<<grid, kThreads, b->smem, b->stream>>>(a);
-        else
-            sbn_bp_kernel<kMaxCard><<<grid, kThreads, b->smem, b->stream>>>(a);
-        SBN_BP_CUDA(cudaGetLastError());
+    if (b->version != 1) return sbn_fail(SBN_E_INVALID, "max-product (version 2) words run through sbn_bp_mpe_host");
+    return run_rows<false>(b, ev, ld_ev, n_rows, n_iterations, damping, tol, ld_out, iterations, [&](int64_t r0, int64_t n) {
         SBN_BP_CUDA(cudaMemcpy2DAsync(out + r0, ld_out * 4, b->d_out, b->cap * 4, n * 4, b->Q, cudaMemcpyDeviceToHost,
                                       b->stream));
-        SBN_BP_CUDA(cudaMemcpyAsync(iterations + r0, b->d_iters, n * 4, cudaMemcpyDeviceToHost, b->stream));
-    }
-    SBN_BP_CUDA(cudaStreamSynchronize(b->stream));
-    return SBN_OK;
+        return SBN_OK;
+    });
+}
+
+int sbn_bp_mpe_host(sbn_bp *b, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int32_t n_iterations, float damping,
+                    float tol, uint8_t *codes, int64_t ld_codes, double *log_p, int32_t *iterations) {
+    if (!b || !log_p || !iterations || (b->n_ev > 0 && !ev) || (b->Q > 0 && !codes))
+        return sbn_fail(SBN_E_INVALID, "null argument");
+    if (b->version != 2) return sbn_fail(SBN_E_INVALID, "sum-product (version 1) words run through sbn_bp_run_host");
+    return run_rows<true>(b, ev, ld_ev, n_rows, n_iterations, damping, tol, ld_codes, iterations, [&](int64_t r0, int64_t n) {
+        if (b->Q > 0)
+            SBN_BP_CUDA(cudaMemcpy2DAsync(codes + r0, ld_codes, b->d_codes, b->cap, n, b->Q, cudaMemcpyDeviceToHost,
+                                          b->stream));
+        SBN_BP_CUDA(cudaMemcpyAsync(log_p + r0, b->d_log_p, n * 8, cudaMemcpyDeviceToHost, b->stream));
+        return SBN_OK;
+    });
 }
 
 void sbn_bp_destroy(sbn_bp *b) {
@@ -455,6 +602,8 @@ void sbn_bp_destroy(sbn_bp *b) {
     cudaFree(b->d_msg);
     cudaFree(b->d_out);
     cudaFree(b->d_iters);
+    cudaFree(b->d_codes);
+    cudaFree(b->d_log_p);
     if (b->stream) cudaStreamDestroy(b->stream);
     delete b;
 }
