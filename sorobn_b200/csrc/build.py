@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.dirname(HERE)
 LIB = os.path.join(PKG, "libsorobn_b200.so")
 SOURCES = [os.path.join(HERE, f) for f in ("sbn_api.cu", "sbn_tiled_u0.cu", "sbn_tiled_u1.cu", "sbn_tiled_u2.cu", "sbn_tiled_c.cu",
-                                            "sbn_chain.cu", "sbn_tma.cu", "sbn_pair.cu", "sbn_triple_rows.cu",
+                                            "sbn_chain.cu", "sbn_tma.cu", "sbn_pair.cu", "sbn_triple_rows.cu", "sbn_contract.cu",
                                             "sbn_join.cu", "sbn_tally.cu", "sbn_bp.cu")]
 HEADERS = [os.path.join(HERE, h) for h in ("sbn_kernels.cuh", "sbn_gibbs.cuh", "sbn_chain.h", "sbn_tma.h", "sbn_pair.h", "sbn_join.h", "sbn_internal.h", "sbn_launch.h",
                                             "sbn_launch_impl.cuh", "sbn_marginal.cuh", "sbn_count.cuh", "sbn_deriv.cuh", "sbn_sample.cuh",

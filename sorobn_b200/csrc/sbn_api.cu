@@ -2073,6 +2073,7 @@ static int create_common(int device, const int32_t *words, int64_t n_words, cons
             SBN_CUDA_P(sbn_tma_set_attrs());
             SBN_CUDA_P(sbn_join_set_attrs());
             SBN_CUDA_P(sbn_triple_rows_set_attrs());
+            SBN_CUDA_P(sbn_contract_set_attrs());
             SBN_CUDA_P(sbn_marginal_set_attrs());
             SBN_CUDA_P(sbn_count_set_attrs());
             SBN_CUDA_P(sbn_deriv_set_attrs());

@@ -576,6 +576,128 @@ SbnPair *plan_triple(sbn_program *P, int i1, int i2, std::vector<int32_t> *tiles
     return pr;
 }
 
+// The expanding product contracted by its consumer (sbn_pair.h, SbnContractParams) for two consecutive launched
+// steps; appends the joint-state and tile words to the pair tile table.  A shape rule only: it never looks at the
+// batch size.
+SbnPair *plan_contract(sbn_program *P, int i1, int i2, std::vector<int32_t> *tiles) {
+    constexpr int T = SBN_PAIR_T, R = SBN_CONTRACT_R;
+    const StepDesc &s1 = P->steps[i1], &s2 = P->steps[i2];
+    if (s1.kind != 1 || s2.kind != 1 || s1.ecards.size() != 1 || s2.ecards.empty()) return nullptr;
+    if (s1.in.size() != 2 || s2.in.size() != 2 || s1.ecards[0] < 2 || s1.ecards[0] > T) return nullptr;
+    for (const StepDesc *s : {&s1, &s2})
+        for (const InDesc &in : s->in)
+            if (!in.batched || !in.is_slot || !in.ev.empty()) return nullptr;
+    // Each step alone runs on the tiled kernel, whose arithmetic the fused kernel repeats: step 1's A and B on
+    // different sides of its tile (fmaf(A, B, acc)); step 2's M and C either both on the A side (the product is
+    // rounded, then summed) or not (fmaf(M, C, acc)).
+    if (s1.tile == 0 || s2.tile == 0 || s1.nu + s1.na != 1) return nullptr;
+    int mi = -1;
+    for (int i = 0; i < 2; ++i)
+        if (s2.in[i].id == s1.out_slot) mi = i;
+    if (mi < 0 || s2.in[1 - mi].id == s1.out_slot || s1.out_slot == P->post_slot) return nullptr;
+    const InDesc &A = s1.in[0], &B = s1.in[1], &M = s2.in[mi], &C = s2.in[1 - mi];
+    const int out_slot = s2.out_slot;
+    if (out_slot == A.id || out_slot == B.id || out_slot == C.id || out_slot == M.id) return nullptr;
+
+    // entry stride in X (A or B) of the variable whose entry stride in M is `m_stride` (a variable of `card` states)
+    bool ok = true;
+    auto via_m = [&](int m_stride, int card, const InDesc &X) -> int64_t {
+        if (m_stride == 0 || card == 1) return 0;
+        const int ax = axis_of_stride(s1.cards, m_stride);
+        if (ax < 0 || s1.cards[ax] != card) {
+            ok = false;
+            return 0;
+        }
+        return X.strides[ax];
+    };
+    // entries an operand spans (dense factors: its largest offset + 1)
+    auto span = [](const InDesc &X, const std::vector<int> &cards, const std::vector<int> &ecards) {
+        int64_t n = 1;
+        for (size_t k = 0; k < cards.size(); ++k) n += static_cast<int64_t>(cards[k] - 1) * X.strides[k];
+        for (size_t k = 0; k < ecards.size(); ++k) n += static_cast<int64_t>(ecards[k] - 1) * X.estrides[k];
+        return n;
+    };
+    const int64_t n_a = span(A, s1.cards, s1.ecards), n_b = span(B, s1.cards, s1.ecards), n_c = span(C, s2.cards, s2.ecards);
+    if (n_a + n_b + n_c > SBN_CONTRACT_MAX_OPERAND) return nullptr;
+    int64_t n_e = 1;
+    for (int c : s2.ecards) n_e *= c;
+    if (n_e > SBN_CONTRACT_MAX_E) return nullptr;
+
+    // z: an output axis A lacks, walked inside the thread; every other output axis is a tile axis
+    const int n2 = static_cast<int>(s2.cards.size());
+    int kz = -1;
+    for (int k = 0; k < n2 && kz < 0; ++k)
+        if (s2.cards[k] > 1 && s2.cards[k] <= T && via_m(M.strides[k], s2.cards[k], A) == 0) kz = k;
+    std::vector<int> rt;
+    int64_t n_tiles = 1;
+    for (int k = 0; k < n2; ++k)
+        if (k != kz) rt.push_back(k), n_tiles *= s2.cards[k];
+    if (n_tiles * (kz >= 0 ? s2.cards[kz] : 1) > SBN_CONTRACT_MAX_WARPS) return nullptr;
+    std::vector<int64_t> os2(n2);
+    int64_t os = 1;
+    for (int k = 0; k < n2; ++k) os2[k] = os, os *= s2.cards[k];
+
+    SbnContractParams q;
+    memset(&q, 0, sizeof q);
+    q.n_a = static_cast<int32_t>(n_a), q.n_b = static_cast<int32_t>(n_b), q.n_c = static_cast<int32_t>(n_c);
+    q.n_e = static_cast<int32_t>(n_e), q.n_tiles = static_cast<int32_t>(n_tiles);
+    q.cj = s1.ecards[0];
+    q.a_j = A.estrides[0] * R, q.b_j = B.estrides[0] * R;
+    q.kz = kz >= 0 ? s2.cards[kz] : 1;
+    if (kz >= 0) {
+        q.b_z = static_cast<int32_t>(via_m(M.strides[kz], s2.cards[kz], B) * R);
+        q.c_z = C.strides[kz] * R;
+        q.o_z = static_cast<int32_t>(os2[kz]);
+    }
+    q.prod2 = s2.nu + s2.na == 2 ? 1 : 0;
+    // joint states of the variables step 2 sums out, first fastest (the tiled kernel's zoff order)
+    std::vector<int32_t> words;
+    std::vector<int> dig(s2.ecards.size(), 0);
+    for (int64_t e = 0; e < n_e; ++e) {
+        int64_t a = 0, b = 0, c = 0;
+        for (size_t k = 0; k < dig.size(); ++k) {
+            a += dig[k] * via_m(M.estrides[k], s2.ecards[k], A);
+            b += dig[k] * via_m(M.estrides[k], s2.ecards[k], B);
+            c += static_cast<int64_t>(dig[k]) * C.estrides[k];
+        }
+        words.insert(words.end(), {static_cast<int32_t>(a * R), static_cast<int32_t>(b * R), static_cast<int32_t>(c * R), 0});
+        for (size_t k = 0; k < dig.size(); ++k) {
+            if (++dig[k] < s2.ecards[k]) break;
+            dig[k] = 0;
+        }
+    }
+    dig.assign(rt.size(), 0);
+    for (int64_t t = 0; t < n_tiles; ++t) {
+        int64_t a = 0, b = 0, c = 0, o = 0;
+        for (size_t k = 0; k < rt.size(); ++k) {
+            const int ax = rt[k];
+            a += dig[k] * via_m(M.strides[ax], s2.cards[ax], A);
+            b += dig[k] * via_m(M.strides[ax], s2.cards[ax], B);
+            c += static_cast<int64_t>(dig[k]) * C.strides[ax];
+            o += dig[k] * os2[ax];
+        }
+        words.insert(words.end(), {static_cast<int32_t>(a * R), static_cast<int32_t>(b * R), static_cast<int32_t>(c * R),
+                                   static_cast<int32_t>(o)});
+        for (size_t k = 0; k < dig.size(); ++k) {
+            if (++dig[k] < s2.cards[rt[k]]) break;
+            dig[k] = 0;
+        }
+    }
+    if (!ok) return nullptr;
+
+    SbnPair *pr = new SbnPair();
+    memset(&pr->q, 0, sizeof pr->q);
+    memset(&pr->t, 0, sizeof pr->t);
+    pr->kind = 2;
+    pr->step1 = i1, pr->step2 = i2;
+    pr->g_in = -1;
+    pr->a_in = 0, pr->b_in = 1, pr->c_in = 1 - mi;
+    pr->k = q;
+    pr->tile_off_pos = static_cast<int64_t>(tiles->size());  // a multiple of 4: every pattern appends rows of 4 or 8 words
+    tiles->insert(tiles->end(), words.begin(), words.end());
+    return pr;
+}
+
 }  // namespace
 
 cudaError_t sbn_pair_set_attrs() {
@@ -629,6 +751,24 @@ cudaError_t sbn_pair_plan(sbn_program *P) {
                 P->pair_first[i1] = static_cast<int>(P->pairs.size());
                 P->pair_first[i2] = -2;
                 P->pairs.push_back(tr);
+                continue;
+            }
+        }
+        // The rule below wants two batched operands in step 2 and the paired-steps rule exactly one, so trying it
+        // here is trying it after both other rules failed.  (With the triples switched off, their shapes stay two
+        // launches.)
+        bool triple_shape = false;
+        if (!triples_on) {
+            std::vector<int32_t> probe;
+            SbnPair *tr = plan_triple(P, i1, i2, &probe);
+            triple_shape = tr != nullptr;
+            delete tr;
+        }
+        if (!triple_shape) {
+            if (SbnPair *ct = plan_contract(P, i1, i2, &tiles)) {
+                P->pair_first[i1] = static_cast<int>(P->pairs.size());
+                P->pair_first[i2] = -2;
+                P->pairs.push_back(ct);
                 continue;
             }
         }
@@ -835,6 +975,18 @@ bool sbn_pair_fits(const sbn_program *P, const SbnPair &pr) {
 cudaError_t sbn_pair_launch(sbn_program *P, const SbnPair &pr, const uint8_t *d_ev, int64_t ld_ev, int64_t n_rows,
                             cudaStream_t stream) {
     if (pr.kind == 1) return triple_launch(P, pr, n_rows, stream);
+    if (pr.kind == 2) {
+        SbnContractParams q = pr.k;
+        const StepDesc &s1 = P->steps[pr.step1], &s2 = P->steps[pr.step2];
+        q.a = P->slots[s1.in[pr.a_in].id].ptr;
+        q.b = P->slots[s1.in[pr.b_in].id].ptr;
+        q.c = P->slots[s2.in[pr.c_in].id].ptr;
+        q.out = P->slots[s2.out_slot].ptr;
+        q.words = P->d_pair_tiles + pr.tile_off_pos;
+        q.ld = P->ld;
+        q.n_rows = static_cast<int32_t>(n_rows);
+        return sbn_contract_launch(q, stream);
+    }
     SbnPairParams q = pr.q;
     const StepDesc &s1 = P->steps[pr.step1], &s2 = P->steps[pr.step2];
     q.f = P->slots[s1.in[pr.f_in].id].ptr;

@@ -120,9 +120,45 @@ struct SbnTripleRows {
     int32_t o_off[SBN_TRIPLE_ROWS_COMBOS];      // output entry of each combination at z = s = 0
 };
 
+// Third pattern: an expanding product that its consumer contracts, all operands batched, no tables,
+//
+//     M[m]   = sum_j A[m, j] B[m, j]             step 1: one eliminated variable j   (e.g. 625 <- B125 x B125)
+//     out[o] = sum_e M[o, e] C[o, e]             step 2: any number of eliminated variables, e = their joint state
+//
+// (the benchmark grid's last two launches: 625 <- B125 x B125, then 5 <- sum_125 B625 x B125).  One CTA takes
+// SBN_CONTRACT_R evidence rows: A, B and C arrive in shared memory as [entry][row] columns (coalesced 16-byte
+// copies, every operand byte read from HBM once), and a thread = (row, output) walks e in the consumer's joint-state
+// order, forming each M[o, e] just before it is used: M is never stored.  A and C are read at every joint state, B
+// only when the state moves it (the grid's B changes at every 25th).  The outputs are numbered tile x KZ + z digit, z
+// being an output axis A lacks (the KZ <= T warps of a tile read the same A entries), or KZ = 1 when there is none.
+// Results are bitwise those of the two tiled launches: each M entry is the tiled kernel's fmaf chain over j from
+// 0.f, each output its chain over e from 0.f, with the product M x C either fused into the fma (the two operands
+// sit on different sides of the consumer's tile) or rounded first (both on the A side, `prod2`).
+#define SBN_CONTRACT_R 32                 // evidence rows per CTA: one warp per tile, one 128-byte line per entry
+#define SBN_CONTRACT_MAX_OPERAND 512      // entries of A + B + C: 64 KB of columns at most (the grid's 375: 48 KB)
+#define SBN_CONTRACT_MAX_E 1024           // joint states step 2 sums out (a 16 KB table in shared memory)
+#define SBN_CONTRACT_MAX_WARPS 16         // threads = SBN_CONTRACT_R x outputs (tiles x KZ)
+struct SbnContractParams {
+    const float *a, *b, *c;
+    float *out;
+    const int32_t *words;         // [n_e][4] = A, B, C column offsets of joint state e, 0; then [n_tiles][4] = A, B, C
+                                  // column offsets of the tile, output entry of its first digit
+    int64_t ld;
+    int32_t n_rows;
+    int32_t n_a, n_b, n_c;        // entries of the operands
+    int32_t n_e, n_tiles;
+    int32_t cj, a_j, b_j;         // step 1: states of j, column strides of j in A and B
+    int32_t kz, b_z, c_z, o_z;    // digits of the z axis; column strides in B and C, entry stride in the output
+    int32_t prod2;                // 1: step 2 rounds M x C before the sum; 0: fmaf(M, C, acc)
+};
+// Column offsets count floats of the [entry][SBN_CONTRACT_R] shared-memory layout (entry offset x R).
+cudaError_t sbn_contract_launch(const SbnContractParams &q, cudaStream_t stream);
+cudaError_t sbn_contract_set_attrs();
+
 // One planned pair (host side).
 struct SbnPair {
-    int kind;                     // 0: two table x frontier steps (SbnPairParams); 1: expanding product + contraction (SbnTripleParams)
+    int kind;                     // 0: two table x frontier steps (SbnPairParams); 1: expanding product + contraction
+                                  // (SbnTripleParams); 2: expanding product contracted by its consumer (SbnContractParams)
     int step1, step2;             // indices into sbn_program::steps
     int f_in;                     // index of the batched operand among step1's inputs
     int g_in;                     // modes GB / GC: index of the second batched operand of step1, else -1
@@ -130,7 +166,8 @@ struct SbnPair {
     SbnPairParams q;              // everything but the run-time pointers
     SbnTripleParams t;
     SbnTripleRows rows;           // kind 1: the row-block variant's view of the operands
-    int a_in, b_in, c_in;         // kind 1: operand indices (A, B among step1's inputs, C among step2's)
+    SbnContractParams k;          // kind 2
+    int a_in, b_in, c_in;         // kinds 1, 2: operand indices (A, B among step1's inputs, C among step2's)
     int64_t tile_off_pos;         // int32 offset into the pair tile table
     int64_t canon_pos;            // float offset into the canonical coefficient buffer
 };
