@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SBN_ABI_VERSION 20
+#define SBN_ABI_VERSION 21
 
 #define SBN_OK 0
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
@@ -332,17 +332,30 @@ int sbn_sampler_run_host(sbn_sampler *sampler, int algo, const uint8_t *ev, int6
  * N_j = sum_k N_jk:
  *   SBN_SCORE_BIC:  sum_jk N_jk ln(N_jk / N_j) - ln(N) q (r - 1) / 2, with 0 ln 0 = 0;
  *   SBN_SCORE_BDEU: sum_j [lgamma(a/q) - lgamma(N_j + a/q) + sum_k (lgamma(N_jk + a/(q r)) - lgamma(a/(q r)))],
- *                   a = ess > 0, the equivalent sample size (ignored by BIC). */
+ *                   a = ess > 0, the equivalent sample size (ignored by BIC).
+ * sbn_tally_tests: conditional-independence tests X _|_ Y | S for constraint-based learning.  A test's words are
+ * those of a family with x as the child and y as parent 1: k x y s1 .. s(k-2), k >= 2, so its table is
+ * [s_(k-2)] .. [s_1][y][x], x fastest, and a configuration z of S is a stratum of r_x r_y contiguous entries.
+ * out[3 t .. 3 t + 2] = statistic, degrees of freedom, p-value of test t, in double.  Per stratum, N_z is its rows,
+ * N_xz = sum_y N_xyz and N_yz = sum_x N_xyz:
+ *   SBN_TEST_G2:   G^2 = 2 sum N_xyz ln(N_xyz N_z / (N_xz N_yz)) over the non-zero cells;
+ *   SBN_TEST_CHI2: X^2 = sum (N_xyz - E)^2 / E, E = N_xz N_yz / N_z, over the cells with E > 0.
+ * dof = sum_z (a_z - 1)(b_z - 1), a_z (b_z) the states of x (y) with N_xz > 0 (N_yz > 0); an empty stratum adds 0.
+ * p = Q(dof / 2, stat / 2), the regularised upper incomplete gamma function, and 1 when dof = 0.  k < 2 and an
+ * unknown kind are SBN_E_INVALID; the words are checked as sbn_tally_counts checks them. */
 typedef struct sbn_tally sbn_tally;
 #define SBN_TALLY_MAX_TABLE (1 << 22)  /* entries of one family's table                         */
 #define SBN_TALLY_SMEM_BINS 32768      /* shared-memory bins of one group; larger tables go global */
 #define SBN_SCORE_BIC 0
 #define SBN_SCORE_BDEU 1
+#define SBN_TEST_G2 0    /* likelihood-ratio G^2 */
+#define SBN_TEST_CHI2 1  /* Pearson X^2          */
 int sbn_tally_create(int device, const uint8_t *codes, int64_t ld, int32_t n_vars, int64_t n_rows, const int32_t *cards,
                      sbn_tally **out);
 int sbn_tally_counts(sbn_tally *tally, const int32_t *words, int64_t n_words, uint64_t *counts, int64_t n_counts);
 int sbn_tally_scores(sbn_tally *tally, const int32_t *words, int64_t n_words, int kind, double ess, double *scores,
                      int64_t n_families);
+int sbn_tally_tests(sbn_tally *tally, const int32_t *words, int64_t n_words, int kind, double *out, int64_t n_tests);
 void sbn_tally_destroy(sbn_tally *tally);
 
 /* ------------------------------------------------------------------ loopy belief propagation

@@ -17,7 +17,9 @@
 //   * global path (sbn_tally_count_global): a family whose table alone exceeds the budget counts with 64-bit global
 //     atomics straight from HBM.
 //
-// sbn_tally_score then reduces every table of the batch to its BIC or BDeu score in double, one CTA per family.
+// sbn_tally_score then reduces every table of the batch to its BIC or BDeu score in double, one CTA per family;
+// sbn_tally_test reduces every table of a batch of conditional-independence tests to its G^2 or X^2 statistic,
+// degrees of freedom and p-value, one CTA per test (constraint-based learning, structure.pc).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -38,6 +40,9 @@ constexpr int kMatchBins = 256;  // up to this many, by warp-aggregated incremen
 constexpr int kMaxAxes = 22;     // members with more than one state: 2^22 >= every table the ABI accepts
 constexpr int kDescWords = 4 + 2 * kMaxAxes;  // off, T, n_ax, pad | (slot, stride) per axis
 constexpr int kScoreThreads = 128;
+constexpr int kTestThreads = 256;
+constexpr int kTestWarps = kTestThreads / 32;
+constexpr int kThreadStratum = 32;  // strata of at most this many cells are reduced one per thread, larger ones one per warp
 constexpr unsigned kFull = 0xffffffffu;
 
 struct FamScore {
@@ -200,6 +205,178 @@ sbn_tally_score(const unsigned long long *__restrict__ counts, const FamScore *_
 
 namespace {
 
+// log(1 + d) - d, by its series where the two terms would cancel
+__device__ double log1pmx(double d) {
+    if (fabs(d) > 0.5) return log1p(d) - d;
+    double pw = d, sum = 0.0;
+    for (int k = 2; k < 100; ++k) {
+        pw *= -d;
+        const double term = pw / k;
+        sum += term;
+        if (fabs(term) <= 1e-17 * fabs(sum)) break;
+    }
+    return sum;
+}
+
+// Q(a, x), the regularised upper incomplete gamma function, for a > 0 and x > 0: the series of P below a + 1, the
+// continued fraction of Q (modified Lentz) above.  The prefactor x^a e^-x / Gamma(a) is taken in the log domain;
+// from a = 10 on through Stirling's series, a log1pmx((x - a) / a) + ln(a / 2 pi) / 2 - (the correction to
+// Stirling), which keeps its absolute error near 1e-13 at a = 2^21 where a ln x and lgamma(a) are both ~3e7.
+__device__ __noinline__ double upper_gamma_q(double a, double x) {
+    double lp;
+    if (a < 10.0) {
+        lp = a * log(x) - x - lgamma(a);
+    } else {
+        const double ia = 1.0 / a, ia2 = ia * ia;
+        const double corr = ia * (1.0 / 12 - ia2 * (1.0 / 360 - ia2 * (1.0 / 1260 - ia2 / 1680)));
+        lp = a * log1pmx((x - a) * ia) + 0.5 * log(a / (2.0 * 3.14159265358979323846)) - corr;
+    }
+    if (x < a + 1.0) {
+        double ap = a, del = 1.0 / a, sum = del;
+        for (int n = 0; n < 1000000; ++n) {
+            ap += 1.0;
+            del *= x / ap;
+            sum += del;
+            if (fabs(del) <= 1e-17 * fabs(sum)) break;
+        }
+        return 1.0 - sum * exp(lp);
+    }
+    constexpr double kTiny = 1e-300;
+    double b = x + 1.0 - a, c = 1.0 / kTiny, d = 1.0 / b, h = d;
+    for (int i = 1; i < 1000000; ++i) {
+        const double an = -i * (i - a);
+        b += 2.0;
+        d = an * d + b;
+        if (fabs(d) < kTiny) d = kTiny;
+        c = b + an / c;
+        if (fabs(c) < kTiny) c = kTiny;
+        d = 1.0 / d;
+        const double del = d * c;
+        h *= del;
+        if (fabs(del - 1.0) <= 1e-16) break;
+    }
+    return exp(lp) * h;
+}
+
+// The contribution of one cell with count n, margins nx = N_xz and ny = N_yz in a stratum of nz rows: G^2 / 2
+// (the factor 2 is applied to the sum) over the non-zero cells, X^2 over the cells whose expected count is > 0.
+__device__ __forceinline__ double test_cell(int kind, double n, double nx, double ny, double nz) {
+    if (kind == SBN_TEST_G2) return n > 0.0 ? n * log(n * nz / (nx * ny)) : 0.0;
+    if (nx == 0.0 || ny == 0.0) return 0.0;
+    const double e = nx * ny / nz, r = n - e;
+    return r * r / e;
+}
+
+}  // namespace
+
+// One CTA per test: the table [..][y][x] of test `blockIdx.x` (x fastest) is a run of strata of rx * ry entries.
+// A stratum of at most kThreadStratum cells is reduced by one thread, recomputing its margins per cell; a larger
+// one by one warp, with its margins in shared memory.  Thread (warp) i takes strata i, i + 256 (8), ..; each
+// thread sums its cells in a fixed order and the CTA adds the threads in a fixed tree, so the result is bitwise
+// reproducible.  Margins and dof are exact integers (every count is below 2^32).
+__global__ void __launch_bounds__(kTestThreads)
+sbn_tally_test(const unsigned long long *__restrict__ counts, const FamScore *__restrict__ fams,
+               const int32_t *__restrict__ ry_of, int kind, double *__restrict__ out) {
+    __shared__ uint32_t marg[kTestWarps][2][256];
+    __shared__ double part[kTestThreads];
+    __shared__ long long dpart[kTestThreads];
+    const FamScore fm = fams[blockIdx.x];
+    const int rx = fm.r, ry = ry_of[blockIdx.x], S = rx * ry;
+    const long long n_strata = fm.T / S;
+    const unsigned long long *tab = counts + fm.off;
+    double acc = 0.0;
+    long long dof = 0;
+    if (S <= kThreadStratum) {
+        for (long long z = threadIdx.x; z < n_strata; z += kTestThreads) {
+            const unsigned long long *c = tab + z * S;
+            unsigned long long nz = 0;
+            int a = 0, b = 0;
+            for (int x = 0; x < rx; ++x) {
+                unsigned long long s = 0;
+                for (int y = 0; y < ry; ++y) s += c[y * rx + x];
+                a += s > 0;
+                nz += s;
+            }
+            if (nz == 0) continue;  // an empty stratum adds nothing
+            for (int y = 0; y < ry; ++y) {
+                unsigned long long s = 0;
+                for (int x = 0; x < rx; ++x) s += c[y * rx + x];
+                b += s > 0;
+            }
+            dof += static_cast<long long>(a - 1) * (b - 1);
+            const double dz = static_cast<double>(nz);
+            for (int y = 0; y < ry; ++y) {
+                unsigned long long ny = 0;
+                for (int x = 0; x < rx; ++x) ny += c[y * rx + x];
+                for (int x = 0; x < rx; ++x) {
+                    unsigned long long nx = 0;
+                    for (int y2 = 0; y2 < ry; ++y2) nx += c[y2 * rx + x];
+                    acc += test_cell(kind, static_cast<double>(c[y * rx + x]), static_cast<double>(nx),
+                                     static_cast<double>(ny), dz);
+                }
+            }
+        }
+    } else {
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+        uint32_t *mx = marg[warp][0], *my = marg[warp][1];
+        for (long long z = warp; z < n_strata; z += kTestWarps) {
+            const unsigned long long *c = tab + z * S;
+            unsigned long long nz = 0;
+            int a = 0, b = 0;
+            for (int x = lane; x < rx; x += 32) {
+                unsigned long long s = 0;
+                for (int y = 0; y < ry; ++y) s += c[y * rx + x];
+                mx[x] = static_cast<uint32_t>(s);
+                a += s > 0;
+                nz += s;
+            }
+            for (int y = lane; y < ry; y += 32) {
+                unsigned long long s = 0;
+                for (int x = 0; x < rx; ++x) s += c[y * rx + x];
+                my[y] = static_cast<uint32_t>(s);
+                b += s > 0;
+            }
+            for (int o = 16; o > 0; o >>= 1) {
+                nz += __shfl_xor_sync(kFull, nz, o);
+                a += __shfl_xor_sync(kFull, a, o);
+                b += __shfl_xor_sync(kFull, b, o);
+            }
+            __syncwarp();
+            if (nz != 0) {
+                if (lane == 0) dof += static_cast<long long>(a - 1) * (b - 1);
+                const double dz = static_cast<double>(nz);
+                for (int i = lane; i < S; i += 32) {
+                    const int y = i / rx, x = i - y * rx;
+                    acc += test_cell(kind, static_cast<double>(c[i]), static_cast<double>(mx[x]),
+                                     static_cast<double>(my[y]), dz);
+                }
+            }
+            __syncwarp();  // every lane is done with the margins before the next stratum rewrites them
+        }
+    }
+    part[threadIdx.x] = acc;
+    dpart[threadIdx.x] = dof;
+    __syncthreads();
+    for (int w = kTestThreads / 2; w > 0; w >>= 1) {
+        if (threadIdx.x < w) {
+            part[threadIdx.x] += part[threadIdx.x + w];
+            dpart[threadIdx.x] += dpart[threadIdx.x + w];
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        const double stat = kind == SBN_TEST_G2 ? 2.0 * part[0] : part[0];
+        const long long df = dpart[0];
+        double p = 1.0;
+        if (df > 0 && stat > 0.0) p = upper_gamma_q(0.5 * static_cast<double>(df), 0.5 * stat);
+        out[3LL * blockIdx.x] = stat;
+        out[3LL * blockIdx.x + 1] = static_cast<double>(df);
+        out[3LL * blockIdx.x + 2] = p;
+    }
+}
+
+namespace {
+
 // One parsed batch: the descriptors of every family (groups' families consecutive), the staged columns of every
 // group, and how each group or global family is launched.
 struct Launch {
@@ -230,6 +407,8 @@ struct sbn_tally {
     int64_t counts_cap = 0;
     void *d_words = nullptr;  // descriptors, staged columns, score records, scores
     int64_t words_cap = 0;
+    void *d_tests = nullptr;  // the y cards of a batch of tests, then its [n_tests][3] results
+    int64_t tests_cap = 0;
     cudaStream_t stream = nullptr;
 };
 
@@ -480,6 +659,44 @@ int sbn_tally_scores(sbn_tally *t, const int32_t *words, int64_t n_words, int ki
     return SBN_OK;
 }
 
+int sbn_tally_tests(sbn_tally *t, const int32_t *words, int64_t n_words, int kind, double *out, int64_t n_tests) {
+    if (!t || !out) return sbn_fail(SBN_E_INVALID, "null argument");
+    if (kind != SBN_TEST_G2 && kind != SBN_TEST_CHI2) return sbn_fail(SBN_E_INVALID, "unknown test kind %d", kind);
+    Batch B;
+    int rc = parse_batch(t, words, n_words, B);
+    if (rc != SBN_OK) return rc;
+    if (n_tests != static_cast<int64_t>(B.fams.size()))
+        return sbn_fail(SBN_E_INVALID, "the words hold %zu tests, not %lld", B.fams.size(), static_cast<long long>(n_tests));
+    // parse_batch has checked every test's words; a test needs x and y
+    std::vector<int32_t> ry(B.fams.size());
+    for (int64_t p = 0, f = 0; p < n_words; p += 1 + words[p], ++f) {
+        if (words[p] < 2) return sbn_fail(SBN_E_INVALID, "test %lld: %d members, at least x and y are needed",
+                                          static_cast<long long>(f), words[p]);
+        ry[f] = t->card[words[p + 2]];
+    }
+    FamScore *d_fams;
+    double *d_scores;
+    rc = run_counts(t, B, &d_fams, &d_scores);
+    if (rc != SBN_OK) return rc;
+    const int64_t ry_bytes = round_up(n_tests * 4, 256);
+    const int64_t need = ry_bytes + n_tests * 3 * static_cast<int64_t>(sizeof(double));
+    if (need > t->tests_cap) {
+        if (t->d_tests) SBN_TALLY_CUDA(cudaFree(t->d_tests));
+        t->d_tests = nullptr;
+        t->tests_cap = 0;
+        SBN_TALLY_CUDA(cudaMalloc(&t->d_tests, need));
+        t->tests_cap = need;
+    }
+    int32_t *d_ry = static_cast<int32_t *>(t->d_tests);
+    double *d_out = reinterpret_cast<double *>(static_cast<char *>(t->d_tests) + ry_bytes);
+    SBN_TALLY_CUDA(cudaMemcpyAsync(d_ry, ry.data(), n_tests * 4, cudaMemcpyHostToDevice, t->stream));
+    sbn_tally_test<<<static_cast<unsigned>(n_tests), kTestThreads, 0, t->stream>>>(t->d_counts, d_fams, d_ry, kind, d_out);
+    SBN_TALLY_CUDA(cudaGetLastError());
+    SBN_TALLY_CUDA(cudaMemcpyAsync(out, d_out, n_tests * 3 * sizeof(double), cudaMemcpyDeviceToHost, t->stream));
+    SBN_TALLY_CUDA(cudaStreamSynchronize(t->stream));
+    return SBN_OK;
+}
+
 void sbn_tally_destroy(sbn_tally *t) {
     if (!t) return;
     cudaSetDevice(t->device);
@@ -487,6 +704,7 @@ void sbn_tally_destroy(sbn_tally *t) {
     cudaFree(t->d_codes);
     cudaFree(t->d_counts);
     cudaFree(t->d_words);
+    cudaFree(t->d_tests);
     if (t->stream) cudaStreamDestroy(t->stream);
     delete t;
 }

@@ -16,7 +16,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libsorobn_
 _lib = None
 
 SBN_OK = 0
-ABI_VERSION = 20
+ABI_VERSION = 21
 
 
 class EngineError(RuntimeError):
@@ -129,6 +129,8 @@ def load():
     lib.sbn_tally_counts.argtypes = [vp, vp, i64, vp, i64]
     lib.sbn_tally_scores.restype = i32
     lib.sbn_tally_scores.argtypes = [vp, vp, i64, i32, c.c_double, vp, i64]
+    lib.sbn_tally_tests.restype = i32
+    lib.sbn_tally_tests.argtypes = [vp, vp, i64, i32, vp, i64]
     lib.sbn_tally_destroy.restype = None
     lib.sbn_tally_destroy.argtypes = [vp]
     lib.sbn_bp_create.restype = i32
@@ -162,7 +164,7 @@ EXPORTS = (
     "sbn_program_joint_host_f64",
     "sbn_program_info", "sbn_program_set_graph", "sbn_program_set_tiled", "sbn_gibbs_create", "sbn_gibbs_run_host",
     "sbn_sampler_run_host", "sbn_gibbs_conditional", "sbn_gibbs_destroy", "sbn_tally_create", "sbn_tally_counts",
-    "sbn_tally_scores", "sbn_tally_destroy", "sbn_bp_create", "sbn_bp_run_host", "sbn_bp_mpe_host", "sbn_bp_destroy",
+    "sbn_tally_scores", "sbn_tally_tests", "sbn_tally_destroy", "sbn_bp_create", "sbn_bp_run_host", "sbn_bp_mpe_host", "sbn_bp_destroy",
     "sbn_host_alloc",
     "sbn_host_free",
 )
@@ -579,6 +581,7 @@ class Tally:
     uploaded once.  A family is a sequence of column ids, the child first and its parents after it."""
 
     SCORES = {"bic": 0, "bdeu": 1}
+    TESTS = {"g2": 0, "chi2": 1}
 
     def __init__(self, codes, cards, device: int | None = None):
         lib = load()
@@ -618,6 +621,16 @@ class Tally:
         out = np.empty(len(families), dtype=np.float64)
         _check(load().sbn_tally_scores(self._h, words.ctypes.data, words.size, self.SCORES[kind], float(ess),
                                        out.ctypes.data, out.size))
+        return out
+
+    def tests(self, tests, kind: str = "g2") -> np.ndarray:
+        """Conditional-independence tests x _|_ y | S, each a sequence of column ids x, y, *S: float64 [n, 3] of
+        (statistic, degrees of freedom, p-value), with the G^2 ("g2") or Pearson X^2 ("chi2") statistic; only
+        these leave the device (include/sorobn_b200.h, sbn_tally_tests)."""
+        words = self._words(tests)
+        out = np.empty((len(tests), 3), dtype=np.float64)
+        _check(load().sbn_tally_tests(self._h, words.ctypes.data, words.size, self.TESTS[kind], out.ctypes.data,
+                                      len(tests)))
         return out
 
     def close(self):
