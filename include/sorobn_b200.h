@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SBN_ABI_VERSION 21
+#define SBN_ABI_VERSION 22
 
 #define SBN_OK 0
 #define SBN_E_INVALID (-1)   /* malformed program / bad argument            */
@@ -374,7 +374,15 @@ void sbn_tally_destroy(sbn_tally *tally);
  * codes[k * ld_codes + b] = the decoded state of the k-th unobserved variable (var id order; codes may be NULL when
  * there is none), log_p[b] = log P(decode, observed cells) in double (-inf for a decode of probability 0, NaN for
  * a row that met a zero sum, whose codes are 0) and iterations[b] as above (0 when every node is observed).
- * Same argument rules as sbn_bp_run_host. */
+ * Same argument rules as sbn_bp_run_host.
+ * sbn_bp_counts_host: expected-counts words of bp.compile_counts_graph (version 3; bp.py "Expected counts"): the
+ * sum-product sweep over every CPT, then per row the belief of every family, summed over the live rows into
+ * counts[n_table_floats] (double, blob order: entry i counts the configuration of table entry i; bp.Graph.perm maps
+ * it to the dense CPTs) without floating-point atomics, so two calls are bitwise equal; log_z[b] = the Bethe
+ * log-likelihood of row b in double (NaN for a dead row, which adds nothing) and iterations[b] as above (0 for a row
+ * dead before its first sweep and when every node is observed).  Same argument rules as sbn_bp_run_host.  Each run
+ * call refuses the words of the others, naming the call that runs them.
+ * sbn_bp_set_tables: new float32 tables of the same size for the handle's words (an EM iteration's CPTs). */
 typedef struct sbn_bp sbn_bp;
 int sbn_bp_create(int device, const int32_t *words, int64_t n_words, const float *tables, int64_t n_table_floats,
                   sbn_bp **out);
@@ -382,6 +390,9 @@ int sbn_bp_run_host(sbn_bp *bp, const uint8_t *ev, int64_t ld_ev, int64_t n_rows
                     float tol, float *out, int64_t ld_out, int32_t *iterations);
 int sbn_bp_mpe_host(sbn_bp *bp, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int32_t n_iterations,
                     float damping, float tol, uint8_t *codes, int64_t ld_codes, double *log_p, int32_t *iterations);
+int sbn_bp_counts_host(sbn_bp *bp, const uint8_t *ev, int64_t ld_ev, int64_t n_rows, int32_t n_iterations,
+                       float damping, float tol, double *counts, double *log_z, int32_t *iterations);
+int sbn_bp_set_tables(sbn_bp *bp, const float *tables, int64_t n_table_floats);
 void sbn_bp_destroy(sbn_bp *bp);
 
 /* Pinned host memory for evidence / posterior staging buffers. */

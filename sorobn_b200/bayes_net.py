@@ -33,7 +33,9 @@ other unobserved variables summed out: one log-sum-exp, then max-sum program per
 family or of chosen groups of variables, one joint program per pattern (planner.build_joint_plan).
 `marginals_many(..., algorithm="bp")` approximates every marginal by loopy belief propagation on the device, one
 row per thread (sorobn_b200/bp.py, csrc/sbn_bp.cu), for networks too wide to eliminate exactly, and
-`mpe_many(..., algorithm="bp")` decodes every row by max-product belief propagation there.
+`mpe_many(..., algorithm="bp")` decodes every row by max-product belief propagation there, and
+`expected_counts(..., algorithm="bp")` / `fit_em(..., algorithm="bp")` take their E-step from the family beliefs of
+sum-product belief propagation (bp.compile_counts_graph), reduced on the device.
 """
 from __future__ import annotations
 
@@ -119,6 +121,21 @@ def _check_possible(index, rows, impossible, consequence):
     if impossible.any():
         raise ValueError(f"{int(impossible.sum())} row(s) have observed cells of probability zero "
                          f"(first: {index[rows[impossible][0]]!r}); {consequence}")
+
+
+class _BpCounts:
+    """The expected-counts graph of one missingness pattern on the device: the engine handle and `perm`, which maps
+    the device's blob-order counts back to the dense CPTs and the dense CPTs to the blob."""
+
+    def __init__(self, net, ev, device):
+        from . import engine
+
+        g = _bp.compile_counts_graph(net, ev)
+        self.perm = g.perm
+        self.runner = engine.BeliefPropagation(g.words, g.tables, device=device)
+
+    def close(self):
+        self.runner.close()
 
 
 class BayesNet:
@@ -394,7 +411,8 @@ class BayesNet:
         return self.partial_fit(X)
 
     # ------------------------------------------------------- expected counts / EM
-    def expected_counts(self, X: pd.DataFrame, likelihoods: dict | None = None) -> dict:
+    def expected_counts(self, X: pd.DataFrame, likelihoods: dict | None = None, algorithm="exact", n_iterations=100,
+                        damping=0.5, tol=1e-5) -> dict:
         """The E-step of expectation-maximisation: for every node v, the sum over the rows of `X` of
         P(v, parents(v) | the row's observed cells), computed on the GPU.
 
@@ -410,7 +428,34 @@ class BayesNet:
         likelihoods: soft (virtual) evidence, {node: values} with one likelihood row per row of `X`, as in
         `query_many`: the counts are then those of P(v, parents(v) | observed cells, likelihoods).  A soft
         node may not be a column of `X`; a row whose cells and likelihoods have probability zero (an
-        all-zero likelihood row makes one) raises ValueError."""
+        all-zero likelihood row makes one) raises ValueError.
+
+        algorithm="bp": each row's family posteriors are the family beliefs of sum-product loopy belief propagation
+        instead (sorobn_b200/bp.py, "Expected counts", defines them), for networks whose induced width the exact
+        planner refuses.  Every CPT is a factor and every unobserved node a variable; messages are swept and damped
+        as in `marginals_many(algorithm="bp")` (n_iterations, damping, tol as there), then the device forms every
+        family belief of the row and sums them over the rows.  One compiled graph per missingness pattern; the same
+        {node: Series} as the exact path, equal to it on polytrees.  A row whose messages or beliefs sum to zero, or
+        whose observed cells alone hit a CPT entry of zero, raises the exact path's ValueError; on loopy networks BP
+        may miss impossible evidence, whose rows then add counts silently.  Rows that did not converge add the
+        beliefs of their last sweep and raise one RuntimeWarning with their count.  No soft evidence."""
+        if algorithm not in ("exact", "bp"):
+            raise ValueError("Unknown algorithm, must be one of: exact, bp")
+        if algorithm == "bp":
+            if likelihoods is not None:
+                self._check_soft_call(algorithm, None)
+            _bp.check_arguments(n_iterations, damping, tol)
+            groups = self._count_patterns(X)
+            net = self._compiled
+            offsets, n_counts = _planner.count_layout(net)
+            # each pattern's graph is fetched right before it runs, as in `sample_many`
+            counts, _, stuck = self._bp_e_step(
+                X, groups, lambda k, ev: self._cached(("bp_counts", ev), lambda: _BpCounts(net, ev, self.device)),
+                n_counts, n_iterations, damping, tol)
+            if stuck:
+                self._warn_bp_stuck(f"{stuck} of {len(X.index)} rows", n_iterations, tol)
+            return {name: pd.Series(counts[offsets[v]:offsets[v] + int(np.prod(net.cpt[v].shape))],
+                                    index=self._family_index(v), name=name) for v, name in enumerate(net.names)}
         groups = self._count_patterns(X)
         soft = self._pattern_soft(likelihoods, X)
         net = self._compiled
@@ -508,7 +553,8 @@ class BayesNet:
             [net.domains[u] for u in ids], names=[net.names[u] for u in ids])) for g, ids, d in zip(entries, gids, dense)}
 
     def fit_em(self, X: pd.DataFrame, max_iter: int = 100, tol: float = 1e-6,
-               likelihoods: dict | None = None) -> "BayesNet":
+               likelihoods: dict | None = None, algorithm="exact", n_iterations=100, damping=0.5,
+               bp_tol=1e-5) -> "BayesNet":
         """Fit the CPTs to `X` by expectation-maximisation, when cells are missing (None / NaN) or nodes
         are latent (no column in `X`).
 
@@ -525,7 +571,22 @@ class BayesNet:
 
         likelihoods: soft evidence (e.g. probabilistic labels of a latent node), as in `expected_counts`.  They
         stay fixed across the iterations, and `em_log_likelihood_` holds sum_b log P(observed cells of b,
-        likelihoods of b), on the scale of the given likelihoods."""
+        likelihoods of b), on the scale of the given likelihoods.
+
+        algorithm="bp": Bethe-EM, for networks whose induced width the exact planner refuses.  Each E-step is
+        `expected_counts(algorithm="bp")` with n_iterations, damping and `bp_tol` (its tol; `tol` stays EM's), one
+        graph compiled per missingness pattern and only its tables replaced per iteration.  Every other rule is the
+        exact one (start, prior_count, write-back, `_P_sizes`, the stopping rule), with the log-likelihood replaced by
+        the sum of the rows' Bethe log-likelihoods (bp.py, "Expected counts"), which `em_log_likelihood_` then
+        holds: exact on polytrees, an approximation of log P on loopy networks.  Bethe-EM is not monotone; a
+        decrease also stops the loop.  On loopy networks BP can miss impossible evidence, whose rows then add counts
+        silently.  Rows that did not converge in some E-step raise one RuntimeWarning per call.  No soft evidence."""
+        if algorithm not in ("exact", "bp"):
+            raise ValueError("Unknown algorithm, must be one of: exact, bp")
+        if algorithm == "bp":
+            if likelihoods is not None:
+                self._check_soft_call(algorithm, None)
+            _bp.check_arguments(n_iterations, damping, bp_tol)
         if int(max_iter) < 1:
             raise ValueError(f"max_iter must be at least 1, not {max_iter}")
         if all(n in self.P for n in self.nodes):
@@ -542,15 +603,29 @@ class BayesNet:
         net = self._compiled
         offsets, n_counts = _planner.count_layout(net)
         n_rows = len(X.index)
-        runners = [_Programs(_planner.build_pattern_plan(net, "counts", ev, soft=soft), self.device) for ev, _, _ in groups]
+        if algorithm == "bp":
+            runners = [_BpCounts(net, ev, self.device) for ev, _, _ in groups]
+        else:
+            runners = [_Programs(_planner.build_pattern_plan(net, "counts", ev, soft=soft), self.device)
+                       for ev, _, _ in groups]
         cpts = [np.array(c, dtype=np.float64) for c in net.cpt]
         lls = []
+        stuck = 0
         try:
             for it in range(int(max_iter)):
-                if it:
-                    for r in runners:
-                        r.set_cpts(cpts)
-                counts, ll = self._e_step(X, groups, lambda k, ev: runners[k], n_counts, lik)
+                if algorithm == "bp":
+                    if it:
+                        flat = np.concatenate([c.reshape(-1) for c in cpts])
+                        for r in runners:
+                            r.runner.set_tables(flat[r.perm])
+                    counts, ll, s = self._bp_e_step(X, groups, lambda k, ev: runners[k], n_counts, n_iterations,
+                                                    damping, bp_tol)
+                    stuck = max(stuck, s)
+                else:
+                    if it:
+                        for r in runners:
+                            r.set_cpts(cpts)
+                    counts, ll = self._e_step(X, groups, lambda k, ev: runners[k], n_counts, lik)
                 lls.append(ll)
                 fam = [counts[offsets[v]:offsets[v] + c.size].reshape(c.shape) for v, c in enumerate(cpts)]
                 if self.prior_count:
@@ -563,6 +638,8 @@ class BayesNet:
         finally:
             for r in runners:
                 r.close()
+        if stuck:
+            self._warn_bp_stuck(f"up to {stuck} of {n_rows} rows per E-step", n_iterations, bp_tol)
         self.em_log_likelihood_ = lls
         self._write_cpts(cpts, keep=[f.reshape(-1) > 0 for f in fam])
         for v, node in enumerate(net.names):
@@ -742,6 +819,26 @@ class BayesNet:
             _check_possible(X.index, rows, np.isnan(prob), "their expected counts are undefined")
             ll += float(np.log(prob).sum()) if lik is None else float(log_ev.sum())
         return counts, ll
+
+    def _bp_e_step(self, X, groups, runner_of, n_counts, n_iterations, damping, tol):
+        """(expected counts [n_counts] in count_layout order, sum of the rows' Bethe log-likelihoods, rows that did
+        not converge) of belief propagation over every pattern; `runner_of(k, observed var ids)` gives pattern k's
+        `_BpCounts`.  Dead rows raise the exact path's ValueError."""
+        counts = np.zeros(n_counts, dtype=np.float64)
+        ll, stuck = 0.0, 0
+        for k, (ev, rows, codes) in enumerate(groups):
+            r = runner_of(k, ev)
+            c, log_z, iters = r.runner.counts(codes, len(rows), n_iterations, damping, tol)
+            _check_possible(X.index, rows, np.isnan(log_z), "their expected counts are undefined")
+            counts[r.perm] += c
+            ll += float(log_z.sum())
+            stuck += int(np.count_nonzero(iters > n_iterations))
+        return counts, ll, stuck
+
+    @staticmethod
+    def _warn_bp_stuck(which, n_iterations, tol):
+        warnings.warn(f"belief propagation: {which} did not converge to tol={tol:g} in {n_iterations} sweeps; they "
+                      "add the beliefs of their last sweep", RuntimeWarning, stacklevel=3)
 
     def sample_many(self, events: pd.DataFrame, n: int = 1, seed: int | None = None,
                     likelihoods: dict | None = None) -> pd.DataFrame:

@@ -66,6 +66,35 @@ maximisers (even on a polytree: A uniform and B = not A decode A=0, B=0), and lo
 dead row reports NaN and codes 0.  A pattern that observes every node has 0 variables and 0 edges: it runs no sweep,
 records 0 and returns only its score.
 
+Expected counts (the E-step of EM; `compile_counts_graph`, `BayesNet.expected_counts(algorithm="bp")`)
+-------------------------------------------------------------------------------------------------------
+Factor graph.  The max-product graph: every CPT is a factor, with nothing pruned, because every family needs counts;
+every unobserved node is a variable; a family whose members are all observed is kept with 0 members.  (In
+sum-product a barren unobserved node sends uniform messages, so keeping it changes no other belief; its family gets
+P(v | pa) b(pa).)
+
+Sweep.  The sum-product sweep above, unchanged: damping, residual, tol, the n_iterations + 1 record, the zero rule and
+the double products with their 2^64 rescale.  As in max-product, a row whose codes hit a 0 entry of a 0-member factor
+is dead before the first sweep: it runs no sweep and records 0, and so does a pattern that observes every node.
+
+Family beliefs.  After the row's last sweep, for every factor f with at least one member,
+    b_f(x_f) ∝ f(x_f, e) prod_{v ∈ f} nu_{v->f}(x_v),
+formed in double from the last sweep's nu and normalised over the configurations of the unobserved members.  A
+0-member factor has belief 1 at the row's codes.  A belief that sums to 0 makes the row dead.
+
+Variable beliefs.  b_v is the normalised product of v's mu (the sum-product belief), formed in double.
+
+Bethe log-likelihood of a row, in double with 0 log 0 = 0:
+    log Z_B = sum_f sum_{x_f} b_f (log f - log b_f) + sum_v (d_v - 1) sum_x b_v log b_v,
+d_v being the number of factors v is an unobserved member of; each 0-member factor adds log f(e).  On a polytree at
+BP's fixed point it equals log P(e) exactly; on a pattern that observes every node it is log P(row).  (The device
+and the replay sum each factor's terms as H / S + log S, with p = f prod nu, S = sum p and H = sum p (log f - log p),
+which is the same number up to rounding.)
+
+Expected counts.  Each live row adds its b_f into the count entry of (x_f, the row's evidence codes).  A dead row adds
+nothing, and its log Z_B is NaN.  The device adds the rows without floating-point atomics, so two runs are bitwise
+equal.
+
 Words (int32; `sbn_bp_create` bounds-checks every one)
 ------------------------------------------------------
     header : MAGIC 1 n_ev n_factors n_vars E n_targets Q n_table_floats fac_pos var_pos tgt_pos
@@ -82,7 +111,9 @@ variables their ids; targets are sorted by name, each at rows q_offset .. q_offs
 
 Version 2 (max-product) has the same layout, with three differences: a factor record may have n_mem = 0; n_vars
 and E may be 0; the target section lists every variable record in variable order, with q_offset = its position,
-its row of the codes output (Q = n_vars).
+its row of the codes output (Q = n_vars).  Version 3 (expected counts) has the version-2 layout and rules.  Every
+factor's blob is its full CPT transposed, evidence axes included, so the blob is a permutation of the dense CPTs
+concatenated in `planner.count_layout` order: `Graph.perm` gives it (tables64 == concat(cpt).reshape(-1)[perm]).
 """
 from __future__ import annotations
 
@@ -93,6 +124,7 @@ import numpy as np
 MAGIC = 0x53424250  # "SBBP"
 VERSION = 1  # sum-product (compile_graph)
 VERSION_MPE = 2  # max-product (compile_mpe_graph)
+VERSION_COUNTS = 3  # expected counts (compile_counts_graph)
 HEADER_WORDS = 12
 MAX_CARD = 256  # states of an unobserved variable (the kernel's widest message)
 
@@ -108,6 +140,7 @@ class Graph:
     q_offsets: tuple
     Q: int
     n_edges: int  # E: entries of one direction of the message state per row
+    perm: np.ndarray | None = None  # version 3: int64, tables64 == concat of the dense CPTs, flattened, [perm]
 
     def message_bytes_per_sweep(self) -> int:
         """Bytes of message state one sweep of one row accesses in the device scratch, as csrc/sbn_bp.cu walks
@@ -163,6 +196,15 @@ def compile_mpe_graph(net, evidence) -> Graph:
     return _compile(net, evidence, set(range(len(net.names))), variables, VERSION_MPE)
 
 
+def compile_counts_graph(net, evidence) -> Graph:
+    """The expected-counts factor graph of `net` given the evidence var ids (module docstring, "Expected counts"):
+    the graph of `compile_mpe_graph` as version-3 words, with `perm` set."""
+    evidence = [int(e) for e in evidence]
+    observed = set(evidence)
+    variables = [v for v in range(len(net.names)) if v not in observed]
+    return _compile(net, evidence, set(range(len(net.names))), variables, VERSION_COUNTS)
+
+
 def _compile(net, evidence, relevant, targets, version) -> Graph:
     """Words and blob of the factors of the `relevant` CPTs (version 1 drops those with every member observed);
     version 1 targets are sorted by name and span their cards, version 2 targets are every variable in order."""
@@ -178,7 +220,11 @@ def _compile(net, evidence, relevant, targets, version) -> Graph:
         if card[v] > MAX_CARD:
             raise ValueError(f"{net.names[v]!r} has {card[v]} states; belief propagation takes at most {MAX_CARD}")
 
-    fac_words, blobs, families = [], [], []
+    fac_words, blobs, families, perms = [], [], [], []
+    if version == VERSION_COUNTS:
+        from .planner import count_layout
+
+        first = count_layout(net)[0]
     edges_of = {v: [] for v in variables}
     E = 0
     off = 0
@@ -193,6 +239,9 @@ def _compile(net, evidence, relevant, targets, version) -> Graph:
         order = list(reversed(evax)) + list(reversed(members))
         arr = np.transpose(np.asarray(net.cpt[v], dtype=np.float64), [scope.index(u) for u in order])
         blobs.append(np.ascontiguousarray(arr).reshape(-1))
+        if version == VERSION_COUNTS:
+            flat = first[v] + np.arange(arr.size, dtype=np.int64).reshape(np.shape(net.cpt[v]))
+            perms.append(np.transpose(flat, [scope.index(u) for u in order]).reshape(-1))
         rec = [v, off, len(members), len(evax)]
         stride = 1
         for u in members:
@@ -235,8 +284,9 @@ def _compile(net, evidence, relevant, targets, version) -> Graph:
     words = np.asarray(header + fac_flat + var_flat + tgt_flat, dtype=np.int64)
     if words.max(initial=0) >= 2**31 or tables64.size >= 2**31:
         raise ValueError("the factor graph does not fit 32-bit words")
+    perm = (np.concatenate(perms) if perms else np.zeros(0, dtype=np.int64)) if version == VERSION_COUNTS else None
     return Graph(words.astype(np.int32), tables64.astype(np.float32), tables64, tuple(families), tuple(variables),
-                 tuple(targets), tuple(q_offsets), Q, E)
+                 tuple(targets), tuple(q_offsets), Q, E, perm)
 
 
 def check_arguments(n_iterations, damping, tol):

@@ -16,7 +16,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libsorobn_
 _lib = None
 
 SBN_OK = 0
-ABI_VERSION = 21
+ABI_VERSION = 22
 
 
 class EngineError(RuntimeError):
@@ -139,6 +139,10 @@ def load():
     lib.sbn_bp_run_host.argtypes = [vp, vp, i64, i64, i32, c.c_float, c.c_float, vp, i64, vp]
     lib.sbn_bp_mpe_host.restype = i32
     lib.sbn_bp_mpe_host.argtypes = [vp, vp, i64, i64, i32, c.c_float, c.c_float, vp, i64, vp, vp]
+    lib.sbn_bp_counts_host.restype = i32
+    lib.sbn_bp_counts_host.argtypes = [vp, vp, i64, i64, i32, c.c_float, c.c_float, vp, vp, vp]
+    lib.sbn_bp_set_tables.restype = i32
+    lib.sbn_bp_set_tables.argtypes = [vp, vp, i64]
     lib.sbn_bp_destroy.restype = None
     lib.sbn_bp_destroy.argtypes = [vp]
     lib.sbn_host_alloc.restype = i32
@@ -164,7 +168,8 @@ EXPORTS = (
     "sbn_program_joint_host_f64",
     "sbn_program_info", "sbn_program_set_graph", "sbn_program_set_tiled", "sbn_gibbs_create", "sbn_gibbs_run_host",
     "sbn_sampler_run_host", "sbn_gibbs_conditional", "sbn_gibbs_destroy", "sbn_tally_create", "sbn_tally_counts",
-    "sbn_tally_scores", "sbn_tally_tests", "sbn_tally_destroy", "sbn_bp_create", "sbn_bp_run_host", "sbn_bp_mpe_host", "sbn_bp_destroy",
+    "sbn_tally_scores", "sbn_tally_tests", "sbn_tally_destroy", "sbn_bp_create", "sbn_bp_run_host", "sbn_bp_mpe_host", "sbn_bp_counts_host",
+    "sbn_bp_set_tables", "sbn_bp_destroy",
     "sbn_host_alloc",
     "sbn_host_free",
 )
@@ -647,8 +652,8 @@ class Tally:
 
 class BeliefPropagation:
     """Loopy belief propagation over one compiled factor graph on one GPU (csrc/sbn_bp.cu): `words` and `tables` are
-    those of `bp.compile_graph` (sum-product, `run`) or of `bp.compile_mpe_graph` (max-product, `mpe`); the
-    algorithm is defined in sorobn_b200/bp.py."""
+    those of `bp.compile_graph` (sum-product, `run`), of `bp.compile_mpe_graph` (max-product, `mpe`) or of
+    `bp.compile_counts_graph` (expected counts, `counts`); the algorithm is defined in sorobn_b200/bp.py."""
 
     def __init__(self, words, tables, device: int | None = None):
         lib = load()
@@ -656,6 +661,7 @@ class BeliefPropagation:
         words = np.ascontiguousarray(words, dtype=np.int32)
         tables = np.ascontiguousarray(tables, dtype=np.float32)
         self.n_ev, self.n_var, self.Q = int(words[2]), int(words[4]), int(words[7])
+        self.n_table_floats = int(words[8])
         self._h = ctypes.c_void_p()
         _check(lib.sbn_bp_create(self.device, words.ctypes.data, words.size, tables.ctypes.data if tables.size else None,
                                  tables.size, ctypes.byref(self._h)))
@@ -691,6 +697,29 @@ class BeliefPropagation:
                                       out.ctypes.data if self.n_var else None, n_rows, log_p.ctypes.data,
                                       iters.ctypes.data))
         return out, log_p, iters
+
+    def counts(self, codes, n_rows: int, n_iterations: int, damping: float, tol: float):
+        """uint8 evidence codes [n_ev, n_rows] -> (expected counts float64 [n_table_floats] in blob order, summed
+        over the live rows (`Graph.perm` maps them to the dense CPTs); Bethe log-likelihood float64 [n_rows], NaN for
+        a dead row; iterations int32 [n_rows] as `run`, 0 for a row dead before its first sweep and when every node
+        is observed)."""
+        n_rows = int(n_rows)
+        codes = np.ascontiguousarray(codes, dtype=np.uint8)
+        if self.n_ev and codes.shape != (self.n_ev, n_rows):
+            raise ValueError(f"evidence codes have shape {codes.shape}, expected {(self.n_ev, n_rows)}")
+        counts = np.empty(self.n_table_floats, dtype=np.float64)
+        log_z = np.empty(n_rows, dtype=np.float64)
+        iters = np.empty(n_rows, dtype=np.int32)
+        _check(load().sbn_bp_counts_host(self._h, codes.ctypes.data if self.n_ev else None, n_rows, n_rows,
+                                         int(n_iterations), float(damping), float(tol),
+                                         counts.ctypes.data if counts.size else None, log_z.ctypes.data,
+                                         iters.ctypes.data))
+        return counts, log_z, iters
+
+    def set_tables(self, tables):
+        """Replace the float32 table blob by `tables` of the same size (the words stay)."""
+        tables = np.ascontiguousarray(tables, dtype=np.float32)
+        _check(load().sbn_bp_set_tables(self._h, tables.ctypes.data if tables.size else None, tables.size))
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:
